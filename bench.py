@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- genotype-cells/s (N x V) into the Gram on B200, the metric BASELINE.json names.
+"""bench.py -- genotype-cells/s (N x V) into the Gram on H100, the metric BASELINE.json names.
 
     python bench.py --gpus N --steps K --warmup W              # this repo's CUDA path (one rank per GPU)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU algorithm (oracle port)
@@ -9,9 +9,9 @@ per GPU (weak scaling: every rank owns `--variants-per-gpu` variants; 8 ranks x 
 Balding-Nichols-like cohort generated on the device (DESIGN.md "Synthetic generator").
 
 A step = one pass of the hot path over the rank's resident genotype matrix:
-    zero S -> tcgen05 Gram kernel over all V variants -> [N > 1: one NCCL all-reduce of S] -> symmetrize.
+    zero S -> wgmma Gram kernel over all V variants -> [N > 1: one NCCL all-reduce of S] -> symmetrize.
 `value`  = N_samples * V_total * steps / time, inputs resident in HBM (X is 2.5 GB per rank, far larger than the
-           126 MB L2, so no flush is needed between iterations), CUDA-event timed, max over ranks.
+           50 MB L2, so no flush is needed between iterations), CUDA-event timed, max over ranks.
 `e2e`    = the same metric through the public API with HOST inputs: pinned RDD[Seq[Int]] rows (CSR) -> H2D ->
            device encode -> Gram -> centering -> eigensolve -> top-2 PCs back on the host, every step.
 `roofline` = the Gram kernel alone against the tensor-core peak (int8 peak taken as 2 x the measured bf16 figure of
@@ -69,17 +69,43 @@ def parse_args():
     ap.add_argument("--c5-samples", type=int, default=10_000)
     ap.add_argument("--c5-variants-per-gpu", type=int, default=1_250_000, help="0 disables the c5_bf16 leg")
     ap.add_argument("--no-legs", action="store_true", help="skip the c3 and c5_bf16 legs (quick kernel A/B runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed (the symmetric Gram) as DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy: float32 when every value is an integer below 2^24 (exact), else float64.
+    An array larger than its share of DUMP_BYTES is cut to a fixed, seeded sample of its rows, written beside it as
+    <name>_rows.npy, so that two builds given the same arguments can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_BYTES // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        exact32 = a.dtype.kind in "iu" and (a.size == 0 or int(np.abs(a).max()) < (1 << 24))
+        a = a.astype(np.float32 if exact32 else np.float64)
+        if a.nbytes > budget:
+            rows = a.shape[0]
+            keep = max(1, min(rows, budget // max(1, a.nbytes // rows) - 1))
+            idx = np.sort(np.random.default_rng(SEED).choice(rows, keep, replace=False))
+            a = a[idx]
+            np.save(os.path.join(out_dir, f"{name}_rows.npy"), idx.astype(np.float64))
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def load_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return {"bf16_tflops": float(d.get("bf16_tflops", 1590.0)),
-                "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", 1400.0)),
-                "hbm_gbs": float(d.get("hbm_gbs", 6650.0)), "source": "measured"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+        return {"bf16_tflops": float(d.get("bf16_tflops", 989.0)),
+                "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", 989.0)),
+                "hbm_gbs": float(d.get("hbm_gbs", 3350.0)), "source": "measured"}
+    # NVIDIA's H100 SXM data sheet (dense bf16, HBM3) -- a ceiling, not a measurement
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "data sheet"}
 
 
 class ClockSampler(threading.Thread):
@@ -323,7 +349,7 @@ def run_b200(args):
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback)")
+        raise SystemExit("bench.py: no CUDA device (the CUDA path has no CPU fallback)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     numa_note = bind_to_gpu_numa_node(local_rank)      # before any pinned host allocation: first touch on the GPU's node
@@ -335,9 +361,9 @@ def run_b200(args):
     dtype = {"i8": native.DTYPE_I8, "bf16": native.DTYPE_BF16, "e2m1": native.DTYPE_E2M1}[args.dtype]
     eb = {"i8": 1, "bf16": 2, "e2m1": 0.5}[args.dtype]
     tdtype = {"i8": torch.int8, "bf16": torch.bfloat16, "e2m1": torch.uint8}[args.dtype]
-    dname = {"i8": "int8", "bf16": "bf16", "e2m1": "e2m1 (4-bit packed cells, fp32 tensor accumulation, exact)"}[args.dtype]
-    if args.dtype == "e2m1" and args.panel_variants % 256:
-        raise SystemExit("--dtype e2m1 needs --panel-variants % 256 == 0")
+    dname = {"i8": "int8", "bf16": "bf16", "e2m1": "e2m1 (4-bit packed cells, expanded to int8 in shared memory, int32 accumulation, exact)"}[args.dtype]
+    if args.dtype == "e2m1" and args.panel_variants % 128:
+        raise SystemExit("--dtype e2m1 needs --panel-variants % 128 == 0")
     ld = ((vpg + 127) // 128) * 128
     peaks = load_peaks()
 
@@ -425,6 +451,8 @@ def run_b200(args):
     clocks = sampler.stop()
     st1 = nat.stats()
     ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"gram": nat.getGram()})
     if world > 1:
         t = torch.tensor([ms], dtype=torch.float64, device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -452,33 +480,17 @@ def run_b200(args):
     fused_close_ms = sum(gt) / len(gt) if fused else None      # closing barrier(s) + gather, incl. waiting for the slowest peer
     ops = float(n) * (n + 1) * vpg                       # SYRK-minimal ops per launch (SURVEY.md 8d)
     achieved_tops = ops / (kernel_ms * 1e-3) / 1e12
-    mxf4 = args.dtype == "e2m1" and os.environ.get("VPCA_E2M1_MXF4", "1") != "0"
-    peak_mult = 1.0 if args.dtype == "bf16" else (4.0 if mxf4 else 2.0)      # dense nominal: bf16 2.25, int8/fp8 4.5, fp4 9 PF
+    peak_mult = 1.0 if args.dtype == "bf16" else 2.0     # H100 SXM dense nominal: bf16 989, int8 1979 TFLOP/s
     peak = peak_mult * peaks["bf16_tflops"]
-    # DRAM traffic of one launch is an ncu number (dram__bytes_read.sum + dram__bytes_write.sum of `ncu --set full`); it
-    # cannot be measured inside this run.  The last capture is kept in profiles/r2_gram_traffic.json together with the
-    # hash of the kernel source it was taken from: a capture of a different kernel version reads as null, never as stale.
-    traffic, traffic_src = None, None
-    tp = ROOT / "profiles" / "r2_gram_traffic.json"
-    if tp.exists():
-        try:
-            tj = json.loads(tp.read_text())
-            src_hash = native.gramSourceFingerprint()     # code only: comments and whitespace do not count
-            ent = tj.get(args.dtype, {})
-            if ent.get("kernel_code_sha256_16") == src_hash:
-                traffic, traffic_src = ent.get("dram_bytes_per_launch"), ent.get("source")
-        except Exception:
-            traffic = None
-    nominal = {1.0: 2250.0, 2.0: 4500.0, 4.0: 9000.0}[peak_mult]
+    nominal = {1.0: 989.0, 2.0: 1979.0}[peak_mult]
     roofline = {"bound": "tensor", "achieved": achieved_tops, "peak": peak, "unit": "TFLOP/s",
-                "frac": achieved_tops / peak, "traffic": traffic, "traffic_source": traffic_src,
+                "frac": achieved_tops / peak,
                 "kernel": "gram_kernel<cta_group=%d>" % st1["gram_cta_group"], "kernel_ms": kernel_ms,
                 "ops_per_launch": ops, "ops_definition": "SYRK-minimal N(N+1)V (int8 MAC = 2 ops)",
-                "peak_source": "%g x %s bf16 burst TFLOP/s of MEASURED_PEAKS.json (nominal dense ratios: int8/fp8 = 2 x bf16, "
-                               "fp4 = 4 x bf16)" % (peak_mult, peaks["source"]),
+                "peak_source": "%g x bf16 TFLOP/s (%s; H100 dense ratio int8 = 2 x bf16)" % (peak_mult, peaks["source"]),
                 "frac_of_nominal": achieved_tops / nominal, "nominal_peak": nominal,
-                "peak_note": ("frac > 1: the denominator is cuBLAS bf16 throughput (x%g), which itself reaches ~75 %% of the "
-                              "nominal tensor peak on this pool; read frac_of_nominal as the utilisation" % peak_mult)
+                "peak_note": ("frac > 1: the denominator is a measured bf16 throughput (x%g) below the nominal tensor "
+                              "peak; read frac_of_nominal as the utilisation" % peak_mult)
                              if achieved_tops > peak else None,
                 "hbm_gbs_algorithmic": (n * vpg * eb + 4.0 * n * n) / (kernel_ms * 1e-3) / 1e9,
                 "hbm_peak_gbs": peaks["hbm_gbs"]}
@@ -752,13 +764,10 @@ def run_b200(args):
             ms4 = sum(t4) / len(t4)
             nat4.finalizeGram()
             torch.cuda.synchronize()
-            mx = os.environ.get("VPCA_E2M1_MXF4", "1") != "0"
-            alt = {"dtype": "e2m1 (4-bit packed cells in HBM, tcgen05 %s, fp32 accumulation flushed to int32; exact)"
-                            % ("kind::mxf4 with unit block scales" if mx else "kind::f8f6f4"),
+            alt = {"dtype": "e2m1 (4-bit packed cells in HBM, expanded to int8 in shared memory, int32 accumulation; exact)",
                    "kernel_ms": ms4, "cells_per_s_kernel": n * vpg / (ms4 * 1e-3),
                    "achieved_tflops_syrk": ops / (ms4 * 1e-3) / 1e12,
-                   "frac_of_fp4_peak_4x_bf16" if mx else "frac_of_2x_bf16_peak":
-                       ops / (ms4 * 1e-3) / 1e12 / ((4.0 if mx else 2.0) * peaks["bf16_tflops"]),
+                   "frac_of_2x_bf16_peak": ops / (ms4 * 1e-3) / 1e12 / (2.0 * peaks["bf16_tflops"]),
                    "gram_bit_identical_to_int8_path": bool(torch.equal(S4, S)) if world == 1 else None}
         del X4, S4
 
@@ -860,7 +869,7 @@ def run_b200(args):
                     carriers += (Xl.view(torch.int8).view(npan, n_leg, P_leg)[pn] != 0).sum(dim=1)
             if world > 1:
                 dist.all_reduce(carriers)
-            mult = {"i8": 2.0, "bf16": 1.0, "e2m1": 4.0 if os.environ.get("VPCA_E2M1_MXF4", "1") != "0" else 2.0}[dtype_name]
+            mult = {"i8": 2.0, "bf16": 1.0, "e2m1": 2.0}[dtype_name]
             ops_l = float(n_leg) * (n_leg + 1) * vpg_leg                      # SYRK-minimal, per GPU
             out = {"workload": f"{n_leg} samples x {vpg_leg} variants per GPU ({vpg_leg * world} total), {dtype_name}",
                    "value": n_leg * vpg_leg * world * k / (ms_l * 1e-3), "unit": UNIT, "steps": k, "seconds": ms_l * 1e-3,
@@ -868,8 +877,8 @@ def run_b200(args):
                    "per_gpu_tops_step": ops_l / (ms_l / k * 1e-3) / 1e12,
                    "per_gpu_tops_kernel": ops_l / (kern_ms * 1e-3) / 1e12 if kern_ms > 0 else None,
                    "frac_of_sustained_peak": ops_l / (ms_l / k * 1e-3) / 1e12 / (mult * peaks["bf16_tflops_sustained"]),
-                   "frac_of_nominal_peak": ops_l / (ms_l / k * 1e-3) / 1e12 / (mult * 2250.0),
-                   "peak_source": "%g x bf16_tflops_sustained (%s) of MEASURED_PEAKS.json; nominal = %g x 2250 TFLOP/s dense"
+                   "frac_of_nominal_peak": ops_l / (ms_l / k * 1e-3) / 1e12 / (mult * 989.0),
+                   "peak_source": "%g x bf16_tflops_sustained (%s) of MEASURED_PEAKS.json; nominal = %g x 989 TFLOP/s dense (H100 SXM)"
                                   % (mult, peaks["source"], mult),
                    "hbm_gbs_algorithmic": (n_leg * vpg_leg * ebytes + 4.0 * n_leg * n_leg) / (ms_l / k * 1e-3) / 1e9,
                    "reduce": "fused peer-memory reduce" if fused_l else ("nccl all-reduce" if world > 1 else "none (1 GPU)"),

@@ -1,5 +1,5 @@
 /*
- * vpca.h -- C ABI of libvpca.so: the B200-native VariantsPca hot path
+ * vpca.h -- C ABI of libvpca.so: the H100-native VariantsPca hot path
  *           (genotype encode -> N x N similarity/Gram accumulation -> centering + top-k eigenvectors).
  *
  * Drop-in boundary.  The reference (googlegenomics/spark-examples) has no FFI; the boundary is the
@@ -23,7 +23,7 @@
  *     driver-side calls made when no accumulate call is in flight.
  *   - device-resident input (on_device tiles, panels) and everything driver-side is ordered on the stream given in
  *     vpca_config.stream (or a private stream); functions that return host data synchronise before returning.
- *   - there is no CPU fallback: vpca_create fails with VPCA_ERR_CUDA when no sm_100 device is usable.
+ *   - there is no CPU fallback: vpca_create fails with VPCA_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef VPCA_H_
 #define VPCA_H_
@@ -54,16 +54,16 @@ typedef enum vpca_status {
 } vpca_status;
 
 typedef enum vpca_dtype {
-    VPCA_DTYPE_I8 = 0,  /* int8 genotype encoding, tcgen05 kind::i8, exact int32 accumulation   */
-    VPCA_DTYPE_BF16 = 1, /* bf16 genotype encoding, tcgen05 kind::f16, fp32 TMEM accumulation flushed
+    VPCA_DTYPE_I8 = 0,  /* int8 genotype encoding, wgmma s8, exact int32 accumulation            */
+    VPCA_DTYPE_BF16 = 1, /* bf16 genotype encoding, wgmma bf16, fp32 register accumulation flushed
                             into the int32 Gram before 2^24 could be reached (exact)              */
-    VPCA_DTYPE_E2M1 = 2  /* 4-bit e2m1 cells (0, 1, 2 exact), two per byte in HBM and in shared memory;
-                            tcgen05 kind::mxf4 (block-scaled FP4 MMA, unit UE8M0 scales kept in TMEM:
-                            twice the int8 MMA rate) with fp32 accumulation, flushed like bf16 (exact).
-                            Half the HBM/L2 bytes per cell.  Dense tiles need ld % 128 == 0 (panels:
-                            % 256), 32-byte alignment and zero cells up to the next multiple of 128
-                            variants; max_multiplicity <= 2.  VPCA_E2M1_MXF4=0 selects kind::f8f6f4
-                            (cells expanded to bytes by TMA, int8 rate) instead.                     */
+    VPCA_DTYPE_E2M1 = 2  /* 4-bit e2m1 cells (0, 1, 2 exact), two per byte in HBM; expanded in shared
+                            memory to int8 holding twice the cell value, wgmma s8 with int32
+                            accumulation, the flush divides by 4 (exact).  Half the HBM/L2 bytes per
+                            cell, but the expansion makes its Gram several times slower than int8
+                            (README): choose it only for the memory footprint.  Dense tiles need ld % 128 == 0 (panels: % 128), 32-byte alignment
+                            and zero cells up to the next multiple of 128 variants;
+                            max_multiplicity <= 2.                                                 */
 } vpca_dtype;
 
 typedef struct vpca_ctx vpca_ctx;
@@ -122,7 +122,7 @@ int vpca_encode_calls(vpca_ctx* ctx, const int64_t* offsets, const int32_t* samp
 
 /* ---- similarity / Gram accumulation (VariantsPca.scala:182-191 getSimilarityMatrix) --------------
  * vpca_accumulate_calls = the body of `mapPartitions` (:184-189) for one batch of rows of Spark
- * partition `partition_id`: encode on device + S_partition += X X^T on tcgen05 tensor cores.  May be
+ * partition `partition_id`: encode on device + S_partition += X X^T on wgmma tensor cores.  May be
  * called many times per partition.  Nothing is visible in the Gram until vpca_commit(partition_id)
  * (task success); vpca_abort discards it (task failure / retry), so a retried task is counted exactly
  * once -- the property the reference gets from returning a fresh matrix per task (:185).
@@ -286,14 +286,14 @@ int vpca_synth_panels_device(vpca_ctx* ctx, uint64_t seed, int64_t v0, int64_t n
 /* ---- introspection ---------------------------------------------------------------------------------- */
 typedef struct vpca_stats {
     int64_t variants_accumulated; /* rows folded into the Gram or into staged partitions                  */
-    int64_t gram_launches;        /* tcgen05 Gram kernel launches                                         */
+    int64_t gram_launches;        /* Gram kernel launches                                                 */
     int64_t kernel_launches;      /* all kernels launched by this ctx                                     */
     int64_t h2d_bytes;            /* bytes copied host -> device by accumulate_* / encode / set_gram      */
     int64_t d2h_bytes;            /* bytes copied device -> host by get_* / compute_pca                   */
     float last_gram_ms;           /* device time of the most recent Gram launch (CUDA events)             */
     float last_eig_ms;            /* device time of the most recent centering + eigensolve                */
-    int32_t gram_cta_group;       /* 1 or 2: tcgen05 cta_group used                                       */
-    int32_t gram_resident;        /* 1 when the last launch kept accumulators in TMEM for the whole K loop */
+    int32_t gram_cta_group;       /* 1 or 2: CTAs per Gram tile                                           */
+    int32_t gram_resident;        /* 1 when the last launch kept accumulators in registers for the whole K loop */
     int32_t eig_method;           /* last vpca_compute_pca: 1 direct reduction, 2 Lanczos, 3 Lanczos abandoned -> direct */
     int32_t eig_iterations;       /* Lanczos steps taken by the last vpca_compute_pca (0 for a direct solve)  */
 } vpca_stats;
@@ -346,14 +346,14 @@ int vpca_accumulate_joined(vpca_ctx* ctx, int64_t partition_id);
  * vpca_debug_tiles: the output tiles the kernel enumerates for n_samples -- 8 int32 per tile {rowA of CTA 0, rowA of CTA 1,
  *   rowB, n_eff (MMA N), weight prefix, flags (1: a 128-block above the diagonal is written transposed, 2: CTA 1 is a
  *   filler), 0, 0}; exact != 0: the exact 128-block cover of the lower triangle (every block of
- *   `for (c1 <- callset; c2 <- callset)`, VariantsPca.scala:186-188, with c2 <= c1 computed exactly once), 0: the 256 x 240
- *   rectangles kind::mxf4 uses.  Returns the tile count (may exceed max_tiles).
- * vpca_debug_plan: the (worker, tile, first k-block, end k-block, TMEM column, TMEM columns of the worker) pieces of one
+ *   `for (c1 <- callset; c2 <- callset)`, VariantsPca.scala:186-188, with c2 <= c1 computed exactly once), 0: the 256 x (<= 256)
+ *   rectangles of the default tiling.  Returns the tile count (may exceed max_tiles).
+ * vpca_debug_plan: the (worker, tile, first k-block, end k-block, accumulator column, accumulator columns of the worker) pieces of one
  *   window of kb_window k-blocks under an equal split -- 6 int32 per piece; returns the piece count, or -(1 + worker) when
  *   a worker would own more pieces than the kernel supports.
  * vpca_debug_rebalance: what the on-device rebalancer does with a candidate speed-weighted split before it publishes it --
  *   `cum` (workers + 1 fractions of a window, cum[0] = 0, cum[workers] = 1; in / out) is repaired so that the accumulators
- *   of every worker fit `col_limit` TMEM columns (512; 480 for kind::mxf4), then the pieces are written like
+ *   of every worker fit `col_limit` accumulator columns (256: one tile), then the pieces are written like
  *   vpca_debug_plan.  Returns the piece count, or VPCA_ERR_STATE when no repair exists (the device keeps the old split). */
 int vpca_debug_rebalance(const int32_t* tiles, int32_t num_tiles, int32_t workers, int32_t kb_window, int32_t col_limit,
                          double* cum, int32_t* out, int32_t max_pieces);

@@ -1,7 +1,7 @@
 /*
  * vpca_oracle.c -- CPU restatement of the VariantsPca hot path.  TEST INFRASTRUCTURE ONLY.
  *
- * This file is the parity oracle for the B200 path.  It is NOT product code: only tests/,
+ * This file is the parity oracle for the CUDA path.  It is NOT product code: only tests/,
  * __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may load it.
  *
  * PINNING: the reference (googlegenomics/spark-examples) ships no tests, fixtures or golden vectors

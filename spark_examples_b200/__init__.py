@@ -1,4 +1,4 @@
-"""spark_examples_b200 -- the B200-native VariantsPca hot path behind the reference's driver API.
+"""spark_examples_b200 -- the H100-native VariantsPca hot path behind the reference's driver API.
 
 Only what the path needs: `csrc/` (CUDA kernels + the C ABI of include/vpca.h, built into libvpca.so),
 `native` (ctypes twin of the JNI class), and the host-side mirror of the reference interface

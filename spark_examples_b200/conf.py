@@ -102,7 +102,7 @@ class PcaConf(GenomicsConf):
             ("debugDatasets", bool, False, False),        # :80
             ("minAlleleFrequency", float, None, False),   # :81
             ("numPc", int, 2, False),                     # :85
-            # ---- additive, B200 side ----
+            # ---- additive, GPU side ----
             ("gpuDevice", int, None, False),              # CUDA ordinal (default: LOCAL_RANK or 0)
             ("gpuDtype", str, "int8", False),             # int8 | bf16 genotype encoding
             ("synthetic", str, None, False),              # "N,V[,seed]": synthetic cohort instead of the retired API

@@ -327,7 +327,7 @@ __global__ void __launch_bounds__(512) tridiag_fused_kernel(double* __restrict__
             double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
             int t = j + 1 + lane;
             if (j > 0) {
-                // 4 independent 8-byte loads per lane in flight (8 was measured slower: 53 vs 42.5 ms at N = 2504)
+                // 4 independent 8-byte loads per lane in flight
                 for (; t + 96 < n; t += 128) {
                     const double r0 = row[t], r1 = row[t + 32], r2 = row[t + 64], r3 = row[t + 96];
                     const double u0 = r0 - (vi * w[t] + wi * vp[t]);
@@ -954,7 +954,7 @@ __device__ __forceinline__ void lz_share(const LzArgs& a, const double* vts, int
     }
 }
 
-// dst[q] = sum over the blocks of src[b][q], q < jc.  148 dependent-latency L2 loads per column if one thread walked the
+// dst[q] = sum over the blocks of src[b][q], q < jc.  one dependent-latency L2 load per block per column if one thread walked the
 // blocks; instead warp w takes the blocks b = w, w + 32, ... (a handful of independent coalesced loads per lane, 32 columns
 // at a time) and the 32 partial sums of a column are added in warp order: deterministic and ~1 L2 latency deep.
 // Ends with a block barrier: dst is complete for every thread.
@@ -1677,13 +1677,13 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
     constexpr int kGraphSteps = 64;
     const size_t fused_smem = 3 * (size_t)n * sizeof(double);
     // one launch per step while every trailing row still gets its own warp (<= ~16 rows per SM-resident block);
-    // beyond that the two-kernel form (one warp per row over a larger grid) is faster (measured: 4096 -> 162 vs 133 ms)
+    // beyond that the two-kernel form (one warp per row over a larger grid) is faster
     const bool fused = n <= 3072 && fused_smem <= 200 * 1024 && getenv("VPCA_EIG_TWO_KERNELS") == nullptr;
     const int big_blocks = (n - 1 + 3) / 4 > 0 ? (n - 1 + 3) / 4 : 1;
     if (w.graph_exec == nullptr || w.graph_n != n || w.graph_fused != fused) {
         if (w.graph_exec != nullptr) cudaGraphExecDestroy(w.graph_exec);
         w.graph_exec = nullptr;
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         if (fused) {

@@ -5,7 +5,7 @@
 // row v lists the callset indices that have `hasVariation` at variant v; the dense equivalent is column v of
 // X in {0,1,..}^N where X[s][v] = number of times s is listed (a sample listed twice counts twice, exactly as the
 // reference's `for (c1 <- callset; c2 <- callset)` at :187 would count it).  The tile is written sample-major
-// (row = sample, contiguous along variants) because that is the K-major operand layout the tcgen05 Gram kernel
+// (row = sample, contiguous along variants) because that is the K-major operand layout the wgmma Gram kernel
 // streams through TMA.
 //
 // HBM-bound scatter: one warp per variant row reads its indices coalesced and adds 1 to X[s][v] with a packed
@@ -263,7 +263,7 @@ static cudaError_t encode_launch(const int64_t* d_off, int64_t base, const IdxT*
     if (e != cudaSuccess || nv <= 0) return e;
     const int threads = 256;
     const int64_t want = (nv * 32 + threads - 1) / threads;
-    const int blocks = (int)(want < 148 * 16 ? (want < 1 ? 1 : want) : 148 * 16);
+    const int blocks = (int)(want < 132 * 16 ? (want < 1 ? 1 : want) : 132 * 16);
     if (elem_bits == 4) {
         const int cap = max_mult > 2 ? 2 : max_mult;
         encode_e2m1_kernel<IdxT><<<blocks, threads, 0, stream>>>(d_off, base, d_idx, nv, n, cap, reinterpret_cast<uint32_t*>(d_x),

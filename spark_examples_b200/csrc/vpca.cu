@@ -267,7 +267,8 @@ struct LaneGuard {
 
 int launch_gram(vpca_ctx* ctx, GramPlan& plan, cudaStream_t stream, cudaEvent_t t0, cudaEvent_t t1, const void* d_x,
                 int64_t nv, int64_t ld, int64_t panel, int32_t* d_target) {
-    // fp32 TMEM accumulation (bf16 / e2m1) is exact only below 2^24: bound the variants one launch may fold.
+    // fp32 accumulation (bf16) is exact only below 2^24: bound the variants one launch may fold (e2m1, whose doubled
+    // cells accumulate 4 S in int32, keeps the same bound).
     // vpca_create guarantees that the bound is at least one panel.
     int64_t limit = nv;
     if (ctx->elem_bits != 8) {
@@ -525,8 +526,8 @@ int vpca_create(const vpca_config* cfg, vpca_ctx** out) {
     CUDA_OK(nullptr, cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     CUDA_OK(nullptr, cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major != 10)
-        return fail(nullptr, VPCA_ERR_UNSUPPORTED, "device %d is sm_%d%d; libvpca is built for sm_100a (B200) only",
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(nullptr, VPCA_ERR_UNSUPPORTED, "device %d is sm_%d%d; libvpca is built for sm_90a (H100) only",
                     cfg->device, prop.major, prop.minor);
     vpca_ctx* ctx = new (std::nothrow) vpca_ctx();
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_NOMEM, "out of host memory");
@@ -1507,7 +1508,7 @@ int vpca_debug_plan(const int32_t* tiles, int32_t num_tiles, int32_t workers, in
     if (tiles == nullptr || num_tiles < 1 || workers < 1 || kb_window < 1 || (out == nullptr && max_pieces > 0))
         return fail(nullptr, VPCA_ERR_BAD_ARG, "vpca_debug_plan: bad argument");
     const int rc = gram_debug_plan(tiles, num_tiles, workers, kb_window, out, max_pieces);
-    if (rc < 0) return fail(nullptr, VPCA_ERR_STATE, "vpca_debug_plan: the accumulators of a worker do not fit TMEM (large-N schedule)");
+    if (rc < 0) return fail(nullptr, VPCA_ERR_STATE, "vpca_debug_plan: the accumulators of a worker do not fit its budget (large-N schedule)");
     return rc;
 }
 

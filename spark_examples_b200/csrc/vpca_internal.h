@@ -9,40 +9,36 @@
 
 namespace vpca {
 
-// ---- Gram (gram_sm100.cu) --------------------------------------------------------------------
+// ---- Gram (gram_sm90.cu) --------------------------------------------------------------------
 struct GramPlan {
-    int cta_group = 2;        // tcgen05 cta_group (1: 128x256 tiles per CTA, 2: 256x256 per CTA pair)
+    int cta_group = 2;        // CTAs per tile (1: 128 x 256 tiles per CTA, 2: 256 x 256 per CTA pair, one A block each)
     int kb_window = 0;        // k-blocks per L2 window (0 -> automatic)
     int num_sms = 0;
-    void* d_tiles = nullptr;  // device tile list (TileDesc, gram_sm100.cu)
-    std::vector<int32_t> h_tiles;   // the same list on the host (8 ints per tile): resident / TMEM-fit decisions
+    void* d_tiles = nullptr;  // device tile list (TileDesc, gram_sm90.cu)
+    std::vector<int32_t> h_tiles;   // the same list on the host (8 ints per tile): resident / accumulator-fit decisions
     int num_tiles = 0;
     int num_full = 0;         // leading full-weight tiles (whole-tile waves of the large-N schedule)
     int total_weight = 0;     // sum over tiles of n_eff / 16
-    int tiles_col_limit = 512;   // TMEM columns the accumulators of one worker may take
+    int tiles_col_limit = 256;   // accumulator columns (B rows) one worker may hold
     bool exact_cover = false; // VPCA_EXACT_COVER=1: the exact 128-block cover of the lower triangle (4.5 % fewer MMAs at
-                              // 2504 samples) instead of square 256 x 256 tiles.  Off by default: its N = 128 tiles need
-                              // 96 B/clk per SM from L2 (A 16 KB + B 8 KB per 256 MMA cycles) where the 256 x 256 tiles
-                              // need 64, and L2 -> SM bandwidth is what the kernel runs against -- measured on B200:
-                              // 2.06 ms vs 1.65 ms per 2504 x 1M Gram (profiles/README.md, round 2)
+                              // 2504 samples) instead of square 256 x 256 tiles.  Off by default: a one-row tile (128 B rows)
+                              // still takes a worker's whole 256-row accumulator, and with one accumulator per worker its
+                              // unequal tiles split less evenly (2504 samples, 66 workers: the busiest worker gets 1.30 x the
+                              // mean share against 1.24 x for the rectangles)
     int tiles_for_n = -1;     // n_samples the tile list was built for
     int tiles_for_cg = 0;
     int tiles_for_bn = 0;
     int tiles_row_lo = 0, tiles_row_hi = 0;   // rows of S the tile list covers
     int own_lo = 0, own_hi = 0;   // band-only context: the rows of S it stores (own_hi == 0: the whole matrix); without
                                   // peers the Gram kernel then computes exactly those rows (owner-computes)
-    bool e2m1_mxf4 = true;    // packed e2m1 cells run through kind::mxf4 (2x MMA rate, unit block scales);
-                              // VPCA_E2M1_MXF4=0 selects kind::f8f6f4 (TMA-expanded cells, int8 rate)
     int last_resident = 0;
     int* d_err = nullptr;     // device debug words written before a watchdog trap
     static constexpr int kMaxWindows = 1 << 16;
-    int sync_lead = 0;        // VPCA_SYNC_LEAD: windows a worker may lead the slowest one by (0 = no pacing; measured
-                              // on B200: pacing only slows every worker to the slowest one, see DESIGN.md)
+    int sync_lead = 0;        // VPCA_SYNC_LEAD: windows a worker may lead the slowest one by (0 = no pacing)
     int* d_win_done = nullptr;
     bool self_b = true;       // VPCA_SELF_B=0: diagonal tiles load their B rows although they are the pair's own A blocks
     bool red64 = true;        // VPCA_RED64=0: one 32-bit red per cell in the flush instead of two cells per 64-bit red
-    double gain = 0.5;        // VPCA_REBALANCE_GAIN: how far a launch moves the shares towards the measured speeds (measured on
-                              // B200, 2504 x 1M int8: 0.5 settles at 1.61 ms within three launches, 0.7 and 1.0 hover at 1.70)
+    double gain = 0.5;        // VPCA_REBALANCE_GAIN: how far a launch moves the shares towards the measured speeds
     bool adaptive = true;     // VPCA_ADAPTIVE=0 keeps the stream-K split equal instead of speed-weighted
     double* d_cum = nullptr;  // cumulative worker shares (workers + 1 doubles) + update counter
     int cum_workers = 0, cum_tiles = 0, cum_kbw = 0, cum_for_n = 0, cum_dev = 0, cum_elem = 0;   // what the split in d_cum was made for
@@ -79,7 +75,7 @@ cudaError_t gram_add_peers(GramPlan& plan, const int32_t* d_src, int64_t count, 
 cudaError_t gram_add_owners(GramPlan& plan, const int32_t* d_src, int n, cudaStream_t stream);
 cudaError_t gram_gather_rows(GramPlan& plan, int32_t* d_S, int n, cudaStream_t stream);
 cudaError_t gram_peer_barrier(GramPlan& plan, cudaStream_t stream);
-cudaError_t gram_preload_kernels(cudaStream_t stream);   // see gram_sm100.cu: lazy module loading vs spinning barriers
+cudaError_t gram_preload_kernels(cudaStream_t stream);   // see gram_sm90.cu: lazy module loading vs spinning barriers
 cudaError_t encode_preload_kernels();
 void gram_plan_free(GramPlan& plan);
 int gram_debug_max_clusters(int cluster_size);

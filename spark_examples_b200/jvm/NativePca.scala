@@ -16,7 +16,7 @@ object NativePca {
 
   val DTYPE_I8 = 0
   val DTYPE_BF16 = 1
-  val DTYPE_E2M1 = 2 // packed 4-bit cells (tcgen05 kind::mxf4 with unit scales; exact for 0/1/2)
+  val DTYPE_E2M1 = 2 // packed 4-bit cells (expanded to int8 on the device; exact for 0/1/2)
 
   // every native method throws on a negative vpca_status: IndexOutOfBoundsException for a sample index outside [0, N)
   // (what Breeze throws at VariantsPca.scala:188), IllegalArgumentException, OutOfMemoryError, else RuntimeException

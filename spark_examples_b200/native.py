@@ -3,7 +3,7 @@ shown in INTEGRATION.md.  One ``NativePca`` object = one ``vpca_ctx`` = one GPU.
 
 There is no CPU fallback: importing this module never fails (so host logic stays testable without a
 GPU), but constructing ``NativePca`` raises ``VpcaError`` when the CUDA library is missing or no
-sm_100 device is usable.
+sm_90 device is usable.
 """
 from __future__ import annotations
 
@@ -586,7 +586,8 @@ def debugTiles(n_samples: int, cta_group: int = 2, exact: bool = True) -> np.nda
 
 
 def debugPlan(tiles: np.ndarray, workers: int, kb_window: int) -> np.ndarray:
-    """(pieces, 6) int32 {worker, tile, kb_lo, kb_hi, tmem_col, tmem_cols_of_worker} of one window (vpca_debug_plan)."""
+    """(pieces, 6) int32 {worker, tile, kb_lo, kb_hi, acc_col, acc_cols_of_worker} of one window (vpca_debug_plan); the
+    columns are B rows of the worker's register accumulator."""
     L = load_library()
     t = np.ascontiguousarray(tiles, dtype=np.int32)
     cap = 8 * int(workers) + 8
@@ -608,18 +609,6 @@ def debugBandTiles(n_samples: int, cta_group: int, row0: int, rows: int) -> np.n
     out = np.zeros((cnt, 8), dtype=np.int32)
     L.vpca_debug_band_tiles(int(n_samples), int(cta_group), int(row0), int(rows), _host_ptr(out), cnt)
     return out
-
-
-def gramSourceFingerprint() -> str:
-    """sha256 (16 hex digits) of csrc/gram_sm100.cu with comments and whitespace removed: what an ncu capture of the Gram
-    kernel is tied to (profiles/r2_gram_traffic.json) -- editing a comment does not orphan a capture, editing code does."""
-    import hashlib
-    import re
-    src = (Path(__file__).resolve().parent / "csrc" / "gram_sm100.cu").read_text()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    src = re.sub(r"//[^\n]*", "", src)
-    src = re.sub(r"\s+", "", src)
-    return hashlib.sha256(src.encode()).hexdigest()[:16]
 
 
 def maxClusters(device: int, cluster_size: int) -> int:

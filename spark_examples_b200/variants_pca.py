@@ -271,7 +271,7 @@ class VariantsPcaDriver:
 
     # -- VariantsPca.scala:182-191 ----------------------------------------------------------------------------------
     def getSimilarityMatrix(self, callsets: CallsRdd) -> SimilarityMatrix:
-        """S = sum over variants of x x^T on the GPU: every partition is one `mapPartitions` task (encode + tcgen05
+        """S = sum over variants of x x^T on the GPU: every partition is one `mapPartitions` task (encode + wgmma
         Gram into a private staging Gram, committed on success); `reduceByKey(_ + _)` across ranks is one all-reduce."""
         nat = self._native(callsets.n_samples)
         nat.reset()

@@ -1,5 +1,5 @@
-"""pytest configuration: `gpu` marks tests that need a B200 (driver: `-m gpu` on the GPU box,
-`-m "not gpu"` in the CPU container)."""
+"""pytest configuration: `gpu` marks tests that need an H100 (`-m gpu` on a GPU machine, `-m "not gpu"` without
+one)."""
 import os
 import sys
 from pathlib import Path
@@ -16,7 +16,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA sm_100 device (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA sm_90 device (H100; run with -m gpu)")
 
 
 def _cuda_available() -> bool:

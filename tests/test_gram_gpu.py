@@ -293,12 +293,13 @@ def test_encode_tile_e2m1(oracle):
     assert np.array_equal(got, _pack_e2m1(want))
 
 
-@pytest.mark.parametrize("mxf4", [1, 0])
+@pytest.mark.parametrize("red64", [1, 0])
 @pytest.mark.parametrize("cta_group", [1, 2])
-def test_gram_e2m1_dense_and_calls(oracle, monkeypatch, cta_group, mxf4):
-    """Packed 4-bit cells through kind::mxf4 (block-scaled, unit scales) and through kind::f8f6f4: same exact Gram."""
+def test_gram_e2m1_dense_and_calls(oracle, monkeypatch, cta_group, red64):
+    """Packed 4-bit cells, expanded to int8 in shared memory: the exact Gram through both flushes (two cells per 64-bit
+    red, or VPCA_RED64=0: one 32-bit red per cell)."""
     _set_env(monkeypatch, cta_group, kb_window=8)
-    monkeypatch.setenv("VPCA_E2M1_MXF4", str(mxf4))
+    monkeypatch.setenv("VPCA_RED64", str(red64))
     from spark_examples_b200 import native
     n, nv = 700, 5003
     X = oracle.c_synth_dense(SEED, n, 0, nv, mode=1)           # dosage 0/1/2: all three codes

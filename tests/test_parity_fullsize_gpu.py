@@ -59,7 +59,7 @@ def test_c2_sample_count_gram_bit_exact_vs_reference_loop(oracle, seed):
 
 
 def test_c2_sample_count_resident_panels_and_eigenvectors(oracle):
-    """The bench path at N = 2504: device-resident panels (int8 and packed e2m1 / kind::mxf4) -> Gram bit-exact against
+    """The bench path at N = 2504: device-resident panels (int8 and packed e2m1) -> Gram bit-exact against
     the reference loop on the same 64 k variants; top-2 eigenvectors against the MLlib recipe and against LAPACK dsyevd."""
     import scipy.linalg
     import torch
@@ -117,7 +117,7 @@ def test_direct_householder_solver_at_benchmark_size(oracle, monkeypatch):
 
 @pytest.mark.parametrize("dtype_name", ["bf16", "e2m1"])
 def test_c5_sample_count_other_encodings_match_int8(oracle, dtype_name):
-    """N = 10 000 (BASELINE configs[4]): bf16 (kind::f16) and packed e2m1 (kind::mxf4) Grams equal the int8 Gram of the
+    """N = 10 000 (BASELINE configs[4]): bf16 and packed e2m1 Grams equal the int8 Gram of the
     same cohort bit for bit, and random rows equal an fp32 matmul (exact: every count < 2^24)."""
     import torch
     from spark_examples_b200 import native

@@ -1,6 +1,6 @@
 """GPU parity tests of centering + eigensolve (VariantsPca.scala:198-231) against the oracle, through the C ABI.
 
-Tolerance (BASELINE.json north_star): top-k eigenvectors within 1e-6 relative, sign-normalised:
+Tolerance: top-k eigenvectors within 1e-6 relative, sign-normalised:
 max_i |u^_i - u_i| / max_i |u_i| <= 1e-6 per component.  Centering is compared bit for bit."""
 import numpy as np
 import pytest

@@ -1,12 +1,13 @@
 """Host-side checks of the Gram kernel's work decomposition (no GPU needed): the tile list and the per-worker pieces
-are computed by the same code the kernel's three roles replay (plan_segments in csrc/gram_sm100.cu), exposed through
+are computed by the same code the kernel's two roles replay (plan_segments in csrc/gram_sm90.cu), exposed through
 vpca_debug_tiles / vpca_debug_plan.
 
 What must hold for S = sum_v x_v x_v^T (VariantsPca.scala:186-188) to come out exact:
   * exact block cover: every 128 x 128 block (col block c <= row block r) of the lower triangle is produced by exactly
     one (A block, B block) product -- directly, or as the mirror image (c > r, written transposed);
   * the pieces of all workers partition every (tile, k-block) unit of a window: nothing twice, nothing missing;
-  * the accumulators of one worker fit the 512 TMEM columns whenever the schedule is declared resident.
+  * the accumulators of one worker fit its budget -- one tile of up to 256 B rows, held in the registers of its two
+    consumer warpgroups -- whenever the schedule is declared resident.
 """
 import numpy as np
 import pytest
@@ -63,7 +64,7 @@ def test_exact_cover_saves_the_redundant_quarter_of_diagonal_tiles():
     assert len(tiles) == 60 and int((tiles[:, 3] == 256).sum()) == 45
 
 
-@pytest.mark.parametrize("cg,workers", [(2, 74), (1, 148)])
+@pytest.mark.parametrize("cg,workers", [(2, 74), (1, 148), (2, 66), (1, 132)])   # H100: 66 CTA pairs / 132 CTAs
 @pytest.mark.parametrize("n,kbw", [(2504, 64), (2504, 32), (2504, 7), (1092, 64), (600, 16), (130, 64), (2000, 128)])
 def test_pieces_partition_every_window_and_fit_tmem(n, kbw, cg, workers):
     tiles = native.debugTiles(n, cg, True)
@@ -72,56 +73,63 @@ def test_pieces_partition_every_window_and_fit_tmem(n, kbw, cg, workers):
     for w, t, lo, hi, col, cols in pieces:
         assert 0 <= lo < hi <= kbw
         seen[t, lo:hi] += 1
-        assert col % 32 == 0 and col + tiles[t, 3] <= cols <= 512
+        assert col % 32 == 0 and col + tiles[t, 3] <= cols <= 256
     assert (seen == 1).all()
-    # accumulators of one worker never overlap in TMEM
+    # accumulators of one worker never overlap
     for w in np.unique(pieces[:, 0]):
         mine = pieces[pieces[:, 0] == w]
         spans = sorted((c, c + ((tiles[t, 3] + 31) // 32) * 32) for _, t, _, _, c, _ in mine)
         assert all(spans[i][1] <= spans[i + 1][0] for i in range(len(spans) - 1))
-    # balance: a worker's share of the weighted work is within one k-block per piece of the mean
+    # one accumulator per worker: a worker owns a piece of one tile per window
+    assert np.bincount(pieces[:, 0], minlength=workers).max() == 1
+    # balance: no worker is given more than the mean share plus what the repair moves to it from a cut tile, and never
+    # more than one whole tile
     work = np.zeros(workers)
     for w, t, lo, hi, _, _ in pieces:
         work[w] += (hi - lo) * (tiles[t, 3] // 16)
     mean = work.sum() / workers
-    assert work.max() - mean <= 16 * 3 + 1
+    assert work.max() <= (tiles[:, 3] // 16).max() * kbw
+    assert work.max() <= 2 * mean + 16
 
 
 def test_large_cohorts_leave_the_resident_schedule():
-    """N = 5000: more accumulators per worker than TMEM holds -> the host must pick the wave schedule (debugPlan reports
+    """N = 5000: more accumulators per worker than its budget holds -> the host must pick the wave schedule (debugPlan reports
     the overflow instead of a plan)."""
     tiles = native.debugTiles(5000, 2, True)
     with pytest.raises(native.VpcaError):
-        native.debugPlan(tiles, 74, 64)
+        native.debugPlan(tiles, 66, 64)
     # whole-tile waves deal out only full-weight two-row tiles, in compact patches of S
     full = tiles[tiles[:, 3] == 256]
     lead = 0
     while lead < len(tiles) and tiles[lead, 3] == 256:
         lead += 1
     assert lead == len(full)
-    wave = tiles[:74]
+    wave = tiles[:66]
     rows_of_x = set(wave[:, 0] // 128) | set(wave[:, 1] // 128) | set(wave[:, 2] // 128) | set(wave[:, 2] // 128 + 1)
     assert len(rows_of_x) <= 40              # ~34 row blocks of X per wave instead of ~150 for a row-major tile order
 
 
-def test_mxf4_rectangles_cover_the_triangle():
-    """kind::mxf4 keeps 256 x (<= 240) rectangles: every cell with row >= col lies in exactly one of them, and the B strips
-    have nearly equal widths (so that tiles have nearly equal weights and an even split never spans three of them)."""
+def test_rectangles_cover_the_triangle():
+    """The default tiling, 256 x (<= 256) rectangles: every cell with row >= col lies in exactly one of them, and the B
+    strips have nearly equal widths (so that tiles have nearly equal weights)."""
     n = 2504
     tiles = native.debugTiles(n, 2, False)
     hit = np.zeros((n, n), np.int8)
     for a0, a1, rb, ne, ws, fl, _, _ in tiles:
-        assert fl == 0 and a1 == a0 + 128 and rb % 16 == 0 and ne % 16 == 0 and ne <= 240
+        assert fl & ~4 == 0 and a1 == a0 + 128 and rb % 16 == 0 and ne % 16 == 0 and ne <= 256
         hit[rb:min(n, rb + ne), a0:min(n, a0 + 256)] += 1
     assert (np.tril(hit) == np.tril(np.ones((n, n), np.int8))).all()
-    assert set(tiles[:, 3]) == {224, 240}
+    assert set(tiles[:, 3]) == {240, 256}
 
 
-@pytest.mark.parametrize("n,exact,col_limit", [(2504, True, 512), (2504, False, 480), (1092, True, 512), (2000, True, 512)])
+# col_limit is the budget handed to the repair (256: the kernel's one 256-row register accumulator; the larger budgets
+# check the same repair when a worker may hold two accumulators)
+@pytest.mark.parametrize("n,exact,col_limit", [(2504, True, 512), (2504, False, 480), (1092, True, 512), (2000, True, 512),
+                                               (2504, False, 256), (1500, False, 256), (1092, True, 256)])
 @pytest.mark.parametrize("seed", [0, 1, 2, 3])
 def test_rebalanced_splits_are_repaired_to_fit_tmem(n, exact, col_limit, seed):
     """The speed-weighted split the device publishes (rebalance_kernel -> repair_split) must keep every worker inside its
-    TMEM budget whatever speeds were measured: skew the shares by up to +-35 % (the clamp of the rebalancer) and check that
+    accumulator budget whatever speeds were measured: skew the shares by up to +-35 % (the clamp of the rebalancer) and check that
     the repaired split still partitions every (tile, k-block) unit and fits `col_limit` columns."""
     workers, kbw = 74, 104
     tiles = native.debugTiles(n, 2, exact)
@@ -145,14 +153,6 @@ def test_rebalanced_splits_are_repaired_to_fit_tmem(n, exact, col_limit, seed):
     want = np.diff(cum)
     got = np.diff(cum2)
     assert got.max() <= want.max() + (want - got).clip(0).sum() + 1e-9
-
-
-def test_mxf4_accumulators_sit_below_the_scale_columns():
-    """kind::mxf4: 240-column accumulators at TMEM columns 0 and 240, block scales at 480 (gram_sm100.cu kSfCol)."""
-    tiles = native.debugTiles(2504, 2, False)
-    assert (tiles[:, 6] == 240).all()
-    pieces = native.debugPlan(tiles, 74, 104)
-    assert pieces[:, 5].max() <= 480 and set(pieces[:, 4]) <= {0, 240}
 
 
 @pytest.mark.parametrize("n,world", [(2504, 8), (1092, 4), (100_000, 8), (777, 2), (10_000, 3)])
@@ -181,9 +181,9 @@ def test_owner_computes_bands_tile_the_triangle_exactly_once(n, world):
 
 
 def test_repair_is_safe_for_any_split_hypothesis():
-    """Property test of repair_split (the last line of defence before a launch: overlapping TMEM accumulators would corrupt
+    """Property test of repair_split (the last line of defence before a launch: overlapping accumulators would corrupt
     S silently): for ANY monotone split of a window -- far outside the +-35 % the rebalancer proposes, including empty and
-    huge shares -- the repaired split either fits every worker into its TMEM budget and still partitions the window, or is
+    huge shares -- the repaired split either fits every worker into its accumulator budget and still partitions the window, or is
     rejected."""
     from hypothesis import given, settings, strategies as st
 
@@ -194,7 +194,7 @@ def test_repair_is_safe_for_any_split_hypothesis():
            st.lists(st.floats(0.0, 4.0, allow_nan=False), min_size=74, max_size=74))
     def check(which, workers, kbw, raw):
         tiles = tiles_by[which]
-        col_limit = 480 if not which[1] else 512
+        col_limit = 256
         share = np.asarray(raw[:workers]) + 1e-9
         cum = np.concatenate([[0.0], np.cumsum(share / share.sum())])
         cum[-1] = 1.0

@@ -1,6 +1,6 @@
 """The CUDA path against vectors produced by the reference's own code (tests/golden/reference_twin.json: the reference's
 Python twin executed, see tests/golden/make_reference_twin_golden.py): the call rows it produced go through the C ABI
-(encode -> tcgen05 Gram -> centering) and every similarity count and every centred double must come out identical.
+(encode -> wgmma Gram -> centering) and every similarity count and every centred double must come out identical.
 (File name: sorted last on purpose, so that this late addition can never mask another GPU test under `-x`.)"""
 import json
 from pathlib import Path

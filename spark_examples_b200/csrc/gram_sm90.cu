@@ -8,6 +8,10 @@
 //   TMA (cp.async.bulk.tensor, SWIZZLE_128B)  ->  shared memory ring  ->  wgmma (s8 -> s32 / bf16 -> f32)
 //   ->  accumulators in the registers of two consumer warpgroups  ->  red.global.add into the lower triangle of S.
 //
+// CTA pairs (VPCA_CTA_GROUP=2, the default) are 2-CTA clusters: both CTAs multiply the same B rows, so B box r is fetched
+// once, by CTA r, and multicast into both CTAs' shared memory, while each CTA loads its own A block.  Per k-block a CTA
+// pulls 32 KB from L2 instead of 48 KB (16 KB instead of 32 KB on a self-B tile).  Both CTAs walk the same k-blocks.
+//
 // Work decomposition ("window-synchronous stream-K"):
 //   * an output tile is the product of A row blocks (128 samples each: one per CTA, so two for a CTA pair with
 //     VPCA_CTA_GROUP=2) and up to 256 B rows; the B rows are the wgmma M side (128 per consumer warpgroup), the A block
@@ -442,8 +446,9 @@ template <int CG, int KIND>
 __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant__ CUtensorMap tmap, const GramArgs a) {
     using C = Cfg<KIND>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const uint32_t smem_base = ptx::smem_u32(smem);
+    // aligned in the shared window itself: a generic pointer of a cluster kernel carries the CTA's rank, and converting
+    // one back to a shared address re-reads it (ptxas re-derived and spilled the base in every k-block)
+    const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES + C::XBUF_BYTES * 2;
     // stage st: the B rows (M operand, 256 rows) then the A block (N operand, 128 rows), as TMA delivers them
     auto sB = [&](uint32_t st) { return smem_base + st * C::STAGE_BYTES; };
@@ -453,18 +458,31 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const uint32_t lane = ptx::lane_id();
+    // CG == 2: the pair is a 2-CTA cluster of a 1-D grid, so its rank in the cluster is blockIdx.x & 1 (taken from
+    // %ctaid: a rank read through inline asm from %cluster_ctarank was spilled and reloaded in every k-block)
     const uint32_t cta_rank = (CG == 2) ? (blockIdx.x & 1u) : 0u;
     const int worker = (CG == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+    // a consumer warpgroup frees a stage in its own CTA and, with CTA pairs, in the peer (whose producer multicasts into it)
+    auto release = [&](uint32_t st) {
+        if constexpr (CG == 2) {
+            ptx::mbar_arrive_cluster(ptx::mapa(empty_bar(st), 0));
+            ptx::mbar_arrive_cluster(ptx::mapa(empty_bar(st), 1));
+        } else {
+            ptx::mbar_arrive(empty_bar(st));
+        }
+    };
 
     if (warp == 0 && ptx::elect_one()) {
         ptx::prefetch_tensormap(&tmap);
         for (uint32_t i = 0; i < (uint32_t)C::STAGES; ++i) {
-            ptx::mbar_init(full_bar(i), 1);    // producer's arrive.expect_tx
-            ptx::mbar_init(empty_bar(i), 2);   // one arrive per consumer warpgroup
+            ptx::mbar_init(full_bar(i), 1);         // producer's arrive.expect_tx
+            ptx::mbar_init(empty_bar(i), 2 * CG);   // one arrive per consumer warpgroup of the cluster
         }
         ptx::fence_mbar_init();
     }
-    __syncthreads();
+    // the peer's barriers must be initialised before the first multicast or remote arrive reaches them
+    if constexpr (CG == 2) ptx::cluster_sync();
+    else __syncthreads();
     if (a.prof != nullptr && threadIdx.x == 0) a.prof[(size_t)blockIdx.x * 4 + 0] = globaltimer_ns();
 
     if (warp < 4) {
@@ -478,8 +496,8 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
             uint32_t it = 0;
             int synced_win = -1;
             while (sc.next(s)) {
-                // CTA r of a pair multiplies its own A block; a filler CTA has nothing to produce
-                if (CG == 2 && cta_rank != 0 && (s.flags & kTileFiller) != 0) continue;
+                // CTA r of a pair multiplies its own A block.  Both CTAs walk every tile, filler tiles included, so that
+                // their k-block sequences (and the stages the multicasts fill) stay in lockstep.
                 const int rowA = (CG == 2 && cta_rank != 0) ? s.rowA1 : s.rowA0;
                 const bool two_boxes = s.n_eff > kBoxRows;
                 const bool self_b = (CG == 2) && (s.flags & kTileSelfB) != 0;   // the A block is half of the B rows
@@ -494,8 +512,16 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
                     const int pnl = kb / a.kb_per_panel;
                     const int kc = (kb - pnl * a.kb_per_panel) * a.kc_per_kb;
                     ptx::mbar_arrive_expect_tx(full_bar(st), tx);
-                    ptx::tma_load_3d(sB(st), &tmap, full_bar(st), kc, s.rowB, pnl);
-                    if (two_boxes) ptx::tma_load_3d(sB(st) + C::BOX_BYTES, &tmap, full_bar(st), kc, s.rowB + kBoxRows, pnl);
+                    if constexpr (CG == 2) {
+                        // B box r is fetched once, by CTA r, into both CTAs (on a self-B tile it is CTA r's A block);
+                        // the empty barrier waited on above counts the consumers of both CTAs
+                        if (two_boxes || cta_rank == 0)
+                            ptx::tma_load_3d_multicast(sB(st) + cta_rank * C::BOX_BYTES, &tmap, full_bar(st), kc,
+                                                       s.rowB + (int)cta_rank * kBoxRows, pnl, 0x3);
+                    } else {
+                        ptx::tma_load_3d(sB(st), &tmap, full_bar(st), kc, s.rowB, pnl);
+                        if (two_boxes) ptx::tma_load_3d(sB(st) + C::BOX_BYTES, &tmap, full_bar(st), kc, s.rowB + kBoxRows, pnl);
+                    }
                     if (!self_b) ptx::tma_load_3d(sA(st), &tmap, full_bar(st), kc, rowA, pnl);
                 }
                 if (a.sync_lead > 0 && leader && s.last_in_win)
@@ -514,8 +540,8 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
         Seg s;
         uint32_t it = 0;
         while (sc.next(s)) {
+            // CTA 1's A block of a filler tile only pads the pair: multiplied in lockstep with CTA 0, never flushed
             const bool filler = (CG == 2) && cta_rank != 0 && (s.flags & kTileFiller) != 0;
-            if (filler) continue;
             const bool self_b = (CG == 2) && (s.flags & kTileSelfB) != 0;
             // m64 blocks of this warpgroup that hold B rows of the tile (n_eff is a multiple of 16)
             const int mrow0 = cw * 128;
@@ -527,6 +553,8 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
                     acc[1][i] = 0;
                 }
             }
+            // the A block follows the 256 B rows; on a self-B tile it is CTA r's half of them
+            const uint32_t a_off = (self_b ? cta_rank : 2u) * (uint32_t)(kBoxRows * 128);
             int pending = -1;   // stage whose wgmmas may still be in flight
             for (int kb = s.kb0; kb < s.kb1; ++kb, ++it) {
                 const uint32_t st = it % C::STAGES, ph = (it / C::STAGES) & 1u;
@@ -555,14 +583,12 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
                     }
                     ptx::fence_proxy_async();   // generic-proxy stores -> visible to wgmma (async proxy)
                     ptx::named_sync(1, 256);
-                    if (threadIdx.x % 128 == 0) ptx::mbar_arrive(empty_bar(st));   // the packed stage is free again
+                    if (threadIdx.x % 128 == 0) release(st);   // the packed stage is free again
                     opB = xb;
-                    opA = xb + 2u * kBoxRows * 128u;
                 } else {
                     opB = sB(st);
-                    opA = sA(st);
                 }
-                if (self_b) opA = opB + cta_rank * (uint32_t)(kBoxRows * 128);
+                opA = opB + a_off;
                 const uint64_t bdesc = make_smem_desc(opA);
                 const uint64_t adesc0 = make_smem_desc(opB + (uint32_t)mrow0 * 128u);
                 const uint64_t adesc1 = make_smem_desc(opB + (uint32_t)(mrow0 + 64) * 128u);
@@ -585,7 +611,7 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
                 ptx::wgmma_fence_acc(acc[0]);
                 ptx::wgmma_fence_acc(acc[1]);
                 if constexpr (KIND != 2) {
-                    if (pending >= 0 && threadIdx.x % 128 == 0) ptx::mbar_arrive(empty_bar((uint32_t)pending));
+                    if (pending >= 0 && threadIdx.x % 128 == 0) release((uint32_t)pending);
                 }
                 pending = (int)st;
             }
@@ -593,9 +619,9 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
             ptx::wgmma_fence_acc(acc[0]);
             ptx::wgmma_fence_acc(acc[1]);
             if constexpr (KIND != 2) {
-                if (pending >= 0 && threadIdx.x % 128 == 0) ptx::mbar_arrive(empty_bar((uint32_t)pending));
+                if (pending >= 0 && threadIdx.x % 128 == 0) release((uint32_t)pending);
             }
-            if (!s.flush) continue;
+            if (!s.flush || filler) continue;
 
             // ---- flush: S[row][col] += D, lower triangle only (or the transposed cell, exact block cover) ----
             const int colA = (CG == 2 && cta_rank != 0) ? s.rowA1 : s.rowA0;
@@ -680,7 +706,9 @@ __global__ void __launch_bounds__(kThreads, 1) gram_kernel(const __grid_constant
         if (a.prof != nullptr && threadIdx.x == 128) a.prof[(size_t)blockIdx.x * 4 + 2] = globaltimer_ns();
     }
 
-    __syncthreads();
+    // no CTA of a pair exits while its peer may still arrive on its barriers
+    if constexpr (CG == 2) ptx::cluster_sync();
+    else __syncthreads();
     if (a.prof != nullptr && threadIdx.x == 0) a.prof[(size_t)blockIdx.x * 4 + 3] = globaltimer_ns();
 }
 
@@ -925,7 +953,47 @@ cudaError_t launch(const CUtensorMap& tmap, const GramArgs& args, int grid, cuda
     cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = C::SMEM_BYTES;
     cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    if (CG == 2) {   // the two CTAs of a worker form a cluster (TMA multicast of the B rows they share)
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+    }
     return cudaLaunchKernelEx(&cfg, gram_kernel<CG, KIND>, tmap, args);
+}
+
+// How many clusters of `cluster_size` CTAs of gram_kernel<2, KIND> (1 CTA per SM: ~200 KB of shared memory each) the
+// current device can hold at once; -1 if the query fails.
+template <int KIND>
+int max_clusters(int cluster_size) {
+    using C = Cfg<KIND>;
+    if (cudaFuncSetAttribute(gram_kernel<2, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess)
+        return -1;
+    if (cluster_size > 8 &&
+        cudaFuncSetAttribute(gram_kernel<2, KIND>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) return -1;
+    int sms = 0, dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)(sms / cluster_size * cluster_size));
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = C::SMEM_BYTES;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cluster_size;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    if (cudaOccupancyMaxActiveClusters(&clusters, gram_kernel<2, KIND>, &cfg) != cudaSuccess) {
+        cudaGetLastError();
+        return -1;
+    }
+    return clusters;
 }
 
 }  // namespace
@@ -1264,11 +1332,21 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
     }
 
     const int cgp = plan.cta_group;
-    const int workers = (cgp == 2) ? plan.num_sms / 2 : plan.num_sms;
     // one k-block = one 128-byte swizzle atom of the operand layout: 128 int8, 64 bf16 or 128 e2m1 cells (64 packed bytes,
     // expanded to one byte each in shared memory)
     const int elems_per_kb = (elem_bits == 16) ? 64 : 128;
     const int kind = (elem_bits == 8) ? 0 : (elem_bits == 16 ? 1 : 2);
+    int workers = plan.num_sms;
+    if (cgp == 2) {
+        // a pair is a 2-CTA cluster: as many pairs as the device holds at once, so that all of them are co-resident
+        int& pairs = plan.max_pairs[kind];
+        if (pairs == 0) pairs = kind == 0 ? max_clusters<0>(2) : (kind == 1 ? max_clusters<1>(2) : max_clusters<2>(2));
+        if (pairs <= 0) {
+            if (err) *err = "cudaOccupancyMaxActiveClusters found no room for a 2-CTA cluster of the Gram kernel";
+            return cudaErrorNotSupported;
+        }
+        workers = std::min(plan.num_sms / 2, pairs);
+    }
 
     CUtensorMap tmap;
     // Panel layout: dim0 = cells of one panel row (bytes for e2m1), dim1 = samples, dim2 = panels.  Row-major input is one
@@ -1425,35 +1503,9 @@ cudaError_t gram_preload_kernels(cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-// How many clusters of `cluster_size` CTAs of the int8 Gram kernel (1 CTA per SM: ~200 KB of shared memory each) the
-// current device can hold at once -- the GPC layout decides whether a 4- or 8-CTA cluster (TMA multicast of a shared
-// operand) could still use every SM.  Diagnostic only.
-int gram_debug_max_clusters(int cluster_size) {
-    using C = Cfg<0>;
-    if (cudaFuncSetAttribute(gram_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess) return -1;
-    if (cluster_size > 8 &&
-        cudaFuncSetAttribute(gram_kernel<2, 0>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) return -1;
-    int sms = 0, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(sms / cluster_size * cluster_size));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = C::SMEM_BYTES;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)cluster_size;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int clusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&clusters, gram_kernel<2, 0>, &cfg) != cudaSuccess) {
-        cudaGetLastError();
-        return -1;
-    }
-    return clusters;
-}
+// How many clusters of `cluster_size` CTAs of the int8 Gram kernel the current device can hold at once -- the GPC
+// layout decides whether a 4- or 8-CTA cluster could still use every SM.  Diagnostic only.
+int gram_debug_max_clusters(int cluster_size) { return max_clusters<0>(cluster_size); }
 
 cudaError_t gram_symmetrize(int32_t* d_S, int n, cudaStream_t stream) {
     const int nb = (n + 31) / 32;

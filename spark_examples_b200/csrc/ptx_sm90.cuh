@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_90a features the Gram kernel uses: mbarrier, TMA (cp.async.bulk.tensor) and
-// warpgroup MMA (wgmma).  Written for `nvcc -gencode arch=compute_90a,code=sm_90a` only.
+// Thin inline-PTX wrappers for the sm_90a features the Gram kernel uses: mbarrier, TMA (cp.async.bulk.tensor, also
+// multicast to a thread-block cluster), cluster addressing and barriers, and warpgroup MMA (wgmma).  Written for `nvcc -gencode arch=compute_90a,code=sm_90a` only.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -70,6 +70,33 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const void* desc,
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(desc)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
+}
+// The same box written to the same shared-memory offset of every CTA of the cluster named in `cta_mask`; each
+// destination CTA's mbarrier at offset `bar` receives the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_3d_multicast(uint32_t smem_dst, const void* desc, uint32_t bar, int32_t c0,
+                                                      int32_t c1, int32_t c2, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(desc)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
+        : "memory");
+}
+// ---------------------------------------------------------------- thread-block cluster
+// shared::cta address of this CTA -> shared::cluster address of the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa(uint32_t saddr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
+    return r;
+}
+// arrive on an mbarrier of any CTA of the cluster (address from mapa).  Default semantics (release at CTA scope): the
+// arrive frees a stage whose readers (wgmma, or the e2m1 expansion's loads) have already completed, and an explicit
+// .release.cluster would put a GPU-wide MEMBAR in front of every arrive (it made the CTA-pair kernel 3x slower).
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+}
+// every thread of every CTA of the cluster: arrive, then wait for all of them
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
 // ---------------------------------------------------------------- wgmma
 // Warpgroup MMA, both operands K-major in shared memory (128-byte swizzle), 64 x 128 accumulator tile of the warpgroup

@@ -11,9 +11,11 @@ namespace vpca {
 
 // ---- Gram (gram_sm90.cu) --------------------------------------------------------------------
 struct GramPlan {
-    int cta_group = 2;        // CTAs per tile (1: 128 x 256 tiles per CTA, 2: 256 x 256 per CTA pair, one A block each)
+    int cta_group = 2;        // CTAs per tile (1: 128 x 256 tiles per CTA; 2: 256 x 256 per CTA pair, one A block each,
+                              // the pair launched as a 2-CTA cluster that fetches the B rows once and multicasts them)
     int kb_window = 0;        // k-blocks per L2 window (0 -> automatic)
     int num_sms = 0;
+    int max_pairs[3] = {};    // 2-CTA clusters of the int8 / bf16 / e2m1 kernel the device holds at once (0: not queried)
     void* d_tiles = nullptr;  // device tile list (TileDesc, gram_sm90.cu)
     std::vector<int32_t> h_tiles;   // the same list on the host (8 ints per tile): resident / accumulator-fit decisions
     int num_tiles = 0;

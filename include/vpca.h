@@ -237,6 +237,44 @@ int vpca_get_centered(vpca_ctx* ctx, double* out);
 /* Tridiagonal form of the centered matrix after the last vpca_compute_pca (diag: n, offdiag: n-1). */
 int vpca_get_tridiagonal(vpca_ctx* ctx, double* diag, double* offdiag);
 
+/* ---- variant loadings and projection (beyond VariantsPca.scala:224-230) ---------------------------------------------
+ * The reference returns U (:226-227) and prints pc1 / pc2 per sample (:229-246); U alone means nothing without the
+ * cohort's genotypes.  With C = J S J (the centering of :199-223) and C u_c = lambda_c u_c (vpca_compute_pca), u_c is
+ * orthogonal to the ones vector, so
+ *   loadings of variant v:   w[v][c] = sum_s x[s][v] u_c[s]      carriers n_v = sum_s x[s][v]   (x as encoded at :56-60)
+ *   projection of cells y:   p_c = sum_v (y_v - n_v / N) w[v][c] / lambda_c
+ * and a reference sample projected with its own loadings gets u_c back, in the units of the pc1 / pc2 columns of :229-246.
+ * Cells are staged and encoded exactly as for the Gram (:56-60, :164; no-calls are 0); every sum runs in a fixed order,
+ * no floating-point atomics, so results are bitwise reproducible.  w[v] depends on column v only: the three input forms
+ * give the same bits.  Driver-side calls: one at a time per context, never concurrent with accumulation.
+ *
+ * After vpca_compute_pca(ctx, k, ...) U and the eigenvalues stay on the device until the next vpca_reset / vpca_set_gram /
+ * vpca_load_partial_gram / vpca_finalize_gram (VPCA_ERR_STATE after that).  Loadings of k' <= k components, k' in [1, 16]:
+ *   out_w[v * k' + c] = sum_s x[s][v] * U[s][c] (FP64), out_count[v] = sum_s x[s][v] (exact).  Rows without carriers are
+ *   legal (w = 0).  VPCA_ERR_INDEX_OUT_OF_RANGE for a sample index >= n_samples; VPCA_ERR_UNSUPPORTED on a band-only
+ *   context.  _panels: device input in the layout of vpca_accumulate_panels, device outputs, ordered on the ctx stream. */
+int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const int32_t* sample_idx, int64_t nv,
+                        double* out_w, int32_t* out_count);
+int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                      double* out_w, int32_t* out_count);
+int vpca_loadings_panels(vpca_ctx* ctx, int32_t k, const void* d_x, int64_t nv, int64_t panel_variants,
+                         double* d_w, int32_t* d_count);
+/* Projection, in a context whose n_samples is the NEW cohort's size M (its Gram is unused).  vpca_project_begin zeroes
+ * the M x k FP64 accumulator (k in [1, 16]); vpca_reset drops it.  Every row passed is a variant of the new cohort,
+ * aligned with w (nv x k, variant-major, as vpca_loadings_* wrote it) and mean (nv, n_v / N of the reference): rows with
+ * no carriers still contribute -mean * w.  Successive calls add up (per call in variant order; across calls in call
+ * order).  VPCA_ERR_STATE before vpca_project_begin.
+ * vpca_project_get: out[s + c*M] = acc[s][c] / evals[c] (column-major like vpca_compute_pca); evals = 1 reads the raw
+ * sums (e.g. to add the sums of several GPUs before dividing). */
+int vpca_project_begin(vpca_ctx* ctx, int32_t k);
+int vpca_project_calls(vpca_ctx* ctx, const int64_t* offsets, const int32_t* sample_idx, int64_t nv, const double* w,
+                       const double* mean);
+int vpca_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                     const double* w, const double* mean);
+int vpca_project_panels(vpca_ctx* ctx, const void* d_x, int64_t nv, int64_t panel_variants, const double* d_w,
+                        const double* d_mean);
+int vpca_project_get(vpca_ctx* ctx, const double* evals, double* out);
+
 /* ---- one process, all GPUs of the box (SURVEY 8b "process model") --------------------------------------------------
  * A vpca_pool is what `class VariantsPcaDriver` holds on a multi-GPU host: one vpca_ctx per GPU, wired with
  * vpca_gram_set_peers_local in VPCA_PEER_OWNER_ROWS mode (VPCA_PEER_REPLICATE when n_samples < 64 x n_gpus).  Spark

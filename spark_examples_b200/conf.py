@@ -112,4 +112,6 @@ class PcaConf(GenomicsConf):
             ("callsParquetPath", str, None, False),       # Parquet file of calls rows (parquet_calls.py): RDD[Seq[Int]] at rest
             ("bedPath", str, None, False),                # PLINK 1 fileset prefix (.bed/.bim/.fam) as the variants source
             ("bedCountedAllele", str, "A1", False),       # which .bim allele is "variation": A1 (PLINK's minor) or A2
+            ("saveLoadings", str, None, False),           # after computePca: write per-variant loadings + counts (.npz)
+            ("projectLoadings", str, None, False),        # project this cohort onto a saved loadings file (no Gram / eigensolve)
         ]

@@ -18,6 +18,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -50,6 +51,15 @@ struct vpca_ctx {
     bool eig_ready = false;
     JoinWork join;        // multi-dataset keying (join.cu); one join at a time (join_mu)
     std::mutex join_mu;
+    int pca_k = 0;        // k of the last vpca_compute_pca whose U / eigenvalues are still valid on the device (0: none)
+    int proj_k = 0;       // k of the projection begun by vpca_project_begin (0: none in progress)
+    double* d_proj_acc = nullptr;    // n x kProjLd partial projection sums (project.cu)
+    double* d_proj_part = nullptr;   // per-panel partial sums of one launch
+    int64_t cap_proj_part = 0;
+    double* d_lp_w = nullptr;        // host-input loadings / projection: one chunk of w (loadings out, projection in)
+    double* d_lp_mean = nullptr;     // and of the means (projection)
+    int32_t* d_lp_count = nullptr;   // and of the carrier counts (loadings)
+    int64_t cap_lp_w = 0, cap_lp_mean = 0, cap_lp_count = 0;
 
     struct Slot {
         int64_t pid = -1;
@@ -402,9 +412,13 @@ void lane_gram_time(vpca_ctx* ctx, vpca_ctx::Lane& L) {
     }
 }
 
-// CSR rows -> encode -> (optionally) Gram, on lane L.  out_tile != nullptr: copy the encoded tile back instead.
+// What a staging loop does with one encoded chunk: rows [v, v + nvc) of the call sit in L.d_x[b] in panel layout
+// (ctx->panel); work is enqueued on L.stream.
+using ChunkFn = std::function<int(vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc)>;
+
+// CSR rows -> encode -> consume(chunk), on lane L.  gram: the consumer launches the Gram (its time is recorded).
 int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, const void* sample_idx, int idx_bytes,
-                  int64_t nv, int32_t* d_target, void* out_tile, int64_t out_ld) {
+                  int64_t nv, const ChunkFn& consume, bool gram) {
     const int bits = ctx->elem_bits;
     // validate the whole offsets array before anything is sized from it
     if (offsets[0] < 0) return fail(ctx, VPCA_ERR_BAD_ARG, "offsets[0] must be >= 0");
@@ -414,7 +428,6 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
     CUDA_OK(ctx, cudaMemsetAsync(L.d_flags, 0, sizeof(int), L.stream));
     int64_t v = 0;
     int chunk = 0;
-    bool launched = false;
     while (v < nv) {
         // largest run of rows that fits both the variant and the index budget
         int64_t vend = std::min(nv, v + ctx->chunk_variants);
@@ -445,23 +458,8 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
         CUDA_OK(ctx, encode_calls(L.d_off[b], offsets[v], L.d_idx[b], idx_bytes, nvc, ctx->n, bits, ctx->max_mult, L.d_x[b], P, P,
                                   L.d_flags, L.stream));
         ctx->c_launches += 2;
-        if (out_tile != nullptr) {
-            // panel layout -> the caller's row-major tile, one 2-D copy per panel (chunk boundaries are multiples of
-            // 128 variants, so 4-bit rows split on byte boundaries)
-            for (int64_t pv = 0; pv < nvc; pv += P) {
-                const int64_t wv = std::min(P, nvc - pv);
-                CUDA_OK(ctx, cudaMemcpy2DAsync(static_cast<char*>(out_tile) + (size_t)(v + pv) * bits / 8,
-                                               (size_t)out_ld * bits / 8,
-                                               static_cast<const char*>(L.d_x[b]) + (size_t)(pv / P) * ctx->n * P * bits / 8,
-                                               (size_t)P * bits / 8, (size_t)(wv * bits + 7) / 8, (size_t)ctx->n,
-                                               cudaMemcpyDeviceToHost, L.stream));
-            }
-            ctx->c_d2h += (nvc * bits + 7) / 8 * (int64_t)ctx->n;
-        } else {
-            int rc = launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b], nvc, P, P, d_target);
-            if (rc != VPCA_OK) return rc;
-            launched = true;
-        }
+        int rc = consume(L, b, v, nvc);
+        if (rc != VPCA_OK) return rc;
         CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
         v = vend;
         ++chunk;
@@ -469,7 +467,7 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
     CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, L.d_flags, sizeof(int), cudaMemcpyDeviceToHost, L.stream));
     // the caller's buffers are read asynchronously: do not return before every copy has completed
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
-    if (launched) lane_gram_time(ctx, L);
+    if (gram && nv > 0) lane_gram_time(ctx, L);
     if (*L.h_flags & 1)
         return fail(ctx, VPCA_ERR_INDEX_OUT_OF_RANGE, "sample index outside [0, %d) (the reference throws at "
                     "VariantsPca.scala:59/:188)", ctx->n);
@@ -479,6 +477,38 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
     return VPCA_OK;
 }
 
+
+// Packed rows (code 0: bitmaps; 1 / 2: PLINK .bed rows counting A1 / A2, see encode.cu) -> encode -> consume(chunk), on
+// lane L; returns after the lane's stream has drained (the caller's buffer is free to reuse).
+int process_packed(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* bits, int64_t nv, int64_t stride_bytes, int code,
+                   const ChunkFn& consume) {
+    // bits beyond sample n-1 in the last byte of a row would be read as carriers of non-existent samples: the kernel
+    // masks them (smp >= n), nothing to validate on the host.
+    const int64_t P = ctx->panel;
+    const int64_t cap_rows = std::min<int64_t>(ctx->chunk_variants, (ctx->chunk_nnz * (int64_t)sizeof(int32_t)) / stride_bytes);
+    if (cap_rows < 32) return fail(ctx, VPCA_ERR_BAD_ARG, "stride_bytes too large for the staging buffer");
+    const int64_t whole = std::max<int64_t>(P, (cap_rows / P) * P);
+    const int64_t step = whole <= cap_rows ? whole : (cap_rows / 32) * 32;
+    int chunk = 0;
+    for (int64_t v = 0; v < nv; v += step, ++chunk) {
+        const int64_t nvc = std::min(step, nv - v);
+        const int b = chunk & 1;
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
+        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b], bits + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
+                                     cudaMemcpyHostToDevice, L.copy_stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
+        ctx->c_h2d += nvc * stride_bytes;
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        CUDA_OK(ctx, encode_bits(reinterpret_cast<const uint8_t*>(L.d_idx[b]), stride_bytes, nvc, ctx->n, ctx->elem_bits,
+                                 L.d_x[b], P, P, code, L.stream));
+        ctx->c_launches += 1;
+        int r = consume(L, b, v, nvc);
+        if (r != VPCA_OK) return r;
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
 
 template <typename T>
 static cudaError_t grow_buffer(T** p, int64_t* cap, int64_t need) {
@@ -607,6 +637,9 @@ int vpca_destroy(vpca_ctx* ctx) {
             if (d != ctx->plan.peer_rank && ctx->plan.peer_S[d] != nullptr) cudaIpcCloseMemHandle(ctx->plan.peer_base[d]);
     if (ctx->own_S) cudaFree(ctx->d_S);
     if (ctx->eig_ready) eig_free(ctx->eig);
+    for (void* p : {(void*)ctx->d_proj_acc, (void*)ctx->d_proj_part, (void*)ctx->d_lp_w, (void*)ctx->d_lp_mean,
+                    (void*)ctx->d_lp_count})
+        cudaFree(p);
     join_free(ctx->join);
     gram_plan_free(ctx->plan);
     for (cudaEvent_t ev : {ctx->ev_t0, ctx->ev_t1, ctx->ev_e0, ctx->ev_e1})
@@ -634,6 +667,8 @@ int vpca_reset(vpca_ctx* ctx) {
     for (auto& s : ctx->slots) s.used = false;
     ctx->finalized = false;
     ctx->pca_done = false;
+    ctx->pca_k = 0;
+    ctx->proj_k = 0;
     ctx->total_variants = 0;
     ctx->inflight_variants = 0;
     ctx->st.variants_accumulated = 0;
@@ -650,7 +685,22 @@ int vpca_encode_calls(vpca_ctx* ctx, const int64_t* offsets, const int32_t* samp
     if (nv == 0) return VPCA_OK;
     LaneGuard lg(ctx);
     if (lg.rc != VPCA_OK) return lg.rc;
-    return process_calls(ctx, *lg.lane, offsets, sample_idx, 4, nv, nullptr, out, ld);
+    const int bits = ctx->elem_bits;
+    const int64_t P = ctx->panel;
+    // panel layout -> the caller's row-major tile, one 2-D copy per panel (chunk boundaries are multiples of 128
+    // variants, so 4-bit rows split on byte boundaries)
+    auto copy_out = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) -> int {
+        for (int64_t pv = 0; pv < nvc; pv += P) {
+            const int64_t wv = std::min(P, nvc - pv);
+            CUDA_OK(ctx, cudaMemcpy2DAsync(static_cast<char*>(out) + (size_t)(v + pv) * bits / 8, (size_t)ld * bits / 8,
+                                           static_cast<const char*>(L.d_x[b]) + (size_t)(pv / P) * ctx->n * P * bits / 8,
+                                           (size_t)P * bits / 8, (size_t)(wv * bits + 7) / 8, (size_t)ctx->n,
+                                           cudaMemcpyDeviceToHost, L.stream));
+        }
+        ctx->c_d2h += (nvc * bits + 7) / 8 * (int64_t)ctx->n;
+        return VPCA_OK;
+    };
+    return process_calls(ctx, *lg.lane, offsets, sample_idx, 4, nv, copy_out, false);
 }
 
 static int accumulate_calls_impl(vpca_ctx* ctx, int64_t partition_id, const int64_t* offsets, const void* sample_idx,
@@ -671,7 +721,10 @@ static int accumulate_calls_impl(vpca_ctx* ctx, int64_t partition_id, const int6
         LaneGuard lg(ctx);
         rc = lg.rc;
         if (rc == VPCA_OK) rc = prepare_slot(ctx, *lg.lane, sc);
-        if (rc == VPCA_OK) rc = process_calls(ctx, *lg.lane, offsets, sample_idx, idx_bytes, nv, sc.target, nullptr, 0);
+        auto gram = [&](vpca_ctx::Lane& L, int b, int64_t, int64_t nvc) -> int {
+            return launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b], nvc, ctx->panel, ctx->panel, sc.target);
+        };
+        if (rc == VPCA_OK) rc = process_calls(ctx, *lg.lane, offsets, sample_idx, idx_bytes, nv, gram, true);
     }
     return sc.end(rc);
 }
@@ -706,31 +759,11 @@ static int accumulate_packed(vpca_ctx* ctx, int64_t partition_id, const uint8_t*
     auto body = [&](vpca_ctx::Lane& L) -> int {
         int r = prepare_slot(ctx, L, sc);
         if (r != VPCA_OK) return r;
-        // bits beyond sample n-1 in the last byte of a row would be read as carriers of non-existent samples: the kernel
-        // masks them (smp >= n), nothing to validate on the host.
-        const int64_t P = ctx->panel;
-        const int64_t cap_rows = std::min<int64_t>(ctx->chunk_variants, (ctx->chunk_nnz * (int64_t)sizeof(int32_t)) / stride_bytes);
-        if (cap_rows < 32) return fail(ctx, VPCA_ERR_BAD_ARG, "stride_bytes too large for the staging buffer");
-        const int64_t whole = std::max<int64_t>(P, (cap_rows / P) * P);
-        const int64_t step = whole <= cap_rows ? whole : (cap_rows / 32) * 32;
-        int chunk = 0;
-        for (int64_t v = 0; v < nv; v += step, ++chunk) {
-            const int64_t nvc = std::min(step, nv - v);
-            const int b = chunk & 1;
-            CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-            CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b], bits + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
-                                         cudaMemcpyHostToDevice, L.copy_stream));
-            CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
-            ctx->c_h2d += nvc * stride_bytes;
-            CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-            CUDA_OK(ctx, encode_bits(reinterpret_cast<const uint8_t*>(L.d_idx[b]), stride_bytes, nvc, ctx->n, ctx->elem_bits,
-                                     L.d_x[b], P, P, code, L.stream));
-            ctx->c_launches += 1;
-            r = launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b], nvc, P, P, sc.target);
-            if (r != VPCA_OK) return r;
-            CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
-        }
-        CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's buffer is free to reuse on return
+        auto gram = [&](vpca_ctx::Lane& L2, int b, int64_t, int64_t nvc) -> int {
+            return launch_gram(ctx, L2.plan, L2.stream, L2.ev_t0, L2.ev_t1, L2.d_x[b], nvc, ctx->panel, ctx->panel, sc.target);
+        };
+        r = process_packed(ctx, L, bits, nv, stride_bytes, code, gram);
+        if (r != VPCA_OK) return r;
         lane_gram_time(ctx, L);
         return VPCA_OK;
     };
@@ -1088,6 +1121,7 @@ int vpca_finalize_gram(vpca_ctx* ctx) {
     }
     ctx->finalized = true;
     ctx->pca_done = false;
+    ctx->pca_k = 0;
     return VPCA_OK;
 }
 
@@ -1146,6 +1180,7 @@ int vpca_load_partial_gram(vpca_ctx* ctx, const int32_t* gram, int64_t variants_
     // the restored counts keep counting against the int32 bound (VariantsPca.scala:185)
     ctx->total_variants = variants_in_gram;
     ctx->inflight_variants = 0;
+    ctx->pca_k = 0;
     return check_overflow(ctx, 0);
 }
 
@@ -1162,6 +1197,7 @@ int vpca_set_gram(vpca_ctx* ctx, const int32_t* gram) {
     ctx->inflight_variants = 0;
     ctx->finalized = true;
     ctx->pca_done = false;
+    ctx->pca_k = 0;
     return VPCA_OK;
 }
 
@@ -1196,6 +1232,7 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
         return fail(ctx, VPCA_ERR_UNSUPPORTED, "computePca is limited to 65535 samples, like the reference (MLlib RowMatrix "
                     "behind VariantsPca.scala:226 refuses more columns); the Gram itself has no such limit");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    ctx->pca_k = 0;   // U is overwritten from here on
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_e0, ctx->stream));
     int rc = run_center(ctx, false);   // row sums + mean; the solver materialises C only if it needs it
     if (rc != VPCA_OK) return rc;
@@ -1219,6 +1256,7 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
     if (non_zero_rows) *non_zero_rows = nz;
     ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
     ctx->pca_done = true;
+    ctx->pca_k = k;
     return VPCA_OK;
 }
 
@@ -1248,6 +1286,222 @@ int vpca_get_tridiagonal(vpca_ctx* ctx, double* diag, double* offdiag) {
     CUDA_OK(ctx, cudaMemcpyAsync(diag, ctx->eig.d_diag, (size_t)ctx->n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaMemcpyAsync(offdiag, ctx->eig.d_off, (size_t)(ctx->n - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return VPCA_OK;
+}
+
+// ---- variant loadings and projection (project.cu) --------------------------------------------------------------
+// Driver-side calls, one at a time per context and never concurrent with accumulation, so the chunk buffers below are
+// the context's own; host-input calls run on a staging lane (encode as for the Gram), panel calls on the ctx stream.
+static constexpr int kProjLd = 16;   // row pitch (doubles) of the projection accumulator
+
+static int loadings_check(vpca_ctx* ctx, int32_t k) {   // caller holds ctx->mu
+    if (ctx->band_rows != ctx->n)
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "loadings need the eigenvectors of the whole Gram; this context stores a row band");
+    if (k < 1 || k > 16) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings: k=%d out of range [1, 16]", k);
+    if (ctx->pca_k == 0)
+        return fail(ctx, VPCA_ERR_STATE, "loadings need a vpca_compute_pca since the last reset / set_gram / "
+                    "load_partial_gram / finalize_gram");
+    if (k > ctx->pca_k) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings of %d components, vpca_compute_pca computed %d", k, ctx->pca_k);
+    return VPCA_OK;
+}
+
+static int project_check(vpca_ctx* ctx) {   // caller holds ctx->mu
+    if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_UNSUPPORTED, "projection needs a context that stores the whole Gram");
+    if (ctx->proj_k == 0) return fail(ctx, VPCA_ERR_STATE, "call vpca_project_begin first");
+    return VPCA_OK;
+}
+
+// The projection of one encoded chunk [v, v + nvc) on lane L: the chunk's slice of w / mean goes to the device on the
+// lane's stream (the single buffer is reused in stream order), then the projection kernels add into the accumulator.
+static int project_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, const double* w, const double* mean) {
+    const int k = ctx->proj_k;
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_lp_w, w + v * k, (size_t)nvc * k * sizeof(double), cudaMemcpyHostToDevice, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_lp_mean, mean + v, (size_t)nvc * sizeof(double), cudaMemcpyHostToDevice, L.stream));
+    ctx->c_h2d += nvc * (k + 1) * (int64_t)sizeof(double);
+    CUDA_OK(ctx, project_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, ctx->d_lp_w, ctx->d_lp_mean, k,
+                                ctx->d_proj_part, ctx->d_proj_acc, kProjLd, L.stream));
+    ctx->c_launches += 2;
+    return VPCA_OK;
+}
+
+static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, int k, double* out_w,
+                          int32_t* out_count) {
+    CUDA_OK(ctx, loadings_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, ctx->eig.d_evecs, k, ctx->d_lp_w,
+                                 ctx->d_lp_count, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_lp_w, (size_t)nvc * k * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(out_count + v, ctx->d_lp_count, (size_t)nvc * sizeof(int32_t), cudaMemcpyDeviceToHost, L.stream));
+    ctx->c_launches += 1;
+    ctx->c_d2h += nvc * (k * (int64_t)sizeof(double) + 4);
+    return VPCA_OK;
+}
+
+// chunk buffers for host-input loadings (project == false) or projection; after LaneGuard (it fixes chunk_variants)
+static int lp_buffers(vpca_ctx* ctx, int k, bool project) {
+    const int64_t cv = ctx->chunk_variants;
+    CUDA_OK(ctx, grow_buffer(&ctx->d_lp_w, &ctx->cap_lp_w, cv * k));
+    if (project) {
+        CUDA_OK(ctx, grow_buffer(&ctx->d_lp_mean, &ctx->cap_lp_mean, cv));
+        CUDA_OK(ctx, grow_buffer(&ctx->d_proj_part, &ctx->cap_proj_part, project_scratch_doubles(ctx->n, cv, ctx->panel, k)));
+    } else {
+        CUDA_OK(ctx, grow_buffer(&ctx->d_lp_count, &ctx->cap_lp_count, cv));
+    }
+    return VPCA_OK;
+}
+
+int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const int32_t* sample_idx, int64_t nv,
+                        double* out_w, int32_t* out_count) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    if (offsets == nullptr || nv < 0 || (nv > 0 && (out_w == nullptr || out_count == nullptr)) ||
+        (nv > 0 && sample_idx == nullptr && offsets[nv] > offsets[0]))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_calls: bad argument");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        int rc = loadings_check(ctx, k);
+        if (rc != VPCA_OK) return rc;
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    int rc = lp_buffers(ctx, k, false);
+    if (rc != VPCA_OK) return rc;
+    auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) {
+        return loadings_chunk(ctx, L, b, v, nvc, k, out_w, out_count);
+    };
+    return process_calls(ctx, *lg.lane, offsets, sample_idx, 4, nv, consume, false);
+}
+
+int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                      double* out_w, int32_t* out_count) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    if (counted_allele != 1 && counted_allele != 2)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: counted_allele must be 1 (A1) or 2 (A2)");
+    if (nv < 0 || (nv > 0 && (rows == nullptr || out_w == nullptr || out_count == nullptr)) || stride_bytes < (ctx->n + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        int rc = loadings_check(ctx, k);
+        if (rc != VPCA_OK) return rc;
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    int rc = lp_buffers(ctx, k, false);
+    if (rc != VPCA_OK) return rc;
+    auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) {
+        return loadings_chunk(ctx, L, b, v, nvc, k, out_w, out_count);
+    };
+    return process_packed(ctx, *lg.lane, rows, nv, stride_bytes, counted_allele, consume);
+}
+
+int vpca_loadings_panels(vpca_ctx* ctx, int32_t k, const void* d_x, int64_t nv, int64_t panel_variants, double* d_w,
+                         int32_t* d_count) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    int rc = loadings_check(ctx, k);
+    if (rc != VPCA_OK) return rc;
+    if (d_x == nullptr || nv < 0 || panel_variants < 128 || (panel_variants % 128) != 0 || (nv > 0 && (d_w == nullptr || d_count == nullptr)))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_panels: panel_variants must be a positive multiple of 128");
+    if ((reinterpret_cast<uintptr_t>(d_x) & 31) != 0) return fail(ctx, VPCA_ERR_BAD_ARG, "panels must be 32-byte aligned");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    CUDA_OK(ctx, loadings_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, ctx->eig.d_evecs, k, d_w, d_count, ctx->stream));
+    ctx->c_launches += nv > 0 ? 1 : 0;
+    return VPCA_OK;
+}
+
+int vpca_project_begin(vpca_ctx* ctx, int32_t k) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_UNSUPPORTED, "projection needs a context that stores the whole Gram");
+    if (k < 1 || k > 16) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_begin: k=%d out of range [1, 16]", k);
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (ctx->d_proj_acc == nullptr) CUDA_OK(ctx, cudaMalloc(&ctx->d_proj_acc, (size_t)ctx->n * kProjLd * sizeof(double)));
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->d_proj_acc, 0, (size_t)ctx->n * kProjLd * sizeof(double), ctx->stream));
+    ctx->proj_k = k;
+    return VPCA_OK;
+}
+
+int vpca_project_calls(vpca_ctx* ctx, const int64_t* offsets, const int32_t* sample_idx, int64_t nv, const double* w,
+                       const double* mean) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        int rc = project_check(ctx);
+        if (rc != VPCA_OK) return rc;
+    }
+    if (offsets == nullptr || nv < 0 || (nv > 0 && (w == nullptr || mean == nullptr)) ||
+        (nv > 0 && sample_idx == nullptr && offsets[nv] > offsets[0]))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_calls: bad argument");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    int rc = lp_buffers(ctx, ctx->proj_k, true);
+    if (rc != VPCA_OK) return rc;
+    auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) { return project_chunk(ctx, L, b, v, nvc, w, mean); };
+    return process_calls(ctx, *lg.lane, offsets, sample_idx, 4, nv, consume, false);
+}
+
+int vpca_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                     const double* w, const double* mean) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        int rc = project_check(ctx);
+        if (rc != VPCA_OK) return rc;
+    }
+    if (counted_allele != 1 && counted_allele != 2)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_bed: counted_allele must be 1 (A1) or 2 (A2)");
+    if (nv < 0 || (nv > 0 && (rows == nullptr || w == nullptr || mean == nullptr)) || stride_bytes < (ctx->n + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    int rc = lp_buffers(ctx, ctx->proj_k, true);
+    if (rc != VPCA_OK) return rc;
+    auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) { return project_chunk(ctx, L, b, v, nvc, w, mean); };
+    return process_packed(ctx, *lg.lane, rows, nv, stride_bytes, counted_allele, consume);
+}
+
+int vpca_project_panels(vpca_ctx* ctx, const void* d_x, int64_t nv, int64_t panel_variants, const double* d_w,
+                        const double* d_mean) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    int rc = project_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    if (d_x == nullptr || nv < 0 || panel_variants < 128 || (panel_variants % 128) != 0 || (nv > 0 && (d_w == nullptr || d_mean == nullptr)))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_panels: panel_variants must be a positive multiple of 128");
+    if ((reinterpret_cast<uintptr_t>(d_x) & 31) != 0) return fail(ctx, VPCA_ERR_BAD_ARG, "panels must be 32-byte aligned");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int64_t need = project_scratch_doubles(ctx->n, nv, panel_variants, ctx->proj_k);
+    if (need > ctx->cap_proj_part) {
+        // the scratch may still be read by an earlier launch on this stream
+        CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+        CUDA_OK(ctx, grow_buffer(&ctx->d_proj_part, &ctx->cap_proj_part, need));
+    }
+    CUDA_OK(ctx, project_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, d_w, d_mean, ctx->proj_k, ctx->d_proj_part,
+                                ctx->d_proj_acc, kProjLd, ctx->stream));
+    ctx->c_launches += 2;
+    return VPCA_OK;
+}
+
+int vpca_project_get(vpca_ctx* ctx, const double* evals, double* out) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    int rc = project_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    if (evals == nullptr || out == nullptr) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_get: NULL argument");
+    const int k = ctx->proj_k, n = ctx->n;
+    std::vector<double> acc((size_t)n * kProjLd);
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    CUDA_OK(ctx, cudaMemcpyAsync(acc.data(), ctx->d_proj_acc, acc.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_d2h += (int64_t)(acc.size() * sizeof(double));
+    for (int c = 0; c < k; ++c)
+        for (int s = 0; s < n; ++s) out[s + (size_t)c * n] = acc[(size_t)s * kProjLd + c] / evals[c];
     return VPCA_OK;
 }
 

@@ -176,6 +176,18 @@ cudaError_t center_gram(EigWork& w, const int32_t* d_S, cudaStream_t stream, boo
 cudaError_t center_matrix(EigWork& w, cudaStream_t stream);
 cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches);
 
+// ---- variant loadings and projection (project.cu) -----------------------------------------------------------------
+// Both read cells in the panel layout (see gram_accumulate; zero cells after nv in the last panel), k in [1, 16].
+// w[v * k + c] = sum_s x[s][v] U[s][c] (FP64, samples summed in order), count[v] = sum_s x[s][v] (exact) for v < nv;
+// U: n x k column-major (ld n).  Never synchronises.
+cudaError_t loadings_launch(const void* d_x, int elem_bits, int n, int64_t nv, int64_t panel, const double* d_U, int k,
+                            double* d_w, int32_t* d_count, cudaStream_t stream);
+// acc[s * acc_ld + c] += sum_v (y[s][v] - mean[v]) w[v * k + c] for the m samples: a partial sum per panel (variants in
+// order) into d_part (project_scratch_doubles entries), then the partials added in panel order.
+cudaError_t project_launch(const void* d_y, int elem_bits, int m, int64_t nv, int64_t panel, const double* d_w,
+                           const double* d_mean, int k, double* d_part, double* d_acc, int acc_ld, cudaStream_t stream);
+int64_t project_scratch_doubles(int m, int64_t nv, int64_t panel, int k);
+
 // ---- synthetic generator (synth.cu) ----------------------------------------------------------------
 cudaError_t synth_dense(uint64_t seed, int n, int64_t v0, int64_t nv, int mode, int elem_bits, void* d_x,
                         int64_t ld, int64_t panel, cudaStream_t stream);

@@ -41,3 +41,24 @@ def allreduce_count(value: int, device=None) -> int:
     t = torch.tensor([int(value)], dtype=torch.int64, device=device if device is not None else "cpu")
     dist.all_reduce(t, op=dist.ReduceOp.SUM)
     return int(t.item())
+
+
+def gather_to_rank0(obj) -> list:
+    """`obj` of every rank in rank order on rank 0 (other ranks get None); a single process gets [obj]."""
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+        return [obj]
+    out = [None] * dist.get_world_size() if dist.get_rank() == 0 else None
+    dist.gather_object(obj, out, dst=0)
+    return out
+
+
+def allreduce_f64(arr, device=None):
+    """Element-wise sum of a float64 numpy array over all ranks (projection partial sums); returns numpy."""
+    import torch
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+        return arr
+    t = torch.from_numpy(arr).to(device if device is not None else "cpu")
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    return t.cpu().numpy()

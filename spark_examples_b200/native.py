@@ -50,6 +50,8 @@ EXPORTED_SYMBOLS = (
     "vpca_pool_accumulate_calls", "vpca_pool_accumulate_calls_u16", "vpca_pool_accumulate_bits", "vpca_pool_accumulate_bed",
     "vpca_pool_commit", "vpca_pool_abort", "vpca_pool_reduce_and_finalize", "vpca_pool_get_gram", "vpca_pool_compute_pca",
     "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan",
+    "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
+    "vpca_project_bed", "vpca_project_panels", "vpca_project_get",
 )
 
 
@@ -248,6 +250,22 @@ def load_library() -> ctypes.CDLL:
     L.vpca_gram_gather.argtypes = [vp]
     L.vpca_debug_gram_profile.restype = ctypes.c_int
     L.vpca_debug_gram_profile.argtypes = [vp, vp, i32]
+    L.vpca_loadings_calls.restype = ctypes.c_int
+    L.vpca_loadings_calls.argtypes = [vp, i32, vp, vp, i64, vp, vp]
+    L.vpca_loadings_bed.restype = ctypes.c_int
+    L.vpca_loadings_bed.argtypes = [vp, i32, vp, i64, i64, i32, vp, vp]
+    L.vpca_loadings_panels.restype = ctypes.c_int
+    L.vpca_loadings_panels.argtypes = [vp, i32, vp, i64, i64, vp, vp]
+    L.vpca_project_begin.restype = ctypes.c_int
+    L.vpca_project_begin.argtypes = [vp, i32]
+    L.vpca_project_calls.restype = ctypes.c_int
+    L.vpca_project_calls.argtypes = [vp, vp, vp, i64, vp, vp]
+    L.vpca_project_bed.restype = ctypes.c_int
+    L.vpca_project_bed.argtypes = [vp, vp, i64, i64, i32, vp, vp]
+    L.vpca_project_panels.restype = ctypes.c_int
+    L.vpca_project_panels.argtypes = [vp, vp, i64, i64, vp, vp]
+    L.vpca_project_get.restype = ctypes.c_int
+    L.vpca_project_get.argtypes = [vp, vp, vp]
     _lib = L
     return L
 
@@ -572,6 +590,69 @@ class NativePca:
         st = VpcaStats()
         self._check(self._lib.vpca_get_stats(self._h, ctypes.byref(st)))
         return {name: getattr(st, name) for name, _ in VpcaStats._fields_}
+
+    # -- variant loadings and projection onto computed principal coordinates (vpca.h, DESIGN.md 6) --------------------
+    def loadingsCalls(self, k: int, offsets, sample_idx):
+        """After computePca(k0 >= k): (w (nv, k) float64, count (nv,) int32) with w[v, c] = sum_s x[s][v] U[s, c] and
+        count[v] = sum_s x[s][v] for the CSR rows given (rows without carriers allowed)."""
+        off, idx = self._csr(offsets, sample_idx)
+        nv = len(off) - 1
+        w = np.zeros((max(nv, 1), int(k)), dtype=np.float64)
+        cnt = np.zeros(max(nv, 1), dtype=np.int32)
+        self._check(self._lib.vpca_loadings_calls(self._h, int(k), _host_ptr(off), _host_ptr(idx) if len(idx) else None, nv,
+                                                  _host_ptr(w), _host_ptr(cnt)))
+        return w[:nv], cnt[:nv]
+
+    def loadingsBed(self, k: int, rows: np.ndarray, counted_allele: int = 1):
+        """Same for PLINK .bed rows (see accumulateBed)."""
+        b = np.ascontiguousarray(rows, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        w = np.zeros((max(b.shape[0], 1), int(k)), dtype=np.float64)
+        cnt = np.zeros(max(b.shape[0], 1), dtype=np.int32)
+        self._check(self._lib.vpca_loadings_bed(self._h, int(k), _host_ptr(b), b.shape[0], b.shape[1], int(counted_allele),
+                                                _host_ptr(w), _host_ptr(cnt)))
+        return w[:b.shape[0]], cnt[:b.shape[0]]
+
+    def loadingsPanels(self, k: int, d_ptr: int, nv: int, panel_variants: int, d_w: int, d_count: int):
+        """Device panels in, device outputs (nv x k float64, nv int32), ordered on the context's stream."""
+        self._check(self._lib.vpca_loadings_panels(self._h, int(k), d_ptr, int(nv), int(panel_variants), d_w, d_count))
+
+    def projectBegin(self, k: int):
+        """Start a projection of this context's n samples onto k components (zeroes the accumulator)."""
+        self._check(self._lib.vpca_project_begin(self._h, int(k)))
+        self._proj_k = int(k)
+
+    def projectCalls(self, offsets, sample_idx, w, mean):
+        """Add sum_v (y[s][v] - mean[v]) w[v, :] for the CSR rows given; w (nv, k) and mean (nv,) align with the rows."""
+        off, idx = self._csr(offsets, sample_idx)
+        nv = len(off) - 1
+        ww = np.ascontiguousarray(w, dtype=np.float64).reshape(nv, -1)
+        mm = np.ascontiguousarray(mean, dtype=np.float64).reshape(nv)
+        self._check(self._lib.vpca_project_calls(self._h, _host_ptr(off), _host_ptr(idx) if len(idx) else None, nv,
+                                                 _host_ptr(ww), _host_ptr(mm)))
+
+    def projectBed(self, rows: np.ndarray, w, mean, counted_allele: int = 1):
+        b = np.ascontiguousarray(rows, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        ww = np.ascontiguousarray(w, dtype=np.float64).reshape(b.shape[0], -1)
+        mm = np.ascontiguousarray(mean, dtype=np.float64).reshape(b.shape[0])
+        self._check(self._lib.vpca_project_bed(self._h, _host_ptr(b), b.shape[0], b.shape[1], int(counted_allele),
+                                               _host_ptr(ww), _host_ptr(mm)))
+
+    def projectPanels(self, d_ptr: int, nv: int, panel_variants: int, d_w: int, d_mean: int):
+        self._check(self._lib.vpca_project_panels(self._h, d_ptr, int(nv), int(panel_variants), d_w, d_mean))
+
+    def projectGet(self, evals) -> np.ndarray:
+        """(n, k) projected coordinates: accumulated sums / evals[c] (evals of ones: the raw sums)."""
+        k = getattr(self, "_proj_k", 0)        # 0: not begun, the library reports VPCA_ERR_STATE before reading evals
+        ev = np.ascontiguousarray(evals, dtype=np.float64).reshape(-1)
+        if k and len(ev) != k:
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"evals must have {k} entries")
+        out = np.zeros(self.n * max(k, 1), dtype=np.float64)
+        self._check(self._lib.vpca_project_get(self._h, _host_ptr(ev), _host_ptr(out)))
+        return out.reshape(max(k, 1), self.n).T.copy()
 
 
 def debugTiles(n_samples: int, cta_group: int = 2, exact: bool = True) -> np.ndarray:

@@ -25,6 +25,7 @@ class CallsBatch:
     """One partition already in `RDD[Seq[Int]]` form (VariantsPca.scala:153-168): CSR rows of sample indices."""
     offsets: np.ndarray   # int64, nv + 1
     idx: np.ndarray       # int32
+    keys: Optional[np.ndarray] = None   # (nv, 2) uint64 murmur3_128 variant keys of the rows (None: rows carry no identity)
 
 
 @dataclass

@@ -177,6 +177,7 @@ class VariantsPcaDriver:
         self._nat: Optional[native.NativePca] = None
         self._gram_tensor = None
         self._torch_stream = None
+        self._bim_cache: Dict[str, list] = {}
 
     # -- VariantsPca.scala:87 ---------------------------------------------------------------------------------------
     @property
@@ -257,13 +258,18 @@ class VariantsPcaDriver:
         # conf.variantSetId().size (:154); sources that are not API variant sets count the datasets they hold
         variantSetCount = len(self.conf.variantSetId()) if self.conf.variantSetId.isSupplied else len(data)
         mapping = self.common.indexes
+        # loadings files key record rows by their variant key (:62-78); a projection keeps the rows without carriers,
+        # which still contribute -mean * w
+        want_keys = self.conf.saveLoadings.isDefined or self.conf.projectLoadings.isDefined
         if variantSetCount == 1:
             parts = []
             for part in data[0].partitions:
                 if isinstance(part, (CallsBatch, SyntheticSlice, BedSlice, ParquetSlice)):
                     parts.append(part)                          # already RDD[Seq[Int]] rows (or their packed form)
                 else:
-                    parts.append(_rows_to_batch([extractCallInfo(v, mapping) for v in part]))
+                    keys = [variantKeyBytes(v) for v in part] if want_keys else None
+                    parts.append(_rows_to_batch([extractCallInfo(v, mapping) for v in part], keys,
+                                                keep_empty=self.conf.projectLoadings.isDefined))
             return CallsRdd(parts, n)
         # keying, join / merge and the concatenation of the calls run on the GPU and feed the encoder there (csrc/join.cu);
         # joinDatasets / mergeDatasets above stay as the record-level mirror of the reference's public methods
@@ -356,6 +362,154 @@ class VariantsPcaDriver:
                     for name, pc1, pc2, dataset in rows:
                         fh.write(f"{name}\t{jdouble(pc1)}\t{jdouble(pc2)}\t{dataset}\n")
                 open(os.path.join(path, "_SUCCESS"), "w").close()
+
+    # -- variant loadings and projection onto saved principal coordinates (beyond :224-230; DESIGN.md 6) ------------
+    def keyKind(self, callsets: CallsRdd) -> str:
+        """How the rows of this cohort are identified in a loadings file: "variant" (murmur3_128 of the variant key,
+        :62-78), "bim" (murmur3_128 of contig, position, A1, A2) or "row" (global row index)."""
+        kinds = set()
+        for p in callsets.partitions:
+            if isinstance(p, JoinedSlice):
+                raise ValueError("--save-loadings / --project-loadings read one dataset; joined multi-dataset input is "
+                                 "not supported")
+            kinds.add("bim" if isinstance(p, BedSlice) else
+                      "variant" if isinstance(p, CallsBatch) and p.keys is not None else "row")
+        if len(kinds) > 1:
+            raise ValueError(f"partitions mix variant identities {sorted(kinds)}")
+        return kinds.pop() if kinds else "row"
+
+    @staticmethod
+    def _counted_allele(callsets: CallsRdd) -> int:
+        """1 / 2: .bed carriers of A1 / A2; 0: `hasVariation` of the calls (:58)."""
+        for p in callsets.partitions:
+            if isinstance(p, BedSlice):
+                return int(p.counted)
+        return 0
+
+    def _partition_keys(self, part, row0: int) -> np.ndarray:
+        """(nv, 2) uint64 identity of every row of a partition (see keyKind)."""
+        if isinstance(part, BedSlice):
+            prefix = part.bed.prefix
+            if prefix not in self._bim_cache:
+                from . import plink
+                self._bim_cache[prefix] = plink.read_bim(prefix)
+            bim = self._bim_cache[prefix][part.v0:part.v0 + part.nv]
+            return np.asarray([_hash_words(bimKeyBytes(b)) for b in bim], np.uint64).reshape(-1, 2)
+        if isinstance(part, CallsBatch) and part.keys is not None:
+            return np.asarray(part.keys, np.uint64).reshape(-1, 2)
+        nv = _partition_len(part)
+        keys = np.zeros((nv, 2), np.uint64)
+        keys[:, 0] = np.arange(row0, row0 + nv, dtype=np.uint64)
+        return keys
+
+    def _partition_loadings(self, nat: native.NativePca, part, k: int, panel: int = 8192):
+        if isinstance(part, SyntheticSlice):
+            import torch
+            dev = self._gram_tensor.device
+            buf = torch.empty(nat.panelBytes(part.nv, panel), dtype=torch.uint8, device=dev)
+            w = torch.empty((part.nv, k), dtype=torch.float64, device=dev)
+            cnt = torch.empty(part.nv, dtype=torch.int32, device=dev)
+            nat.synthPanelsDevice(part.seed, part.v0, part.nv, 0, buf.data_ptr(), panel)
+            nat.loadingsPanels(k, buf.data_ptr(), part.nv, panel, w.data_ptr(), cnt.data_ptr())
+            torch.cuda.current_stream().synchronize()
+            return w.cpu().numpy(), cnt.cpu().numpy()
+        if isinstance(part, BedSlice):
+            return nat.loadingsBed(k, part.rows(), part.counted)
+        off, idx = _partition_csr(part)
+        return nat.loadingsCalls(k, off, idx)
+
+    def saveLoadings(self, callsets: CallsRdd, path: Optional[str] = None):
+        """After computePca: the loadings w = X^T U (numPc columns) and carrier counts of every variant of this run,
+        streamed through the GPU a second time, written by rank 0 as one .npz (rows in partition order)."""
+        path = path if path is not None else self.conf.saveLoadings()
+        kind = self.keyKind(callsets)
+        k = self.conf.numPc()
+        starts = _partition_starts(callsets)
+        mine = {}
+        for pid, part in enumerate(callsets.partitions):
+            if vdist.partition_owner(pid, self._world) != self._rank:
+                continue
+            w, cnt = self._partition_loadings(self._nat, part, k)
+            mine[pid] = (self._partition_keys(part, starts[pid]), np.asarray(w, np.float64).reshape(-1, k),
+                         np.asarray(cnt, np.int32))
+        gathered = vdist.gather_to_rank0(mine)
+        if self._rank != 0:
+            return
+        merged = {}
+        for d in gathered:
+            merged.update(d)
+        order = sorted(merged)
+
+        def cat(i, empty):
+            return np.concatenate([merged[p][i] for p in order]) if order else empty
+        with open(path, "wb") as fh:
+            np.savez(fh, loadings=cat(1, np.zeros((0, k))), count=cat(2, np.zeros(0, np.int32)),
+                     n_samples=np.int64(len(self.common.indexes)), eigenvalues=np.asarray(self.eigenvalues[:k], np.float64),
+                     counted_allele=np.int32(self._counted_allele(callsets)), keys=cat(0, np.zeros((0, 2), np.uint64)),
+                     key_kind=np.str_(kind))
+
+    def projectLoadings(self, callsets: CallsRdd, path: Optional[str] = None) -> List[Tuple[str, float, float]]:
+        """Place this cohort in the PC space of a saved loadings file, without a Gram or an eigensolve: every row whose
+        key is in the file goes through the GPU projection (rows without carriers too); file variants this cohort
+        lacks contribute nothing (mean imputation).  Returns computePca's (callset id, pc1, pc2) rows."""
+        path = path if path is not None else self.conf.projectLoadings()
+        kind = self.keyKind(callsets)
+        with np.load(path, allow_pickle=False) as f:
+            W, count, keys = f["loadings"], f["count"], f["keys"]
+            n_ref, evals = int(f["n_samples"]), np.asarray(f["eigenvalues"], np.float64)
+            file_kind, file_counted = str(f["key_kind"]), int(f["counted_allele"])
+        if file_kind != kind:
+            raise ValueError(f"{path} identifies variants by {file_kind!r} keys, this cohort's rows by {kind!r} keys")
+        counted = self._counted_allele(callsets)
+        if file_counted != counted:
+            raise ValueError(f"{path} counts allele {file_counted}, this cohort counts allele {counted} (0: hasVariation)")
+        k = W.shape[1] if W.ndim == 2 else 0
+        if k < 2:
+            raise ValueError(f"{path} holds {k} component(s); pc1 and pc2 need at least 2")
+        mean = count.astype(np.float64) / n_ref
+        index = {(int(a), int(b)): i for i, (a, b) in enumerate(keys)}
+        rowCount = len(self.common.indexes)
+        nat = self._native(rowCount)
+        nat.reset()
+        nat.projectBegin(k)
+        starts = _partition_starts(callsets)
+        for pid, part in enumerate(callsets.partitions):
+            if vdist.partition_owner(pid, self._world) != self._rank:
+                continue
+            rows = np.asarray([index.get((int(a), int(b)), -1) for a, b in self._partition_keys(part, starts[pid])],
+                              np.int64).reshape(-1)
+            sel = rows >= 0
+            if sel.any():
+                self._partition_project(nat, part, sel, W[rows[sel]], mean[rows[sel]])
+        if self._world > 1:
+            raw = vdist.allreduce_f64(nat.projectGet(np.ones(k)), self._gram_tensor.device)
+            P = raw / evals[None, :]
+        else:
+            P = nat.projectGet(evals)
+        self.eigenvalues = evals
+        self.components = P
+        reverse = {i: cid for cid, i in self.common.indexes.items()}
+        return [(reverse[i], float(P[i, 0]), float(P[i, 1])) for i in range(rowCount)]
+
+    def _partition_project(self, nat: native.NativePca, part, sel: np.ndarray, w: np.ndarray, mean: np.ndarray,
+                           panel: int = 8192):
+        if isinstance(part, SyntheticSlice):
+            # rows are born on the device: all of them go, unmatched rows with w = 0 and mean = 0
+            import torch
+            dev = self._gram_tensor.device
+            W_full = np.zeros((part.nv, w.shape[1]), np.float64)
+            m_full = np.zeros(part.nv, np.float64)
+            W_full[sel], m_full[sel] = w, mean
+            buf = torch.empty(nat.panelBytes(part.nv, panel), dtype=torch.uint8, device=dev)
+            dw, dm = torch.from_numpy(W_full).to(dev), torch.from_numpy(m_full).to(dev)
+            nat.synthPanelsDevice(part.seed, part.v0, part.nv, 0, buf.data_ptr(), panel)
+            nat.projectPanels(buf.data_ptr(), part.nv, panel, dw.data_ptr(), dm.data_ptr())
+            torch.cuda.current_stream().synchronize()       # the buffers must outlive the kernels that read them
+        elif isinstance(part, BedSlice):
+            nat.projectBed(part.rows()[sel], w, mean, part.counted)
+        else:
+            off, idx = _select_rows(*_partition_csr(part), sel)
+            nat.projectCalls(off, idx, w, mean)
 
     def reportIoStats(self):                                                     # :281
         self.common.reportIoStats()
@@ -459,20 +613,68 @@ def joined_rows_on_host(p: JoinedSlice) -> CallsBatch:
     return CallsBatch(off, np.asarray([c for r in out for c in r], np.int32))
 
 
-def _rows_to_batch(rows: Iterable[Sequence[CallData]]) -> CallsBatch:
-    """VariantsPca.scala:164-167: keep calls with variation, drop empty variants, project to the callset index."""
-    kept = []
-    for calls in rows:
+def _rows_to_batch(rows: Iterable[Sequence[CallData]], keys: Optional[Sequence[bytes]] = None,
+                   keep_empty: bool = False) -> CallsBatch:
+    """VariantsPca.scala:164-167: keep calls with variation, drop empty variants, project to the callset index.
+    keys: the variant key bytes of the rows (:65-73), hashed into CallsBatch.keys for the rows kept; keep_empty: keep
+    the rows without carriers (a projection needs them)."""
+    kept, kept_keys = [], []
+    for v, calls in enumerate(rows):
         r = [c.callsetId for c in calls if c.hasVariation]
-        if len(r) > 0:
+        if len(r) > 0 or keep_empty:
             kept.append(r)
+            if keys is not None:
+                kept_keys.append(_hash_words(keys[v]))
     off = np.zeros(len(kept) + 1, np.int64)
     if kept:
         off[1:] = np.cumsum([len(r) for r in kept])
         idx = np.concatenate([np.asarray(r, np.int32) for r in kept])
     else:
         idx = np.zeros(0, np.int32)
-    return CallsBatch(off, idx)
+    if keys is None:
+        return CallsBatch(off, idx)
+    return CallsBatch(off, idx, np.asarray(kept_keys, np.uint64).reshape(-1, 2))
+
+
+def _hash_words(key: bytes) -> Tuple[int, int]:
+    """murmur3_128 of `key` as its two little-endian 64-bit halves (what vpca_hash_keys returns)."""
+    h1, h2 = struct.unpack("<QQ", bytes.fromhex(murmur3_128(key)))
+    return h1, h2
+
+
+def bimKeyBytes(b) -> bytes:
+    """Key bytes of a .bim record: contig, NUL, position (int64 little-endian), A1, NUL, A2."""
+    return b.contig.encode("utf-8") + b"\0" + struct.pack("<q", b.position) + b.a1.encode("utf-8") + b"\0" + b.a2.encode("utf-8")
+
+
+def _partition_len(part) -> int:
+    return len(part.offsets) - 1 if isinstance(part, CallsBatch) else int(part.nv)
+
+
+def _partition_starts(callsets: CallsRdd) -> List[int]:
+    """Global row index of the first row of every partition."""
+    starts, r = [], 0
+    for p in callsets.partitions:
+        starts.append(r)
+        r += _partition_len(p)
+    return starts
+
+
+def _partition_csr(part):
+    """CSR rows of a calls partition; a Parquet row group keeps its rows without carriers (row keys stay aligned)."""
+    if isinstance(part, ParquetSlice):
+        return part.file.read_row_group(part.row_group)
+    return part.offsets, part.idx
+
+
+def _select_rows(off: np.ndarray, idx: np.ndarray, sel: np.ndarray):
+    """The CSR rows where `sel` is true."""
+    off = np.asarray(off, np.int64)
+    counts = np.diff(off)
+    row_of = np.repeat(np.arange(len(counts)), counts)
+    new_off = np.zeros(int(sel.sum()) + 1, np.int64)
+    np.cumsum(counts[sel], out=new_off[1:])
+    return new_off, np.asarray(idx[off[0]:off[-1]], np.int32)[sel[row_of]]
 
 
 def main(args: Optional[Sequence[str]] = None):
@@ -487,8 +689,17 @@ def main(args: Optional[Sequence[str]] = None):
     data = driver.getData
     filtered = [driver.filterDataset(d) for d in data]
     callsRdd = driver.getCallsRdd(filtered)
-    simMatrix = driver.getSimilarityMatrix(callsRdd)
-    result = driver.computePca(simMatrix)
+    if conf.projectLoadings.isDefined:
+        if conf.saveLoadings.isDefined:
+            raise ValueError("--project-loadings computes no principal components to save; drop --save-loadings")
+        result = driver.projectLoadings(callsRdd)
+    else:
+        if conf.saveLoadings.isDefined:
+            driver.keyKind(callsRdd)                    # reject unsupported input before the Gram
+        simMatrix = driver.getSimilarityMatrix(callsRdd)
+        result = driver.computePca(simMatrix)
+        if conf.saveLoadings.isDefined:
+            driver.saveLoadings(callsRdd)
     driver.emitResult(result)
     driver.reportIoStats()
     driver.stop()

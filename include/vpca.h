@@ -230,8 +230,26 @@ int vpca_set_gram(vpca_ctx* ctx, const int32_t* gram);
  *   vecs : n_samples x k, column-major -- the layout of `pca.toArray` (:227); vecs[i + c*n] is PC c of
  *          sample i.  Each column is unit-norm and sign-normalised (largest-|.| entry positive).
  *   evals: k eigenvalues of the centered matrix, descending (may be NULL).
- *   non_zero_rows: `rowSums.filter(_ > 0).size` (:207), may be NULL. */
+ *   non_zero_rows: `rowSums.filter(_ > 0).size` (:207), may be NULL.
+ * Like MLlib's RowMatrix, limited to 65 535 samples, and needs the whole Gram in this context plus an N x N FP64
+ * workspace; for a Gram held as row bands, or for more samples, use vpca_compute_pca_bands below. */
 int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int32_t* non_zero_rows);
+/* Top-k principal coordinates of a Gram stored as row bands in `world` contexts of this process (beyond
+ * VariantsPca.scala:224-227: no replica of S and no N x N FP64 matrix, no 65 535-sample limit).
+ *   ctxs[q] holds rows [row0_q, row0_q + rows_q) (vpca_config.gram_band_row0 / _rows); the bands cover [0, N) in rank order
+ *   with no gap or overlap, all with the same n_samples; a context that stores the whole Gram is the band [0, N), so
+ *   world = 1 with an ordinary context is legal.  Every context must be finalized (VPCA_ERR_STATE otherwise); owner-flush
+ *   (VPCA_PEER_OWNER_ROWS + vpca_gram_gather) and owner-computes (no peers) bands are both accepted.  The bands are only
+ *   read.  1 <= world <= 16, 1 <= k <= min(N, max(num_pc of ctxs[0], 16)), else VPCA_ERR_BAD_ARG.
+ *   vecs / evals / non_zero_rows as for vpca_compute_pca.
+ * Lanczos with full reorthogonalisation driven from ctxs[0]; each step's product S v is sharded over the bands (every
+ * stored lower-triangle cell read once, for its row and for its transpose) and the partials are added in rank order, so
+ * repeated calls on the same bands give the same bits.  There is no direct-solver fallback (it would need the N x N
+ * matrix): breakdown (e.g. a zero Gram), no convergence within the step budget (VPCA_EIG_MAXIT) or an eigenvalue missed
+ * by a single Krylov sequence returns VPCA_ERR_UNSUPPORTED, with the reason in vpca_last_error(ctxs[0]).  ctxs[0]'s
+ * vpca_stats report the solve (eig_method 4).  Driver-side: no accumulation may be in flight in any of the contexts. */
+int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, double* vecs, double* evals,
+                           int32_t* non_zero_rows);
 /* The centered matrix itself (row-major N x N doubles) for parity tests of :199-223. */
 int vpca_get_centered(vpca_ctx* ctx, double* out);
 /* Tridiagonal form of the centered matrix after the last vpca_compute_pca (diag: n, offdiag: n-1). */
@@ -332,8 +350,9 @@ typedef struct vpca_stats {
     float last_eig_ms;            /* device time of the most recent centering + eigensolve                */
     int32_t gram_cta_group;       /* 1 or 2: CTAs per Gram tile                                           */
     int32_t gram_resident;        /* 1 when the last launch kept accumulators in registers for the whole K loop */
-    int32_t eig_method;           /* last vpca_compute_pca: 1 direct reduction, 2 Lanczos, 3 Lanczos abandoned -> direct */
-    int32_t eig_iterations;       /* Lanczos steps taken by the last vpca_compute_pca (0 for a direct solve)  */
+    int32_t eig_method;           /* last vpca_compute_pca: 1 direct reduction, 2 Lanczos, 3 Lanczos abandoned -> direct;
+                                     4 Lanczos on row bands (vpca_compute_pca_bands, reported by ctxs[0])    */
+    int32_t eig_iterations;       /* Lanczos steps taken by the last solve (0 for a direct solve)             */
 } vpca_stats;
 int vpca_get_stats(vpca_ctx* ctx, vpca_stats* out);
 /* Diagnostic (set VPCA_GRAM_PROF=1 before the first Gram launch): per-CTA timestamps of the last Gram launch,

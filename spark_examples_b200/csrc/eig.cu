@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 
 #include "vpca_internal.h"
 
@@ -1358,6 +1359,224 @@ __global__ void lz_lock_kernel(double* __restrict__ VT, int n, int cap, const do
     for (int c = 0; c < k; ++c) VT[(size_t)i * cap + c] = Z[(size_t)c * n + i];
 }
 
+// ------------------------------------------------- Lanczos on a Gram held as row bands (vpca_compute_pca_bands)
+// The five-kernel Lanczos above with its mat-vec sharded over the contexts that hold the bands.  Rank q stores rows
+// [row0, row0 + rows) of S, of which only the cells j <= i are meaningful (the upper part of a band-only allocation is not
+// the transpose and is never read).  Its partial product covers what those cells give:
+//   y_i += sum_{j <= i} S_ij v_j  (its rows)        y_j += S_ij v_i  for j < i  (the transpose, columns [0, row0 + rows))
+// Every stored cell is read once per step and feeds both FMAs.  The band's lower part is cut into kBandTR x kBandTC tiles;
+// a tile writes one row partial per row and one column partial per column into scratch, and band_reduce_kernel adds them
+// per output entry in tile order (row partials first, then column partials).  No floating-point atomics: fixed order.
+constexpr int kBandTR = 64;                   // rows per tile (two 32-row halves, each reduced by a warp transpose)
+constexpr int kBandThreads = 256;
+constexpr int kBandTC = 4 * kBandThreads;     // columns per tile: 4 adjacent cells (one int4) per thread
+
+// Row i of the band, cells [c, c + 4) clipped to j <= i; 0 for rows past the band and for cells above the diagonal.
+template <bool VEC>
+__device__ __forceinline__ int4 band_load(const int32_t* __restrict__ S, int n, int row0, int i, int iend, int c) {
+    int4 s = make_int4(0, 0, 0, 0);
+    if (i >= iend || c > i) return s;
+    const int32_t* p = S + (size_t)(i - row0) * n + c;
+    if (VEC && c + 3 <= i) return __ldg(reinterpret_cast<const int4*>(p));
+    s.x = __ldg(p);
+    if (c + 1 <= i) s.y = __ldg(p + 1);
+    if (c + 2 <= i) s.z = __ldg(p + 2);
+    if (c + 3 <= i) s.w = __ldg(p + 3);
+    return s;
+}
+
+// 32 values per lane in, lane l out with the sum over the warp of value l (fixed order: 31 exchanges, not 32 reductions).
+// Stage OFF: the lane with bit OFF set keeps the upper half of its live values, its partner the lower half.
+template <int OFF, typename T>
+__device__ __forceinline__ void warp_transpose_stage(T (&rp)[32], int lane) {
+    const bool up = (lane & OFF) != 0;
+#pragma unroll
+    for (int r = 0; r < OFF; ++r) {
+        const T send = up ? rp[r] : rp[r + OFF];
+        const T keep = up ? rp[r + OFF] : rp[r];
+        rp[r] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+    }
+}
+
+template <typename T>
+__device__ __forceinline__ T warp_transpose_sum(T (&rp)[32], int lane) {
+    warp_transpose_stage<16>(rp, lane);
+    warp_transpose_stage<8>(rp, lane);
+    warp_transpose_stage<4>(rp, lane);
+    warp_transpose_stage<2>(rp, lane);
+    warp_transpose_stage<1>(rp, lane);
+    return rp[0];
+}
+
+// grid (ceil((row0 + rows) / kBandTC), ceil(rows / kBandTR)).  T = double: the partials of S v.  T = long long: the same
+// traversal with v = 1 in exact integer arithmetic, i.e. the partial row sums of the symmetric S.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kBandThreads, 2) band_tile_kernel(const int32_t* __restrict__ S, int n, int row0, int rows,
+                                                                   const double* __restrict__ v, T* __restrict__ rowp,
+                                                                   T* __restrict__ colp) {
+    constexpr bool kDot = std::is_same<T, double>::value;
+    __shared__ double vrow[kBandTR];
+    __shared__ T rsum[kBandThreads / 32][kBandTR];
+    const int i0 = row0 + (int)blockIdx.y * kBandTR;
+    const int iend = min(row0 + rows, i0 + kBandTR);
+    const int c0 = (int)blockIdx.x * kBandTC;
+    if (c0 >= iend) return;                       // the tile lies above the diagonal: no stored cell
+    const int ncols = row0 + rows;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int c = c0 + (int)threadIdx.x * 4;
+    double vc[4] = {0.0, 0.0, 0.0, 0.0};
+    if constexpr (kDot) {
+        if (threadIdx.x < kBandTR) vrow[threadIdx.x] = i0 + (int)threadIdx.x < iend ? v[i0 + threadIdx.x] : 0.0;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) vc[e] = c + e < ncols ? v[c + e] : 0.0;
+        __syncthreads();
+    }
+    T cacc[4] = {0, 0, 0, 0};
+#pragma unroll 1
+    for (int h = 0; h < kBandTR / 32; ++h) {
+        T rp[32];
+#pragma unroll
+        for (int r0 = 0; r0 < 32; r0 += 8) {
+            int4 sv[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) sv[u] = band_load<VEC>(S, n, row0, i0 + h * 32 + r0 + u, iend, c);   // 8 loads in flight
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+                const int i = i0 + h * 32 + r0 + u;
+                const int32_t s[4] = {sv[u].x, sv[u].y, sv[u].z, sv[u].w};
+                // cells above the diagonal were loaded as 0; the diagonal cell (column i) feeds the row only
+                if constexpr (kDot) {
+                    const double vi = vrow[h * 32 + r0 + u];
+                    double d[4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) d[e] = lz_i2d(s[e]);
+                    rp[r0 + u] = (d[0] * vc[0] + d[1] * vc[1]) + (d[2] * vc[2] + d[3] * vc[3]);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) cacc[e] += (c + e < i ? d[e] : 0.0) * vi;
+                } else {
+                    rp[r0 + u] = ((long long)s[0] + s[1]) + ((long long)s[2] + s[3]);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) cacc[e] += c + e < i ? s[e] : 0;
+                }
+            }
+        }
+        const T mine = warp_transpose_sum(rp, lane);   // this warp's 128 columns of row i0 + 32 h + lane
+        rsum[wid][h * 32 + lane] = mine;
+    }
+    __syncthreads();
+    if (threadIdx.x < kBandTR) {
+        const int i = i0 + (int)threadIdx.x;
+        if (i < iend) {
+            T acc = 0;
+#pragma unroll
+            for (int w = 0; w < kBandThreads / 32; ++w) acc += rsum[w][threadIdx.x];
+            rowp[(size_t)blockIdx.x * rows + (i - row0)] = acc;
+        }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+        if (c + e < ncols) colp[(size_t)blockIdx.y * ncols + c + e] = cacc[e];
+}
+
+// y[t], t < row0 + rows: the row partials of row t (tiles 0 .. t / kBandTC, all launched and written), then the column
+// partials of column t from the row tiles that hold a row below t (the others contribute nothing and are skipped).
+template <typename T>
+__global__ void band_reduce_kernel(const T* __restrict__ rowp, const T* __restrict__ colp, int row0, int rows,
+                                   T* __restrict__ y) {
+    const int ncols = row0 + rows;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= ncols) return;
+    const int ntr = (rows + kBandTR - 1) / kBandTR;
+    T acc = 0;
+    if (t >= row0)
+        for (int tc = 0; tc <= t / kBandTC; ++tc) acc += rowp[(size_t)tc * rows + (t - row0)];
+    const int d = t - row0 + 1;
+    for (int tr = d > 0 ? d / kBandTR : 0; tr < ntr; ++tr) acc += colp[(size_t)tr * ncols + t];
+    y[t] = acc;
+}
+
+struct BandEnds {
+    int end[16];   // rank q's partial covers [0, end[q])
+};
+
+// rowSums (VariantsPca.scala:206) of the whole S from the ranks' exact partial sums, added in rank order; rbar = rowSums / N
+__global__ void band_rowsum_kernel(const long long* __restrict__ slots, int n, int world, BandEnds be,
+                                   double* __restrict__ rowsum, double* __restrict__ rbar) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    long long acc = 0;
+#pragma unroll
+    for (int q = 0; q < 16; ++q)
+        if (q < world && i < be.end[q]) acc += slots[(size_t)q * n + i];
+    const double r = (double)acc;   // integer-valued and < 2^53
+    rowsum[i] = r;
+    rbar[i] = __ddiv_rn(r, (double)n);
+}
+
+// Step j, part 1 (one block): beta_j = ||w_in|| from the partial sums lz_update_kernel left, sc = {1 / beta_j, sum(v_j),
+// rbar . v_j}.  Breakdown (zero or non-finite norm) sets the flag and every later kernel of the step returns.
+__global__ void __launch_bounds__(1024) band_norm_kernel(const double* __restrict__ part, int npart,
+                                                         const double* __restrict__ wbuf, const double* __restrict__ rbar,
+                                                         int n, double* __restrict__ beta, double* __restrict__ sc,
+                                                         int* __restrict__ st) {
+    __shared__ double red[33];
+    const int j = st[0];
+    if (st[1] != 0 || j >= st[3]) return;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    double s = 0.0;
+    for (int p = tid; p < npart; p += nt) s += part[p];
+    const double nrm = sqrt(block_sum(s, red));
+    if (!(nrm > 0.0) || !(nrm <= DBL_MAX)) {
+        if (tid == 0) st[1] = 2;
+        return;
+    }
+    const double* __restrict__ win = wbuf + (size_t)(j & 1) * n;
+    double s1 = 0.0, s2 = 0.0;
+    for (int i = tid; i < n; i += nt) {
+        const double x = win[i];
+        s1 += x;
+        s2 += rbar[i] * x;
+    }
+    s1 = block_sum(s1, red);
+    s2 = block_sum(s2, red);
+    if (tid == 0) {
+        const double inv = 1.0 / nrm;
+        beta[j] = nrm;
+        sc[0] = inv;
+        sc[1] = s1 * inv;
+        sc[2] = s2 * inv;
+    }
+}
+
+// Step j, part 2: v_j = w_in / beta_j -> V[:, j] and the vector the ranks multiply
+__global__ void band_scale_kernel(const double* __restrict__ wbuf, int n, const double* __restrict__ sc,
+                                  double* __restrict__ V, double* __restrict__ v, const int* __restrict__ st) {
+    const int j = st[0];
+    if (st[1] != 0 || j >= st[3]) return;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double x = wbuf[(size_t)(j & 1) * n + i] * sc[0];
+    V[(size_t)j * n + i] = x;
+    v[i] = x;
+}
+
+// Step j, part 3: S v_j = the ranks' partials added in rank order, then the centring applied to the vector as in
+// lz_persist_kernel: (C v)_i = (S v)_i - rbar_i sum(v) - rbar . v + mean sum(v)  -> w_out
+__global__ void band_combine_kernel(const double* __restrict__ slots, int n, int world, BandEnds be,
+                                    const double* __restrict__ rbar, const double* __restrict__ sc,
+                                    const double* __restrict__ scal, double* __restrict__ wbuf, const int* __restrict__ st) {
+    const int j = st[0];
+    if (st[1] != 0 || j >= st[3]) return;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    double y = 0.0;
+#pragma unroll
+    for (int q = 0; q < 16; ++q)
+        if (q < world && i < be.end[q]) y += slots[(size_t)q * n + i];
+    const double s1 = sc[1], s2 = sc[2], mm = scal[0];
+    wbuf[(size_t)((j + 1) & 1) * n + i] = y - rbar[i] * s1 - s2 + mm * s1;
+}
+
 }  // namespace
 
 cudaError_t eig_alloc(EigWork& w, int n, int kmax) {
@@ -1730,6 +1949,244 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
     backtransform_kernel<<<k, 512, 0, stream>>>(w.d_C, n, w.d_tau, w.d_evecs);
     nl += 3;
     if (launches) *launches += nl;
+    return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------- band Lanczos, host side
+void band_part_free(BandPart& p) {
+    cudaFree(p.d_v); cudaFree(p.d_y); cudaFree(p.d_scratch);
+    if (p.ev_done != nullptr) cudaEventDestroy(p.ev_done);
+    p = BandPart{};
+}
+
+void band_eig_free(BandEigWork& w) {
+    cudaFree(w.d_V); cudaFree(w.d_w); cudaFree(w.d_small); cudaFree(w.d_slots); cudaFree(w.d_rowsum); cudaFree(w.d_rbar);
+    cudaFree(w.d_scal); cudaFree(w.d_evals); cudaFree(w.d_evecs); cudaFree(w.d_lu); cudaFree(w.d_nz); cudaFree(w.d_st);
+    if (w.ev_v != nullptr) cudaEventDestroy(w.ev_v);
+    w = BandEigWork{};
+}
+
+namespace {
+
+constexpr size_t kBandSmallFixed = 5 * (size_t)kLzCap + 16 + 4 + 16 + 4;   // + kLzCap * kmax (Y) + npart
+
+// Buffers of one rank (on the current device, which is the rank's).  The scratch holds ceil((row0 + rows) / kBandTC) x rows
+// row partials and ceil(rows / kBandTR) x (row0 + rows) column partials.
+cudaError_t band_part_prepare(BandPart& p) {
+    if (p.alloc_n == p.n && p.alloc_row0 == p.row0 && p.alloc_rows == p.rows) return cudaSuccess;
+    cudaFree(p.d_v); cudaFree(p.d_y); cudaFree(p.d_scratch);
+    p.d_v = p.d_y = p.d_scratch = nullptr;
+    p.alloc_n = 0;
+    const size_t ncols = (size_t)p.row0 + p.rows;
+    const size_t ntc = (ncols + kBandTC - 1) / kBandTC, ntr = ((size_t)p.rows + kBandTR - 1) / kBandTR;
+    p.scratch_doubles = ntc * p.rows + ntr * ncols;
+    cudaError_t e;
+    if ((e = cudaMalloc(&p.d_v, (size_t)p.n * sizeof(double))) != cudaSuccess) return e;
+    if ((e = cudaMalloc(&p.d_y, ncols * sizeof(double))) != cudaSuccess) return e;
+    if ((e = cudaMalloc(&p.d_scratch, p.scratch_doubles * sizeof(double))) != cudaSuccess) return e;
+    if (p.ev_done == nullptr && (e = cudaEventCreateWithFlags(&p.ev_done, cudaEventDisableTiming)) != cudaSuccess) return e;
+    p.alloc_n = p.n;
+    p.alloc_row0 = p.row0;
+    p.alloc_rows = p.rows;
+    return cudaSuccess;
+}
+
+// The rank's partial of S v (T = double) or of the row sums (T = long long, v unused) into y[0, row0 + rows), on its stream.
+template <typename T>
+cudaError_t band_product(const BandPart& p, const double* v, T* y) {
+    const int ncols = p.row0 + p.rows;
+    const dim3 grid((unsigned)((ncols + kBandTC - 1) / kBandTC), (unsigned)((p.rows + kBandTR - 1) / kBandTR));
+    T* rowp = reinterpret_cast<T*>(p.d_scratch);
+    T* colp = rowp + (size_t)grid.x * p.rows;
+    const bool vec = (p.n & 3) == 0 && (reinterpret_cast<uintptr_t>(p.d_S) & 15) == 0;
+    if (vec) band_tile_kernel<T, true><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
+    else band_tile_kernel<T, false><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
+    band_reduce_kernel<T><<<(ncols + 255) / 256, 256, 0, p.stream>>>(rowp, colp, p.row0, p.rows, y);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int kmax, int k, int64_t* launches,
+                          int* outcome) {
+    *outcome = 4;
+    BandPart& p0 = *parts[0];
+    const int n = p0.n, dev0 = p0.device;
+    const int npart = (n + 31) / 32;
+    cudaStream_t s0 = p0.stream;
+    cudaError_t e;
+#define VPCA_TRY(x) if ((e = (x)) != cudaSuccess) return e
+    // ---- workspace: rank 0's solver state, every rank's share
+    VPCA_TRY(cudaSetDevice(dev0));
+    if (w.d_V == nullptr || w.n != n || w.kmax != kmax) {
+        band_eig_free(w);
+        w.n = n;
+        w.kmax = kmax;
+        VPCA_TRY(cudaMalloc(&w.d_V, (size_t)n * kLzCap * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_w, 2 * (size_t)n * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_small, (kBandSmallFixed + (size_t)kLzCap * kmax + npart) * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_slots, 16 * (size_t)n * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_rowsum, (size_t)n * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_rbar, (size_t)n * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_scal, 16 * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_evals, (size_t)kmax * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_evecs, (size_t)n * kmax * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_lu, 8 * (size_t)kLzCap * sizeof(double)));
+        VPCA_TRY(cudaMalloc(&w.d_nz, sizeof(int)));
+        VPCA_TRY(cudaMalloc(&w.d_st, 8 * sizeof(int)));
+        VPCA_TRY(cudaEventCreateWithFlags(&w.ev_v, cudaEventDisableTiming));
+        VPCA_TRY(cudaMemset(w.d_small, 0, (kBandSmallFixed + (size_t)kLzCap * kmax + npart) * sizeof(double)));
+    }
+    for (int q = 0; q < world; ++q) {
+        VPCA_TRY(cudaSetDevice(parts[q]->device));
+        VPCA_TRY(band_part_prepare(*parts[q]));
+    }
+    VPCA_TRY(cudaSetDevice(dev0));
+    VPCA_TRY(cudaFuncSetAttribute(invit_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    double* alpha = w.d_small;
+    double* beta = alpha + kLzCap;
+    double* h1 = beta + kLzCap;
+    double* h2 = h1 + kLzCap;
+    double* e2 = h2 + kLzCap;
+    double* Y = e2 + kLzCap;
+    double* theta2 = Y + (size_t)kLzCap * kmax;
+    double* res = theta2 + 16;
+    double* scal2 = res + 4;
+    double* sc = scal2 + 16;
+    double* part = sc + 4;
+    BandEnds be{};
+    for (int q = 0; q < 16; ++q) be.end[q] = q < world ? parts[q]->row0 + parts[q]->rows : 0;
+    int64_t nl = 0;
+
+    // Every rank's partial of one traversal lands in rank 0's slot q; rank 0's stream waits for all of them.
+    auto gather = [&](auto* slot_type, const double* v) -> cudaError_t {
+        using T = std::remove_pointer_t<decltype(slot_type)>;
+        cudaError_t ce;
+        for (int q = 1; q < world; ++q) {
+            BandPart& p = *parts[q];
+            if ((ce = cudaSetDevice(p.device)) != cudaSuccess) return ce;
+            if ((ce = cudaStreamWaitEvent(p.stream, w.ev_v, 0)) != cudaSuccess) return ce;   // rank 0 is done with slot q
+            if (v != nullptr &&
+                (ce = cudaMemcpyPeerAsync(p.d_v, p.device, v, dev0, (size_t)n * sizeof(double), p.stream)) != cudaSuccess)
+                return ce;
+            if ((ce = band_product<T>(p, p.d_v, reinterpret_cast<T*>(p.d_y))) != cudaSuccess) return ce;
+            if ((ce = cudaMemcpyPeerAsync(w.d_slots + (size_t)q * n, dev0, p.d_y, p.device,
+                                          (size_t)(p.row0 + p.rows) * sizeof(double), p.stream)) != cudaSuccess) return ce;
+            if ((ce = cudaEventRecord(p.ev_done, p.stream)) != cudaSuccess) return ce;
+            nl += 2;
+        }
+        if ((ce = cudaSetDevice(dev0)) != cudaSuccess) return ce;
+        if ((ce = band_product<T>(p0, v, reinterpret_cast<T*>(w.d_slots))) != cudaSuccess) return ce;
+        for (int q = 1; q < world; ++q)
+            if ((ce = cudaStreamWaitEvent(s0, parts[q]->ev_done, 0)) != cudaSuccess) return ce;
+        nl += 2;
+        return cudaSuccess;
+    };
+    // One Lanczos step: normalise on rank 0, v_j to every rank, the sharded product, the partials back in rank order,
+    // centring, then both Gram-Schmidt passes with the five-kernel form's kernels.  No host synchronisation.
+    auto step = [&]() -> cudaError_t {
+        cudaError_t ce;
+        band_norm_kernel<<<1, 1024, 0, s0>>>(part, npart, w.d_w, w.d_rbar, n, beta, sc, w.d_st);
+        band_scale_kernel<<<(n + 255) / 256, 256, 0, s0>>>(w.d_w, n, sc, w.d_V, p0.d_v, w.d_st);
+        if (world > 1 && (ce = cudaEventRecord(w.ev_v, s0)) != cudaSuccess) return ce;
+        if ((ce = gather((double*)nullptr, p0.d_v)) != cudaSuccess) return ce;
+        band_combine_kernel<<<(n + 255) / 256, 256, 0, s0>>>(w.d_slots, n, world, be, w.d_rbar, sc, w.d_scal, w.d_w, w.d_st);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h1, w.d_st);
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h1, alpha, part, w.d_st, 1);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h2, w.d_st);
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h2, alpha, part, w.d_st, 2);
+        nl += 7;
+        return cudaGetLastError();
+    };
+
+    // ---- row sums (exact, int64), matrixMean and non_zero_rows (VariantsPca.scala:206-211)
+    if (world > 1) VPCA_TRY(cudaEventRecord(w.ev_v, s0));   // the ranks write rank 0's slots after its earlier work
+    VPCA_TRY(gather((long long*)nullptr, nullptr));
+    band_rowsum_kernel<<<(n + 255) / 256, 256, 0, s0>>>(reinterpret_cast<const long long*>(w.d_slots), n, world, be,
+                                                         w.d_rowsum, w.d_rbar);
+    matrix_mean_kernel<<<1, 1024, 0, s0>>>(w.d_rowsum, n, w.d_scal, w.d_nz);
+    nl += 2;
+
+    // ---- main run: the convergence test and its step budget are those of lanczos_topk's five-kernel form
+    const double tol = 1e-12;
+    int max_iter = kLzMaxIter;
+    if (const char* mi = getenv("VPCA_EIG_MAXIT")) max_iter = std::max(kLzChunk, std::min(kLzMaxIter, atoi(mi)));
+    int hst[8] = {0, 0, 0, max_iter, 0, 0, 0, 0};
+    double hres[2] = {0.0, 0.0};
+    VPCA_TRY(cudaMemcpyAsync(w.d_st, hst, sizeof(hst), cudaMemcpyHostToDevice, s0));
+    lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w, n, 0x5eedULL, part);
+    nl += 1;
+    int m = 0, m_prev = 0;
+    bool converged = false;
+    double rho_prev = 0.0;
+    const int max_chunks = std::min(max_iter, n - 1) / kLzChunk;
+    *outcome = 4;
+    for (int chunk = 1; chunk <= max_chunks; ++chunk) {
+        for (int g = 0; g < kLzChunk; ++g) VPCA_TRY(step());
+        m = chunk * kLzChunk;
+        if (chunk > 4 && (chunk & 1) && chunk != max_chunks) continue;
+        bisect_kernel<<<k, 256, 0, s0>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
+        invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), s0>>>(alpha, beta + 1, m, k, w.d_evals,
+                                                                                           w.d_scal, w.d_lu, Y);
+        lz_check_kernel<<<1, 32, 0, s0>>>(part, npart, Y, m, k, w.d_scal, w.d_st, res, tol);
+        nl += 3;
+        VPCA_TRY(cudaMemcpyAsync(hst, w.d_st, sizeof(hst), cudaMemcpyDeviceToHost, s0));
+        VPCA_TRY(cudaMemcpyAsync(hres, res, sizeof(hres), cudaMemcpyDeviceToHost, s0));
+        VPCA_TRY(cudaStreamSynchronize(s0));
+        if (hst[1] == 1) {
+            converged = true;
+            break;
+        }
+        if (hst[1] != 0) {
+            *outcome = 2;
+            break;
+        }
+        const double rho = hres[0];
+        if (m >= 96 && rho > 1e-3) break;   // no separated top of the spectrum: hopeless within kLzMaxIter
+        if (m_prev >= 32 && rho < rho_prev) {
+            const double rate = std::log(rho_prev / rho) / (m - m_prev);
+            if (m + 1.5 * std::log(rho / tol) / rate > max_iter + 2 * kLzChunk) break;
+        }
+        rho_prev = rho;
+        m_prev = m;
+    }
+    w.last_iters = m;
+    if (launches) *launches += nl;
+    nl = 0;
+    if (!converged) return cudaGetLastError();
+
+    // ---- Ritz vectors, unit norm, sign rule
+    lz_ritz_kernel<<<dim3(npart, k), 256, 0, s0>>>(w.d_V, n, Y, m, w.d_evecs);
+    lz_finish_kernel<<<k, 512, 0, s0>>>(w.d_evecs, n);
+    nl += 2;
+    // ---- deflated verification run (as in the five-kernel form): the k Ritz vectors become the first k basis columns, a
+    // fresh start vector is made orthogonal to them and one chunk runs; a Ritz value above theta_k means a missed eigenvalue
+    if (k + kLzChunk < n) {
+        VPCA_TRY(cudaMemcpyAsync(w.d_V, w.d_evecs, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice, s0));
+        int vst[4] = {k - 1, 0, 0, k + kLzChunk};
+        VPCA_TRY(cudaMemcpyAsync(w.d_st, vst, sizeof(vst), cudaMemcpyHostToDevice, s0));
+        lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w + (size_t)(k & 1) * n, n, 0xfaceULL, part);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h1, w.d_st);
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h1, alpha, part, w.d_st, 1);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h2, w.d_st);
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h2, alpha, part, w.d_st, 2);
+        nl += 5;
+        for (int g = 0; g < kLzChunk; ++g) VPCA_TRY(step());
+        bisect_kernel<<<1, 256, 0, s0>>>(alpha + k, beta + k + 1, kLzChunk, e2, theta2, scal2);
+        lz_verify_kernel<<<1, 1, 0, s0>>>(w.d_evals, k, theta2, w.d_scal, w.d_st);
+        nl += 2;
+        VPCA_TRY(cudaMemcpyAsync(hst, w.d_st, sizeof(hst), cudaMemcpyDeviceToHost, s0));
+        VPCA_TRY(cudaStreamSynchronize(s0));
+        if (launches) *launches += nl;
+        if (hst[1] != 1) {
+            *outcome = hst[1] == 3 ? 3 : 2;
+            return cudaGetLastError();
+        }
+    } else if (launches) {
+        *launches += nl;
+    }
+#undef VPCA_TRY
+    *outcome = 0;
     return cudaGetLastError();
 }
 

@@ -49,6 +49,8 @@ struct vpca_ctx {
     GramPlan plan;        // schedule state of the launches on `stream` (device-resident input)
     EigWork eig;
     bool eig_ready = false;
+    BandEigWork band_eig;   // vpca_compute_pca_bands with this context as rank 0: the solver's state
+    BandPart band_part;     // vpca_compute_pca_bands: this context's share of the sharded mat-vec
     JoinWork join;        // multi-dataset keying (join.cu); one join at a time (join_mu)
     std::mutex join_mu;
     int pca_k = 0;        // k of the last vpca_compute_pca whose U / eigenvalues are still valid on the device (0: none)
@@ -637,6 +639,8 @@ int vpca_destroy(vpca_ctx* ctx) {
             if (d != ctx->plan.peer_rank && ctx->plan.peer_S[d] != nullptr) cudaIpcCloseMemHandle(ctx->plan.peer_base[d]);
     if (ctx->own_S) cudaFree(ctx->d_S);
     if (ctx->eig_ready) eig_free(ctx->eig);
+    band_eig_free(ctx->band_eig);
+    band_part_free(ctx->band_part);
     for (void* p : {(void*)ctx->d_proj_acc, (void*)ctx->d_proj_part, (void*)ctx->d_lp_w, (void*)ctx->d_lp_mean,
                     (void*)ctx->d_lp_count})
         cudaFree(p);
@@ -1286,6 +1290,86 @@ int vpca_get_tridiagonal(vpca_ctx* ctx, double* diag, double* offdiag) {
     CUDA_OK(ctx, cudaMemcpyAsync(diag, ctx->eig.d_diag, (size_t)ctx->n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaMemcpyAsync(offdiag, ctx->eig.d_off, (size_t)(ctx->n - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return VPCA_OK;
+}
+
+// Top-k of a Gram stored as row bands in `world` contexts (eig.cu, band_eig_topk): Lanczos driven from rank 0 with the
+// mat-vec sharded over the bands.  Neither S nor the FP64 centred matrix is ever assembled, so neither the 65 535-sample
+// limit of vpca_compute_pca nor its N x N workspace applies.  The direct reduction that backs the one-GPU Lanczos needs
+// C, so there is no fallback here: every Lanczos failure is reported as VPCA_ERR_UNSUPPORTED.
+int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, double* vecs, double* evals,
+                           int32_t* non_zero_rows) {
+    if (ctxs == nullptr || world < 1 || world > 16)
+        return fail(nullptr, VPCA_ERR_BAD_ARG, "vpca_compute_pca_bands: world must be in [1, 16]");
+    for (int r = 0; r < world; ++r)
+        if (ctxs[r] == nullptr) return fail(ctxs[0], VPCA_ERR_BAD_ARG, "vpca_compute_pca_bands: ctxs[%d] is NULL", r);
+    vpca_ctx* c0 = ctxs[0];
+    const int n = c0->n;
+    const int kmax = std::max(c0->num_pc, 16);
+    if (vecs == nullptr || k < 1 || k > n || k > kmax)
+        return fail(c0, VPCA_ERR_BAD_ARG, "vpca_compute_pca_bands: k=%d out of range [1, %d]", k, std::min(n, kmax));
+    // n, band_row0 and band_rows are fixed at vpca_create: the bands can be checked before any lock is taken
+    int next = 0;
+    for (int r = 0; r < world; ++r) {
+        const vpca_ctx* c = ctxs[r];
+        if (c->n != n) return fail(c0, VPCA_ERR_BAD_ARG, "ctxs[%d] has %d samples, ctxs[0] %d", r, c->n, n);
+        for (int q = 0; q < r; ++q)
+            if (ctxs[q] == c) return fail(c0, VPCA_ERR_BAD_ARG, "ctxs[%d] and ctxs[%d] are the same context", q, r);
+        if (c->band_row0 != next)
+            return fail(c0, VPCA_ERR_BAD_ARG, "the bands must cover [0, %d) in rank order: ctxs[%d] stores rows [%d, %d), "
+                        "expected a band starting at row %d", n, r, c->band_row0, c->band_row0 + c->band_rows, next);
+        next = c->band_row0 + c->band_rows;
+    }
+    if (next != n) return fail(c0, VPCA_ERR_BAD_ARG, "the bands end at row %d, not at %d", next, n);
+    std::vector<std::unique_lock<std::mutex>> locks;   // rank order
+    locks.reserve(world);
+    for (int r = 0; r < world; ++r) locks.emplace_back(ctxs[r]->mu);
+    BandPart* parts[16];
+    for (int r = 0; r < world; ++r) {
+        vpca_ctx* c = ctxs[r];
+        if (!c->finalized) return fail(c0, VPCA_ERR_STATE, "ctxs[%d]: call vpca_finalize_gram first", r);
+        for (auto& L : c->lanes)
+            if (L.busy) return fail(c0, VPCA_ERR_STATE, "ctxs[%d]: an accumulate call is in flight", r);
+        BandPart& p = c->band_part;
+        p.device = c->cfg.device;
+        p.stream = c->stream;
+        p.d_S = c->d_S;
+        p.n = n;
+        p.row0 = c->band_row0;
+        p.rows = c->band_rows;
+        parts[r] = &p;
+    }
+    CUDA_OK(c0, cudaSetDevice(c0->cfg.device));
+    CUDA_OK(c0, cudaEventRecord(c0->ev_e0, c0->stream));
+    int64_t launches = 0;
+    int outcome = 0;
+    const cudaError_t e = band_eig_topk(c0->band_eig, parts, world, kmax, k, &launches, &outcome);
+    cudaSetDevice(c0->cfg.device);
+    c0->c_launches += launches;
+    if (e != cudaSuccess)
+        return fail(c0, e == cudaErrorMemoryAllocation ? VPCA_ERR_NOMEM : VPCA_ERR_CUDA, "band eigensolver: %s",
+                    cudaGetErrorString(e));
+    CUDA_OK(c0, cudaEventRecord(c0->ev_e1, c0->stream));
+    c0->st.eig_method = 4;
+    c0->st.eig_iterations = c0->band_eig.last_iters;
+    c0->eig_timed = true;
+    if (outcome != 0) {
+        CUDA_OK(c0, cudaStreamSynchronize(c0->stream));
+        const char* why = outcome == 2 ? "Lanczos broke down (a zero Gram, or a Krylov space exhausted before convergence)"
+                        : outcome == 3 ? "the deflated verification run found an eigenvalue above the computed ones (a "
+                                         "multiple top eigenvalue)"
+                                       : "Lanczos did not converge within the step budget (kLzMaxIter, VPCA_EIG_MAXIT)";
+        return fail(c0, VPCA_ERR_UNSUPPORTED, "vpca_compute_pca_bands after %d steps: %s; the bands have no direct-solver "
+                    "fallback", c0->band_eig.last_iters, why);
+    }
+    const size_t nb = (size_t)n * k * sizeof(double);
+    CUDA_OK(c0, cudaMemcpyAsync(vecs, c0->band_eig.d_evecs, nb, cudaMemcpyDeviceToHost, c0->stream));
+    if (evals) CUDA_OK(c0, cudaMemcpyAsync(evals, c0->band_eig.d_evals, k * sizeof(double), cudaMemcpyDeviceToHost, c0->stream));
+    int nz = 0;
+    CUDA_OK(c0, cudaMemcpyAsync(&nz, c0->band_eig.d_nz, sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
+    CUDA_OK(c0, cudaStreamSynchronize(c0->stream));
+    if (non_zero_rows) *non_zero_rows = nz;
+    c0->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
     return VPCA_OK;
 }
 

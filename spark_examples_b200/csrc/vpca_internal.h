@@ -176,6 +176,49 @@ cudaError_t center_gram(EigWork& w, const int32_t* d_S, cudaStream_t stream, boo
 cudaError_t center_matrix(EigWork& w, cudaStream_t stream);
 cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches);
 
+// ---- top-k of a Gram held as row bands across contexts (eig.cu, vpca_compute_pca_bands) ------------------------------
+// One rank's share: its band of S (rows [row0, row0 + rows), lower-triangle cells meaningful) and the buffers of its part
+// of the sharded mat-vec, all on the rank's device.  Owned by the rank's context, kept between solves.
+struct BandPart {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    const int32_t* d_S = nullptr;   // row row0 of the band
+    int n = 0, row0 = 0, rows = 0;
+    double* d_v = nullptr;          // n: the Lanczos vector of the step
+    double* d_y = nullptr;          // row0 + rows: the partial product (or partial row sums as int64)
+    double* d_scratch = nullptr;    // tile row partials, then tile column partials
+    size_t scratch_doubles = 0;
+    int alloc_n = 0, alloc_row0 = -1, alloc_rows = 0;
+    cudaEvent_t ev_done = nullptr;  // the partial has landed on rank 0
+};
+void band_part_free(BandPart& p);
+
+// Solver state on rank 0: the Lanczos basis (n x kLzCap), w ping-pong, the small Lanczos scalars, `world` slots of n
+// doubles for the partials, row sums; no n x n matrix.
+struct BandEigWork {
+    int n = 0, kmax = 0;
+    double* d_V = nullptr;
+    double* d_w = nullptr;       // 2 n
+    double* d_small = nullptr;   // alpha | beta | h1 | h2 | e2 | Y | theta2 | res | scal2 | sc | part
+    double* d_slots = nullptr;   // 16 n
+    double* d_rowsum = nullptr;  // n
+    double* d_rbar = nullptr;    // n
+    double* d_scal = nullptr;    // 16: [0] matrixMean, [2] ||T||
+    double* d_evals = nullptr;   // kmax
+    double* d_evecs = nullptr;   // n x kmax, column-major
+    double* d_lu = nullptr;      // 8 kLzCap: inverse-iteration scratch
+    int* d_nz = nullptr;
+    int* d_st = nullptr;         // {step, flag, ticket, step cap}
+    cudaEvent_t ev_v = nullptr;  // v_j is ready on rank 0
+    int last_iters = 0;
+};
+void band_eig_free(BandEigWork& w);
+// outcome: 0 converged (d_evals / d_evecs / d_nz hold the answer), 2 breakdown, 3 a missed eigenvalue found by the
+// deflated verification run, 4 no convergence within the step budget.  Synchronises rank 0's stream at every convergence
+// test; the bands are only read.
+cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int kmax, int k, int64_t* launches,
+                          int* outcome);
+
 // ---- variant loadings and projection (project.cu) -----------------------------------------------------------------
 // Both read cells in the panel layout (see gram_accumulate; zero cells after nv in the last panel), k in [1, 16].
 // w[v * k + c] = sum_s x[s][v] U[s][c] (FP64, samples summed in order), count[v] = sum_s x[s][v] (exact) for v < nv;

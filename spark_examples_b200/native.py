@@ -51,7 +51,7 @@ EXPORTED_SYMBOLS = (
     "vpca_pool_commit", "vpca_pool_abort", "vpca_pool_reduce_and_finalize", "vpca_pool_get_gram", "vpca_pool_compute_pca",
     "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan",
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
-    "vpca_project_bed", "vpca_project_panels", "vpca_project_get",
+    "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
 )
 
 
@@ -226,6 +226,8 @@ def load_library() -> ctypes.CDLL:
     L.vpca_set_gram.argtypes = [vp, vp]
     L.vpca_compute_pca.restype = ctypes.c_int
     L.vpca_compute_pca.argtypes = [vp, i32, vp, vp, ctypes.POINTER(i32)]
+    L.vpca_compute_pca_bands.restype = ctypes.c_int
+    L.vpca_compute_pca_bands.argtypes = [ctypes.POINTER(vp), i32, i32, vp, vp, ctypes.POINTER(i32)]
     L.vpca_get_centered.restype = ctypes.c_int
     L.vpca_get_centered.argtypes = [vp, vp]
     L.vpca_get_tridiagonal.restype = ctypes.c_int
@@ -730,6 +732,25 @@ def ownerRowBands(n_samples: int, world: int) -> list:
         out.append((prev, int(ends[q]) - prev))
         prev = int(ends[q])
     return out
+
+
+def computePcaBands(contexts, k: int = 2):
+    """Top-k principal coordinates of a Gram held as row bands by `contexts` (rank order, bands covering [0, N); a context
+    that stores the whole Gram is the band [0, N)) -> (vecs (N, k), evals (k,), nonZeroRows), like NativePca.computePca
+    but with no 65 535-sample limit and no N x N workspace (vpca_compute_pca_bands).  Failures of the solver raise
+    VpcaError with code VPCA_ERR_UNSUPPORTED; there is no fallback."""
+    L = load_library()
+    if not contexts:
+        raise VpcaError(VPCA_ERR_BAD_ARG, "at least one context")
+    n = contexts[0].n
+    arr = (ctypes.c_void_p * len(contexts))(*[c._h.value if c._h is not None else None for c in contexts])
+    flat = np.empty(n * max(int(k), 1), dtype=np.float64)
+    evals = np.empty(max(int(k), 1), dtype=np.float64)
+    nz = ctypes.c_int32(0)
+    rc = L.vpca_compute_pca_bands(arr, len(contexts), int(k), _host_ptr(flat), _host_ptr(evals), ctypes.byref(nz))
+    if rc != VPCA_OK:
+        contexts[0]._raise(rc, contexts[0]._h)
+    return flat[: n * k].reshape(k, n).T.copy(), evals[:k].copy(), int(nz.value)
 
 
 def setPeersLocal(contexts, mode: str = "owner_rows"):

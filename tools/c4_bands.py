@@ -13,7 +13,14 @@ Times the Gram launches with CUDA events per device (max over devices = the job)
   * diag(S) = carrier counts of the whole cohort, per band;
   * whole sampled rows of every band (its first, its last and random ones: the lower-triangle part, columns 0..row) and
     random 256 x 256 blocks against an exact fp32 matmul of the same shards (0/1 cells, counts < 2^24, TF32 off).
-vpca_compute_pca is not called: like MLlib's RowMatrix it is limited to 65 535 samples (VariantsPca.scala:226)."""
+`--pca K` then computes the top K principal coordinates straight from the bands (vpca_compute_pca_bands: Lanczos with the
+mat-vec sharded over the band contexts; no replica of S, no N x N FP64 matrix, no 65 535-sample limit) and reports
+`pca_ms` (host clock around the call, which synchronises), `lanczos_steps`, and checks computed from the genotype shards,
+not from S: the residual ||J X X^T J u_c - lambda_c u_c|| / lambda_1 of every pair in FP64 (panel by panel), and the
+orthonormality of U.
+
+`--gpus N` sets the number of band contexts (ranks); with fewer visible devices they share them round robin (8 band
+contexts on one H100 hold the 40 GB Gram of config 4, but not its 50 GB of genotypes as well: lower --variants there)."""
 import argparse
 import json
 import sys
@@ -30,7 +37,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--samples", type=int, default=100_000)
     ap.add_argument("--variants", type=int, default=500_000, help="whole cohort; split evenly over the GPUs")
-    ap.add_argument("--gpus", type=int, default=0, help="0 = all visible")
+    ap.add_argument("--gpus", type=int, default=0, help="band contexts (ranks); 0 = one per visible device; more than the "
+                    "visible devices share them round robin")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--panel", type=int, default=8192)
     ap.add_argument("--check-rows", type=int, default=3, help="sampled whole rows per band checked against fp32 matmul")
@@ -38,29 +46,35 @@ def main():
                     help="owner-flush: every GPU holds a variant shard and its kernel adds each tile into the band of the row's "
                          "owner over NVLink; owner-computes: every GPU holds ALL variants and computes only its own band (no "
                          "traffic between GPUs at all; 50 GB of genotypes per GPU)")
+    ap.add_argument("--pca", type=int, default=0, help="K > 0: also compute the top K principal coordinates from the bands "
+                    "(vpca_compute_pca_bands) and check them against the genotype shards")
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     world = args.gpus or torch.cuda.device_count()
+    ndev = torch.cuda.device_count()
+    devs = [r % ndev for r in range(world)]
     n, P = args.samples, args.panel
     computes = args.mode == "owner-computes"
     per = args.variants if computes else (args.variants + world - 1) // world
     bands = native.ownerRowBands(n, world)
     ctxs, bufs, streams = [], [], []
     total_v = per if computes else per * world
-    report = {"config": f"{n} samples x {total_v} variants over {world} GPU(s), one process, band-only Grams, {args.mode}",
+    report = {"config": f"{n} samples x {total_v} variants, {world} band context(s) on {len(set(devs))} GPU(s), one process, "
+                        f"band-only Grams, {args.mode}",
               "n": n, "variants_per_gpu": per, "world": world, "panel": P,
               "band_rows": [b[1] for b in bands], "band_gb": [round(b[1] * n * 4 / 2 ** 30, 2) for b in bands]}
     try:
         for r in range(world):
-            torch.cuda.set_device(r)
-            s = torch.cuda.Stream(device=r)
+            torch.cuda.set_device(devs[r])
+            s = torch.cuda.Stream(device=devs[r])
             streams.append(s)
-            ctxs.append(native.NativePca(n, device=r, stream=s.cuda_stream, max_multiplicity=1, gram_band=bands[r]))
+            ctxs.append(native.NativePca(n, device=devs[r], stream=s.cuda_stream, max_multiplicity=1, num_pc=max(2, args.pca),
+                                         gram_band=bands[r]))
         if not computes:
             native.setPeersLocal(ctxs, "owner_rows")
         for r, c in enumerate(ctxs):
-            torch.cuda.set_device(r)
-            buf = torch.zeros(c.panelBytes(per, P), dtype=torch.uint8, device=f"cuda:{r}")
+            torch.cuda.set_device(devs[r])
+            buf = torch.zeros(c.panelBytes(per, P), dtype=torch.uint8, device=f"cuda:{devs[r]}")
             bufs.append(buf)
             c.synthPanelsDevice(20240901, 0 if computes else r * per, per, 0, buf.data_ptr(), P)
         for c in ctxs:
@@ -73,7 +87,7 @@ def main():
                 c.synchronize()       # every band is zero before any rank adds into it
             ev = []
             for r, c in enumerate(ctxs):
-                torch.cuda.set_device(r)
+                torch.cuda.set_device(devs[r])
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 with torch.cuda.stream(streams[r]):
                     a.record()
@@ -116,7 +130,7 @@ def main():
             sel = x[:, rows, :]                                            # slice or index list
             return sel.permute(1, 0, 2).reshape(sel.shape[1], npan * P).to(torch.float32)
 
-        shard_devs = [0] if computes else list(range(world))     # owner-computes: every device holds the whole cohort
+        shard_devs = [0] if computes else list(range(world))     # owner-computes: every rank holds the whole cohort
         carriers = torch.zeros(n, dtype=torch.int64)
         for r in shard_devs:
             x = bufs[r].view(torch.int8)[: npan * n * P].view(npan, n, P)
@@ -132,7 +146,7 @@ def main():
                 ok_diag = ok_diag and int(got[row][row]) == int(carriers[row])
             want = {row: torch.zeros(row + 1, dtype=torch.float64) for row in pick}
             for r in shard_devs:
-                torch.cuda.set_device(r)
+                torch.cuda.set_device(devs[r])
                 xr = shard_rows(r, pick)                                   # (len(pick), K)
                 for r0 in range(0, max(pick) + 1, 8192):             # columns beyond the last sampled row are never needed
                     r1 = min(n, r0 + 8192)
@@ -149,11 +163,13 @@ def main():
             gb = c.gramBand(br, min(256, row0 + rows - br))[:, bc:bc + 256].astype(np.int64)
             wb = torch.zeros(gb.shape, dtype=torch.float64)
             for r in shard_devs:
-                torch.cuda.set_device(r)
+                torch.cuda.set_device(devs[r])
                 wb += (shard_rows(r, slice(br, br + gb.shape[0])) @ shard_rows(r, slice(bc, bc + gb.shape[1])).t()).to(torch.float64).cpu()
             ok_blocks = ok_blocks and bool(np.array_equal(gb, wb.numpy().astype(np.int64)))
         report["checks"] = {"diag_equals_carrier_counts": ok_diag, "sampled_rows_exact_vs_fp32_matmul": ok_rows,
                             "random_256_blocks_exact": ok_blocks, "rows_checked_per_band": args.check_rows + 2}
+        if args.pca > 0:
+            report.update(principal_coordinates(args.pca, ctxs, bufs, devs, shard_devs, n, per, P))
     finally:
         for c in ctxs:
             try:
@@ -166,6 +182,46 @@ def main():
     print(line, flush=True)
     if args.out:
         Path(args.out).write_text(line + "\n")
+
+
+def principal_coordinates(k, ctxs, bufs, devs, shard_devs, n, per, P):
+    """Top-k PCs from the bands, timed on the host around the (synchronising) call, and checked against the genotypes:
+    with JX the column-centred cells, (J X X^T J) U = JX ((JX)^T U) is accumulated in FP64, 1024 variants at a time."""
+    import time
+    for c in ctxs:
+        c.finalizeGram()              # a band stays a band of the lower triangle: nothing is mirrored
+    torch.cuda.set_device(devs[0])
+    t0 = time.perf_counter()
+    vecs, evals, nz = native.computePcaBands(ctxs, k)
+    pca_ms = (time.perf_counter() - t0) * 1e3
+    st = ctxs[0].stats()
+    out = {"pca_k": k, "pca_ms": round(pca_ms, 1), "pca_device_ms": round(st["last_eig_ms"], 1),
+           "lanczos_steps": st["eig_iterations"], "eigenvalues": [float(x) for x in evals], "non_zero_rows": nz}
+    npan = (per + P - 1) // P
+    CU = torch.zeros((n, k), dtype=torch.float64, device=f"cuda:{devs[0]}")
+    for r in shard_devs:
+        dev = f"cuda:{devs[r]}"
+        torch.cuda.set_device(devs[r])
+        U = torch.from_numpy(vecs).to(dev)
+        acc = torch.zeros((n, k), dtype=torch.float64, device=dev)
+        x = bufs[r].view(torch.int8)[: npan * n * P].view(npan, n, P)
+        for p_ in range(npan):
+            width = min(P, per - p_ * P)                              # cells of this panel that hold variants
+            for b0 in range(0, width, 1024):
+                b1 = min(b0 + 1024, width)
+                xb = x[p_, :, b0:b1].to(torch.float64)
+                xb -= xb.mean(dim=0, keepdim=True)                    # J X: every variant column centred over the samples
+                acc += xb @ (xb.t() @ U)
+        CU += acc.to(CU.device)
+    torch.cuda.set_device(devs[0])
+    U = torch.from_numpy(vecs).to(CU.device)
+    lam = torch.from_numpy(evals).to(CU.device)
+    res = (torch.linalg.vector_norm(CU - U * lam[None, :], dim=0) / lam[0]).cpu().numpy()
+    orth = float((U.t() @ U - torch.eye(k, dtype=torch.float64, device=CU.device)).abs().max())
+    out["pca_checks"] = {"residual_over_lambda1": [float(x) for x in res], "residuals_below_1e-9": bool(np.all(res <= 1e-9)),
+                         "max_abs_UtU_minus_I": orth, "orthonormal_to_1e-10": orth <= 1e-10,
+                         "descending_eigenvalues": bool(np.all(np.diff(evals) <= 0))}
+    return out
 
 
 main()

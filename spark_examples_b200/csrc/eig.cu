@@ -8,7 +8,8 @@
 //             are the eigenvectors of C for its k largest eigenvalues; we compute them from C directly:
 //   N >= 512 (default): Lanczos with full reorthogonalisation for the top k pairs only -- as ONE persistent cooperative
 //               kernel per 16-step chunk that reads the int32 Gram S itself and applies the centring to the vector
-//               (lz_persist_kernel below); the five-kernel CUDA-graph form of round 1 remains for N > 16384;
+//               (lz_persist_kernel below) while its shared-memory working set fits one block (N <= 10 752 on 132 SMs);
+//               past that the five-kernel CUDA-graph form on the FP64 matrix C;
 //   small N, VPCA_EIG=direct, and the fallback of the Krylov solver:
 //               1. Householder tridiagonalisation  C = Q T Q^T           (N steps, 1-2 kernels per step, not blocked)
 //               2. k largest eigenvalues of T by Sturm-count multisection (parallel over shifts)
@@ -643,9 +644,10 @@ __global__ void __launch_bounds__(512) backtransform_kernel(const double* __rest
 // above, on m instead of N) give Ritz values theta and vectors z = V y whose residual is |beta_m y_m|.  One step
 // costs one pass over C (50 MB from L2 at N = 2504) instead of the N steps the reduction needs, and population
 // structure separates the top of the spectrum, so a few dozen steps reach |beta_m y_m| <= 1e-12 ||T||.
-// Graph form (N > 16384, VPCA_LZ_PERSIST=0): five launches per step (matvec | V^T w | w -= V h | V^T w | w -= V h), step
-// index and stop flag in device memory so that kLzChunk steps replay from one CUDA graph; the host looks at the residual
-// after a replay.  Persistent form (default): see lz_persist_kernel further down.
+// Graph form (past N = 10 752 on 132 SMs, where the persistent kernel's shared memory no longer fits a block, and
+// VPCA_LZ_PERSIST=0): five launches per step (matvec | V^T w | w -= V h | V^T w | w -= V h), step index and stop flag in
+// device memory so that kLzChunk steps replay from one CUDA graph; the host looks at the residual after a replay.
+// Persistent form (default): see lz_persist_kernel further down.
 // Anything unusual -- breakdown, slow convergence, a larger eigenvalue found by the deflated re-run that guards
 // against a missed copy of a multiple eigenvalue -- falls back to the direct reduction, which remains the
 // reference-grade path.  Every reduction has a fixed order: the result is run-to-run deterministic.
@@ -844,7 +846,7 @@ __global__ void lz_verify_kernel(const double* __restrict__ theta, int k, const 
 }
 
 
-// ------------------------------------------------------------------ Lanczos, persistent form (n <= kLzPersistMaxN)
+// ------------------------------------------------- Lanczos, persistent form (while its shared memory fits one block)
 // The five launches of a step (and the 80 of a 16-step chunk) become ONE cooperative launch per chunk: 1024 threads on
 // every SM, block b owns the rows [b R, (b + 1) R) of everything (R = ceil(n / blocks)), and a step is three phases
 // separated by grid-wide barriers (an atomic counter in L2, ~1-2 us each instead of a kernel boundary):
@@ -858,7 +860,6 @@ __global__ void lz_verify_kernel(const double* __restrict__ theta, int k, const 
 //   C  the same with hpart2, alpha_j = h_j + h2_j, w_out rows = y.
 // VT is row-major (n x cap) so that one block's slice is contiguous in the Lanczos index q: the dot products and the
 // updates of a block read only its own R rows, coalesced.  Summation orders are fixed: run-to-run deterministic.
-constexpr int kLzPersistMaxN = 16384;   // w_in staged in shared memory: 8 n bytes
 constexpr int kLzThreads = 1024;
 constexpr int kLzSeg = 512;             // columns per warp task of the matvec
 constexpr int kLzVtCols = 32;           // leading basis columns of the block's rows that are mirrored in shared memory
@@ -1643,11 +1644,16 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     cudaError_t e;
 #define VPCA_TRY(x) if ((e = (x)) != cudaSuccess) return e
     if (w.d_V == nullptr) {
-        // persistent form: one 1024-thread block per SM, launched cooperatively (all blocks co-resident)
-        int dev = 0, sms = 0, coop = 0;
+        // persistent form: one 1024-thread block per SM, launched cooperatively (all blocks co-resident), with as much
+        // dynamic shared memory as the device grants one block beside the kernel's static arrays
+        int dev = 0, sms = 0, coop = 0, optin = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+        cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        cudaFuncAttributes fa{};
+        VPCA_TRY(cudaFuncGetAttributes(&fa, lz_persist_kernel));
+        w.lz_smem_max = (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
         const char* lp = getenv("VPCA_LZ_PERSIST");
         w.lz_blocks = (coop != 0 && sms > 0 && !(lp != nullptr && atoi(lp) == 0)) ? sms : 0;
     }
@@ -1679,21 +1685,22 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     double* part = scal2 + 16;
     int64_t nl = 0;
     const int upd_blocks = npart, mv_blocks = (n + 3) / 4;
-    // persistent form: one cooperative launch per chunk (see lz_persist_kernel); the five-kernel graph is kept for
-    // cohorts whose start vector does not fit shared memory and as VPCA_LZ_PERSIST=0
-    const bool persist = w.lz_blocks > 0 && n <= kLzPersistMaxN;
     double* hpart = part + npart;
-    const int rows_per = persist ? (n + w.lz_blocks - 1) / w.lz_blocks : 0;
+    // the persistent kernel's shared-memory layout (lz_persist_kernel): two length-n vectors plus per-block buffers that
+    // grow with rows_per = n / SMs -- 222 448 bytes at N = 10 752 on 132 SMs, past the 227 KB a block may use soon after
+    const int rows_per = w.lz_blocks > 0 ? (n + w.lz_blocks - 1) / w.lz_blocks : 0;
     const size_t base_smem =
         ((((size_t)n + 1) & ~(size_t)1) + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1) +
          ((((size_t)rows_per * ((n + kLzSeg - 1) / kLzSeg)) + 1) & ~(size_t)1) + (size_t)rows_per * kLzVtCols + (((size_t)n + 1) & ~(size_t)1) +
          (size_t)kLzVtCols * kLzVtCols + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1)) * sizeof(double);
-    // what is left of the 227 KB a block may use (minus the kernel's ~9 KB of static shared memory) holds rows of S
+    // persistent form (one cooperative launch per chunk) whenever that layout fits; otherwise, and with VPCA_LZ_PERSIST=0,
+    // the five-kernel graph form, which needs only the FP64 matrix C
+    const bool persist = w.lz_blocks > 0 && base_smem <= w.lz_smem_max;
+    // what is left of the block's shared memory holds rows of S
     int rows_smem = 0;
-    {
-        const size_t budget = 232448 - 10240 - 1024;
+    if (persist) {
         const size_t row_bytes = (size_t)((n + 3) & ~3) * sizeof(int32_t);
-        if (persist && base_smem < budget) rows_smem = (int)std::min<size_t>((size_t)rows_per, (budget - base_smem) / row_bytes);
+        rows_smem = (int)std::min<size_t>((size_t)rows_per, (w.lz_smem_max - base_smem) / row_bytes);
         if (const char* sr = getenv("VPCA_LZ_SROWS"); sr != nullptr) rows_smem = std::min(rows_smem, std::max(0, atoi(sr)));
     }
     const size_t persist_smem = base_smem + (size_t)rows_smem * ((n + 3) & ~3) * sizeof(int32_t);

@@ -163,6 +163,7 @@ struct EigWork {
     long long* d_lzprof = nullptr; // VPCA_LZ_PROF=1: phase timestamps of block 0 (first 64 steps)
     bool c_valid = false;       // d_C holds the centred matrix of the last center_gram()
     int lz_blocks = 0;          // blocks of the persistent kernel (= SMs; 0: cooperative launch unavailable or VPCA_LZ_PERSIST=0)
+    size_t lz_smem_max = 0;     // dynamic shared memory a block of the persistent kernel may take (opt-in limit - static)
     const int32_t* d_S = nullptr;   // the (symmetrised) int32 Gram the last center_gram() read
     cudaGraphExec_t lz_graph = nullptr;   // kLzChunk Lanczos steps
     int last_method = 0;        // 1 direct, 2 Lanczos, 3 Lanczos abandoned -> direct

@@ -1,0 +1,444 @@
+"""Every eigensolver path behind vpca_compute_pca, and the band solver's unaligned edges, against an FP64 reference.
+
+`eig_topk` / `lanczos_topk` (csrc/eig.cu) choose a path from N, N mod 4, the SM count and environment switches:
+
+  persistent Lanczos (one cooperative launch per 16-step chunk, reads the int32 Gram S), while its shared memory fits
+      mat-vec  regw       N % 4 == 0 and the 512-column segments fill the warps (1092, 2504, 8192, ...)
+               task list  N % 4 == 0 otherwise (5632, 10 000, 10 752, ...)
+               scalar     N % 4 != 0
+      rows of S kept in shared memory as far as they fit, the rest read from L2 (VPCA_LZ_SROWS caps them)
+  graph-form Lanczos (five kernels per step on the FP64 matrix C): past that fit (~10 750 on 132 SMs), VPCA_LZ_PERSIST=0
+  direct reduction: fused step kernel up to N = 3072, two kernels above (or VPCA_EIG_TWO_KERNELS); inverse iteration
+      out of shared memory up to N = 3200, out of global memory above
+  Lanczos that gives up hands over to the direct reduction (eig_method 3)
+
+Each test names the path it exercises and proves that it ran: `eig_method`, and -- both Lanczos forms report 2 -- the
+`kernel_launches` delta of the call: the persistent form needs fewer launches than steps, the graph form at least five
+per step, the direct reduction 64 (fused) or 128 (two kernels) per 64-step graph replay.
+
+Reference: the cohort is the synthetic generator's cells X (N x nv, 0/1) and the Gram kernel builds S = X X^T from them
+(pinned bit for bit by test_gram_gpu.py).  The centred Gram is C = J S J = (JX)(JX)^T, so its top eigenpairs come from the
+small FP64 eigh of (JX)^T (JX): lambda and u = JX v / sqrt(lambda).  Residuals C u - lambda u = JX ((JX)^T u) - lambda u
+cost O(N nv) without forming C."""
+import math
+import os
+from contextlib import contextmanager
+
+import numpy as np
+import pytest
+
+pytestmark = pytest.mark.gpu
+
+SEED = 20240901
+P = 1024          # variants per panel
+NV = 4096         # variants of every cohort below 65 535 samples
+K = 4             # the generator's five populations give four well separated components
+
+# static shared memory of lz_persist_kernel (`ptxas -v`: red, red2, red3); with the device's opt-in limit it decides the
+# largest N the persistent form takes.  Update it with the kernel.
+LZ_STATIC_SMEM = 9488
+LZ_ENV = ("VPCA_EIG", "VPCA_EIG_MAXIT", "VPCA_EIG_TWO_KERNELS", "VPCA_LZ_PERSIST", "VPCA_LZ_SROWS", "VPCA_LZ_SPECULATE")
+
+
+# ---------------------------------------------------------------------------------------------------- reference helpers
+class Reference:
+    """FP64 top eigenpairs of the centred Gram of the cells X, from the nv x nv eigh of (JX)^T (JX)"""
+
+    def __init__(self, X, k):
+        import torch
+        X = X.to(torch.float64)
+        self.n = X.shape[0]
+        self.nz = int((X.sum(dim=1) > 0).sum())                 # rows of S with a positive sum: samples with a carrier
+        self.JX = X - X.mean(dim=0, keepdim=True)
+        del X
+        lam, V = torch.linalg.eigh(self.JX.t() @ self.JX)
+        lam, V = lam.flip(0)[:k], V.flip(1)[:, :k]
+        self.U = ((self.JX @ V) / lam.sqrt()).cpu().numpy()
+        self.lam = lam.cpu().numpy()
+
+    def residuals(self, vecs, evals):
+        """||C u - lambda u|| / lambda_1 per column, C u = JX ((JX)^T u)"""
+        import torch
+        u = torch.from_numpy(vecs).to(self.JX.device)
+        r = self.JX @ (self.JX.t() @ u) - u * torch.from_numpy(evals).to(self.JX.device)[None, :]
+        return (torch.linalg.norm(r, dim=0) / float(self.lam[0])).cpu().numpy()
+
+    def gaps_allow(self, k):
+        """the top k + 1 eigenvalues are far enough apart for two solvers' vectors to agree to 1e-8"""
+        return k >= len(self.lam) or np.min(np.abs(np.diff(self.lam[: k + 1]))) / self.lam[0] > 1e-4
+
+
+def synth_cells(n, nv):
+    """The generator's cells of n samples x nv variants on cuda:0 in panel layout (uint8) and as an (n, nv) int8 view"""
+    import torch
+    from spark_examples_b200 import native
+    assert nv % P == 0
+    with native.NativePca(n, max_multiplicity=1, gram_band=(0, min(n, 64))) as gen:   # a generator, not an N x N Gram
+        buf = torch.zeros(gen.panelBytes(nv, P), dtype=torch.uint8, device="cuda:0")
+        torch.cuda.synchronize()
+        gen.synthPanelsDevice(SEED, 0, nv, 0, buf.data_ptr(), P)
+        gen.synchronize()
+    X = buf.view(torch.int8).view(nv // P, n, P).permute(1, 0, 2).reshape(n, nv)
+    return buf, X
+
+
+def check_pairs(ref, vecs, evals, nz, k):
+    """The assertions every solve below must meet against the FP64 reference"""
+    from oracle import oracle
+    n = ref.n
+    assert vecs.shape == (n, k) and evals.shape == (k,)
+    assert nz == ref.nz
+    assert np.allclose(evals, ref.lam[:k], rtol=1e-10, atol=0), (evals, ref.lam[:k])
+    err = oracle.eigvec_rel_err(vecs, ref.U[:, :k])
+    assert np.all(err <= 1e-6), err
+    res = ref.residuals(vecs, evals)
+    assert np.all(res <= 1e-11), res
+    assert np.abs(vecs.T @ vecs - np.eye(k)).max() <= 1e-10
+    assert np.allclose(np.linalg.norm(vecs, axis=0), 1.0, atol=1e-12)
+    for c in range(k):
+        assert vecs[np.argmax(np.abs(vecs[:, c])), c] > 0               # sign rule: largest-|.| entry positive
+
+
+def check_agree(a, b, k, ref, vec_tol=1e-8, eval_rtol=1e-11):
+    """two solves of the same Gram: eigenvalues to eval_rtol, vectors to vec_tol where the gaps allow"""
+    from oracle import oracle
+    assert np.allclose(a.evals, b.evals, rtol=eval_rtol, atol=0), (a.evals, b.evals)
+    if ref.gaps_allow(k):
+        err = oracle.eigvec_rel_err(a.vecs, b.vecs)
+        assert np.all(err <= vec_tol), err
+
+
+# --------------------------------------------------------------------------------------------------------- solve helpers
+@contextmanager
+def solver_env(env):
+    """exactly the given solver switches, whatever the caller's environment holds"""
+    saved = {key: os.environ.pop(key, None) for key in LZ_ENV}
+    os.environ.update(env or {})
+    try:
+        yield
+    finally:
+        for key in LZ_ENV:
+            os.environ.pop(key, None)
+            if saved[key] is not None:
+                os.environ[key] = saved[key]
+
+
+class Solve:
+    def __init__(self, out, before, after):
+        self.vecs, self.evals, self.nz = out
+        self.method = after["eig_method"]
+        self.iters = after["eig_iterations"]
+        self.launches = after["kernel_launches"] - before["kernel_launches"]
+
+    def __repr__(self):
+        return f"Solve(method={self.method}, iters={self.iters}, launches={self.launches})"
+
+
+def gram_context(n, buf, nv, k):
+    """a fresh full context whose finalized Gram the Gram kernel built from the cells"""
+    from spark_examples_b200 import native
+    nat = native.NativePca(n, max_multiplicity=1, num_pc=k)
+    try:
+        nat.accumulatePanels(buf.data_ptr(), nv, P)
+        nat.finalizeGram()
+    except Exception:
+        nat.close()
+        raise
+    return nat
+
+
+def compute_pca(nat, k, env=None):
+    """vpca_compute_pca under exactly the switches in env (the context must not have solved by Lanczos yet if env sets
+    VPCA_LZ_PERSIST: the form is fixed at a context's first Lanczos solve)"""
+    with solver_env(env):
+        before = nat.stats()
+        out = nat.computePca(k)
+        return Solve(out, before, nat.stats())
+
+
+def solve(n, buf, nv, k, env=None):
+    with gram_context(n, buf, nv, k) as nat:
+        return compute_pca(nat, k, env)
+
+
+def compute_pca_bands(ctxs, k):
+    from spark_examples_b200 import native
+    with solver_env(None):
+        before = ctxs[0].stats()
+        out = native.computePcaBands(ctxs, k)
+        return Solve(out, before, ctxs[0].stats())
+
+
+def assert_persistent(s):
+    assert s.method == 2, s
+    assert 16 <= s.iters <= 320 and s.launches < s.iters, s          # one cooperative launch per 16 steps + the checks
+
+
+def assert_graph(s):
+    assert s.method == 2, s
+    assert 16 <= s.iters <= 320 and s.launches >= 5 * s.iters, s     # 80 launches per 16-step chunk
+
+
+def assert_direct(s, n, fused):
+    # row sums + mean (2), ceil(n / 64) replays of the 64-step graph (1 or 2 launches per step), bisection, inverse
+    # iteration, back-transformation (3)
+    assert s.method == 1 and s.iters == 0, s
+    assert s.launches == 2 + (1 if fused else 2) * 64 * math.ceil(n / 64) + 3, s
+
+
+def need_free_hbm(gib):
+    import torch
+    free, _ = torch.cuda.mem_get_info()
+    if free < gib * 2 ** 30:
+        pytest.skip(f"needs {gib:.0f} GB of free HBM")
+
+
+def graph_form_gib(n):
+    """S (int32) + C (FP64) + the Krylov basis + the reference's cells, with room to spare"""
+    return 1.3 * (12 * n * n + 8 * 400 * n + 24 * n * NV) / 2 ** 30 + 1
+
+
+def persist_smem(n, sms):
+    """dynamic shared memory lz_persist_kernel needs at n on `sms` SMs (base_smem in lanczos_topk, eig.cu)"""
+    cap, seg, vt = 384, 512, 32
+    rows = -(-n // sms)
+    even = lambda x: (x + 1) & ~1
+    return 8 * (even(n) + cap + even(rows) + even(rows * -(-n // seg)) + rows * vt + even(n) + vt * vt + cap + even(rows))
+
+
+def last_persistent_n():
+    """the largest N whose persistent-form working set fits one block of this device (10 752 on 132 SMs)"""
+    import torch
+    props = torch.cuda.get_device_properties(0)
+    limit = props.shared_memory_per_block_optin - LZ_STATIC_SMEM
+    n = 4096
+    while persist_smem(n + 1, props.multi_processor_count) <= limit:
+        n += 1
+    return n
+
+
+def resolve(n):
+    return {"last_fit": last_persistent_n, "past_fit": lambda: last_persistent_n() + 1}.get(n, lambda: n)()
+
+
+# ------------------------------------------------------------------------------------------ 1. persistent Lanczos
+@pytest.mark.parametrize("n", [1092, 2503, 5632, 8192, 10_000, "last_fit"],
+                         ids=["regw-all-rows-smem", "scalar", "tasklist-some-rows-smem", "regw-one-row-smem",
+                              "tasklist-rows-from-L2", "tasklist-last-N-that-fits"])
+def test_persistent_lanczos_matvec_variants(n):
+    """Persistent Lanczos, each mat-vec variant: regw (one w segment in registers per warp) at 1092 with every row of S in
+    shared memory and at 8192 with one; the scalar mat-vec at 2503 (N % 4 != 0); the (row, segment) task list at 5632,
+    10 000 and the largest N whose shared-memory working set still fits a block, rows mostly or all read from L2."""
+    n = resolve(n)
+    buf, X = synth_cells(n, NV)
+    s = solve(n, buf, NV, K)
+    assert_persistent(s)
+    check_pairs(Reference(X, K), s.vecs, s.evals, s.nz, K)
+    if n == 1092:                        # and the MLlib recipe itself, where it is cheap
+        from oracle import oracle
+        with gram_context(n, buf, NV, K) as nat:
+            S = nat.getGram()
+        want, _ = oracle.compute_pca(S, K)
+        assert np.all(oracle.eigvec_rel_err(s.vecs, want) <= 1e-6)
+
+
+@pytest.mark.parametrize("env", [{"VPCA_LZ_SROWS": "0"}, {"VPCA_LZ_SPECULATE": "0"}], ids=["no-rows-in-smem", "no-speculation"])
+def test_persistent_lanczos_switches(env):
+    """Persistent Lanczos at 2504 with every row of S read from L2 (VPCA_LZ_SROWS=0), and with the verification run
+    enqueued only after the host has seen convergence (VPCA_LZ_SPECULATE=0): the same pairs as the default run."""
+    n = 2504
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    default, switched = solve(n, buf, NV, K), solve(n, buf, NV, K, env)
+    for s in (default, switched):
+        assert_persistent(s)
+        check_pairs(ref, s.vecs, s.evals, s.nz, K)
+    check_agree(switched, default, K, ref)
+
+
+# ------------------------------------------------------------------------------------------- 2. graph-form Lanczos
+@pytest.mark.parametrize("n", [1092, 2503])
+def test_graph_lanczos_forced(n):
+    """Graph-form Lanczos (lz_matvec_kernel on the FP64 C, lz_dots / lz_update, lz_ritz_kernel, and the column-major
+    deflated verification run) forced with VPCA_LZ_PERSIST=0, against the persistent form and the reference."""
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    graph, persistent = solve(n, buf, NV, K, {"VPCA_LZ_PERSIST": "0"}), solve(n, buf, NV, K)
+    assert_graph(graph)
+    assert_persistent(persistent)
+    check_pairs(ref, graph.vecs, graph.evals, graph.nz, K)
+    check_agree(graph, persistent, K, ref)
+
+
+@pytest.mark.parametrize("n", ["past_fit", 12_000, 16_384, 16_385, 20_000])
+def test_graph_lanczos_past_the_persistent_fit(n):
+    """Graph-form Lanczos chosen by the solver itself: from the first N whose persistent working set no longer fits a
+    block of shared memory (10 753 on 132 SMs) on, where the persistent kernel cannot be launched."""
+    n = resolve(n)
+    need_free_hbm(graph_form_gib(n))
+    buf, X = synth_cells(n, NV)
+    s = solve(n, buf, NV, K)
+    assert_graph(s)
+    check_pairs(Reference(X, K), s.vecs, s.evals, s.nz, K)
+
+
+def test_graph_lanczos_at_the_sample_limit():
+    """Graph-form Lanczos at N = 65 535, vpca_compute_pca's limit: S is 17 GB, C 34 GB, and center_kernel's grid is
+    exactly 65 535 rows high.  k = 2 on the structured cohort converges without a hand-over to the direct solver."""
+    import torch
+    n, nv, k = 65_535, 2048, 2
+    need_free_hbm(60)
+    buf, X = synth_cells(n, nv)
+    with gram_context(n, buf, nv, k) as nat:
+        s = compute_pca(nat, k)
+    torch.cuda.empty_cache()
+    assert_graph(s)
+    check_pairs(Reference(X, k), s.vecs, s.evals, s.nz, k)
+
+
+# ------------------------------------------------------------------------------------------------ 3. direct solver
+@pytest.mark.parametrize("n,fused", [(3072, True), (3073, False), (3200, False), (3201, False), (4096, False)],
+                         ids=["fused-smem-invit", "two-kernel-smem-invit", "two-kernel-last-smem-invit",
+                              "two-kernel-global-invit", "two-kernel-global-invit-4096"])
+def test_direct_solver(n, fused):
+    """Direct reduction (VPCA_EIG=direct) on both sides of its switches: the fused step kernel up to N = 3072 and
+    tridiag_small + tridiag_big above; inverse iteration with its 8 N doubles in shared memory up to N = 3200
+    (invit_kernel<true>) and in global memory above (invit_kernel<false>)."""
+    buf, X = synth_cells(n, NV)
+    s = solve(n, buf, NV, K, {"VPCA_EIG": "direct"})
+    assert_direct(s, n, fused)
+    check_pairs(Reference(X, K), s.vecs, s.evals, s.nz, K)
+
+
+def test_direct_solver_two_kernels_forced():
+    """The two-kernel direct reduction forced with VPCA_EIG_TWO_KERNELS=1 at 1092, against the fused form."""
+    n = 1092
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    two = solve(n, buf, NV, K, {"VPCA_EIG": "direct", "VPCA_EIG_TWO_KERNELS": "1"})
+    fused = solve(n, buf, NV, K, {"VPCA_EIG": "direct"})
+    assert_direct(two, n, fused=False)
+    assert_direct(fused, n, fused=True)
+    for s in (two, fused):
+        check_pairs(ref, s.vecs, s.evals, s.nz, K)
+    check_agree(two, fused, K, ref)
+
+
+# ------------------------------------------------------------------------------------------ 4. hand-over above 3072
+def test_abandoned_lanczos_hands_over_above_3072():
+    """Lanczos that gives up hands over to the two-kernel direct reduction: six components reach into the bulk and need
+    more than 32 steps, so with VPCA_EIG_MAXIT=32 the solve falls back -- and then it is the direct solve, bit for bit."""
+    n, k = 4000, 6
+    buf, X = synth_cells(n, NV)
+    cut = solve(n, buf, NV, k, {"VPCA_EIG_MAXIT": "32"})
+    direct = solve(n, buf, NV, k, {"VPCA_EIG": "direct"})
+    assert cut.method == 3 and cut.iters == 32, cut
+    assert_direct(direct, n, fused=False)
+    assert cut.launches > direct.launches
+    assert np.array_equal(cut.vecs, direct.vecs) and np.array_equal(cut.evals, direct.evals)
+    check_pairs(Reference(X, k), cut.vecs, cut.evals, cut.nz, k)
+
+
+# --------------------------------------------------------------------------------------------------- 5. band solver
+def band_contexts(n, buf, nv, bands, k):
+    """owner-computes band contexts (no peers, every variant fed to each) storing rows [row0, row0 + rows) each"""
+    from spark_examples_b200 import native
+    ctxs = []
+    try:
+        for band in bands:
+            ctxs.append(native.NativePca(n, max_multiplicity=1, num_pc=k, gram_band=band))
+        for c in ctxs:
+            c.accumulatePanels(buf.data_ptr(), nv, P)
+        for c in ctxs:
+            c.synchronize()
+            c.finalizeGram()
+        return ctxs
+    except Exception:
+        close_all(ctxs)
+        raise
+
+
+def close_all(ctxs):
+    for c in ctxs:
+        try:
+            c.synchronize()
+        except Exception:
+            pass
+    for c in ctxs:
+        c.close()
+
+
+def bands_from_edges(edges):
+    return [(a, b - a) for a, b in zip(edges[:-1], edges[1:])]
+
+
+@pytest.mark.parametrize("n", [2503, 3001])
+def test_band_solver_scalar_loads(n):
+    """Band solver on one full context with N % 4 != 0: band_tile_kernel<T, false> (scalar loads, the diagonal clipped
+    cell by cell) for both the exact row sums and every mat-vec, against the reference and vpca_compute_pca."""
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    with gram_context(n, buf, NV, K) as nat:
+        bands = compute_pca_bands([nat], K)
+        full = compute_pca(nat, K)
+    assert bands.method == 4 and 16 <= bands.iters <= 320, bands
+    assert_persistent(full)
+    check_pairs(ref, bands.vecs, bands.evals, bands.nz, K)
+    check_agree(bands, full, K, ref)
+    assert bands.nz == full.nz
+
+
+# band bounds off every multiple of 4, 32 and 64, one single-row band, two that straddle a 1024-column tile boundary
+UNALIGNED_EDGES = [0, 1, 64, 1064, 2063]
+
+
+@pytest.mark.parametrize("n", [2503, 2504], ids=["scalar-loads", "vector-loads"])
+def test_band_solver_unaligned_bands(n):
+    """Band solver on hand-made owner-computes bands [0, 1), [1, 64), [64, 1064), [1064, 2063), [2063, N): the diagonal
+    clipping of band_load inside a 4-cell group, with scalar (N % 4 != 0) and int4 loads, and tiles cut by band ends."""
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    ctxs = band_contexts(n, buf, NV, bands_from_edges(UNALIGNED_EDGES + [n]), K)
+    try:
+        bands = compute_pca_bands(ctxs, K)
+    finally:
+        close_all(ctxs)
+    assert bands.method == 4, bands
+    check_pairs(ref, bands.vecs, bands.evals, bands.nz, K)
+    full = solve(n, buf, NV, K)
+    check_agree(bands, full, K, ref)
+
+
+def test_band_solver_world_16():
+    """Band solver with 16 owner-computes bands (BandEnds' maximum), uneven and unaligned: the rank-order sums of the
+    partial products over all 16 slots."""
+    n = 3001
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    edges = [round(q * n / 16) + (q % 3 if 0 < q < 16 else 0) for q in range(17)]
+    ctxs = band_contexts(n, buf, NV, bands_from_edges(edges), K)
+    try:
+        bands = compute_pca_bands(ctxs, K)
+    finally:
+        close_all(ctxs)
+    assert bands.method == 4, bands
+    check_pairs(ref, bands.vecs, bands.evals, bands.nz, K)
+    check_agree(bands, solve(n, buf, NV, K), K, ref)
+
+
+# ------------------------------------------------------------------------------------ 6. cross-solver agreement
+@pytest.mark.parametrize("n", [12_000, 20_000])
+def test_graph_lanczos_and_band_solver_agree(n):
+    """Two independent mat-vecs of the same Gram past the persistent fit: the graph-form Lanczos on the FP64 C
+    (vpca_compute_pca) and the band solver on the int32 lower triangle (vpca_compute_pca_bands, world 1)."""
+    need_free_hbm(graph_form_gib(n))
+    buf, X = synth_cells(n, NV)
+    ref = Reference(X, K)
+    with gram_context(n, buf, NV, K) as nat:
+        graph = compute_pca(nat, K)
+        bands = compute_pca_bands([nat], K)
+    assert_graph(graph)
+    assert bands.method == 4, bands
+    for s in (graph, bands):
+        check_pairs(ref, s.vecs, s.evals, s.nz, K)
+    check_agree(graph, bands, K, ref)

@@ -1774,6 +1774,9 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     for (int chunk = 1; chunk <= max_chunks; ++chunk) {
         VPCA_TRY(run_chunk(0));
         m = chunk * kLzChunk;
+        // fewer steps than wanted pairs (k > 16): T has no k Ritz pairs, and the residual of the missing ones is noise
+        // that would only feed the convergence-rate forecast below
+        if (m < k) continue;
         // look at the residual after every replay up to 64 steps, then after every other one
         if (chunk > 4 && (chunk & 1) && chunk != max_chunks) continue;
         bisect_kernel<<<k, 256, 0, stream>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
@@ -2131,6 +2134,7 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     for (int chunk = 1; chunk <= max_chunks; ++chunk) {
         for (int g = 0; g < kLzChunk; ++g) VPCA_TRY(step());
         m = chunk * kLzChunk;
+        if (m < k) continue;   // as in lanczos_topk: no k Ritz pairs yet
         if (chunk > 4 && (chunk & 1) && chunk != max_chunks) continue;
         bisect_kernel<<<k, 256, 0, s0>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
         invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), s0>>>(alpha, beta + 1, m, k, w.d_evals,

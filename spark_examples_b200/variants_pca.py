@@ -32,6 +32,8 @@ from .records import Call, CallData, Variant
 from .parquet_calls import ParquetSlice
 from .variants_common import BedSlice, CallsBatch, JoinedSlice, SyntheticSlice, VariantsCommon, VariantsDataset
 
+MAX_LOADING_PC = 16   # components vpca_loadings_* / vpca_project_* handle (include/vpca.h)
+
 
 # ------------------------------------------------------------------------------------------------------------------
 # companion-object functions (VariantsPca.scala:54-78)
@@ -695,6 +697,9 @@ def main(args: Optional[Sequence[str]] = None):
         result = driver.projectLoadings(callsRdd)
     else:
         if conf.saveLoadings.isDefined:
+            if conf.numPc() > MAX_LOADING_PC:           # vpca_loadings_* take k <= 16: refuse before the Gram
+                raise ValueError(f"--save-loadings stores at most {MAX_LOADING_PC} components; "
+                                 f"--num-pc {conf.numPc()} asks for more")
             driver.keyKind(callsRdd)                    # reject unsupported input before the Gram
         simMatrix = driver.getSimilarityMatrix(callsRdd)
         result = driver.computePca(simMatrix)

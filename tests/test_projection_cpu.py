@@ -232,6 +232,23 @@ def test_rejections(tmp_path, oracle, fake_native):
     assert all(not n.X for n in fake_native)
 
 
+def test_save_loadings_refuses_more_than_16_components_before_the_gram(tmp_path, monkeypatch, oracle, fake_native):
+    """Loadings hold at most 16 components: --num-pc 17 with --save-loadings fails before any Gram is requested, not
+    after the Gram and the eigensolve."""
+    d = oracle.c_synth_dense(9, 40, 0, 100, 1).astype(np.int64)
+    plink.write_fileset(str(tmp_path / "r"), d)
+    grams = []
+    gram = VariantsPcaDriver.getSimilarityMatrix
+    monkeypatch.setattr(VariantsPcaDriver, "getSimilarityMatrix", lambda self, calls: grams.append(1) or gram(self, calls))
+    argv = ["--bed-path", str(tmp_path / "r"), "--save-loadings", str(tmp_path / "r.npz")]
+    with pytest.raises(ValueError, match="at most 16 components"):
+        variants_pca.main(argv + ["--num-pc", "17"])
+    assert grams == [] and all(not n.X and not n.staged for n in fake_native)
+    assert not (tmp_path / "r.npz").exists()
+    variants_pca.main(argv + ["--num-pc", "16"])                 # 16 is still accepted
+    assert len(grams) == 1
+
+
 def test_row_keys_for_in_memory_calls(tmp_path, oracle, fake_native):
     """CSR partitions carry no identity: rows are keyed by their global index, so a re-run on the same rows matches."""
     X = oracle.c_synth_dense(4, 30, 0, 90, 0).astype(np.int64)

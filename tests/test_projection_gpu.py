@@ -12,6 +12,10 @@ from projection_ref import dense_to_csr, np_loadings, np_project
 pytestmark = pytest.mark.gpu
 
 P = 1024   # panel width of the device-resident inputs below
+# component counts that launch every KMAX instantiation of project.cu (2, 4, 8, 16) at and past its lower and upper
+# bound; at KMAX 16 loadings_kernel runs 2 variants per thread (VT) instead of 4, and project_kernel stages w in
+# 256-variant tiles from KMAX 8 on
+KS = (1, 2, 4, 5, 8, 9, 16)
 
 
 def _cohort(oracle, n, nv, seed=20240901):
@@ -37,14 +41,14 @@ def _bed_rows(tmp_path, X, name="c"):
     return bed.rows(0, bed.n_variants)
 
 
-def _panels(X, dtype):
+def _panels(X, dtype, panel=P):
     """(N, V) cells -> device panel layout (torch uint8 buffer) of the dtype, zero cells after V."""
     import torch
     n, nv = X.shape
-    npan = (nv + P - 1) // P
-    Xp = np.zeros((n, npan * P), np.int64)
+    npan = (nv + panel - 1) // panel
+    Xp = np.zeros((n, npan * panel), np.int64)
     Xp[:, :nv] = X
-    pan = np.ascontiguousarray(Xp.reshape(n, npan, P).transpose(1, 0, 2))     # (panels, n, P)
+    pan = np.ascontiguousarray(Xp.reshape(n, npan, panel).transpose(1, 0, 2))     # (panels, n, panel)
     if dtype == 0:
         host = pan.astype(np.int8).view(np.uint8)
     elif dtype == 1:
@@ -59,26 +63,40 @@ def _rel(a, b):
     return np.max(np.abs(a - b), axis=0) / np.max(np.abs(b), axis=0)
 
 
-@pytest.mark.parametrize("n,nv", [(257, 3000), (1092, 8000)])
+@pytest.mark.parametrize("n,nv", [(257, 3000), (1092, 8000), (257, 3001), (1092, 3001)])
 @pytest.mark.parametrize("dtype", [0, 1, 2], ids=["int8", "bf16", "e2m1"])
 def test_loadings_match_numpy(oracle, n, nv, dtype):
+    """Loadings of k' = 1 .. 16 components (KS) from one computePca(16), from CSR calls and from panels 384 and 1024
+    variants wide: numpy's X^T U to 1e-12, and every column the same bits whatever k' and input -- each column is summed
+    over the samples in order by every KMAX / VT instantiation.  N = 1092 takes U in five 256-sample tiles at KMAX 16,
+    the last one partial; nv = 3001 leaves a partial last panel and a thread with one variant of its pair."""
+    import torch
     from spark_examples_b200 import native
     X = _cohort(oracle, n, nv)
-    import torch
-    nat, U, _ = _reference(native, X, 4, dtype)
+    nat, U, _ = _reference(native, X, 16, dtype)
+    csr = dense_to_csr(X)
+    panels = {}
     with nat:
-        w, cnt = nat.loadingsCalls(4, *dense_to_csr(X))
-        w2, _ = nat.loadingsCalls(2, *dense_to_csr(X))
-        d_x = _panels(X, dtype)                                    # the kernel's own decode of each element type
-        dw = torch.zeros((nv, 4), dtype=torch.float64, device="cuda")
-        dc = torch.zeros(nv, dtype=torch.int32, device="cuda")
-        nat.loadingsPanels(4, d_x.data_ptr(), nv, P, dw.data_ptr(), dc.data_ptr())
-        nat.synchronize()
+        calls = {k: nat.loadingsCalls(k, *csr) for k in KS}
+        for pw in (384, 1024):
+            d_x = _panels(X, dtype, pw)                            # the kernel's own decode of each element type
+            for k in KS:
+                dw = torch.zeros((nv, k), dtype=torch.float64, device="cuda")
+                dc = torch.zeros(nv, dtype=torch.int32, device="cuda")
+                nat.loadingsPanels(k, d_x.data_ptr(), nv, pw, dw.data_ptr(), dc.data_ptr())
+                panels[pw, k] = dw, dc
+            nat.synchronize()
     W, C = np_loadings(X, U)
-    assert np.array_equal(cnt, C) and np.array_equal(dc.cpu().numpy(), C)
-    assert np.array_equal(dw.cpu().numpy().view(np.uint64), w.view(np.uint64))
-    assert np.all(_rel(w, W) <= 1e-12), _rel(w, W)
-    assert np.array_equal(w2, w[:, :2])                            # a column does not depend on how many are asked for
+    w16 = calls[16][0]
+    assert np.all(_rel(w16, W) <= 1e-12), _rel(w16, W)
+    for k in KS:
+        w, cnt = calls[k]
+        assert np.array_equal(cnt, C), k
+        assert np.array_equal(w.view(np.uint64), w16[:, :k].view(np.uint64)), k   # independent of how many are asked for
+        for pw in (384, 1024):
+            dw, dc = panels[pw, k]
+            assert np.array_equal(dc.cpu().numpy(), C), (pw, k)
+            assert np.array_equal(dw.cpu().numpy().view(np.uint64), w.view(np.uint64)), (pw, k)
 
 
 def test_loadings_bit_identical_across_inputs_and_runs(oracle, tmp_path):
@@ -102,49 +120,60 @@ def test_loadings_bit_identical_across_inputs_and_runs(oracle, tmp_path):
 
 
 def test_self_projection_reproduces_the_eigenvectors(oracle):
+    """Projecting the reference samples with their own loadings gives U back, at k = 4 and 16 (KMAX 4 and 16)."""
     from spark_examples_b200 import native
     X = _cohort(oracle, 1092, 8000)
     n = X.shape[0]
-    nat, U, evals = _reference(native, X, 4)
+    nat, U, evals = _reference(native, X, 16)
     off, idx = dense_to_csr(X)
     with nat:
-        w, cnt = nat.loadingsCalls(4, off, idx)
-    with native.NativePca(n) as proj:
-        proj.projectBegin(4)
-        proj.projectCalls(off, idx, w, cnt / n)
-        got = proj.projectGet(evals)
-    err = oracle.eigvec_rel_err(got, U)
-    print(f"self-projection eigvec_rel_err per component: {err}")
-    assert np.all(err <= 1e-6)
+        w, cnt = nat.loadingsCalls(16, off, idx)
+    assert np.all(evals > 1e-3 * evals[0])                        # every pair has lambda well above zero
+    for k in (4, 16):
+        with native.NativePca(n) as proj:
+            proj.projectBegin(k)
+            proj.projectCalls(off, idx, np.ascontiguousarray(w[:, :k]), cnt / n)
+            got = proj.projectGet(evals[:k])
+        err = oracle.eigvec_rel_err(got, U[:, :k])
+        print(f"self-projection k={k} eigvec_rel_err per component: {err}")
+        assert np.all(err <= 1e-6), (k, err)
 
 
 def test_held_out_samples_match_numpy_through_every_input(oracle, tmp_path):
+    """M = 200 held-out samples (not a multiple of 128) projected with k = 3, 5, 8, 9 and 16 components through CSR
+    calls, .bed rows and panels 384 (one 256- and one 128-variant tile of w from KMAX 8 on) and 1024 variants wide:
+    numpy to 1e-10, and each component the same bits whatever k -- every column is summed in the same order."""
     import torch
     from spark_examples_b200 import native
     X = _cohort(oracle, 900, 5000)
     n1 = 700
     R, Y = X[:n1], X[n1:]
     m = Y.shape[0]
-    nat, U, evals = _reference(native, R, 3)
+    nat, U, evals = _reference(native, R, 16)
     with nat:
-        w, cnt = nat.loadingsCalls(3, *dense_to_csr(R))
-    want = np_project(Y, w, cnt, n1, evals)
+        loadings = {k: nat.loadingsCalls(k, *dense_to_csr(R)) for k in (3, 5, 8, 9, 16)}
+    cnt = loadings[16][1]
     mean = cnt / n1
+    rows, y_csr, d_y = _bed_rows(tmp_path, Y), dense_to_csr(Y), {pw: _panels(Y, 0, pw) for pw in (384, 1024)}
     outs = {}
     with native.NativePca(m) as proj:
-        proj.projectBegin(3)
-        proj.projectCalls(*dense_to_csr(Y), w, mean)
-        outs["calls"] = proj.projectGet(evals)
-        proj.projectBegin(3)
-        proj.projectBed(_bed_rows(tmp_path, Y), w, mean, 1)
-        outs["bed"] = proj.projectGet(evals)
-        proj.projectBegin(3)
-        d_y = _panels(Y, 0)
-        dw, dm = torch.from_numpy(w).cuda(), torch.from_numpy(mean).cuda()
-        proj.projectPanels(d_y.data_ptr(), Y.shape[1], P, dw.data_ptr(), dm.data_ptr())
-        outs["panels"] = proj.projectGet(evals)
-    for name, got in outs.items():
-        assert np.all(_rel(got, want) <= 1e-10), (name, _rel(got, want))
+        for k, (w, _) in loadings.items():
+            proj.projectBegin(k)
+            proj.projectCalls(*y_csr, w, mean)
+            outs[k, "calls"] = proj.projectGet(evals[:k])
+            proj.projectBegin(k)
+            proj.projectBed(rows, w, mean, 1)
+            outs[k, "bed"] = proj.projectGet(evals[:k])
+            dw, dm = torch.from_numpy(w).cuda(), torch.from_numpy(mean).cuda()
+            for pw in (384, 1024):
+                proj.projectBegin(k)
+                proj.projectPanels(d_y[pw].data_ptr(), Y.shape[1], pw, dw.data_ptr(), dm.data_ptr())
+                outs[k, f"panels{pw}"] = proj.projectGet(evals[:k])
+    want = np_project(Y, loadings[16][0], cnt, n1, evals)
+    for (k, name), got in outs.items():
+        assert got.shape == (m, k)
+        assert np.all(_rel(got, want[:, :k]) <= 1e-10), (k, name, _rel(got, want[:, :k]))
+        assert np.array_equal(got.view(np.uint64), outs[16, name][:, :k].view(np.uint64)), (k, name)
 
 
 def test_partial_overlap_equals_zeroed_rows_and_runs_are_reproducible(oracle):
@@ -229,12 +258,21 @@ def _tsv(lines):
 
 
 def test_cli_save_then_project_bed(oracle, tmp_path, capsys):
+    """--save-loadings then --project-loadings through the driver, with --num-pc 2 (the default) and 16 (the most
+    components loadings hold)."""
+    for num_pc in (2, 16):
+        (tmp_path / f"pc{num_pc}").mkdir()
+        _cli_save_then_project_bed(oracle, tmp_path / f"pc{num_pc}", capsys, num_pc)
+
+
+def _cli_save_then_project_bed(oracle, tmp_path, capsys, num_pc):
     from spark_examples_b200 import plink, variants_pca
     d = oracle.c_synth_dense(7, 400, 0, 3000, 1).astype(np.int64)   # dosage 0/1/2
     n, nv = d.shape
     plink.write_fileset(str(tmp_path / "ref"), d)
     lpath = str(tmp_path / "ref.loadings.npz")
-    variants_pca.main(["--bed-path", str(tmp_path / "ref"), "--variants-per-partition", "1000", "--save-loadings", lpath])
+    variants_pca.main(["--bed-path", str(tmp_path / "ref"), "--variants-per-partition", "1000", "--save-loadings", lpath,
+                       "--num-pc", str(num_pc)])
     first = _tsv([ln for ln in capsys.readouterr().out.splitlines() if ln.count("\t") == 3])
     variants_pca.main(["--bed-path", str(tmp_path / "ref"), "--variants-per-partition", "700", "--project-loadings", lpath])
     again = _tsv([ln for ln in capsys.readouterr().out.splitlines() if ln.count("\t") == 3])
@@ -243,6 +281,7 @@ def test_cli_save_then_project_bed(oracle, tmp_path, capsys):
         assert np.all(np.abs(first[name] - again[name]) <= 1e-6), name
     # a sample subset, variants shuffled and partly missing, in a second fileset
     f = np.load(lpath)
+    assert f["loadings"].shape == (nv, num_pc) and f["eigenvalues"].shape == (num_pc,)
     rng = np.random.default_rng(3)
     subset = np.sort(rng.choice(n, 120, replace=False))
     cols = rng.permutation(nv)[: nv - 400]

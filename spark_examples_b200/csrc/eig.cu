@@ -65,26 +65,49 @@ __global__ void rowsum_kernel(const int32_t* __restrict__ S, int n, double* __re
     if (lane == 0) rowsum[row] = (double)acc;
 }
 
-// scal[0] = matrixMean (:211), nz = rowSums.filter(_ > 0).size (:207)
+// Round to nearest even of a 128-bit integer: shift it below 2^63, folding the bits shifted out into bit 0 (a sticky bit
+// far below the rounding position of the 53-bit significand), convert once and scale back by the exact power of two.
+__device__ double i128_to_double_rn(__int128 x) {
+    const bool neg = x < 0;
+    unsigned __int128 m = neg ? (unsigned __int128)(-x) : (unsigned __int128)x;
+    int shift = 0;
+    while ((m >> 63) != 0) {
+        m = (m >> 1) | (m & 1);
+        ++shift;
+    }
+    const double d = scalbn(__ull2double_rn((unsigned long long)m), shift);
+    return neg ? -d : d;
+}
+
+// scal[0] = matrixMean (:211), nz = rowSums.filter(_ > 0).size (:207).
+// The reference adds the row sums as doubles (`reduce(_ + _)`, :210); once their total passes 2^53 (at N = 65 535 from a
+// mean count of about 2^21 shared variants on) that sum depends on the order of the additions.  Here they are added as
+// integers -- every row sum is an integer below 2^53, so converting it is exact -- in 128 bits, since N row sums can pass
+// 2^63 in the band path, and the total is rounded to a double once: matrixMean = RN(RN(RN(sum S) / N) / N), whatever
+// the order.
 __global__ void matrix_mean_kernel(const double* __restrict__ rowsum, int n, double* __restrict__ scal,
                                    int* __restrict__ nz) {
-    __shared__ double red[33];
+    __shared__ __int128 red[kSmallThreads];
     __shared__ int cnt;
     if (threadIdx.x == 0) cnt = 0;
     __syncthreads();
-    double acc = 0.0;
+    __int128 acc = 0;
     int c = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const double r = rowsum[i];
-        acc += r;   // exact: integer-valued partial sums below 2^53, so the order of `reduce(_ + _)` (:210) is immaterial
+        acc += (long long)r;
         c += (r > 0.0);
     }
-    const double tot = block_sum(acc, red);
+    red[threadIdx.x] = acc;
     atomicAdd(&cnt, c);
     __syncthreads();
+    for (int s = blockDim.x / 2; s > 0; s >>= 1) {   // blockDim.x is a power of two
+        if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+        __syncthreads();
+    }
     if (threadIdx.x == 0) {
         const double rc = (double)n;
-        scal[0] = __ddiv_rn(__ddiv_rn(tot, rc), rc);
+        scal[0] = __ddiv_rn(__ddiv_rn(i128_to_double_rn(red[0]), rc), rc);
         *nz = cnt;
     }
 }

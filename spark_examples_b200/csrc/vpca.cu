@@ -972,8 +972,8 @@ int vpca_commit(vpca_ctx* ctx, int64_t partition_id) {
             CUDA_OK(ctx, gram_add_owners(ctx->plan, s->d_S, ctx->n, ctx->stream));
         else if (ctx->plan.num_peers > 1)
             CUDA_OK(ctx, gram_add_peers(ctx->plan, s->d_S, (int64_t)ctx->n * ctx->n, ctx->stream));
-        else
-            CUDA_OK(ctx, gram_add(ctx->d_S, s->d_S, (int64_t)ctx->n * ctx->n, ctx->stream));
+        else   // an owner-computes band staged only its own rows, at the band Gram's own offsets
+            CUDA_OK(ctx, gram_add(ctx->d_S, s->d_S, (int64_t)ctx->band_rows * ctx->n, ctx->stream));
         CUDA_OK(ctx, cudaEventRecord(s->ev_free, ctx->stream));
         ctx->c_launches += 1;
     }
@@ -1771,7 +1771,8 @@ int vpca_owner_row_bands(int32_t n_samples, int32_t world, int32_t* row_end) {
     for (int q = 0; q < world; ++q) {
         int end = (q + 1 == world) ? n : (int)(std::sqrt((double)(q + 1) / world) * n / 32.0 + 0.5) * 32;
         end = std::max(end, prev + 32);
-        if (q + 1 < world) end = std::min(end, n - 32 * (world - 1 - q));
+        // leave 32 rows for each later band without leaving the multiples of 32 (n itself need not be one)
+        if (q + 1 < world) end = std::min(end, (n / 32) * 32 - 32 * (world - 1 - q));
         row_end[q] = end;
         prev = end;
     }

@@ -247,7 +247,12 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
  * repeated calls on the same bands give the same bits.  There is no direct-solver fallback (it would need the N x N
  * matrix): breakdown (e.g. a zero Gram), no convergence within the step budget (VPCA_EIG_MAXIT) or an eigenvalue missed
  * by a single Krylov sequence returns VPCA_ERR_UNSUPPORTED, with the reason in vpca_last_error(ctxs[0]).  ctxs[0]'s
- * vpca_stats report the solve (eig_method 4).  Driver-side: no accumulation may be in flight in any of the contexts. */
+ * vpca_stats report the solve (eig_method 4).  Driver-side: no accumulation may be in flight in any of the contexts.
+ * On success every context in ctxs holds U (N x k, FP64, column-major) and the k eigenvalues on its own device for the
+ * loadings below, as after vpca_compute_pca: ctxs[0] reads its solver's vectors, every other context gets a copy of the
+ * first min(k, 16) columns in a buffer of N x 16 doubles it allocates on the first such solve (cudaMemcpyPeerAsync after
+ * the solve, also between contexts on one device).  The call clears U on every context it names before it starts, so a
+ * failed solve leaves no vectors behind; the most recent successful vpca_compute_pca / _bands of a context wins. */
 int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, double* vecs, double* evals,
                            int32_t* non_zero_rows);
 /* The centered matrix itself (row-major N x N doubles) for parity tests of :199-223. */
@@ -266,18 +271,27 @@ int vpca_get_tridiagonal(vpca_ctx* ctx, double* diag, double* offdiag);
  * no floating-point atomics, so results are bitwise reproducible.  w[v] depends on column v only: the three input forms
  * give the same bits.  Driver-side calls: one at a time per context, never concurrent with accumulation.
  *
- * After vpca_compute_pca(ctx, k, ...) U and the eigenvalues stay on the device until the next vpca_reset / vpca_set_gram /
- * vpca_load_partial_gram / vpca_finalize_gram (VPCA_ERR_STATE after that).  Loadings of k' <= k components, k' in [1, 16]:
+ * After vpca_compute_pca(ctx, k, ...), or a vpca_compute_pca_bands(..., k, ...) that named ctx, U and the eigenvalues stay
+ * on the device until the next vpca_reset / vpca_set_gram / vpca_load_partial_gram / vpca_finalize_gram of this context or
+ * the next band solve that names it; the most recent successful solve wins.  Without them: VPCA_ERR_STATE on a context
+ * that stores the whole Gram, VPCA_ERR_UNSUPPORTED on a band-only one (never solved, reset, or named by a failed band
+ * solve).  A band-only context with U from a band solve computes loadings of any variants, whatever rows it stores; its
+ * host forms run on the staging lanes it has for staged partitions.  Loadings of k' <= k components, k' in [1, 16]:
  *   out_w[v * k' + c] = sum_s x[s][v] * U[s][c] (FP64), out_count[v] = sum_s x[s][v] (exact).  Rows without carriers are
- *   legal (w = 0).  VPCA_ERR_INDEX_OUT_OF_RANGE for a sample index >= n_samples; VPCA_ERR_UNSUPPORTED on a band-only
- *   context.  _panels: device input in the layout of vpca_accumulate_panels, device outputs, ordered on the ctx stream. */
+ *   legal (w = 0).  VPCA_ERR_INDEX_OUT_OF_RANGE for a sample index >= n_samples.  _panels: device input in the layout of
+ *   vpca_accumulate_panels, device outputs, ordered on the ctx stream.
+ * Up to 65 535 samples a thread sums each variant over all samples in order; above, the samples are cut into 4 ranges
+ * whose bounds depend on n_samples alone and the 4 partials are added in range order.  Either way w[v] depends on column
+ * v, U and n_samples only: every rank, input form and panel width gives it the same bits.  (Diagnostic:
+ * VPCA_LOADINGS_KERNEL=whole|split forces one of the two orders at any n_samples.) */
 int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const int32_t* sample_idx, int64_t nv,
                         double* out_w, int32_t* out_count);
 int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
                       double* out_w, int32_t* out_count);
 int vpca_loadings_panels(vpca_ctx* ctx, int32_t k, const void* d_x, int64_t nv, int64_t panel_variants,
                          double* d_w, int32_t* d_count);
-/* Projection, in a context whose n_samples is the NEW cohort's size M (its Gram is unused).  vpca_project_begin zeroes
+/* Projection, in a context whose n_samples is the NEW cohort's size M (its Gram is unused; a band-only context is refused
+ * with VPCA_ERR_UNSUPPORTED, so a cohort placed on the axes of a band solve is projected in an ordinary context).  vpca_project_begin zeroes
  * the M x k FP64 accumulator (k in [1, 16]); vpca_reset drops it.  Every row passed is a variant of the new cohort,
  * aligned with w (nv x k, variant-major, as vpca_loadings_* wrote it) and mean (nv, n_v / N of the reference): rows with
  * no carriers still contribute -mean * w.  Successive calls add up (per call in variant order; across calls in call

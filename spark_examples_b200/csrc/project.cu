@@ -11,6 +11,9 @@
 //   loadings_kernel: a thread owns VT adjacent variants of a panel and walks ALL samples in order 0 .. N-1; U goes
 //     through shared memory in sample tiles.  w[v] depends on column v alone, so it is the same bits whichever path
 //     (CSR, .bed, panels) staged the cells and whatever the panel width.
+//   above kSplitMinN samples the sum is cut into kRanges fixed ranges whose bounds depend on N alone, the range sums
+//     added in range order: loadings_split_kernel (k <= 8) gives each range its own warps, loadings_ranged_kernel
+//     (k > 8) walks the ranges one after another in each thread.  w[v] is still a function of column v, U and N only.
 //   project_kernel: a thread owns one sample and walks the variants of one panel in order; the panel's slice of w and of
 //     the means goes through shared memory in variant tiles.  Each panel leaves a partial sum per (sample, component);
 //     project_reduce_kernel adds the partials into the accumulator in panel order.
@@ -19,6 +22,8 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <cstdlib>
+#include <cstring>
 
 #include "vpca_internal.h"
 
@@ -55,13 +60,39 @@ __device__ __forceinline__ uint64_t load_word(const uint8_t* p) {
 }
 
 // ---- loadings ------------------------------------------------------------------------------------------------------
+// acc[i][c] += x[s][v0 + i] U[s][c] and cnt[i] += x[s][v0 + i] for the ts sample rows of a tile, in order, from the
+// thread's cells `r` (row_bytes apart) and the tile's U in shared memory (su[s * KMAX + c]).
+template <int BITS, int KMAX, int VT>
+__device__ __forceinline__ void sum_tile(const uint8_t* r, int64_t row_bytes, const double* su, int ts,
+                                         double (&acc)[VT][KMAX], int (&cnt)[VT]) {
+    constexpr int WB = VT * BITS / 8; // bytes of my VT cells in one sample row
+#pragma unroll 8
+    for (int s = 0; s < ts; ++s) {
+        const uint64_t word = load_word<WB>(r + (int64_t)s * row_bytes);
+        double u[KMAX];
+#pragma unroll
+        for (int c = 0; c < KMAX; c += 2) {
+            const double2 uu = *reinterpret_cast<const double2*>(&su[s * KMAX + c]);
+            u[c] = uu.x;
+            u[c + 1] = uu.y;
+        }
+#pragma unroll
+        for (int i = 0; i < VT; ++i) {
+            const int m = cell_value<BITS>(word, i);
+            cnt[i] += m;
+            const double d = int_to_f64(m);
+#pragma unroll
+            for (int c = 0; c < KMAX; ++c) acc[i][c] = fma(d, u[c], acc[i][c]);
+        }
+    }
+}
+
 // grid (panels, ceil(P / (kThreads * VT))).  U: n x k column-major (ld n).  w: nv x k variant-major, count: nv.
 template <int BITS, int KMAX, int VT>
 __global__ void __launch_bounds__(kThreads) loadings_kernel(const uint8_t* __restrict__ x, int n, int64_t nv,
                                                             int64_t panel, const double* __restrict__ U, int k,
                                                             double* __restrict__ w, int32_t* __restrict__ count) {
     constexpr int TS = 4096 / KMAX;   // samples of U per shared-memory tile (32 KB)
-    constexpr int WB = VT * BITS / 8; // bytes of my VT cells in one sample row
     __shared__ __align__(16) double su[TS * KMAX];
     const int64_t p = blockIdx.x;
     const int64_t vloc = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * VT;
@@ -86,28 +117,160 @@ __global__ void __launch_bounds__(kThreads) loadings_kernel(const uint8_t* __res
         }
         __syncthreads();
         if (!active) continue;
-        const uint8_t* r = col + (int64_t)s0 * row_bytes;
-#pragma unroll 8
-        for (int s = 0; s < ts; ++s) {
-            const uint64_t word = load_word<WB>(r + (int64_t)s * row_bytes);
-            double u[KMAX];
+        sum_tile<BITS, KMAX, VT>(col + (int64_t)s0 * row_bytes, row_bytes, su, ts, acc, cnt);
+    }
+    if (!active) return;
 #pragma unroll
-            for (int c = 0; c < KMAX; c += 2) {
-                const double2 uu = *reinterpret_cast<const double2*>(&su[s * KMAX + c]);
-                u[c] = uu.x;
-                u[c + 1] = uu.y;
+    for (int i = 0; i < VT; ++i) {
+        const int64_t v = vg + i;
+        if (v >= nv) break;
+        count[v] = cnt[i];
+#pragma unroll
+        for (int c = 0; c < KMAX; ++c)
+            if (c < k) w[v * k + c] = acc[i][c];
+    }
+}
+
+// Above kSplitMinN samples the sum over the samples is cut into kRanges ranges of `span` samples (the last one shorter),
+// span = round_up(ceil(n / kRanges), 32), each summed in order from zero, and the range partials are added in range
+// order: w = ((p_0 + p_1) + p_2) + p_3.  The bounds and the order depend on n alone -- not on nv, the panel width, the
+// input form or k -- so every path gives w[v] the same bits.  Two kernels sum in this order:
+//   loadings_ranged_kernel: loadings_kernel's grid, each thread summing the ranges one after another (a second set of
+//     accumulators); used at KMAX 16, where 2 variants per thread already give enough CTAs;
+//   loadings_split_kernel (below): the ranges side by side in the warps of a CTA, for KMAX <= 8.
+constexpr int kRanges = 4;
+
+__host__ __device__ inline int split_span(int n) { return ((n + kRanges - 1) / kRanges + 31) / 32 * 32; }
+
+template <int BITS, int KMAX, int VT>
+__global__ void __launch_bounds__(kThreads) loadings_ranged_kernel(const uint8_t* __restrict__ x, int n, int64_t nv,
+                                                                   int64_t panel, const double* __restrict__ U, int k,
+                                                                   double* __restrict__ w, int32_t* __restrict__ count) {
+    constexpr int TS = 4096 / KMAX;
+    __shared__ __align__(16) double su[TS * KMAX];
+    const int64_t p = blockIdx.x;
+    const int64_t vloc = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * VT;
+    const int64_t vg = p * panel + vloc;
+    const bool active = vloc < panel && vg < nv;
+    const int64_t row_bytes = panel * BITS / 8;
+    const uint8_t* col = x + (p * (int64_t)n * panel + vloc) * BITS / 8;
+    const int span = split_span(n);
+    double acc[VT][KMAX];   // the sum of the running range
+    double tot[VT][KMAX];   // the sum of the ranges so far
+    int cnt[VT];
+#pragma unroll
+    for (int i = 0; i < VT; ++i) cnt[i] = 0;
+#pragma unroll 1
+    for (int jr = 0; jr < kRanges; ++jr) {
+        const int lo = min(n, jr * span), hi = min(n, (jr + 1) * span);
+#pragma unroll
+        for (int i = 0; i < VT; ++i)
+#pragma unroll
+            for (int c = 0; c < KMAX; ++c) acc[i][c] = 0.0;
+        for (int s0 = lo; s0 < hi; s0 += TS) {
+            const int ts = min(TS, hi - s0);
+            __syncthreads();
+            for (int q = threadIdx.x; q < ts * KMAX; q += kThreads) {
+                const int s = q / KMAX, c = q - s * KMAX;
+                su[q] = c < k ? U[(int64_t)c * n + s0 + s] : 0.0;
             }
+            __syncthreads();
+            if (active) sum_tile<BITS, KMAX, VT>(col + (int64_t)s0 * row_bytes, row_bytes, su, ts, acc, cnt);
+        }
+#pragma unroll
+        for (int i = 0; i < VT; ++i)
+#pragma unroll
+            for (int c = 0; c < KMAX; ++c) tot[i][c] = jr == 0 ? acc[i][c] : tot[i][c] + acc[i][c];
+    }
+    if (!active) return;
+#pragma unroll
+    for (int i = 0; i < VT; ++i) {
+        const int64_t v = vg + i;
+        if (v >= nv) break;
+        count[v] = cnt[i];
+#pragma unroll
+        for (int c = 0; c < KMAX; ++c)
+            if (c < k) w[v * k + c] = tot[i][c];
+    }
+}
+
+// ---- loadings, sample axis split across warps ----------------------------------------------------------------------
+// The range order of loadings_ranged_kernel, with the ranges side by side: a CTA is G x kRanges warps, warp (group g,
+// range j) owns the VT adjacent variants of lane l of group g and sums range j in order; the range partials are then
+// added in shared memory, range by range.  The grid has kRanges times the warps of loadings_kernel's for the same
+// variants, which is what keeps enough loads in flight when few variants meet many samples.
+// G (variant groups per CTA) only decides which variants a CTA covers, never an order: 2 at KMAX 2 (half the re-reads of
+// U per variant); 1 at KMAX 4 and 8, where the accumulators take up to ~200 registers and two CTAs per SM hide each
+// other's tile barriers.
+__host__ __device__ constexpr int split_groups(int kmax) { return kmax <= 2 ? 2 : 1; }
+
+// grid (panels, ceil(P / (32 * G * VT))), 32 * kRanges * G threads.  Arguments as for loadings_kernel.
+template <int BITS, int KMAX, int VT>
+__global__ void __launch_bounds__(32 * kRanges * split_groups(KMAX), 2)
+    loadings_split_kernel(const uint8_t* __restrict__ x, int n, int64_t nv, int64_t panel, const double* __restrict__ U,
+                          int k, double* __restrict__ w, int32_t* __restrict__ count) {
+    constexpr int G = split_groups(KMAX);
+    constexpr int NT = 32 * kRanges * G;
+    constexpr int TS = 1024 / KMAX;    // samples of U per range and tile (kRanges tiles: 32 KB)
+    constexpr int R = VT * KMAX;       // partial sums per thread
+    __shared__ __align__(16) double su[kRanges * TS * KMAX];   // later: the range partials, G x R x 32
+    __shared__ int scnt[G * VT * 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int g = warp % G, j = warp / G;
+    const int span = split_span(n);
+    const int lo = min(n, j * span), hi = min(n, (j + 1) * span);
+    const int64_t p = blockIdx.x;
+    const int64_t vloc = (((int64_t)blockIdx.y * G + g) * 32 + lane) * VT;
+    const int64_t vg = p * panel + vloc;
+    const bool active = vloc < panel && vg < nv;
+    const int64_t row_bytes = panel * BITS / 8;
+    const uint8_t* col = x + (p * (int64_t)n * panel + vloc) * BITS / 8;
+    double acc[VT][KMAX];
+    int cnt[VT];
+#pragma unroll
+    for (int i = 0; i < VT; ++i) {
+        cnt[i] = 0;
+#pragma unroll
+        for (int c = 0; c < KMAX; ++c) acc[i][c] = 0.0;
+    }
+    for (int t0 = 0; t0 < span; t0 += TS) {   // every warp takes the same number of tiles: the barriers line up
+        __syncthreads();
+        for (int q = threadIdx.x; q < kRanges * TS * KMAX; q += NT) {
+            const int jr = q / (TS * KMAX), rem = q - jr * (TS * KMAX);
+            const int s = rem / KMAX, c = rem - s * KMAX;
+            const int sg = jr * span + t0 + s;
+            su[q] = (c < k && t0 + s < span && sg < n) ? U[(int64_t)c * n + sg] : 0.0;
+        }
+        __syncthreads();
+        const int s0 = lo + t0;
+        const int ts = min(TS, hi - s0);
+        if (!active || ts <= 0) continue;
+        sum_tile<BITS, KMAX, VT>(col + (int64_t)s0 * row_bytes, row_bytes, su + j * TS * KMAX, ts, acc, cnt);
+    }
+    // range partials, added in range order; lanes are the fastest index, so the shared accesses do not conflict
+    double* red = su + g * R * 32 + lane;
+    int* rc = scnt + g * VT * 32 + lane;
+#pragma unroll 1
+    for (int jr = 0; jr < kRanges; ++jr) {
+        __syncthreads();
+        if (j != jr) continue;
+#pragma unroll
+        for (int i = 0; i < VT; ++i) {
+            if (jr > 0) cnt[i] += rc[i * 32];
+#pragma unroll
+            for (int c = 0; c < KMAX; ++c)
+                if (jr > 0) acc[i][c] = red[(i * KMAX + c) * 32] + acc[i][c];
+        }
+        if (jr < kRanges - 1) {
 #pragma unroll
             for (int i = 0; i < VT; ++i) {
-                const int m = cell_value<BITS>(word, i);
-                cnt[i] += m;
-                const double d = int_to_f64(m);
+                rc[i * 32] = cnt[i];
 #pragma unroll
-                for (int c = 0; c < KMAX; ++c) acc[i][c] = fma(d, u[c], acc[i][c]);
+                for (int c = 0; c < KMAX; ++c) red[(i * KMAX + c) * 32] = acc[i][c];
             }
         }
     }
-    if (!active) return;
+    if (j != kRanges - 1 || !active) return;
 #pragma unroll
     for (int i = 0; i < VT; ++i) {
         const int64_t v = vg + i;
@@ -195,12 +358,25 @@ int kmax_for(int k) { return k <= 2 ? 2 : k <= 4 ? 4 : k <= 8 ? 8 : 16; }
 
 template <int BITS, int KMAX>
 void launch_loadings(const void* d_x, int n, int64_t nv, int64_t panel, const double* d_U, int k, double* d_w,
-                     int32_t* d_count, cudaStream_t stream) {
+                     int32_t* d_count, bool split, cudaStream_t stream) {
     constexpr int VT = KMAX >= 16 ? 2 : 4;
     const int64_t npanels = (nv + panel - 1) / panel;
+    const uint8_t* x = static_cast<const uint8_t*>(d_x);
     const dim3 grid((unsigned)npanels, (unsigned)((panel + kThreads * VT - 1) / (kThreads * VT)));
-    loadings_kernel<BITS, KMAX, VT><<<grid, kThreads, 0, stream>>>(static_cast<const uint8_t*>(d_x), n, nv, panel, d_U, k,
-                                                                   d_w, d_count);
+    if constexpr (KMAX >= 16) {
+        // 2 variants per thread leave enough CTAs already; the warp split would re-read U 4 x as often
+        if (split) {
+            loadings_ranged_kernel<BITS, KMAX, VT><<<grid, kThreads, 0, stream>>>(x, n, nv, panel, d_U, k, d_w, d_count);
+            return;
+        }
+    } else if (split) {
+        constexpr int G = split_groups(KMAX);
+        constexpr int CV = 32 * G * VT;   // variants of one CTA
+        const dim3 sgrid((unsigned)npanels, (unsigned)((panel + CV - 1) / CV));
+        loadings_split_kernel<BITS, KMAX, VT><<<sgrid, 32 * kRanges * G, 0, stream>>>(x, n, nv, panel, d_U, k, d_w, d_count);
+        return;
+    }
+    loadings_kernel<BITS, KMAX, VT><<<grid, kThreads, 0, stream>>>(x, n, nv, panel, d_U, k, d_w, d_count);
 }
 
 template <int BITS, int KMAX>
@@ -216,12 +392,12 @@ void launch_project(const void* d_y, int m, int64_t nv, int64_t panel, const dou
 
 template <int BITS>
 void loadings_bits(const void* d_x, int n, int64_t nv, int64_t panel, const double* d_U, int k, double* d_w,
-                   int32_t* d_count, cudaStream_t stream) {
+                   int32_t* d_count, bool split, cudaStream_t stream) {
     switch (kmax_for(k)) {
-        case 2: launch_loadings<BITS, 2>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream); break;
-        case 4: launch_loadings<BITS, 4>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream); break;
-        case 8: launch_loadings<BITS, 8>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream); break;
-        default: launch_loadings<BITS, 16>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream); break;
+        case 2: launch_loadings<BITS, 2>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
+        case 4: launch_loadings<BITS, 4>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
+        case 8: launch_loadings<BITS, 8>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
+        default: launch_loadings<BITS, 16>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
     }
 }
 
@@ -241,9 +417,16 @@ void project_bits(const void* d_y, int m, int64_t nv, int64_t panel, const doubl
 cudaError_t loadings_launch(const void* d_x, int elem_bits, int n, int64_t nv, int64_t panel, const double* d_U, int k,
                             double* d_w, int32_t* d_count, cudaStream_t stream) {
     if (nv <= 0) return cudaSuccess;
-    if (elem_bits == 8) loadings_bits<8>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream);
-    else if (elem_bits == 16) loadings_bits<16>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream);
-    else loadings_bits<4>(d_x, n, nv, panel, d_U, k, d_w, d_count, stream);
+    // VPCA_LOADINGS_KERNEL=whole|split forces one kernel (to time both at one N, or to test the split below the
+    // threshold); the default is the split above kSplitMinN samples
+    bool split = n > kSplitMinN;
+    if (const char* e = getenv("VPCA_LOADINGS_KERNEL")) {
+        if (strcmp(e, "whole") == 0) split = false;
+        else if (strcmp(e, "split") == 0) split = true;
+    }
+    if (elem_bits == 8) loadings_bits<8>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream);
+    else if (elem_bits == 16) loadings_bits<16>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream);
+    else loadings_bits<4>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream);
     return cudaGetLastError();
 }
 

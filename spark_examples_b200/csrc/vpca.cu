@@ -53,7 +53,10 @@ struct vpca_ctx {
     BandPart band_part;     // vpca_compute_pca_bands: this context's share of the sharded mat-vec
     JoinWork join;        // multi-dataset keying (join.cu); one join at a time (join_mu)
     std::mutex join_mu;
-    int pca_k = 0;        // k of the last vpca_compute_pca whose U / eigenvalues are still valid on the device (0: none)
+    int pca_k = 0;        // k of the last solve whose U / eigenvalues are still valid on the device (0: none)
+    const double* d_U = nullptr;     // that U (n x min(pca_k, 16), column-major): eig.d_evecs after vpca_compute_pca;
+                                     // band_eig.d_evecs or d_band_U after vpca_compute_pca_bands
+    double* d_band_U = nullptr;      // n x 16: this rank's copy of U from a band solve driven by another context
     int proj_k = 0;       // k of the projection begun by vpca_project_begin (0: none in progress)
     double* d_proj_acc = nullptr;    // n x kProjLd partial projection sums (project.cu)
     double* d_proj_part = nullptr;   // per-panel partial sums of one launch
@@ -642,7 +645,7 @@ int vpca_destroy(vpca_ctx* ctx) {
     band_eig_free(ctx->band_eig);
     band_part_free(ctx->band_part);
     for (void* p : {(void*)ctx->d_proj_acc, (void*)ctx->d_proj_part, (void*)ctx->d_lp_w, (void*)ctx->d_lp_mean,
-                    (void*)ctx->d_lp_count})
+                    (void*)ctx->d_lp_count, (void*)ctx->d_band_U})
         cudaFree(p);
     join_free(ctx->join);
     gram_plan_free(ctx->plan);
@@ -1261,6 +1264,7 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
     ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
     ctx->pca_done = true;
     ctx->pca_k = k;
+    ctx->d_U = ctx->eig.d_evecs;
     return VPCA_OK;
 }
 
@@ -1324,6 +1328,7 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
     std::vector<std::unique_lock<std::mutex>> locks;   // rank order
     locks.reserve(world);
     for (int r = 0; r < world; ++r) locks.emplace_back(ctxs[r]->mu);
+    for (int r = 0; r < world; ++r) ctxs[r]->pca_k = 0;   // a failed solve leaves no U behind, never a stale one
     BandPart* parts[16];
     for (int r = 0; r < world; ++r) {
         vpca_ctx* c = ctxs[r];
@@ -1367,9 +1372,35 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
     if (evals) CUDA_OK(c0, cudaMemcpyAsync(evals, c0->band_eig.d_evals, k * sizeof(double), cudaMemcpyDeviceToHost, c0->stream));
     int nz = 0;
     CUDA_OK(c0, cudaMemcpyAsync(&nz, c0->band_eig.d_nz, sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
+    // U for the loadings on every rank: rank 0 reads its solver's vectors, every other rank gets a copy of the first
+    // min(k, 16) columns on its own device, in stream order after the solve (ev_e1), as v_j travels during it
+    const int kc = std::min(k, 16);
+    for (int r = 1; r < world; ++r) {
+        vpca_ctx* c = ctxs[r];
+        CUDA_OK(c0, cudaSetDevice(c->cfg.device));
+        if (c->d_band_U == nullptr) {
+            const cudaError_t ae = cudaMalloc(&c->d_band_U, (size_t)n * 16 * sizeof(double));
+            if (ae != cudaSuccess) {
+                c->d_band_U = nullptr;
+                return fail(c0, VPCA_ERR_NOMEM, "ctxs[%d]: U for the loadings: %s", r, cudaGetErrorString(ae));
+            }
+        }
+        CUDA_OK(c0, cudaStreamWaitEvent(c->stream, c0->ev_e1, 0));
+        CUDA_OK(c0, cudaMemcpyPeerAsync(c->d_band_U, c->cfg.device, c0->band_eig.d_evecs, c0->cfg.device,
+                                        (size_t)n * kc * sizeof(double), c->stream));
+    }
+    for (int r = 1; r < world; ++r) {   // the source is rank 0's solver state, which the next solve overwrites
+        CUDA_OK(c0, cudaSetDevice(ctxs[r]->cfg.device));
+        CUDA_OK(c0, cudaStreamSynchronize(ctxs[r]->stream));
+    }
+    CUDA_OK(c0, cudaSetDevice(c0->cfg.device));
     CUDA_OK(c0, cudaStreamSynchronize(c0->stream));
     if (non_zero_rows) *non_zero_rows = nz;
     c0->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
+    for (int r = 0; r < world; ++r) {
+        ctxs[r]->pca_k = k;
+        ctxs[r]->d_U = r == 0 ? c0->band_eig.d_evecs : ctxs[r]->d_band_U;
+    }
     return VPCA_OK;
 }
 
@@ -1378,14 +1409,17 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
 // the context's own; host-input calls run on a staging lane (encode as for the Gram), panel calls on the ctx stream.
 static constexpr int kProjLd = 16;   // row pitch (doubles) of the projection accumulator
 
-static int loadings_check(vpca_ctx* ctx, int32_t k) {   // caller holds ctx->mu
-    if (ctx->band_rows != ctx->n)
-        return fail(ctx, VPCA_ERR_UNSUPPORTED, "loadings need the eigenvectors of the whole Gram; this context stores a row band");
+// On success *U is the U the loadings read (valid until the next solve, reset or Gram change of this context).
+static int loadings_check(vpca_ctx* ctx, int32_t k, const double** U) {   // caller holds ctx->mu
+    if (ctx->band_rows != ctx->n && ctx->pca_k == 0)
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "loadings on a context that stores a row band need the eigenvectors of a "
+                    "successful vpca_compute_pca_bands that named it, since its last reset / finalize_gram");
     if (k < 1 || k > 16) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings: k=%d out of range [1, 16]", k);
     if (ctx->pca_k == 0)
-        return fail(ctx, VPCA_ERR_STATE, "loadings need a vpca_compute_pca since the last reset / set_gram / "
-                    "load_partial_gram / finalize_gram");
-    if (k > ctx->pca_k) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings of %d components, vpca_compute_pca computed %d", k, ctx->pca_k);
+        return fail(ctx, VPCA_ERR_STATE, "loadings need a vpca_compute_pca or vpca_compute_pca_bands since the last reset / "
+                    "set_gram / load_partial_gram / finalize_gram");
+    if (k > ctx->pca_k) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings of %d components, the last solve computed %d", k, ctx->pca_k);
+    *U = ctx->d_U;
     return VPCA_OK;
 }
 
@@ -1408,9 +1442,9 @@ static int project_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int
     return VPCA_OK;
 }
 
-static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, int k, double* out_w,
-                          int32_t* out_count) {
-    CUDA_OK(ctx, loadings_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, ctx->eig.d_evecs, k, ctx->d_lp_w,
+static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, const double* U, int k,
+                          double* out_w, int32_t* out_count) {
+    CUDA_OK(ctx, loadings_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, U, k, ctx->d_lp_w,
                                  ctx->d_lp_count, L.stream));
     CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_lp_w, (size_t)nvc * k * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
     CUDA_OK(ctx, cudaMemcpyAsync(out_count + v, ctx->d_lp_count, (size_t)nvc * sizeof(int32_t), cudaMemcpyDeviceToHost, L.stream));
@@ -1438,9 +1472,10 @@ int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const 
     if (offsets == nullptr || nv < 0 || (nv > 0 && (out_w == nullptr || out_count == nullptr)) ||
         (nv > 0 && sample_idx == nullptr && offsets[nv] > offsets[0]))
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_calls: bad argument");
+    const double* U = nullptr;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
-        int rc = loadings_check(ctx, k);
+        int rc = loadings_check(ctx, k, &U);
         if (rc != VPCA_OK) return rc;
     }
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
@@ -1450,7 +1485,7 @@ int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const 
     int rc = lp_buffers(ctx, k, false);
     if (rc != VPCA_OK) return rc;
     auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) {
-        return loadings_chunk(ctx, L, b, v, nvc, k, out_w, out_count);
+        return loadings_chunk(ctx, L, b, v, nvc, U, k, out_w, out_count);
     };
     return process_calls(ctx, *lg.lane, offsets, sample_idx, 4, nv, consume, false);
 }
@@ -1462,9 +1497,10 @@ int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv,
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: counted_allele must be 1 (A1) or 2 (A2)");
     if (nv < 0 || (nv > 0 && (rows == nullptr || out_w == nullptr || out_count == nullptr)) || stride_bytes < (ctx->n + 3) / 4)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    const double* U = nullptr;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
-        int rc = loadings_check(ctx, k);
+        int rc = loadings_check(ctx, k, &U);
         if (rc != VPCA_OK) return rc;
     }
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
@@ -1474,7 +1510,7 @@ int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv,
     int rc = lp_buffers(ctx, k, false);
     if (rc != VPCA_OK) return rc;
     auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) {
-        return loadings_chunk(ctx, L, b, v, nvc, k, out_w, out_count);
+        return loadings_chunk(ctx, L, b, v, nvc, U, k, out_w, out_count);
     };
     return process_packed(ctx, *lg.lane, rows, nv, stride_bytes, counted_allele, consume);
 }
@@ -1483,13 +1519,14 @@ int vpca_loadings_panels(vpca_ctx* ctx, int32_t k, const void* d_x, int64_t nv, 
                          int32_t* d_count) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    int rc = loadings_check(ctx, k);
+    const double* U = nullptr;
+    int rc = loadings_check(ctx, k, &U);
     if (rc != VPCA_OK) return rc;
     if (d_x == nullptr || nv < 0 || panel_variants < 128 || (panel_variants % 128) != 0 || (nv > 0 && (d_w == nullptr || d_count == nullptr)))
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_panels: panel_variants must be a positive multiple of 128");
     if ((reinterpret_cast<uintptr_t>(d_x) & 31) != 0) return fail(ctx, VPCA_ERR_BAD_ARG, "panels must be 32-byte aligned");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    CUDA_OK(ctx, loadings_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, ctx->eig.d_evecs, k, d_w, d_count, ctx->stream));
+    CUDA_OK(ctx, loadings_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, U, k, d_w, d_count, ctx->stream));
     ctx->c_launches += nv > 0 ? 1 : 0;
     return VPCA_OK;
 }

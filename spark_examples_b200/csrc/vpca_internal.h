@@ -223,7 +223,9 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
 // ---- variant loadings and projection (project.cu) -----------------------------------------------------------------
 // Both read cells in the panel layout (see gram_accumulate; zero cells after nv in the last panel), k in [1, 16].
 // w[v * k + c] = sum_s x[s][v] U[s][c] (FP64, samples summed in order), count[v] = sum_s x[s][v] (exact) for v < nv;
-// U: n x k column-major (ld n).  Never synchronises.
+// U: n x k column-major (ld n).  Never synchronises.  Above kSplitMinN samples the samples are summed in 4 ranges whose
+// bounds depend on n alone, the range sums added in range order (project.cu): w[v] still depends on n, column v and U only.
+constexpr int kSplitMinN = 65535;
 cudaError_t loadings_launch(const void* d_x, int elem_bits, int n, int64_t nv, int64_t panel, const double* d_U, int k,
                             double* d_w, int32_t* d_count, cudaStream_t stream);
 // acc[s * acc_ld + c] += sum_v (y[s][v] - mean[v]) w[v * k + c] for the m samples: a partial sum per panel (variants in

@@ -595,8 +595,11 @@ class NativePca:
 
     # -- variant loadings and projection onto computed principal coordinates (vpca.h, DESIGN.md 6) --------------------
     def loadingsCalls(self, k: int, offsets, sample_idx):
-        """After computePca(k0 >= k): (w (nv, k) float64, count (nv,) int32) with w[v, c] = sum_s x[s][v] U[s, c] and
-        count[v] = sum_s x[s][v] for the CSR rows given (rows without carriers allowed)."""
+        """After computePca(k0 >= k), or a computePcaBands(..., k0 >= k) that named this context (band-only contexts
+        included; the most recent solve wins): (w (nv, k) float64, count (nv,) int32) with w[v, c] = sum_s x[s][v] U[s, c]
+        and count[v] = sum_s x[s][v] for the CSR rows given (rows without carriers allowed).  Without a valid U:
+        VPCA_ERR_STATE on a full context, VPCA_ERR_UNSUPPORTED on a band-only one.  Above 65 535 samples the samples are
+        summed in 4 fixed ranges (vpca.h); w[v] depends on column v, U and N only, whatever the input form."""
         off, idx = self._csr(offsets, sample_idx)
         nv = len(off) - 1
         w = np.zeros((max(nv, 1), int(k)), dtype=np.float64)
@@ -606,7 +609,7 @@ class NativePca:
         return w[:nv], cnt[:nv]
 
     def loadingsBed(self, k: int, rows: np.ndarray, counted_allele: int = 1):
-        """Same for PLINK .bed rows (see accumulateBed)."""
+        """Same for PLINK .bed rows (see accumulateBed), with the same U and the same bits."""
         b = np.ascontiguousarray(rows, dtype=np.uint8)
         if b.ndim != 2:
             raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
@@ -617,7 +620,8 @@ class NativePca:
         return w[:b.shape[0]], cnt[:b.shape[0]]
 
     def loadingsPanels(self, k: int, d_ptr: int, nv: int, panel_variants: int, d_w: int, d_count: int):
-        """Device panels in, device outputs (nv x k float64, nv int32), ordered on the context's stream."""
+        """Device panels in, device outputs (nv x k float64, nv int32), ordered on the context's stream; U as for
+        loadingsCalls, and the same bits whatever the panel width."""
         self._check(self._lib.vpca_loadings_panels(self._h, int(k), d_ptr, int(nv), int(panel_variants), d_w, d_count))
 
     def projectBegin(self, k: int):
@@ -738,7 +742,9 @@ def computePcaBands(contexts, k: int = 2):
     """Top-k principal coordinates of a Gram held as row bands by `contexts` (rank order, bands covering [0, N); a context
     that stores the whole Gram is the band [0, N)) -> (vecs (N, k), evals (k,), nonZeroRows), like NativePca.computePca
     but with no 65 535-sample limit and no N x N workspace (vpca_compute_pca_bands).  Failures of the solver raise
-    VpcaError with code VPCA_ERR_UNSUPPORTED; there is no fallback."""
+    VpcaError with code VPCA_ERR_UNSUPPORTED; there is no fallback.  On success every context holds U (the first
+    min(k, 16) columns) and the eigenvalues on its own device, so each rank can call loadings* on its variants; the call
+    clears U on every context first, so after a failed solve they have none."""
     L = load_library()
     if not contexts:
         raise VpcaError(VPCA_ERR_BAD_ARG, "at least one context")

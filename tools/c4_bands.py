@@ -18,6 +18,10 @@ mat-vec sharded over the band contexts; no replica of S, no N x N FP64 matrix, n
 `pca_ms` (host clock around the call, which synchronises), `lanczos_steps`, and checks computed from the genotype shards,
 not from S: the residual ||J X X^T J u_c - lambda_c u_c|| / lambda_1 of every pair in FP64 (panel by panel), and the
 orthonormality of U.
+`--loadings` (with --pca) then has every rank compute the variant loadings w = X^T U of the variants it holds
+(vpca_loadings_panels on its band-only context, which holds U after the band solve; owner-computes ranks split the panels
+between them), timed with CUDA events per rank, checked against FP64 X^T U from the genotype shards, and projects 4096
+sampled reference samples in an ordinary 4096-sample context with those loadings: they must come back to their rows of U.
 
 `--gpus N` sets the number of band contexts (ranks); with fewer visible devices they share them round robin (8 band
 contexts on one H100 hold the 40 GB Gram of config 4, but not its 50 GB of genotypes as well: lower --variants there)."""
@@ -48,8 +52,12 @@ def main():
                          "traffic between GPUs at all; 50 GB of genotypes per GPU)")
     ap.add_argument("--pca", type=int, default=0, help="K > 0: also compute the top K principal coordinates from the bands "
                     "(vpca_compute_pca_bands) and check them against the genotype shards")
+    ap.add_argument("--loadings", action="store_true", help="with --pca: every rank computes the loadings of its variants; "
+                    "checked against FP64 X^T U, and 4096 sampled reference samples projected back onto U")
     ap.add_argument("--out", default="")
     args = ap.parse_args()
+    if args.loadings and args.pca <= 0:
+        ap.error("--loadings needs --pca K")
     world = args.gpus or torch.cuda.device_count()
     ndev = torch.cuda.device_count()
     devs = [r % ndev for r in range(world)]
@@ -169,7 +177,11 @@ def main():
         report["checks"] = {"diag_equals_carrier_counts": ok_diag, "sampled_rows_exact_vs_fp32_matmul": ok_rows,
                             "random_256_blocks_exact": ok_blocks, "rows_checked_per_band": args.check_rows + 2}
         if args.pca > 0:
-            report.update(principal_coordinates(args.pca, ctxs, bufs, devs, shard_devs, n, per, P))
+            pcs, vecs, evals = principal_coordinates(args.pca, ctxs, bufs, devs, shard_devs, n, per, P)
+            report.update(pcs)
+            if args.loadings:
+                report.update(loadings_and_projection(min(args.pca, 16), ctxs, bufs, devs, streams, computes, n, per, P,
+                                                      vecs, evals))
     finally:
         for c in ctxs:
             try:
@@ -221,6 +233,77 @@ def principal_coordinates(k, ctxs, bufs, devs, shard_devs, n, per, P):
     out["pca_checks"] = {"residual_over_lambda1": [float(x) for x in res], "residuals_below_1e-9": bool(np.all(res <= 1e-9)),
                          "max_abs_UtU_minus_I": orth, "orthonormal_to_1e-10": orth <= 1e-10,
                          "descending_eigenvalues": bool(np.all(np.diff(evals) <= 0))}
+    return out, vecs, evals
+
+
+def loadings_and_projection(k, ctxs, bufs, devs, streams, computes, n, per, P, vecs, evals, m=4096):
+    """Every rank's loadings of the variants it holds (owner-computes: panels split evenly between the ranks), the second
+    of two launches timed with CUDA events on the rank's stream; FP64 X^T U of the same panels as the reference; then m sampled reference samples
+    projected with the loadings in an ordinary m-sample context on device 0."""
+    world = len(ctxs)
+    npan = (per + P - 1) // P
+    # (buffer rank, first panel, end panel) of the variants each rank computes
+    if computes:
+        parts = [(r, r * npan // world, (r + 1) * npan // world) for r in range(world)]
+    else:
+        parts = [(r, 0, npan) for r in range(world)]
+    outs, ev = [], []
+    for r, c in enumerate(ctxs):
+        b, p0, p1 = parts[r]
+        nv = max(0, min(per, p1 * P) - p0 * P)
+        torch.cuda.set_device(devs[r])
+        dev = f"cuda:{devs[r]}"
+        w = torch.empty((max(nv, 1), k), dtype=torch.float64, device=dev)      # every row is written on the ctx stream
+        cnt = torch.empty(max(nv, 1), dtype=torch.int32, device=dev)
+        a, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        with torch.cuda.stream(streams[r]):
+            # one untimed launch first: the first launch of a kernel in a process also loads its module
+            c.loadingsPanels(k, bufs[b].data_ptr() + p0 * n * P, nv, P, w.data_ptr(), cnt.data_ptr())
+            a.record()
+            c.loadingsPanels(k, bufs[b].data_ptr() + p0 * n * P, nv, P, w.data_ptr(), cnt.data_ptr())
+            e.record()
+        outs.append((w[:nv], cnt[:nv], nv))
+        ev.append((a, e))
+    for c in ctxs:
+        c.synchronize()
+    ms = [a.elapsed_time(e) for a, e in ev]
+    out = {"loadings_k": k, "loadings_ms_per_rank": [round(x, 2) for x in ms], "loadings_ms_job": round(max(ms), 2),
+           "loadings_variants_per_rank": [o[2] for o in outs]}
+    rel, counts_ok = 0.0, True
+    rng = np.random.default_rng(11)
+    pick = torch.from_numpy(np.sort(rng.choice(n, m, replace=False)))
+    torch.cuda.set_device(devs[0])
+    with native.NativePca(m, device=devs[0], max_multiplicity=1) as proj:
+        proj.projectBegin(k)
+        for r in range(world):
+            b, p0, p1 = parts[r]
+            w, cnt, nv = outs[r]
+            if nv == 0:
+                continue
+            torch.cuda.set_device(devs[b])
+            x = bufs[b].view(torch.int8)[: npan * n * P].view(npan, n, P)[p0:p1]
+            U = torch.from_numpy(np.ascontiguousarray(vecs[:, :k])).to(x.device)
+            want = torch.cat([x[q, :, b0:b0 + 1024].to(torch.float64).t() @ U                 # 1024 variants at a time
+                              for q in range(p1 - p0) for b0 in range(0, P, 1024)])[:nv]
+            cw = torch.cat([(x[q] != 0).sum(dim=0) for q in range(p1 - p0)])[:nv]
+            got = w.to(want.device)
+            rel = max(rel, float(((got - want).abs().amax(dim=0) / want.abs().amax(dim=0)).max()))
+            counts_ok = counts_ok and bool(torch.equal(cnt.to(cw.device).to(torch.int64), cw.to(torch.int64)))
+            y = x[:, pick.to(x.device), :].contiguous().to("cuda:%d" % devs[0])     # the sampled rows, same panels
+            torch.cuda.set_device(devs[0])
+            wy = got.to(y.device).contiguous()
+            mean = (cnt.to(y.device).to(torch.float64) / n).contiguous()
+            torch.cuda.synchronize()                          # the inputs are ready before the projection's own stream reads them
+            proj.projectPanels(y.data_ptr(), nv, P, wy.data_ptr(), mean.data_ptr())
+            proj.synchronize()
+            del y, wy, mean
+        P_got = proj.projectGet(evals[:k])
+    u = vecs[pick.numpy(), :k]
+    err = np.max(np.abs(P_got - u), axis=0) / np.max(np.abs(vecs[:, :k]), axis=0)
+    out["loadings_checks"] = {"max_rel_err_vs_fp64_XtU": rel, "loadings_within_1e-12": rel <= 1e-12,
+                              "counts_exact": counts_ok, "projected_samples": m,
+                              "self_projection_err_over_max_u": [float(x) for x in err],
+                              "self_projection_within_1e-9": bool(np.all(err <= 1e-9))}
     return out
 
 

@@ -307,6 +307,37 @@ int vpca_project_panels(vpca_ctx* ctx, const void* d_x, int64_t nv, int64_t pane
                         const double* d_mean);
 int vpca_project_get(vpca_ctx* ctx, const double* evals, double* out);
 
+/* ---- KING-robust kinship between the samples (beyond VariantsPca.scala: which samples to leave out of the PCA) ------------
+ * Related samples add excess sharing to S (VariantsPca.scala:182-191) that the top components can pick up as an axis of
+ * their own; the usual remedy is kinship first, PCs of an unrelated subset, projection of the relatives (above).  The
+ * estimator is KING-robust's between-family kinship (Manichaikul et al., Bioinformatics 26:2867, 2010; PLINK 2's
+ * --make-king-table).  PLINK 1 .bed rows (as vpca_accumulate_bed) are encoded into three int8 indicator planes stacked as
+ * 3N rows -- het (code 10), hom A1 (00), hom A2 (11); a missing call (01) sets none -- and G = Y Y^T runs on the int8 Gram
+ * kernel, exact int32, with a Gram schedule of its own.  For a pair a < b (lower-triangle entries of G, DESIGN.md 7):
+ *   HETHET = G[b][a]   IBS0 = G[2N+b][N+a] + G[2N+a][N+b]   HET1_HOM2 = G[N+b][a] + G[2N+b][a]
+ *   HET2_HOM1 = G[N+a][b] + G[2N+a][b]   NSNP = the four + G[N+b][N+a] + G[2N+b][2N+a]   (variants both samples called)
+ *   KINSHIP = (HETHET - 2 IBS0) / (2 HETHET + HET1_HOM2 + HET2_HOM1), numerator and denominator exact int64 converted to
+ *   double, one correctly rounded division: bit-reproducible; NaN when the denominator is 0.
+ * Driver-side calls: one at a time per context, never concurrent with accumulation.  The planes are int8 whatever
+ * cfg.dtype is.  The 3N x 3N int32 counts (9 N^2 x 4 bytes: 17 GB at the limit) are allocated on the first
+ * vpca_kinship_bed; vpca_reset zeroes them; vpca_set_gram / finalize_gram / compute_pca* and accumulation leave them alone,
+ * and kinship calls leave the PCA Gram alone.  VPCA_ERR_UNSUPPORTED when n_samples > 21 845 (3N <= 65 535) or on a
+ * band-only context.
+ * vpca_kinship_bed: adds the rows (stride_bytes >= ceil(n_samples / 4)) to the counts; successive calls add up, and any split
+ *   of the rows into calls gives the same counts.  Rows are staged on a lane (H2D overlapped with the previous chunk's
+ *   work); returns after the last chunk is counted.  VPCA_ERR_OVERFLOW, before any row is staged, when the kinship
+ *   variants would pass 2^31 - 1.
+ * vpca_kinship_pairs: selects pairs -- every pair, NaN included, when min_kinship = -INFINITY, else KINSHIP >= min_kinship
+ *   (NaN never passes) -- and writes the first min(total, max_pairs) in order of b, then a (row-major lower triangle):
+ *   out_ids[2p] = a, out_ids[2p + 1] = b (a < b); out_counts[5p ..] = NSNP, HETHET, IBS0, HET1_HOM2, HET2_HOM1;
+ *   out_kinship[p].  *n_pairs = the total selected (may exceed max_pairs); max_pairs = 0 with NULL outputs counts only.
+ *   May be called any number of times on the same counts.  Two passes (count + scan, then emit in row batches through a
+ *   bounded device scratch), no sort, no floating-point atomics.  VPCA_ERR_STATE when no kinship row was added since
+ *   vpca_create / vpca_reset. */
+int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes);
+int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int32_t* out_ids, int32_t* out_counts,
+                       double* out_kinship, int64_t* n_pairs);
+
 /* ---- one process, all GPUs of the box (SURVEY 8b "process model") --------------------------------------------------
  * A vpca_pool is what `class VariantsPcaDriver` holds on a multi-GPU host: one vpca_ctx per GPU, wired with
  * vpca_gram_set_peers_local in VPCA_PEER_OWNER_ROWS mode (VPCA_PEER_REPLICATE when n_samples < 64 x n_gpus).  Spark

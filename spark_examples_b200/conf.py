@@ -114,4 +114,6 @@ class PcaConf(GenomicsConf):
             ("bedCountedAllele", str, "A1", False),       # which .bim allele is "variation": A1 (PLINK's minor) or A2
             ("saveLoadings", str, None, False),           # after computePca: write per-variant loadings + counts (.npz)
             ("projectLoadings", str, None, False),        # project this cohort onto a saved loadings file (no Gram / eigensolve)
+            ("makeKingTable", str, None, False),          # --bed-path runs: write KING-robust kinship of the sample pairs here
+            ("kingTableFilter", float, None, False),      # keep only the pairs with KINSHIP >= this (PLINK 2's flag names)
         ]

@@ -200,7 +200,85 @@ __global__ void bits_to_cells_kernel(const uint8_t* __restrict__ bits, int64_t s
     }
 }
 
+// .bed rows -> the three int8 indicator planes of kinship (DESIGN.md 7): in a tile of 3n rows, row s is "sample s is
+// heterozygous" (code 10), row n + s "homozygous A1" (00), row 2n + s "homozygous A2" (11); a missing call (01) sets no
+// plane.  The same 32 x 32 ballot transpose as bits_to_cells_kernel, done for the three planes at once; padding samples
+// (smp >= n, PLINK's 00 bits) write nothing.  Always int8, whatever the context's dtype.
+__device__ __forceinline__ void store_i8_cells(uint8_t* dst, uint32_t mine) {   // bit j -> byte j (0 / 1), 32 bytes
+    uint32_t o[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+        const uint32_t nib = (mine >> (4 * q)) & 0xFu;
+        o[q] = (nib & 1u) | ((nib & 2u) << 7) | ((nib & 4u) << 14) | ((nib & 8u) << 21);
+    }
+    uint4* d = reinterpret_cast<uint4*>(dst);
+    d[0] = make_uint4(o[0], o[1], o[2], o[3]);
+    d[1] = make_uint4(o[4], o[5], o[6], o[7]);
+}
+
+__global__ void bed_planes_kernel(const uint8_t* __restrict__ rows, int64_t stride, int64_t nv, int n,
+                                  uint8_t* __restrict__ x, int64_t panel) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int words = (n + 31) / 32;
+    const int64_t vgroups = (nv + 31) / 32;
+    if (warp >= vgroups * words) return;
+    const int64_t vg = warp / words;
+    const int k = (int)(warp - vg * words);
+    const int64_t v = vg * 32 + lane;
+    uint32_t het = 0, hom1 = 0, hom2 = 0;
+    if (v < nv) {
+        const uint8_t* row = rows + v * stride + (size_t)k * 8;
+        const int64_t avail = stride - (int64_t)k * 8;
+        uint64_t w = 0;
+#pragma unroll
+        for (int b = 0; b < 8; ++b)
+            if (b < avail) w |= (uint64_t)row[b] << (8 * b);
+        const uint32_t lo = compress_even_bits(w), hi = compress_even_bits(w >> 1);
+        het = ~lo & hi;
+        hom1 = ~lo & ~hi;
+        hom2 = lo & hi;
+    }
+    uint32_t m_het = 0, m_hom1 = 0, m_hom2 = 0;
+#pragma unroll
+    for (int b = 0; b < 32; ++b) {
+        const uint32_t h = __ballot_sync(0xffffffffu, (het >> b) & 1u);
+        const uint32_t p1 = __ballot_sync(0xffffffffu, (hom1 >> b) & 1u);
+        const uint32_t p2 = __ballot_sync(0xffffffffu, (hom2 >> b) & 1u);
+        if (lane == b) {
+            m_het = h;
+            m_hom1 = p1;
+            m_hom2 = p2;
+        }
+    }
+    const int smp = k * 32 + lane;
+    if (smp >= n) return;
+    const int64_t v0 = vg * 32, pnl = v0 / panel;
+    uint8_t* base = x + pnl * 3 * (int64_t)n * panel + (v0 - pnl * panel);
+    store_i8_cells(base + (int64_t)smp * panel, m_het);
+    store_i8_cells(base + ((int64_t)n + smp) * panel, m_hom1);
+    store_i8_cells(base + (2 * (int64_t)n + smp) * panel, m_hom2);
+}
+
 }  // namespace
+
+cudaError_t encode_bed_planes(const uint8_t* d_rows, int64_t stride, int64_t nv, int n, void* d_x, int64_t panel,
+                              cudaStream_t stream) {
+    if (nv <= 0) return cudaSuccess;
+    const int64_t rows3 = 3 * (int64_t)n;
+    // every cell of the touched 32-variant groups is written: only a partial last panel needs zeroing
+    const int64_t npanels = (nv + panel - 1) / panel;
+    if (npanels * panel != ((nv + 31) / 32) * 32) {
+        cudaError_t e = cudaMemsetAsync(static_cast<char*>(d_x) + (size_t)(npanels - 1) * rows3 * panel, 0,
+                                        (size_t)rows3 * panel, stream);
+        if (e != cudaSuccess) return e;
+    }
+    const int64_t warps = ((nv + 31) / 32) * ((n + 31) / 32);
+    const int threads = 256;
+    const int64_t blocks = (warps * 32 + threads - 1) / threads;
+    bed_planes_kernel<<<(unsigned)blocks, threads, 0, stream>>>(d_rows, stride, nv, n, static_cast<uint8_t*>(d_x), panel);
+    return cudaGetLastError();
+}
 
 cudaError_t encode_bits(const uint8_t* d_bits, int64_t stride, int64_t nv, int n, int elem_bits, void* d_x, int64_t ld,
                         int64_t panel, int code, cudaStream_t stream) {
@@ -290,6 +368,7 @@ cudaError_t encode_preload_kernels() {
     VPCA_LOAD((encode_bf16_kernel<int32_t>)); VPCA_LOAD((encode_bf16_kernel<uint16_t>));
     VPCA_LOAD((encode_e2m1_kernel<int32_t>)); VPCA_LOAD((encode_e2m1_kernel<uint16_t>));
     VPCA_LOAD((bits_to_cells_kernel<8>)); VPCA_LOAD((bits_to_cells_kernel<4>)); VPCA_LOAD((bits_to_cells_kernel<16>));
+    VPCA_LOAD(bed_planes_kernel);
 #undef VPCA_LOAD
     return e;
 }

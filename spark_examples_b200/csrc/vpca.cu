@@ -65,6 +65,14 @@ struct vpca_ctx {
     double* d_lp_mean = nullptr;     // and of the means (projection)
     int32_t* d_lp_count = nullptr;   // and of the carrier counts (loadings)
     int64_t cap_lp_w = 0, cap_lp_mean = 0, cap_lp_count = 0;
+    // kinship (vpca_kinship_bed / _pairs): the 3n x 3n int32 Gram of the indicator planes, allocated on the first call, with
+    // a Gram schedule and plane staging of its own (the PCA Gram's tiles and stream-K split are never touched)
+    int32_t* d_kin = nullptr;
+    GramPlan kin_plan;
+    void* d_kin_x[2] = {nullptr, nullptr};
+    int64_t kin_chunk = 0, kin_panel = 0;   // rows per staged chunk, variants per panel of the 3n-row plane tile
+    int64_t kin_variants = 0;               // rows added since creation / the last vpca_reset
+    KinPairWork kin_pairs;
 
     struct Slot {
         int64_t pid = -1;
@@ -648,6 +656,10 @@ int vpca_destroy(vpca_ctx* ctx) {
                     (void*)ctx->d_lp_count, (void*)ctx->d_band_U})
         cudaFree(p);
     join_free(ctx->join);
+    cudaFree(ctx->d_kin);
+    for (void* p : ctx->d_kin_x) cudaFree(p);
+    gram_plan_free(ctx->kin_plan);
+    kin_pair_free(ctx->kin_pairs);
     gram_plan_free(ctx->plan);
     for (cudaEvent_t ev : {ctx->ev_t0, ctx->ev_t1, ctx->ev_e0, ctx->ev_e1})
         if (ev) cudaEventDestroy(ev);
@@ -671,6 +683,9 @@ int vpca_reset(vpca_ctx* ctx) {
         if (L.busy) return fail(ctx, VPCA_ERR_STATE, "vpca_reset while an accumulate call is in flight");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     CUDA_OK(ctx, cudaMemsetAsync(ctx->d_S, 0, (size_t)ctx->band_rows * ctx->n * sizeof(int32_t), ctx->stream));
+    if (ctx->d_kin != nullptr)
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin, 0, (size_t)9 * ctx->n * ctx->n * sizeof(int32_t), ctx->stream));
+    ctx->kin_variants = 0;
     for (auto& s : ctx->slots) s.used = false;
     ctx->finalized = false;
     ctx->pca_done = false;
@@ -1623,6 +1638,152 @@ int vpca_project_get(vpca_ctx* ctx, const double* evals, double* out) {
     ctx->c_d2h += (int64_t)(acc.size() * sizeof(double));
     for (int c = 0; c < k; ++c)
         for (int s = 0; s < n; ++s) out[s + (size_t)c * n] = acc[(size_t)s * kProjLd + c] / evals[c];
+    return VPCA_OK;
+}
+
+// ---- KING-robust kinship (kinship.cu, DESIGN.md 7) --------------------------------------------------------------
+// Driver-side calls like the loadings: one at a time per context, never concurrent with accumulation.  Rows are staged on
+// a lane (their H2D copy overlaps the encode and Gram of the previous chunk); the planes and the Gram are the kinship's own.
+static int kinship_check(vpca_ctx* ctx) {
+    if (ctx->n > kKinMaxN)
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "kinship is limited to %d samples (the 3N x 3N plane Gram must stay below 2^32 "
+                    "cells); this context has %d", kKinMaxN, ctx->n);
+    if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_UNSUPPORTED, "kinship needs a context that stores the whole Gram");
+    return VPCA_OK;
+}
+
+// Plane staging geometry and buffers, and the kinship Gram (zeroed on the lane's stream), on the first call.
+static int kinship_buffers(vpca_ctx* ctx, vpca_ctx::Lane& L) {
+    const int64_t R = 3 * (int64_t)ctx->n, budget = 256ll << 20;   // bytes per plane staging buffer
+    if (ctx->kin_panel == 0) {
+        const int64_t p = std::max<int64_t>(128, (budget / R / 128) * 128);
+        ctx->kin_panel = std::min<int64_t>(ctx->panel, p);
+        ctx->kin_chunk = std::max<int64_t>(ctx->kin_panel, (budget / R / ctx->kin_panel) * ctx->kin_panel);
+        for (int b = 0; b < 2; ++b) {
+            cudaError_t e = cudaMalloc(&ctx->d_kin_x[b], (size_t)R * ctx->kin_chunk);
+            if (e != cudaSuccess) {
+                cudaFree(ctx->d_kin_x[0]);
+                ctx->d_kin_x[0] = ctx->d_kin_x[1] = nullptr;
+                ctx->kin_panel = ctx->kin_chunk = 0;
+                return fail(ctx, VPCA_ERR_NOMEM, "kinship plane staging: %s", cudaGetErrorString(e));
+            }
+        }
+    }
+    if (ctx->d_kin == nullptr) {
+        const size_t bytes = (size_t)R * R * sizeof(int32_t);
+        cudaError_t e = cudaMalloc(&ctx->d_kin, bytes);
+        if (e != cudaSuccess) {
+            ctx->d_kin = nullptr;
+            return fail(ctx, VPCA_ERR_NOMEM, "kinship Gram of %lld x %lld int32: %s", (long long)R, (long long)R,
+                        cudaGetErrorString(e));
+        }
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin, 0, bytes, L.stream));
+    }
+    return VPCA_OK;
+}
+
+int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int rc = kinship_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    if (nv < 0 || (nv > 0 && rows == nullptr) || stride_bytes < (ctx->n + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_kinship_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->kin_variants + nv > 2147483647ll)
+            return fail(ctx, VPCA_ERR_OVERFLOW, "%lld kinship variants could overflow an int32 count",
+                        (long long)(ctx->kin_variants + nv));
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    rc = kinship_buffers(ctx, L);
+    if (rc != VPCA_OK) return rc;
+    const int n = ctx->n;
+    const int64_t R = 3 * (int64_t)n, P = ctx->kin_panel;
+    const int64_t cap_rows = (ctx->chunk_nnz * (int64_t)sizeof(int32_t)) / stride_bytes;   // raw rows in L.d_idx[b]
+    if (cap_rows < 32) return fail(ctx, VPCA_ERR_BAD_ARG, "stride_bytes too large for the staging buffer");
+    const int64_t step = std::min(ctx->kin_chunk, (cap_rows / 32) * 32);
+    int chunk = 0;
+    for (int64_t v = 0; v < nv; v += step, ++chunk) {
+        const int64_t nvc = std::min(step, nv - v);
+        const int b = chunk & 1;
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
+        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b], rows + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
+                                     cudaMemcpyHostToDevice, L.copy_stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
+        ctx->c_h2d += nvc * stride_bytes;
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        CUDA_OK(ctx, encode_bed_planes(reinterpret_cast<const uint8_t*>(L.d_idx[b]), stride_bytes, nvc, n, ctx->d_kin_x[b], P,
+                                       L.stream));
+        std::string msg;
+        cudaError_t e = gram_accumulate(ctx->kin_plan, ctx->d_kin_x[b], 8, (int)R, nvc, P, P, ctx->d_kin, L.stream, &msg);
+        if (e != cudaSuccess)
+            return fail(ctx, VPCA_ERR_CUDA, "kinship Gram launch failed: %s %s [the kinship counts may hold a partial "
+                        "batch, call vpca_reset]", cudaGetErrorString(e), msg.c_str());
+        ctx->c_launches += 2;
+        ctx->c_gram += 1;
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    ctx->kin_variants += nv;
+    return VPCA_OK;
+}
+
+int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int32_t* out_ids, int32_t* out_counts,
+                       double* out_kinship, int64_t* n_pairs) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int rc = kinship_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    if (n_pairs == nullptr || max_pairs < 0 ||
+        (max_pairs > 0 && (out_ids == nullptr || out_counts == nullptr || out_kinship == nullptr)))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_kinship_pairs: bad argument");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->kin_variants == 0)
+            return fail(ctx, VPCA_ERR_STATE, "no kinship rows since the context was created or reset: call vpca_kinship_bed");
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    const int n = ctx->n, tile_rows = (n + 31) / 32;
+    const bool all = std::isinf(min_kinship) && min_kinship < 0;
+    KinPairWork& w = ctx->kin_pairs;
+    cudaError_t e = kin_pair_alloc(w, n);
+    if (e != cudaSuccess) return fail(ctx, VPCA_ERR_NOMEM, "kinship pair scratch: %s", cudaGetErrorString(e));
+    CUDA_OK(ctx, kin_count(w, ctx->d_kin, n, min_kinship, all, ctx->stream));
+    std::vector<int32_t> row_total(n);
+    CUDA_OK(ctx, cudaMemcpyAsync(row_total.data(), w.d_row_total, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                                 ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_launches += 2;
+    std::vector<int64_t> start(n + 1, 0);   // output position of the first pair of row b (row-major lower triangle)
+    for (int b = 0; b < n; ++b) start[b + 1] = start[b] + row_total[b];
+    *n_pairs = start[n];
+    const int64_t limit = std::min(start[n], max_pairs);
+    if (limit == 0) return VPCA_OK;
+    CUDA_OK(ctx, cudaMemcpyAsync(w.d_row_start, start.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
+    ctx->c_h2d += (int64_t)n * 8;
+    auto row_end = [&](int bt) { return start[std::min(n, 32 * bt)]; };   // position after tile rows [0, bt)
+    for (int lo = 0; lo < tile_rows && row_end(lo) < limit;) {
+        int hi = lo + 1;   // as many tile rows as the scratch holds (one always fits, kin_pair_alloc)
+        while (hi < tile_rows && row_end(hi + 1) - row_end(lo) <= w.cap && row_end(hi) < limit) ++hi;
+        const int64_t base = row_end(lo), end = std::min(row_end(hi), limit), cnt = end - base;
+        if (cnt > 0) {
+            CUDA_OK(ctx, kin_emit(w, ctx->d_kin, n, min_kinship, all, lo, hi, base, end, ctx->stream));
+            CUDA_OK(ctx, cudaMemcpyAsync(out_ids + 2 * base, w.d_ids, (size_t)cnt * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                                         ctx->stream));
+            CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 5 * base, w.d_counts, (size_t)cnt * 5 * sizeof(int32_t),
+                                         cudaMemcpyDeviceToHost, ctx->stream));
+            CUDA_OK(ctx, cudaMemcpyAsync(out_kinship + base, w.d_kin, (size_t)cnt * sizeof(double), cudaMemcpyDeviceToHost,
+                                         ctx->stream));
+            ctx->c_launches += 1;
+            ctx->c_d2h += cnt * 36;
+        }
+        lo = hi;
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     return VPCA_OK;
 }
 

@@ -100,7 +100,34 @@ cudaError_t encode_calls(const int64_t* d_off, int64_t base, const void* d_idx, 
 cudaError_t encode_bits(const uint8_t* d_bits, int64_t stride, int64_t nv, int n, int elem_bits, void* d_x, int64_t ld,
                         int64_t panel, int code, cudaStream_t stream);
 
-// ---- multi-dataset keying: variant keys, join, merge (join.cu) ---------------------------------------------
+// PLINK .bed rows (`stride` bytes apart) -> the three int8 kinship planes in panel layout over 3n rows: row s het, row
+// n + s hom A1, row 2n + s hom A2 (missing calls and padding samples set nothing).  Zeroes a partial last panel first.
+cudaError_t encode_bed_planes(const uint8_t* d_rows, int64_t stride, int64_t nv, int n, void* d_x, int64_t panel,
+                              cudaStream_t stream);
+
+// ---- KING-robust kinship pairs from the 3n x 3n plane Gram (kinship.cu) ----------------------------------------------
+constexpr int kKinMaxN = 21845;   // 3n <= 65 535: the plane Gram stays below 2^32 cells
+// Device scratch of vpca_kinship_pairs, owned by the context and kept between calls.
+struct KinPairWork {
+    int n = 0;
+    int32_t* d_seg = nullptr;        // n x ceil(n / 32): selected pairs per (row b, 32-column tile), then their row-wise scan
+    int32_t* d_row_total = nullptr;  // n: selected pairs per row b
+    int64_t* d_row_start = nullptr;  // n: output position of the first selected pair of row b
+    int32_t* d_ids = nullptr;        // cap pairs: 2 ids, 5 counts, 1 kinship each
+    int32_t* d_counts = nullptr;
+    double* d_kin = nullptr;
+    int64_t cap = 0;
+};
+void kin_pair_free(KinPairWork& w);
+cudaError_t kin_pair_alloc(KinPairWork& w, int n);
+// Pass 1: w.d_seg / w.d_row_total for the threshold (select_all: every pair, NaN included).  Never synchronises.
+cudaError_t kin_count(KinPairWork& w, const int32_t* d_G, int n, double min_kinship, bool select_all, cudaStream_t stream);
+// Pass 2: the selected pairs of tile rows [bt_lo, bt_hi) whose output position p lies in [base, end) go to scratch slot
+// p - base (needs w.d_row_start).  Never synchronises.
+cudaError_t kin_emit(KinPairWork& w, const int32_t* d_G, int n, double min_kinship, bool select_all, int bt_lo, int bt_hi,
+                     int64_t base, int64_t end, cudaStream_t stream);
+
+// ---- multi-dataset keying: variant keys, join, merge (join.cu)---------------------------------------------
 struct JoinWork {
     uint64_t* d_hash = nullptr;      // 2 per row: MurmurHash3_x64_128 of the variant key
     int32_t* d_table = nullptr;      // open-addressing table of row indices (-1 = empty)

@@ -52,7 +52,10 @@ EXPORTED_SYMBOLS = (
     "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan",
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
+    "vpca_kinship_bed", "vpca_kinship_pairs",
 )
+
+KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
 
 
 class VpcaError(RuntimeError):
@@ -268,6 +271,10 @@ def load_library() -> ctypes.CDLL:
     L.vpca_project_panels.argtypes = [vp, vp, i64, i64, vp, vp]
     L.vpca_project_get.restype = ctypes.c_int
     L.vpca_project_get.argtypes = [vp, vp, vp]
+    L.vpca_kinship_bed.restype = ctypes.c_int
+    L.vpca_kinship_bed.argtypes = [vp, vp, i64, i64]
+    L.vpca_kinship_pairs.restype = ctypes.c_int
+    L.vpca_kinship_pairs.argtypes = [vp, ctypes.c_double, i64, vp, vp, vp, ctypes.POINTER(i64)]
     _lib = L
     return L
 
@@ -659,6 +666,30 @@ class NativePca:
         out = np.zeros(self.n * max(k, 1), dtype=np.float64)
         self._check(self._lib.vpca_project_get(self._h, _host_ptr(ev), _host_ptr(out)))
         return out.reshape(max(k, 1), self.n).T.copy()
+
+    # -- KING-robust kinship between the samples (vpca.h, DESIGN.md 7) -------------------------------------------------
+    def kinshipBed(self, rows: np.ndarray):
+        """Add PLINK .bed rows ((nv, stride) uint8, see accumulateBed) to the kinship counts of every sample pair; calls
+        add up, and the PCA Gram is not touched.  Synchronises."""
+        b = np.ascontiguousarray(rows, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        self._check(self._lib.vpca_kinship_bed(self._h, _host_ptr(b) if b.size else None, b.shape[0], b.shape[1]))
+
+    def kinshipPairs(self, min_kinship: float = float("-inf"), max_pairs: Optional[int] = None):
+        """-> (ids (P, 2) int32 with a < b, counts (P, 5) int32 NSNP, HETHET, IBS0, HET1_HOM2, HET2_HOM1, kinship (P,)
+        float64) of the pairs with KINSHIP >= min_kinship (-inf: every pair, NaN ones included), ordered by b then a.
+        max_pairs: keep only the first max_pairs (None: all of them)."""
+        total = ctypes.c_int64(0)
+        self._check(self._lib.vpca_kinship_pairs(self._h, float(min_kinship), 0, None, None, None, ctypes.byref(total)))
+        p = int(total.value) if max_pairs is None else min(int(total.value), int(max_pairs))
+        ids = np.zeros((max(p, 1), 2), np.int32)
+        counts = np.zeros((max(p, 1), 5), np.int32)
+        kin = np.zeros(max(p, 1), np.float64)
+        if p > 0:
+            self._check(self._lib.vpca_kinship_pairs(self._h, float(min_kinship), p, _host_ptr(ids), _host_ptr(counts),
+                                                     _host_ptr(kin), ctypes.byref(total)))
+        return ids[:p], counts[:p], kin[:p]
 
 
 def debugTiles(n_samples: int, cta_group: int = 2, exact: bool = True) -> np.ndarray:

@@ -46,6 +46,12 @@ def read_fam(path: str) -> List[Tuple[str, str]]:
     return out
 
 
+def read_fam_ids(path: str) -> List[Tuple[str, str]]:
+    """[(FID, IID)] (.fam columns 1 and 2) in file order."""
+    with open(_prefix(path) + ".fam", "r", encoding="utf-8") as fh:
+        return [(f[0], f[1]) for f in (line.split() for line in fh) if len(f) >= 2]
+
+
 @dataclass(frozen=True)
 class BimRecord:
     contig: str

@@ -297,7 +297,10 @@ class VariantsPcaDriver:
                     nat.joinRows(part.mode, part.keys, part.offsets, part.idx, part.n_left, part.variant_set_count)
                     nat.accumulateJoined(pid)                   # the joined rows never leave the device
                 elif isinstance(part, BedSlice):
-                    nat.accumulateBed(pid, part.rows(), part.counted)
+                    rows = part.rows()
+                    if self.conf.makeKingTable.isDefined:
+                        nat.kinshipBed(rows)                    # the same rows, three genotype planes (DESIGN.md 7)
+                    nat.accumulateBed(pid, rows, part.counted)
                 else:
                     nat.accumulateCalls(pid, part.offsets, part.idx)
                 nat.commit(pid)
@@ -513,6 +516,19 @@ class VariantsPcaDriver:
             off, idx = _select_rows(*_partition_csr(part), sel)
             nat.projectCalls(off, idx, w, mean)
 
+    # -- KING-robust kinship of the sample pairs (beyond the reference; DESIGN.md 7) --------------------------------------
+    def writeKingTable(self, path: Optional[str] = None, min_kinship: Optional[float] = None):
+        """After getSimilarityMatrix of a --bed-path run with --make-king-table: rank 0 writes the pairs (filtered by
+        --king-table-filter) in PLINK 2's .kin0 columns."""
+        if self._rank != 0:
+            return
+        path = path if path is not None else self.conf.makeKingTable()
+        if min_kinship is None:
+            min_kinship = self.conf.kingTableFilter() if self.conf.kingTableFilter.isDefined else float("-inf")
+        from . import plink
+        ids, counts, kin = self._nat.kinshipPairs(min_kinship)
+        write_king_table(path, plink.read_fam_ids(self.conf.bedPath()), ids, counts, kin)
+
     def reportIoStats(self):                                                     # :281
         self.common.reportIoStats()
         if self._nat is not None:
@@ -586,6 +602,43 @@ class VariantsPcaDriver:
         nat.synthPanelsDevice(part.seed, part.v0, part.nv, 0, buf.data_ptr(), panel)
         nat.accumulatePanels(buf.data_ptr(), part.nv, panel)
         torch.cuda.current_stream().synchronize()      # `buf` must outlive the kernels that read it
+
+
+KING_HEADER = "#FID1\tIID1\tFID2\tIID2\tNSNP\tHETHET\tIBS0\tKINSHIP\n"
+
+
+def write_king_table(path: str, fam: Sequence[Tuple[str, str]], ids: np.ndarray, counts: np.ndarray,
+                     kinship: np.ndarray, batch: int = 1 << 16) -> None:
+    """Tab-separated KING table: one line per pair (ids[p] = (a, b), a < b; counts[p] = NSNP, HETHET, IBS0, HET1_HOM2,
+    HET2_HOM1), FID / IID from .fam columns 1 and 2; KINSHIP as the shortest text that reads back as the same double."""
+    with open(path, "w", encoding="utf-8") as fh:
+        fh.write(KING_HEADER)
+        for p0 in range(0, len(ids), batch):
+            lines = []
+            for (a, b), c, k in zip(ids[p0:p0 + batch].tolist(), counts[p0:p0 + batch].tolist(),
+                                    kinship[p0:p0 + batch].tolist()):
+                fa, fb = fam[a], fam[b]
+                lines.append(f"{fa[0]}\t{fa[1]}\t{fb[0]}\t{fb[1]}\t{c[0]}\t{c[1]}\t{c[2]}\t{k!r}\n")
+            fh.write("".join(lines))
+
+
+def check_king_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
+    """Refuse --make-king-table / --king-table-filter runs the kinship path cannot serve, before any GPU work:
+    without n_samples the flag combinations, with it the cohort size."""
+    if conf.kingTableFilter.isDefined and not conf.makeKingTable.isDefined:
+        raise ValueError("--king-table-filter needs --make-king-table")
+    if not conf.makeKingTable.isDefined:
+        return
+    if not conf.bedPath.isDefined:
+        raise ValueError("--make-king-table needs genotype classes (het / hom): give a PLINK fileset with --bed-path")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("--make-king-table runs on one GPU; launch a single process (WORLD_SIZE=1)")
+    if conf.checkpointPath.isDefined:
+        raise ValueError("--make-king-table counts every partition in one pass; it cannot resume from --checkpoint-path")
+    if conf.projectLoadings.isDefined:
+        raise ValueError("--project-loadings builds no similarity matrix for --make-king-table to ride on")
+    if n_samples is not None and n_samples > native.KINSHIP_MAX_SAMPLES:
+        raise ValueError(f"--make-king-table is limited to {native.KINSHIP_MAX_SAMPLES} samples; the cohort has {n_samples}")
 
 
 def joined_rows_on_host(p: JoinedSlice) -> CallsBatch:
@@ -682,12 +735,14 @@ def _select_rows(off: np.ndarray, idx: np.ndarray, sel: np.ndarray):
 def main(args: Optional[Sequence[str]] = None):
     """VariantsPcaDriver.main (VariantsPca.scala:38-50)."""
     conf = PcaConf(list(sys.argv[1:] if args is None else args))
+    check_king_flags(conf)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         import torch
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl")
     driver = VariantsPcaDriver(conf)
+    check_king_flags(conf, len(driver.common.indexes))
     data = driver.getData
     filtered = [driver.filterDataset(d) for d in data]
     callsRdd = driver.getCallsRdd(filtered)
@@ -706,6 +761,8 @@ def main(args: Optional[Sequence[str]] = None):
         if conf.saveLoadings.isDefined:
             driver.saveLoadings(callsRdd)
     driver.emitResult(result)
+    if conf.makeKingTable.isDefined:
+        driver.writeKingTable()
     driver.reportIoStats()
     driver.stop()
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:

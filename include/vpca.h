@@ -338,6 +338,29 @@ int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t str
 int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int32_t* out_ids, int32_t* out_counts,
                        double* out_kinship, int64_t* n_pairs);
 
+/* ---- principal coordinates of an unrelated subset (kinship, then PCs of the unrelated, then the relatives placed) -------
+ * vpca_compute_pca_subset: the PCs of the samples K with keep[s] != 0 (keep: n_samples bytes), M = |K| >= 2, from the
+ * finalized Gram of all the samples -- no genotype is read again (DESIGN.md 8).  S[K, K] is copied into an M x M buffer and
+ * centred and solved exactly as vpca_compute_pca does in an M-sample context (VPCA_EIG, the same eigensolver selection,
+ * sign rule and fallback), on a workspace of its own that is allocated on the first call and again whenever M changes.
+ *   vecs (n_samples x k, column-major): rows of kept samples hold u_c -- the bits of vpca_set_gram(S[K, K]) +
+ *     vpca_compute_pca in an M-sample context; rows of removed samples r hold their projection onto the axes of K,
+ *       p_c(r) = (sum_{j in K} S[r][j] u_c[j] - (1/M) sum_{j in K} rho_j u_c[j]) / lambda_c     rho_j = sum_{i in K} S[j][i]
+ *     which is vpca_project_* of r's genotypes with the kept samples' loadings (FP64, sums in a fixed order, no
+ *     floating-point atomics).  All samples kept: the bits of vpca_compute_pca.
+ *   evals: the k eigenvalues of the subset (may be NULL); non_zero_rows: the nonzero row sums of S[K, K] (may be NULL).
+ * Afterwards vpca_loadings_* return the kept samples' loadings: w[v][c] = sum_{s in K} x[s][v] u_c[s] and
+ * count[v] = sum_{s in K} x[s][v], with the bits of vpca_loadings_* in an M-sample context fed only the kept columns (they
+ * always sum the samples in the whole order, so this holds unless VPCA_LOADINGS_KERNEL=split forces that context's split);
+ * projection is unaffected; vpca_get_tridiagonal returns VPCA_ERR_STATE; vpca_stats report this solve's eig_method /
+ * eig_iterations.  The next vpca_compute_pca / _bands, vpca_reset, vpca_set_gram, vpca_load_partial_gram or
+ * vpca_finalize_gram ends the subset state as it ends U.  The Gram and the kinship counts are only read.
+ * Checked in vpca_compute_pca's order: VPCA_ERR_BAD_ARG for keep / vecs NULL, M < 2 or k outside
+ * [1, min(M, max(num_pc, 16))]; then VPCA_ERR_STATE before vpca_finalize_gram; then VPCA_ERR_UNSUPPORTED on a band-only
+ * context or above 65 535 samples.  k > 16 (num_pc > 16) is served in full; the loadings afterwards take k' <= 16. */
+int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, double* vecs, double* evals,
+                            int32_t* non_zero_rows);
+
 /* ---- one process, all GPUs of the box (SURVEY 8b "process model") --------------------------------------------------
  * A vpca_pool is what `class VariantsPcaDriver` holds on a multi-GPU host: one vpca_ctx per GPU, wired with
  * vpca_gram_set_peers_local in VPCA_PEER_OWNER_ROWS mode (VPCA_PEER_REPLICATE when n_samples < 64 x n_gpus).  Spark

@@ -116,4 +116,6 @@ class PcaConf(GenomicsConf):
             ("projectLoadings", str, None, False),        # project this cohort onto a saved loadings file (no Gram / eigensolve)
             ("makeKingTable", str, None, False),          # --bed-path runs: write KING-robust kinship of the sample pairs here
             ("kingTableFilter", float, None, False),      # keep only the pairs with KINSHIP >= this (PLINK 2's flag names)
+            ("kingCutoff", float, None, False),           # --bed-path runs: PCs of a maximal set without KINSHIP > this; the
+                                                          # relatives projected onto them (PLINK 2's flag name)
         ]

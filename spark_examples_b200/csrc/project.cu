@@ -14,6 +14,10 @@
 //   above kSplitMinN samples the sum is cut into kRanges fixed ranges whose bounds depend on N alone, the range sums
 //     added in range order: loadings_split_kernel (k <= 8) gives each range its own warps, loadings_ranged_kernel
 //     (k > 8) walks the ranges one after another in each thread.  w[v] is still a function of column v, U and N only.
+//   masked loadings (after vpca_compute_pca_subset): loadings_kernel<..., MASK = true> reads U with zero rows for the
+//     samples outside the PCA set and a keep byte per sample next to the U tile; the count adds only kept cells.  A zero U
+//     row leaves every accumulator's bits unchanged (fma(d, 0, a) = a, as a never holds -0), so w[v] has the bits of the
+//     same kernel run over the kept samples alone.
 //   project_kernel: a thread owns one sample and walks the variants of one panel in order; the panel's slice of w and of
 //     the means goes through shared memory in variant tiles.  Each panel leaves a partial sum per (sample, component);
 //     project_reduce_kernel adds the partials into the accumulator in panel order.
@@ -61,10 +65,11 @@ __device__ __forceinline__ uint64_t load_word(const uint8_t* p) {
 
 // ---- loadings ------------------------------------------------------------------------------------------------------
 // acc[i][c] += x[s][v0 + i] U[s][c] and cnt[i] += x[s][v0 + i] for the ts sample rows of a tile, in order, from the
-// thread's cells `r` (row_bytes apart) and the tile's U in shared memory (su[s * KMAX + c]).
-template <int BITS, int KMAX, int VT>
+// thread's cells `r` (row_bytes apart) and the tile's U in shared memory (su[s * KMAX + c]).  MASK: cnt[i] only counts the
+// rows whose keep byte sk[s] is nonzero.
+template <int BITS, int KMAX, int VT, bool MASK = false>
 __device__ __forceinline__ void sum_tile(const uint8_t* r, int64_t row_bytes, const double* su, int ts,
-                                         double (&acc)[VT][KMAX], int (&cnt)[VT]) {
+                                         double (&acc)[VT][KMAX], int (&cnt)[VT], const uint8_t* sk = nullptr) {
     constexpr int WB = VT * BITS / 8; // bytes of my VT cells in one sample row
 #pragma unroll 8
     for (int s = 0; s < ts; ++s) {
@@ -79,7 +84,8 @@ __device__ __forceinline__ void sum_tile(const uint8_t* r, int64_t row_bytes, co
 #pragma unroll
         for (int i = 0; i < VT; ++i) {
             const int m = cell_value<BITS>(word, i);
-            cnt[i] += m;
+            if constexpr (MASK) cnt[i] += sk[s] ? m : 0;
+            else cnt[i] += m;
             const double d = int_to_f64(m);
 #pragma unroll
             for (int c = 0; c < KMAX; ++c) acc[i][c] = fma(d, u[c], acc[i][c]);
@@ -88,12 +94,15 @@ __device__ __forceinline__ void sum_tile(const uint8_t* r, int64_t row_bytes, co
 }
 
 // grid (panels, ceil(P / (kThreads * VT))).  U: n x k column-major (ld n).  w: nv x k variant-major, count: nv.
-template <int BITS, int KMAX, int VT>
+// MASK: keep (n bytes) selects the samples the count adds up; their tile of keep bytes follows the U tile in shared memory.
+template <int BITS, int KMAX, int VT, bool MASK = false>
 __global__ void __launch_bounds__(kThreads) loadings_kernel(const uint8_t* __restrict__ x, int n, int64_t nv,
                                                             int64_t panel, const double* __restrict__ U, int k,
-                                                            double* __restrict__ w, int32_t* __restrict__ count) {
+                                                            double* __restrict__ w, int32_t* __restrict__ count,
+                                                            const uint8_t* __restrict__ keep = nullptr) {
     constexpr int TS = 4096 / KMAX;   // samples of U per shared-memory tile (32 KB)
-    __shared__ __align__(16) double su[TS * KMAX];
+    __shared__ __align__(16) double su[TS * KMAX + (MASK ? TS / 8 : 0)];
+    uint8_t* sk = reinterpret_cast<uint8_t*>(su + TS * KMAX);
     const int64_t p = blockIdx.x;
     const int64_t vloc = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * VT;
     const int64_t vg = p * panel + vloc;
@@ -115,9 +124,11 @@ __global__ void __launch_bounds__(kThreads) loadings_kernel(const uint8_t* __res
             const int s = q / KMAX, c = q - s * KMAX;
             su[q] = c < k ? U[(int64_t)c * n + s0 + s] : 0.0;
         }
+        if constexpr (MASK)
+            for (int s = threadIdx.x; s < ts; s += kThreads) sk[s] = keep[s0 + s];
         __syncthreads();
         if (!active) continue;
-        sum_tile<BITS, KMAX, VT>(col + (int64_t)s0 * row_bytes, row_bytes, su, ts, acc, cnt);
+        sum_tile<BITS, KMAX, VT, MASK>(col + (int64_t)s0 * row_bytes, row_bytes, su, ts, acc, cnt, sk);
     }
     if (!active) return;
 #pragma unroll
@@ -358,11 +369,15 @@ int kmax_for(int k) { return k <= 2 ? 2 : k <= 4 ? 4 : k <= 8 ? 8 : 16; }
 
 template <int BITS, int KMAX>
 void launch_loadings(const void* d_x, int n, int64_t nv, int64_t panel, const double* d_U, int k, double* d_w,
-                     int32_t* d_count, bool split, cudaStream_t stream) {
+                     int32_t* d_count, bool split, const uint8_t* d_keep, cudaStream_t stream) {
     constexpr int VT = KMAX >= 16 ? 2 : 4;
     const int64_t npanels = (nv + panel - 1) / panel;
     const uint8_t* x = static_cast<const uint8_t*>(d_x);
     const dim3 grid((unsigned)npanels, (unsigned)((panel + kThreads * VT - 1) / (kThreads * VT)));
+    if (d_keep != nullptr) {   // a subset solve: n <= 65 535, the whole order
+        loadings_kernel<BITS, KMAX, VT, true><<<grid, kThreads, 0, stream>>>(x, n, nv, panel, d_U, k, d_w, d_count, d_keep);
+        return;
+    }
     if constexpr (KMAX >= 16) {
         // 2 variants per thread leave enough CTAs already; the warp split would re-read U 4 x as often
         if (split) {
@@ -392,12 +407,12 @@ void launch_project(const void* d_y, int m, int64_t nv, int64_t panel, const dou
 
 template <int BITS>
 void loadings_bits(const void* d_x, int n, int64_t nv, int64_t panel, const double* d_U, int k, double* d_w,
-                   int32_t* d_count, bool split, cudaStream_t stream) {
+                   int32_t* d_count, bool split, const uint8_t* d_keep, cudaStream_t stream) {
     switch (kmax_for(k)) {
-        case 2: launch_loadings<BITS, 2>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
-        case 4: launch_loadings<BITS, 4>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
-        case 8: launch_loadings<BITS, 8>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
-        default: launch_loadings<BITS, 16>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream); break;
+        case 2: launch_loadings<BITS, 2>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream); break;
+        case 4: launch_loadings<BITS, 4>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream); break;
+        case 8: launch_loadings<BITS, 8>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream); break;
+        default: launch_loadings<BITS, 16>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream); break;
     }
 }
 
@@ -415,7 +430,7 @@ void project_bits(const void* d_y, int m, int64_t nv, int64_t panel, const doubl
 }  // namespace
 
 cudaError_t loadings_launch(const void* d_x, int elem_bits, int n, int64_t nv, int64_t panel, const double* d_U, int k,
-                            double* d_w, int32_t* d_count, cudaStream_t stream) {
+                            double* d_w, int32_t* d_count, const uint8_t* d_keep, cudaStream_t stream) {
     if (nv <= 0) return cudaSuccess;
     // VPCA_LOADINGS_KERNEL=whole|split forces one kernel (to time both at one N, or to test the split below the
     // threshold); the default is the split above kSplitMinN samples
@@ -424,9 +439,9 @@ cudaError_t loadings_launch(const void* d_x, int elem_bits, int n, int64_t nv, i
         if (strcmp(e, "whole") == 0) split = false;
         else if (strcmp(e, "split") == 0) split = true;
     }
-    if (elem_bits == 8) loadings_bits<8>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream);
-    else if (elem_bits == 16) loadings_bits<16>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream);
-    else loadings_bits<4>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, stream);
+    if (elem_bits == 8) loadings_bits<8>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream);
+    else if (elem_bits == 16) loadings_bits<16>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream);
+    else loadings_bits<4>(d_x, n, nv, panel, d_U, k, d_w, d_count, split, d_keep, stream);
     return cudaGetLastError();
 }
 

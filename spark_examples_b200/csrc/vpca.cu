@@ -57,6 +57,17 @@ struct vpca_ctx {
     const double* d_U = nullptr;     // that U (n x min(pca_k, 16), column-major): eig.d_evecs after vpca_compute_pca;
                                      // band_eig.d_evecs or d_band_U after vpca_compute_pca_bands
     double* d_band_U = nullptr;      // n x 16: this rank's copy of U from a band solve driven by another context
+    // vpca_compute_pca_subset: a solver of its own for the m kept samples (ctx->eig is never touched), their m x m Gram,
+    // U scattered to n x 16 with zero rows for the removed samples (d_U points here after a subset solve, which is what
+    // makes the loadings apply d_sub_keep), the n x k output, the sample lists and the keep bytes
+    EigWork sub_eig;
+    int32_t* d_sub_S = nullptr;
+    int64_t cap_sub_S = 0;
+    double* d_sub_U = nullptr;
+    double* d_sub_vecs = nullptr;    // n x max(num_pc, 16) (the first k columns used)
+    double* d_sub_t = nullptr;       // max(num_pc, 16): sum_j rho_j u_c[j]
+    int32_t* d_sub_idx = nullptr;    // n: kept samples, then removed ones, each in increasing order
+    uint8_t* d_sub_keep = nullptr;   // n: 1 for kept samples
     int proj_k = 0;       // k of the projection begun by vpca_project_begin (0: none in progress)
     double* d_proj_acc = nullptr;    // n x kProjLd partial projection sums (project.cu)
     double* d_proj_part = nullptr;   // per-panel partial sums of one launch
@@ -653,8 +664,10 @@ int vpca_destroy(vpca_ctx* ctx) {
     band_eig_free(ctx->band_eig);
     band_part_free(ctx->band_part);
     for (void* p : {(void*)ctx->d_proj_acc, (void*)ctx->d_proj_part, (void*)ctx->d_lp_w, (void*)ctx->d_lp_mean,
-                    (void*)ctx->d_lp_count, (void*)ctx->d_band_U})
+                    (void*)ctx->d_lp_count, (void*)ctx->d_band_U, (void*)ctx->d_sub_S, (void*)ctx->d_sub_U,
+                    (void*)ctx->d_sub_vecs, (void*)ctx->d_sub_t, (void*)ctx->d_sub_idx, (void*)ctx->d_sub_keep})
         cudaFree(p);
+    if (ctx->sub_eig.n != 0) eig_free(ctx->sub_eig);
     join_free(ctx->join);
     cudaFree(ctx->d_kin);
     for (void* p : ctx->d_kin_x) cudaFree(p);
@@ -1312,6 +1325,96 @@ int vpca_get_tridiagonal(vpca_ctx* ctx, double* diag, double* offdiag) {
     return VPCA_OK;
 }
 
+// Principal coordinates of the kept samples K from S[K, K], the removed samples placed from their Gram rows (subset.cu,
+// DESIGN.md 8).  The solve is vpca_compute_pca's centring and eigensolver on an m-sample workspace of its own, so the
+// kept rows have the bits of vpca_compute_pca in an m-sample context holding S[K, K].
+int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, double* vecs, double* evals,
+                            int32_t* non_zero_rows) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    // checked in vpca_compute_pca's order: arguments, then the Gram's state, then what the context can hold
+    if (keep == nullptr || vecs == nullptr) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_compute_pca_subset: NULL argument");
+    const int n = ctx->n;
+    std::vector<int32_t> idx;
+    idx.reserve(n);
+    for (int s = 0; s < n; ++s)
+        if (keep[s]) idx.push_back(s);
+    const int m = (int)idx.size();
+    for (int s = 0; s < n; ++s)
+        if (!keep[s]) idx.push_back(s);
+    const int kmax = std::max(ctx->num_pc, 16);
+    if (m < 2) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_compute_pca_subset: %d kept samples, at least 2 needed", m);
+    if (k < 1 || k > m || k > kmax)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_compute_pca_subset: k=%d out of range [1, %d]", k, std::min(m, kmax));
+    if (!ctx->finalized) return fail(ctx, VPCA_ERR_STATE, "call vpca_finalize_gram first");
+    if (ctx->band_rows != ctx->n)
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "vpca_compute_pca_subset needs a context that stores the whole Gram");
+    if (n > 65535)
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "vpca_compute_pca_subset is limited to 65535 samples, like vpca_compute_pca");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    ctx->pca_k = 0;   // U is overwritten from here on
+    ctx->pca_done = false;   // the tridiagonal form of ctx->eig does not belong to this solve
+    if (ctx->sub_eig.n != m) {
+        if (ctx->sub_eig.n != 0) eig_free(ctx->sub_eig);
+        const cudaError_t e = eig_alloc(ctx->sub_eig, m, kmax);
+        if (e != cudaSuccess) {
+            eig_free(ctx->sub_eig);
+            return fail(ctx, VPCA_ERR_NOMEM, "subset eigensolver workspace: %s", cudaGetErrorString(e));
+        }
+    }
+    if (ctx->d_sub_U == nullptr) {
+        // U keeps the 16 columns the loadings read; the output and t take every component a solve may ask for
+        cudaError_t e = cudaMalloc(&ctx->d_sub_U, (size_t)n * 16 * sizeof(double));
+        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_vecs, (size_t)n * kmax * sizeof(double));
+        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_t, (size_t)kmax * sizeof(double));
+        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_idx, (size_t)n * sizeof(int32_t));
+        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_keep, (size_t)n);
+        if (e != cudaSuccess) {
+            for (void* p : {(void*)ctx->d_sub_U, (void*)ctx->d_sub_vecs, (void*)ctx->d_sub_t, (void*)ctx->d_sub_idx})
+                cudaFree(p);
+            ctx->d_sub_U = ctx->d_sub_vecs = ctx->d_sub_t = nullptr;
+            ctx->d_sub_idx = nullptr;
+            ctx->d_sub_keep = nullptr;
+            return fail(ctx, VPCA_ERR_NOMEM, "subset buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(ctx, grow_buffer(&ctx->d_sub_S, &ctx->cap_sub_S, (int64_t)m * m));
+    std::vector<uint8_t> keep01(n);
+    for (int s = 0; s < n; ++s) keep01[s] = keep[s] != 0;
+    CUDA_OK(ctx, cudaEventRecord(ctx->ev_e0, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sub_idx, idx.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sub_keep, keep01.data(), (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->c_h2d += (int64_t)n * 5;
+    CUDA_OK(ctx, subset_gather(ctx->d_S, n, ctx->d_sub_idx, m, ctx->d_sub_S, ctx->stream));
+    EigWork& w = ctx->sub_eig;
+    CUDA_OK(ctx, center_gram(w, ctx->d_sub_S, ctx->stream, false));
+    {   // VPCA_EIG as for vpca_compute_pca
+        const char* em = getenv("VPCA_EIG");
+        w.mode = (em != nullptr && strcmp(em, "direct") == 0) ? 1 : (em != nullptr && strcmp(em, "lanczos") == 0) ? 2 : 0;
+    }
+    int64_t launches = 3;
+    CUDA_OK(ctx, eig_topk(w, k, ctx->stream, &launches));
+    CUDA_OK(ctx, subset_place(ctx->d_S, n, ctx->d_sub_idx, m, w.d_evecs, w.d_evals, w.d_rowsum, k, ctx->d_sub_U,
+                              ctx->d_sub_vecs, ctx->d_sub_t, ctx->stream));
+    launches += m < n ? 3 : 1;
+    ctx->c_launches += launches;
+    CUDA_OK(ctx, cudaEventRecord(ctx->ev_e1, ctx->stream));
+    ctx->st.eig_method = w.last_method;
+    ctx->st.eig_iterations = w.last_iters;
+    ctx->eig_timed = true;
+    const size_t nb = (size_t)n * k * sizeof(double);
+    CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->d_sub_vecs, nb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, w.d_evals, k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    int nz = 0;
+    CUDA_OK(ctx, cudaMemcpyAsync(&nz, w.d_nz, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    if (non_zero_rows) *non_zero_rows = nz;
+    ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
+    ctx->pca_k = k;
+    ctx->d_U = ctx->d_sub_U;
+    return VPCA_OK;
+}
+
 // Top-k of a Gram stored as row bands in `world` contexts (eig.cu, band_eig_topk): Lanczos driven from rank 0 with the
 // mat-vec sharded over the bands.  Neither S nor the FP64 centred matrix is ever assembled, so neither the 65 535-sample
 // limit of vpca_compute_pca nor its N x N workspace applies.  The direct reduction that backs the one-GPU Lanczos needs
@@ -1424,8 +1527,9 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
 // the context's own; host-input calls run on a staging lane (encode as for the Gram), panel calls on the ctx stream.
 static constexpr int kProjLd = 16;   // row pitch (doubles) of the projection accumulator
 
-// On success *U is the U the loadings read (valid until the next solve, reset or Gram change of this context).
-static int loadings_check(vpca_ctx* ctx, int32_t k, const double** U) {   // caller holds ctx->mu
+// On success *U is the U the loadings read (valid until the next solve, reset or Gram change of this context), and *keep
+// the keep bytes of the subset solve that made it (nullptr after any other solve).
+static int loadings_check(vpca_ctx* ctx, int32_t k, const double** U, const uint8_t** keep) {   // caller holds ctx->mu
     if (ctx->band_rows != ctx->n && ctx->pca_k == 0)
         return fail(ctx, VPCA_ERR_UNSUPPORTED, "loadings on a context that stores a row band need the eigenvectors of a "
                     "successful vpca_compute_pca_bands that named it, since its last reset / finalize_gram");
@@ -1435,6 +1539,7 @@ static int loadings_check(vpca_ctx* ctx, int32_t k, const double** U) {   // cal
                     "set_gram / load_partial_gram / finalize_gram");
     if (k > ctx->pca_k) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings of %d components, the last solve computed %d", k, ctx->pca_k);
     *U = ctx->d_U;
+    *keep = ctx->d_U == ctx->d_sub_U ? ctx->d_sub_keep : nullptr;
     return VPCA_OK;
 }
 
@@ -1457,10 +1562,10 @@ static int project_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int
     return VPCA_OK;
 }
 
-static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, const double* U, int k,
-                          double* out_w, int32_t* out_count) {
+static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, const double* U,
+                          const uint8_t* keep, int k, double* out_w, int32_t* out_count) {
     CUDA_OK(ctx, loadings_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, U, k, ctx->d_lp_w,
-                                 ctx->d_lp_count, L.stream));
+                                 ctx->d_lp_count, keep, L.stream));
     CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_lp_w, (size_t)nvc * k * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
     CUDA_OK(ctx, cudaMemcpyAsync(out_count + v, ctx->d_lp_count, (size_t)nvc * sizeof(int32_t), cudaMemcpyDeviceToHost, L.stream));
     ctx->c_launches += 1;
@@ -1488,9 +1593,10 @@ int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const 
         (nv > 0 && sample_idx == nullptr && offsets[nv] > offsets[0]))
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_calls: bad argument");
     const double* U = nullptr;
+    const uint8_t* keep = nullptr;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
-        int rc = loadings_check(ctx, k, &U);
+        int rc = loadings_check(ctx, k, &U, &keep);
         if (rc != VPCA_OK) return rc;
     }
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
@@ -1500,7 +1606,7 @@ int vpca_loadings_calls(vpca_ctx* ctx, int32_t k, const int64_t* offsets, const 
     int rc = lp_buffers(ctx, k, false);
     if (rc != VPCA_OK) return rc;
     auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) {
-        return loadings_chunk(ctx, L, b, v, nvc, U, k, out_w, out_count);
+        return loadings_chunk(ctx, L, b, v, nvc, U, keep, k, out_w, out_count);
     };
     return process_calls(ctx, *lg.lane, offsets, sample_idx, 4, nv, consume, false);
 }
@@ -1513,9 +1619,10 @@ int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv,
     if (nv < 0 || (nv > 0 && (rows == nullptr || out_w == nullptr || out_count == nullptr)) || stride_bytes < (ctx->n + 3) / 4)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
     const double* U = nullptr;
+    const uint8_t* keep = nullptr;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
-        int rc = loadings_check(ctx, k, &U);
+        int rc = loadings_check(ctx, k, &U, &keep);
         if (rc != VPCA_OK) return rc;
     }
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
@@ -1525,7 +1632,7 @@ int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv,
     int rc = lp_buffers(ctx, k, false);
     if (rc != VPCA_OK) return rc;
     auto consume = [&](vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc) {
-        return loadings_chunk(ctx, L, b, v, nvc, U, k, out_w, out_count);
+        return loadings_chunk(ctx, L, b, v, nvc, U, keep, k, out_w, out_count);
     };
     return process_packed(ctx, *lg.lane, rows, nv, stride_bytes, counted_allele, consume);
 }
@@ -1535,13 +1642,14 @@ int vpca_loadings_panels(vpca_ctx* ctx, int32_t k, const void* d_x, int64_t nv, 
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     std::lock_guard<std::mutex> lk(ctx->mu);
     const double* U = nullptr;
-    int rc = loadings_check(ctx, k, &U);
+    const uint8_t* keep = nullptr;
+    int rc = loadings_check(ctx, k, &U, &keep);
     if (rc != VPCA_OK) return rc;
     if (d_x == nullptr || nv < 0 || panel_variants < 128 || (panel_variants % 128) != 0 || (nv > 0 && (d_w == nullptr || d_count == nullptr)))
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_panels: panel_variants must be a positive multiple of 128");
     if ((reinterpret_cast<uintptr_t>(d_x) & 31) != 0) return fail(ctx, VPCA_ERR_BAD_ARG, "panels must be 32-byte aligned");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    CUDA_OK(ctx, loadings_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, U, k, d_w, d_count, ctx->stream));
+    CUDA_OK(ctx, loadings_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, U, k, d_w, d_count, keep, ctx->stream));
     ctx->c_launches += nv > 0 ? 1 : 0;
     return VPCA_OK;
 }

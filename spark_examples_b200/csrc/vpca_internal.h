@@ -253,13 +253,27 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
 // U: n x k column-major (ld n).  Never synchronises.  Above kSplitMinN samples the samples are summed in 4 ranges whose
 // bounds depend on n alone, the range sums added in range order (project.cu): w[v] still depends on n, column v and U only.
 constexpr int kSplitMinN = 65535;
+// d_keep != nullptr (n bytes, after a subset solve; needs n <= kSplitMinN): count[v] adds only the samples whose keep byte is
+// nonzero, U is zero on the others, and the samples are summed in the whole order whatever VPCA_LOADINGS_KERNEL says.
 cudaError_t loadings_launch(const void* d_x, int elem_bits, int n, int64_t nv, int64_t panel, const double* d_U, int k,
-                            double* d_w, int32_t* d_count, cudaStream_t stream);
+                            double* d_w, int32_t* d_count, const uint8_t* d_keep, cudaStream_t stream);
 // acc[s * acc_ld + c] += sum_v (y[s][v] - mean[v]) w[v * k + c] for the m samples: a partial sum per panel (variants in
 // order) into d_part (project_scratch_doubles entries), then the partials added in panel order.
 cudaError_t project_launch(const void* d_y, int elem_bits, int m, int64_t nv, int64_t panel, const double* d_w,
                            const double* d_mean, int k, double* d_part, double* d_acc, int acc_ld, cudaStream_t stream);
 int64_t project_scratch_doubles(int m, int64_t nv, int64_t panel, int k);
+
+// ---- principal coordinates of a subset of the samples (subset.cu, vpca_compute_pca_subset) ------------------------------
+// d_idx: the m kept samples in increasing order, then the r removed ones in increasing order (m + r = n).
+// S_KK[q1 * m + q2] = S[idx[q1]][idx[q2]] for q1, q2 < m (S: the finalized n x n Gram).  Never synchronises.
+cudaError_t subset_gather(const int32_t* d_S, int n, const int32_t* d_idx, int m, int32_t* d_SKK, cudaStream_t stream);
+// From the subset solve (u: m x k column-major, ld m; evals: k; rowsum: the m row sums of S_KK):
+//   U[c * n + s]    = u_c of sample s for kept s, 0 for removed s (c < 16; the buffer the masked loadings read)
+//   vecs[c * n + s] = u_c of sample s for kept s, p_c(s) for removed s (c < k, any k), where
+//   p_c(r) = (sum_q S[r][idx[q]] u_c[q] - (sum_q rowsum[q] u_c[q]) / m) / evals[c]
+// both sums over q in a fixed order (subset.cu), no floating-point atomics; d_t: k doubles of scratch.  Never synchronises.
+cudaError_t subset_place(const int32_t* d_S, int n, const int32_t* d_idx, int m, const double* d_u, const double* d_evals,
+                         const double* d_rowsum, int k, double* d_U, double* d_vecs, double* d_t, cudaStream_t stream);
 
 // ---- synthetic generator (synth.cu) ----------------------------------------------------------------
 cudaError_t synth_dense(uint64_t seed, int n, int64_t v0, int64_t nv, int mode, int elem_bits, void* d_x,

@@ -52,7 +52,7 @@ EXPORTED_SYMBOLS = (
     "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan",
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
-    "vpca_kinship_bed", "vpca_kinship_pairs",
+    "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
@@ -275,6 +275,8 @@ def load_library() -> ctypes.CDLL:
     L.vpca_kinship_bed.argtypes = [vp, vp, i64, i64]
     L.vpca_kinship_pairs.restype = ctypes.c_int
     L.vpca_kinship_pairs.argtypes = [vp, ctypes.c_double, i64, vp, vp, vp, ctypes.POINTER(i64)]
+    L.vpca_compute_pca_subset.restype = ctypes.c_int
+    L.vpca_compute_pca_subset.argtypes = [vp, vp, i32, vp, vp, ctypes.POINTER(i32)]
     _lib = L
     return L
 
@@ -690,6 +692,20 @@ class NativePca:
             self._check(self._lib.vpca_kinship_pairs(self._h, float(min_kinship), p, _host_ptr(ids), _host_ptr(counts),
                                                      _host_ptr(kin), ctypes.byref(total)))
         return ids[:p], counts[:p], kin[:p]
+
+    def computePcaSubset(self, keep, k: int = 2):
+        """PCs of the samples with keep[s] true, from the Gram of all of them (DESIGN.md 8) -> (vecs (n, k), evals (k,),
+        nonZeroRows of S[K, K]): kept rows hold their eigenvectors, removed rows their projection onto the same axes.
+        Afterwards the loadings calls return the kept samples' loadings."""
+        kb = np.ascontiguousarray(np.asarray(keep).reshape(-1) != 0, dtype=np.uint8)
+        if kb.shape[0] != self.n:
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"keep must have {self.n} entries")
+        flat = np.empty(self.n * k, dtype=np.float64)
+        evals = np.empty(k, dtype=np.float64)
+        nz = ctypes.c_int32(0)
+        self._check(self._lib.vpca_compute_pca_subset(self._h, _host_ptr(kb), int(k), _host_ptr(flat), _host_ptr(evals),
+                                                      ctypes.byref(nz)))
+        return flat.reshape(k, self.n).T.copy(), evals, int(nz.value)
 
 
 def debugTiles(n_samples: int, cta_group: int = 2, exact: bool = True) -> np.ndarray:

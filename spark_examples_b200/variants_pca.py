@@ -180,6 +180,7 @@ class VariantsPcaDriver:
         self._gram_tensor = None
         self._torch_stream = None
         self._bim_cache: Dict[str, list] = {}
+        self.pcaSamples: Optional[int] = None   # samples the last computePca solved for (fewer under --king-cutoff)
 
     # -- VariantsPca.scala:87 ---------------------------------------------------------------------------------------
     @property
@@ -298,7 +299,7 @@ class VariantsPcaDriver:
                     nat.accumulateJoined(pid)                   # the joined rows never leave the device
                 elif isinstance(part, BedSlice):
                     rows = part.rows()
-                    if self.conf.makeKingTable.isDefined:
+                    if self.conf.makeKingTable.isDefined or self.conf.kingCutoff.isDefined:
                         nat.kinshipBed(rows)                    # the same rows, three genotype planes (DESIGN.md 7)
                     nat.accumulateBed(pid, rows, part.counted)
                 else:
@@ -343,12 +344,33 @@ class VariantsPcaDriver:
                 S[i, j] = v                                                      # IndexError like Breeze at :216
             nat = self._native(rowCount)
             nat.setGram(S)
-        vecs, evals, nonZeroRows = nat.computePca(numPc)
-        print(f"Non zero rows in matrix: {nonZeroRows} / {rowCount}.")           # :208
+        if self.conf.kingCutoff.isDefined:
+            vecs, evals, nonZeroRows = self._computePcaUnrelated(nat, rowCount, numPc)
+        else:
+            vecs, evals, nonZeroRows = nat.computePca(numPc)
+            self.pcaSamples = rowCount
+            print(f"Non zero rows in matrix: {nonZeroRows} / {rowCount}.")       # :208
         self.eigenvalues = evals
         self.components = vecs                                                   # all numPc columns (Python twin prints them)
         reverse = {i: cid for cid, i in self.common.indexes.items()}             # :228
         return [(reverse[i], float(vecs[i, 0]), float(vecs[i, 1])) for i in range(rowCount)]   # :229-230
+
+    def _computePcaUnrelated(self, nat: native.NativePca, rowCount: int, numPc: int):
+        """--king-cutoff X: the PCs of a maximal set of samples without a pair of KINSHIP > X, from the same Gram; every
+        other sample is projected onto them from its Gram row (DESIGN.md 8).  The kinship counts rode on the Gram pass."""
+        cutoff = self.conf.kingCutoff()
+        ids, _, kin = nat.kinshipPairs(np.nextafter(cutoff, np.inf))              # exactly the pairs with KINSHIP > X
+        keep = king_cutoff_keep(rowCount, ids, kin, cutoff)
+        m = int(keep.sum())
+        check_king_cutoff_kept(m, numPc)
+        print(f"KING cutoff {cutoff!r}: {m} of {rowCount} samples kept, {rowCount - m} projected.")
+        if self.conf.outputPath.isDefined and self._rank == 0:
+            from . import plink
+            write_king_cutoff_ids(self.conf.outputPath(), plink.read_fam_ids(self.conf.bedPath()), keep)
+        vecs, evals, nonZeroRows = nat.computePcaSubset(keep, numPc)
+        print(f"Non zero rows in matrix: {nonZeroRows} / {m}.")                  # :208, of the kept samples' matrix
+        self.pcaSamples = m
+        return vecs, evals, nonZeroRows
 
     # -- VariantsPca.scala:233-246 ----------------------------------------------------------------------------------
     def emitResult(self, result: Sequence[Tuple[str, float, float]], out=None):
@@ -449,7 +471,7 @@ class VariantsPcaDriver:
             return np.concatenate([merged[p][i] for p in order]) if order else empty
         with open(path, "wb") as fh:
             np.savez(fh, loadings=cat(1, np.zeros((0, k))), count=cat(2, np.zeros(0, np.int32)),
-                     n_samples=np.int64(len(self.common.indexes)), eigenvalues=np.asarray(self.eigenvalues[:k], np.float64),
+                     n_samples=np.int64(self.pcaSamples or len(self.common.indexes)), eigenvalues=np.asarray(self.eigenvalues[:k], np.float64),
                      counted_allele=np.int32(self._counted_allele(callsets)), keys=cat(0, np.zeros((0, 2), np.uint64)),
                      key_kind=np.str_(kind))
 
@@ -623,22 +645,68 @@ def write_king_table(path: str, fam: Sequence[Tuple[str, str]], ids: np.ndarray,
 
 
 def check_king_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
-    """Refuse --make-king-table / --king-table-filter runs the kinship path cannot serve, before any GPU work:
-    without n_samples the flag combinations, with it the cohort size."""
+    """Refuse --make-king-table / --king-table-filter / --king-cutoff runs the kinship path cannot serve, before any GPU
+    work: without n_samples the flag combinations, with it the cohort size."""
     if conf.kingTableFilter.isDefined and not conf.makeKingTable.isDefined:
         raise ValueError("--king-table-filter needs --make-king-table")
-    if not conf.makeKingTable.isDefined:
-        return
-    if not conf.bedPath.isDefined:
-        raise ValueError("--make-king-table needs genotype classes (het / hom): give a PLINK fileset with --bed-path")
-    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
-        raise ValueError("--make-king-table runs on one GPU; launch a single process (WORLD_SIZE=1)")
-    if conf.checkpointPath.isDefined:
-        raise ValueError("--make-king-table counts every partition in one pass; it cannot resume from --checkpoint-path")
-    if conf.projectLoadings.isDefined:
-        raise ValueError("--project-loadings builds no similarity matrix for --make-king-table to ride on")
-    if n_samples is not None and n_samples > native.KINSHIP_MAX_SAMPLES:
-        raise ValueError(f"--make-king-table is limited to {native.KINSHIP_MAX_SAMPLES} samples; the cohort has {n_samples}")
+    if conf.kingCutoff.isDefined and not np.isfinite(conf.kingCutoff()):
+        raise ValueError(f"--king-cutoff must be a finite kinship, not {conf.kingCutoff()!r}")
+    for flag, opt in (("--make-king-table", conf.makeKingTable), ("--king-cutoff", conf.kingCutoff)):
+        if not opt.isDefined:
+            continue
+        if not conf.bedPath.isDefined:
+            raise ValueError(f"{flag} needs genotype classes (het / hom): give a PLINK fileset with --bed-path")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            raise ValueError(f"{flag} runs on one GPU; launch a single process (WORLD_SIZE=1)")
+        if conf.checkpointPath.isDefined:
+            raise ValueError(f"{flag} counts every partition in one pass; it cannot resume from --checkpoint-path")
+        if conf.projectLoadings.isDefined:
+            raise ValueError(f"--project-loadings builds no similarity matrix for {flag} to ride on")
+        if n_samples is not None and n_samples > native.KINSHIP_MAX_SAMPLES:
+            raise ValueError(f"{flag} is limited to {native.KINSHIP_MAX_SAMPLES} samples; the cohort has {n_samples}")
+
+
+def check_king_cutoff_kept(kept: int, num_pc: int) -> None:
+    """Refuse a --king-cutoff selection that leaves too few samples for the PCs asked for."""
+    if kept < 2 or kept < num_pc:
+        raise ValueError(f"--king-cutoff keeps {kept} samples: at least max(2, --num-pc = {num_pc}) are needed")
+
+
+def king_cutoff_keep(n: int, ids, kinship, cutoff: float) -> np.ndarray:
+    """(n,) bool: a maximal set of samples without a pair of KINSHIP > cutoff (NaN is never related), chosen
+    deterministically.  While related pairs remain, the sample with the most remaining related partners is removed (the
+    larger index on a tie); then, in increasing index order, a removed sample returns when none of its relatives is in
+    the set.  PLINK 2's --king-cutoff follows the same greedy idea; its tie-breaking is not reproduced."""
+    ids = np.asarray(ids, np.int64).reshape(-1, 2)
+    kin = np.asarray(kinship, np.float64).reshape(-1)
+    partners: List[set] = [set() for _ in range(n)]
+    for a, b in ids[kin > cutoff].tolist():
+        if a != b:
+            partners[a].add(b)
+            partners[b].add(a)
+    removed = np.zeros(n, bool)
+    degree = np.array([len(p) for p in partners], np.int64)
+    while n and degree.max() > 0:
+        r = int(np.flatnonzero(degree == degree.max())[-1])
+        removed[r] = True
+        degree[r] = 0
+        for j in partners[r]:
+            if not removed[j]:
+                degree[j] -= 1
+    for r in np.flatnonzero(removed).tolist():
+        if all(removed[j] for j in partners[r]):
+            removed[r] = False
+    return ~removed
+
+
+def write_king_cutoff_ids(prefix: str, fam: Sequence[Tuple[str, str]], keep: np.ndarray) -> None:
+    """PLINK 2's --king-cutoff outputs: prefix.king.cutoff.in.id (the kept samples) and .out.id (the removed ones),
+    `#FID<TAB>IID` then one line per sample in fileset order."""
+    keep = np.asarray(keep, bool)
+    for suffix, sel in ((".king.cutoff.in.id", keep), (".king.cutoff.out.id", ~keep)):
+        with open(prefix + suffix, "w", encoding="utf-8") as fh:
+            fh.write("#FID\tIID\n")
+            fh.write("".join(f"{fam[s][0]}\t{fam[s][1]}\n" for s in np.flatnonzero(sel).tolist()))
 
 
 def joined_rows_on_host(p: JoinedSlice) -> CallsBatch:

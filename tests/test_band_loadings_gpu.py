@@ -82,6 +82,7 @@ def _contexts(n, nv, world, form, cells=None, num_pc=2, dtype=0, panel=P):
             with torch.cuda.device(devs[r]):
                 if cells is None:
                     buf = torch.zeros(c.panelBytes(v1 - v0, panel), dtype=torch.uint8, device=f"cuda:{devs[r]}")
+                    torch.cuda.synchronize(devs[r])   # zeroed before the context's own stream writes the cells
                     c.synthPanelsDevice(SEED, v0, v1 - v0, 0, buf.data_ptr(), panel)
                 else:
                     buf = _panel_buffer(np.ascontiguousarray(cells[:, v0:v1]), devs[r], panel, dtype)
@@ -293,6 +294,7 @@ def _generated_cells(n, nv):
     from spark_examples_b200 import native
     with native.NativePca(n, max_multiplicity=1, gram_band=(0, 64)) as gen:
         buf = torch.zeros(gen.panelBytes(nv, nv), dtype=torch.uint8, device="cuda:0")
+        torch.cuda.synchronize(0)   # zeroed before the context's own stream writes the cells
         gen.synthPanelsDevice(SEED, 0, nv, 0, buf.data_ptr(), nv)
         gen.synchronize()
     return buf.view(torch.int8).view(n, nv)
@@ -321,6 +323,7 @@ def test_band_loadings_past_the_reference_sample_limit():
                 for r, c in enumerate(ctxs):
                     v0, v1 = shards[r]
                     b2 = torch.zeros(c.panelBytes(v1 - v0, 2048), dtype=torch.uint8, device=f"cuda:{_devices(world)[r]}")
+                    torch.cuda.synchronize(_devices(world)[r])   # zeroed before the context's own stream writes the cells
                     c.synthPanelsDevice(SEED, v0, v1 - v0, 0, b2.data_ptr(), 2048)
                     wide.append(_panel_loadings(c, k, b2, v1 - v0, 2048))
                     del b2

@@ -52,6 +52,7 @@ def _contexts(n, nv, world, form, cells=None, num_pc=2):
             with torch.cuda.device(devs[r]):
                 if cells is None:
                     buf = torch.zeros(c.panelBytes(v1 - v0, P), dtype=torch.uint8, device=f"cuda:{devs[r]}")
+                    torch.cuda.synchronize(devs[r])   # zeroed before the context's own stream writes the cells
                     c.synthPanelsDevice(SEED, v0, v1 - v0, 0, buf.data_ptr(), P)
                 else:
                     buf = _panel_buffer(np.ascontiguousarray(cells[:, v0:v1]), devs[r])
@@ -171,6 +172,7 @@ def test_band_pca_past_the_reference_sample_limit():
     # the same cells, regenerated by the same generator into one buffer
     with native.NativePca(n, max_multiplicity=1, gram_band=(0, 64)) as gen:     # a generator, not a 20 GB Gram
         buf = torch.zeros(gen.panelBytes(nv, nv), dtype=torch.uint8, device="cuda:0")
+        torch.cuda.synchronize(0)   # zeroed before the context's own stream writes the cells
         gen.synthPanelsDevice(SEED, 0, nv, 0, buf.data_ptr(), nv)
         gen.synchronize()
     X = buf.view(torch.int8).view(n, nv).to(torch.float64)

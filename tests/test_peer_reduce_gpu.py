@@ -90,6 +90,7 @@ def _panels(ctx, dev, v0, nv):
     import torch
     with torch.cuda.device(dev):
         buf = torch.zeros(ctx.panelBytes(nv, P), dtype=torch.uint8, device=f"cuda:{dev}")
+        torch.cuda.synchronize(dev)   # zeroed before the context's own stream writes the cells
     ctx.synthPanelsDevice(SEED, v0, nv, 1, buf.data_ptr(), P)
     return buf
 

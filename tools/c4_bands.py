@@ -83,6 +83,9 @@ def main():
         for r, c in enumerate(ctxs):
             torch.cuda.set_device(devs[r])
             buf = torch.zeros(c.panelBytes(per, P), dtype=torch.uint8, device=f"cuda:{devs[r]}")
+            # the zeros are written on torch's stream, the cells on the context's own non-blocking stream: without this
+            # wait the two race, and zeros landing after the cells leave the ranks' copies of the cohort different
+            torch.cuda.synchronize(devs[r])
             bufs.append(buf)
             c.synthPanelsDevice(20240901, 0 if computes else r * per, per, 0, buf.data_ptr(), P)
         for c in ctxs:

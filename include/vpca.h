@@ -361,6 +361,34 @@ int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int
 int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, double* vecs, double* evals,
                             int32_t* non_zero_rows);
 
+/* ---- LD pruning of the variants (beyond VariantsPca.scala: which variants go into S, VariantsPca.scala:182-191) ---------
+ * Blocks of correlated nearby variants make the top components follow local haplotype structure instead of ancestry; the
+ * usual remedy is to keep roughly independent variants only.  For variants i < j, over the samples called at both, with x
+ * and y their A1 counts (0 / 1 / 2) and n, Sx, Sy, Sxx, Syy, Sxy the exact integer sums:
+ *   cov = n Sxy - Sx Sy   vx = n Sxx - Sx^2   vy = n Syy - Sy^2     (int64, exact)
+ *   r2 = (double(cov) * double(cov)) / (double(vx) * double(vy))     (each operation rounded once)
+ * i and j are in LD iff vx > 0 && vy > 0 && r2 > r2_max.  The rows (PLINK 1 .bed, as vpca_accumulate_bed) are unpacked into
+ * three int8 planes per chunk of variants -- A1 count, its square, called -- with the samples as the K axis, and every sum
+ * is one lower-triangle entry of their Gram on the int8 Gram kernel (DESIGN.md 9).  The result does not depend on which
+ * allele is counted (x -> 2 - x leaves r2 unchanged).
+ * vpca_ld_prune_bed: window_lo[j] (nv entries, 0 <= window_lo[j] <= j, non-decreasing) is the first variant of j's window;
+ *   keep[j] (nv bytes) = 1 iff no kept variant i with window_lo[j] <= i < j is in LD with j (keep-first, in order; the
+ *   unique set in which no two kept variants of a window are in LD and every pruned variant is in LD with an earlier kept
+ *   one of its window).  *n_pairs = the number of in-LD pairs (i, j) with window_lo[j] <= i < j; the first
+ *   min(total, max_pairs) of them, in order of j, then i, go to out_pairs[2p] = i, out_pairs[2p + 1] = j and out_r2[p];
+ *   max_pairs = 0 with NULL outputs counts only.  Driver-side and synchronous; int8 planes whatever cfg.dtype is.  The
+ *   variants are walked in chunks that overlap by H = max_j (j - window_lo[j]), the samples in pieces of at most 32 768,
+ *   so device memory grows with H but not with the number of samples or variants, apart from nv keep bytes: up to about
+ *   2.8 GB at H = VPCA_LD_MAX_WINDOW (a 24 576 x 24 576 int32 Gram).  Buffers are allocated on the first call and freed
+ *   by vpca_destroy; the PCA Gram, U, the kinship counts and the subset state are left alone.
+ *   VPCA_ERR_BAD_ARG, before any row is staged: rows, window_lo, keep or n_pairs NULL, stride_bytes < ceil(n_samples / 4),
+ *   a window_lo outside [0, j] or decreasing, r2_max not finite or outside [0, 1), max_pairs > 0 with NULL outputs.
+ *   VPCA_ERR_UNSUPPORTED, before any row is staged, when H > VPCA_LD_MAX_WINDOW. */
+#define VPCA_LD_MAX_WINDOW 4096
+int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const int64_t* window_lo,
+                      double r2_max, uint8_t* keep, int64_t max_pairs, int64_t* out_pairs, double* out_r2,
+                      int64_t* n_pairs);
+
 /* ---- one process, all GPUs of the box (SURVEY 8b "process model") --------------------------------------------------
  * A vpca_pool is what `class VariantsPcaDriver` holds on a multi-GPU host: one vpca_ctx per GPU, wired with
  * vpca_gram_set_peers_local in VPCA_PEER_OWNER_ROWS mode (VPCA_PEER_REPLICATE when n_samples < 64 x n_gpus).  Spark

@@ -118,4 +118,6 @@ class PcaConf(GenomicsConf):
             ("kingTableFilter", float, None, False),      # keep only the pairs with KINSHIP >= this (PLINK 2's flag names)
             ("kingCutoff", float, None, False),           # --bed-path runs: PCs of a maximal set without KINSHIP > this; the
                                                           # relatives projected onto them (PLINK 2's flag name)
+            ("ldPrune", float, None, False),              # --bed-path runs: keep-first LD pruning, r2 > this within a window
+            ("ldWindowKb", float, 500.0, False),          # the window of --ld-prune: same contig, positions <= this many kb apart
         ]

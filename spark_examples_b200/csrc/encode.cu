@@ -260,7 +260,49 @@ __global__ void bed_planes_kernel(const uint8_t* __restrict__ rows, int64_t stri
     store_i8_cells(base + (2 * (int64_t)n + smp) * panel, m_hom2);
 }
 
+// .bed rows -> the three int8 planes of LD pruning (DESIGN.md 9) for samples [s0, s0 + len) of a chunk of c variant rows:
+// in a tile of 3c rows, row v is the A1 count D (00 -> 2, 10 -> 1, 11 -> 0), row c + v is Q = D^2, row 2c + v is M = 1 if
+// called; a missing call (01) is 0 in all three.  Samples are the K axis here, so this is a plain unpack: a thread reads 4
+// bytes (16 samples) of one row and writes 16 cells of each plane.  Rows v >= nv and samples >= n are written as zero, so
+// every cell of the ceil(len / panel) panels is defined.
+__global__ void ld_planes_kernel(const uint8_t* __restrict__ rows, int64_t pitch, int64_t width, int nv, int c, int64_t s0,
+                                 int64_t len, int n, uint8_t* __restrict__ x, int64_t panel) {
+    const int64_t groups = ((len + panel - 1) / panel) * panel / 16;   // 16-sample groups per row
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= groups * c) return;
+    const int v = (int)(t / groups);
+    const int64_t q = t - (int64_t)v * groups, sl = q * 16;
+    uint32_t w = 0x55555555u;   // all missing
+    if (v < nv && 4 * q < width) w = *reinterpret_cast<const uint32_t*>(rows + (int64_t)v * pitch + 4 * q);
+    uint32_t d[4] = {0, 0, 0, 0}, sq[4] = {0, 0, 0, 0}, m[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const uint32_t code = (w >> (2 * j)) & 3u;
+        const bool ok = code != 1u && s0 + sl + j < n;
+        const uint32_t dv = ok ? (code == 0u ? 2u : (code == 2u ? 1u : 0u)) : 0u;
+        d[j >> 2] |= dv << (8 * (j & 3));
+        sq[j >> 2] |= (dv * dv) << (8 * (j & 3));
+        m[j >> 2] |= (ok ? 1u : 0u) << (8 * (j & 3));
+    }
+    const int64_t pnl = sl / panel, col = sl - pnl * panel, R = 3 * (int64_t)c;
+    uint8_t* base = x + pnl * R * panel + col;
+    *reinterpret_cast<uint4*>(base + (int64_t)v * panel) = make_uint4(d[0], d[1], d[2], d[3]);
+    *reinterpret_cast<uint4*>(base + ((int64_t)c + v) * panel) = make_uint4(sq[0], sq[1], sq[2], sq[3]);
+    *reinterpret_cast<uint4*>(base + (2 * (int64_t)c + v) * panel) = make_uint4(m[0], m[1], m[2], m[3]);
+}
+
 }  // namespace
+
+cudaError_t encode_ld_planes(const uint8_t* d_rows, int64_t pitch, int64_t width, int nv, int c, int64_t s0, int64_t len,
+                             int n, void* d_x, int64_t panel, cudaStream_t stream) {
+    if (len <= 0) return cudaSuccess;
+    const int64_t threads_total = ((len + panel - 1) / panel) * panel / 16 * c;
+    const int threads = 256;
+    const int64_t blocks = (threads_total + threads - 1) / threads;
+    ld_planes_kernel<<<(unsigned)blocks, threads, 0, stream>>>(d_rows, pitch, width, nv, c, s0, len, n,
+                                                               static_cast<uint8_t*>(d_x), panel);
+    return cudaGetLastError();
+}
 
 cudaError_t encode_bed_planes(const uint8_t* d_rows, int64_t stride, int64_t nv, int n, void* d_x, int64_t panel,
                               cudaStream_t stream) {
@@ -369,6 +411,7 @@ cudaError_t encode_preload_kernels() {
     VPCA_LOAD((encode_e2m1_kernel<int32_t>)); VPCA_LOAD((encode_e2m1_kernel<uint16_t>));
     VPCA_LOAD((bits_to_cells_kernel<8>)); VPCA_LOAD((bits_to_cells_kernel<4>)); VPCA_LOAD((bits_to_cells_kernel<16>));
     VPCA_LOAD(bed_planes_kernel);
+    VPCA_LOAD(ld_planes_kernel);
 #undef VPCA_LOAD
     return e;
 }

@@ -84,6 +84,16 @@ struct vpca_ctx {
     int64_t kin_chunk = 0, kin_panel = 0;   // rows per staged chunk, variants per panel of the 3n-row plane tile
     int64_t kin_variants = 0;               // rows added since creation / the last vpca_reset
     KinPairWork kin_pairs;
+    // LD pruning (vpca_ld_prune_bed): the 3c x 3c plane Gram of one chunk, its plane tile, double-buffered raw rows, the
+    // chunk's window starts, the pair scratch and the keep bytes; all grow-only, with a Gram schedule of their own
+    int32_t* d_ld_G = nullptr;
+    void* d_ld_x = nullptr;
+    uint8_t* d_ld_rows[2] = {nullptr, nullptr};
+    int64_t* d_ld_wlo = nullptr;
+    uint8_t* d_ld_keep = nullptr;
+    int64_t cap_ld_G = 0, cap_ld_x = 0, cap_ld_rows = 0, cap_ld_wlo = 0, cap_ld_keep = 0, cap_ld_words = 0;
+    GramPlan ld_plan;
+    LdWork ld;
 
     struct Slot {
         int64_t pid = -1;
@@ -673,6 +683,11 @@ int vpca_destroy(vpca_ctx* ctx) {
     for (void* p : ctx->d_kin_x) cudaFree(p);
     gram_plan_free(ctx->kin_plan);
     kin_pair_free(ctx->kin_pairs);
+    for (void* p : {(void*)ctx->d_ld_G, ctx->d_ld_x, (void*)ctx->d_ld_rows[0], (void*)ctx->d_ld_rows[1], (void*)ctx->d_ld_wlo,
+                    (void*)ctx->d_ld_keep, (void*)ctx->ld.d_bits, (void*)ctx->ld.d_seg, (void*)ctx->ld.d_row_total,
+                    (void*)ctx->ld.d_row_start, (void*)ctx->ld.d_total, (void*)ctx->ld.d_pairs, (void*)ctx->ld.d_r2})
+        cudaFree(p);
+    gram_plan_free(ctx->ld_plan);
     gram_plan_free(ctx->plan);
     for (cudaEvent_t ev : {ctx->ev_t0, ctx->ev_t1, ctx->ev_e0, ctx->ev_e1})
         if (ev) cudaEventDestroy(ev);
@@ -1892,6 +1907,218 @@ int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int
         lo = hi;
     }
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return VPCA_OK;
+}
+
+// ---- LD pruning (ld.cu, DESIGN.md 9) ----------------------------------------------------------------------------------
+// Driver-side and synchronous.  The variants are walked in chunks of c rows that overlap by H = max_j (j - window_lo[j]);
+// a chunk decides the rows it does not share with the previous one, whose windows then lie inside it.  The samples of a
+// chunk are split into pieces of at most kLdMaxPiece, each staged on a lane (its H2D copy overlaps the previous piece's
+// encode and Gram) and added into the same plane Gram, so staging is bounded whatever the cohort size.
+namespace {
+constexpr int64_t kLdMaxPiece = 32768;            // samples per staged piece
+constexpr int64_t kLdPlaneBudget = 256ll << 20;   // bytes of the plane tile of one piece
+constexpr int64_t kLdWindowBytes = 16ll << 20;    // bytes of one panel of the plane tile (the Gram kernel's L2 window)
+
+// (re)allocates *p for `need` elements of `elem` bytes unless it already holds `cap` >= need
+cudaError_t ld_grow_bytes(void** p, int64_t& cap, int64_t need, size_t elem) {
+    if (need <= cap) return cudaSuccess;
+    cudaFree(*p);
+    *p = nullptr;
+    cap = 0;
+    cudaError_t e = cudaMalloc(p, (size_t)need * elem);
+    if (e == cudaSuccess) cap = need;
+    return e;
+}
+#define ld_grow(ptr, cap, need) ld_grow_bytes(reinterpret_cast<void**>(&(ptr)), (cap), (need), sizeof(*(ptr)))
+
+// Grows every buffer of one call: the 3c x 3c Gram, the plane tile (x_bytes), two row buffers (row_bytes each), the window
+// starts and the row arrays (c), the bit words (c T), a pair scratch that holds a whole row tile (32 rows of at most 32 T
+// pairs) and the keep bytes (nv).
+cudaError_t ld_buffers(vpca_ctx* ctx, int64_t c, int T, int64_t x_bytes, int64_t row_bytes, int64_t nv) {
+    LdWork& w = ctx->ld;
+    cudaError_t e = ld_grow(ctx->d_ld_G, ctx->cap_ld_G, 9 * c * c);
+    if (e == cudaSuccess) {
+        e = ld_grow_bytes(&ctx->d_ld_x, ctx->cap_ld_x, x_bytes, 1);
+    }
+    if (e == cudaSuccess && row_bytes > ctx->cap_ld_rows) {
+        int64_t c0 = 0, c1 = 0;
+        cudaFree(ctx->d_ld_rows[0]);
+        cudaFree(ctx->d_ld_rows[1]);
+        ctx->d_ld_rows[0] = ctx->d_ld_rows[1] = nullptr;
+        ctx->cap_ld_rows = 0;
+        e = ld_grow(ctx->d_ld_rows[0], c0, row_bytes);
+        if (e == cudaSuccess) e = ld_grow(ctx->d_ld_rows[1], c1, row_bytes);
+        if (e == cudaSuccess) ctx->cap_ld_rows = row_bytes;
+    }
+    if (e == cudaSuccess) e = ld_grow(ctx->d_ld_wlo, ctx->cap_ld_wlo, c);
+    if (e == cudaSuccess) e = ld_grow(ctx->d_ld_keep, ctx->cap_ld_keep, nv);
+    if (e == cudaSuccess && c * T > w.cap_words) {
+        int64_t cb = 0, cs = 0;
+        cudaFree(w.d_bits);
+        cudaFree(w.d_seg);
+        w.d_bits = nullptr;
+        w.d_seg = nullptr;
+        w.cap_words = 0;
+        e = ld_grow(w.d_bits, cb, c * T);
+        if (e == cudaSuccess) e = ld_grow(w.d_seg, cs, c * T);
+        if (e == cudaSuccess) w.cap_words = c * T;
+    }
+    if (e == cudaSuccess && c > w.cap_rows) {
+        int64_t ct = 0, cs = 0;
+        cudaFree(w.d_row_total);
+        cudaFree(w.d_row_start);
+        w.d_row_total = nullptr;
+        w.d_row_start = nullptr;
+        w.cap_rows = 0;
+        e = ld_grow(w.d_row_total, ct, c);
+        if (e == cudaSuccess) e = ld_grow(w.d_row_start, cs, c);
+        if (e == cudaSuccess) w.cap_rows = c;
+    }
+    const int64_t pairs = std::max<int64_t>(int64_t(1) << 20, 1024 * (int64_t)T);
+    if (e == cudaSuccess && pairs > w.cap) {
+        int64_t cp = 0, cr = 0;
+        cudaFree(w.d_pairs);
+        cudaFree(w.d_r2);
+        w.d_pairs = nullptr;
+        w.d_r2 = nullptr;
+        w.cap = 0;
+        e = ld_grow(w.d_pairs, cp, 2 * pairs);
+        if (e == cudaSuccess) e = ld_grow(w.d_r2, cr, pairs);
+        if (e == cudaSuccess) w.cap = pairs;
+    }
+    if (e == cudaSuccess && w.d_total == nullptr) e = cudaMalloc(&w.d_total, sizeof(int64_t));
+    return e;
+}
+#undef ld_grow
+}   // namespace
+
+int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const int64_t* window_lo,
+                      double r2_max, uint8_t* keep, int64_t max_pairs, int64_t* out_pairs, double* out_r2,
+                      int64_t* n_pairs) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    const int n = ctx->n;
+    if (rows == nullptr || window_lo == nullptr || keep == nullptr || n_pairs == nullptr || nv < 0 ||
+        stride_bytes < (n + 3) / 4 || max_pairs < 0 || (max_pairs > 0 && (out_pairs == nullptr || out_r2 == nullptr)))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_ld_prune_bed: bad argument (rows, window_lo, keep and n_pairs must be set, "
+                    "stride_bytes >= ceil(n_samples / 4))");
+    if (!std::isfinite(r2_max) || r2_max < 0.0 || r2_max >= 1.0)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_ld_prune_bed: r2_max must be in [0, 1), not %g", r2_max);
+    int64_t H = 0;
+    for (int64_t j = 0; j < nv; ++j) {
+        const int64_t lo = window_lo[j];
+        if (lo < 0 || lo > j || (j > 0 && lo < window_lo[j - 1]))
+            return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_ld_prune_bed: window_lo[%lld] = %lld must lie in [window_lo[j - 1], j]",
+                        (long long)j, (long long)lo);
+        H = std::max(H, j - lo);
+    }
+    if (H > kLdMaxWindow) {
+        int64_t j = 0;
+        while (j - window_lo[j] <= kLdMaxWindow) ++j;
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "vpca_ld_prune_bed: the window of variant %lld reaches back %lld variants; "
+                    "the limit is %d", (long long)j, (long long)(j - window_lo[j]), kLdMaxWindow);
+    }
+    *n_pairs = 0;
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+
+    // geometry: c = 2H minimises the Gram per decided variant, 4.5 c^2 / (c - H) products per sample (DESIGN.md 9)
+    int64_t c = ((std::max<int64_t>(2 * H, 1024) + 31) / 32) * 32;
+    if (nv <= c) c = ((nv + 31) / 32) * 32;
+    const int T = (int)((H + 31) / 32) + 1;
+    const int64_t R = 3 * c;
+    const int64_t n128 = ((int64_t)n + 127) / 128 * 128;
+    const int64_t P = std::min(n128, std::max<int64_t>(128, std::min<int64_t>(8192, kLdWindowBytes / R / 128 * 128)));
+    int64_t piece = std::max(P, std::min(kLdMaxPiece, kLdPlaneBudget / R) / P * P);
+    piece = std::min(piece, ((int64_t)n + P - 1) / P * P);
+    const int64_t rp = piece / 4;                       // staged bytes per row and piece
+    const int64_t row_bytes = ((int64_t)n + 3) / 4;     // meaningful bytes of a .bed row
+
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    LdWork& w = ctx->ld;
+    {
+        cudaError_t e = ld_buffers(ctx, c, T, R * piece, c * rp, nv);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "LD pruning buffers for chunks of %lld variants: %s", (long long)c,
+                        cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(ctx, cudaMemsetAsync(w.d_total, 0, sizeof(int64_t), L.stream));
+    int64_t listed = 0;                   // pairs counted (and listed) before the current chunk while listing
+    bool listing = max_pairs > 0;
+    std::vector<int32_t> row_total((size_t)c);
+    std::vector<int64_t> start((size_t)c + 1);
+    int unit = 0;                         // staged pieces so far: selects the row buffer
+    for (int64_t s = 0;;) {
+        const int64_t e_end = std::min(s + c, nv);
+        LdChunk ch{ctx->d_ld_G, ctx->d_ld_wlo, s, (int)c, (int)(e_end - s), s == 0 ? 0 : (int)H, T, r2_max};
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_ld_G, 0, (size_t)(R * R) * sizeof(int32_t), L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_wlo, window_lo + s, (size_t)ch.nc * sizeof(int64_t), cudaMemcpyHostToDevice,
+                                     L.stream));
+        ctx->c_h2d += ch.nc * 8;
+        for (int64_t s0 = 0; s0 < n; s0 += piece, ++unit) {
+            const int64_t len = std::min<int64_t>(piece, n - s0);
+            const int64_t width = std::min(rp, row_bytes - s0 / 4);
+            const int b = unit & 1;
+            CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
+            CUDA_OK(ctx, cudaMemcpy2DAsync(ctx->d_ld_rows[b], (size_t)rp, rows + (size_t)s * stride_bytes + s0 / 4,
+                                           (size_t)stride_bytes, (size_t)width, (size_t)ch.nc, cudaMemcpyHostToDevice,
+                                           L.copy_stream));
+            CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
+            ctx->c_h2d += width * ch.nc;
+            CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+            CUDA_OK(ctx, encode_ld_planes(ctx->d_ld_rows[b], rp, width, ch.nc, (int)c, s0, len, n, ctx->d_ld_x, P, L.stream));
+            CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));   // the row buffer is free again
+            std::string msg;
+            cudaError_t e = gram_accumulate(ctx->ld_plan, ctx->d_ld_x, 8, (int)R, len, P, P, ctx->d_ld_G, L.stream, &msg);
+            if (e != cudaSuccess)
+                return fail(ctx, VPCA_ERR_CUDA, "LD plane Gram launch failed: %s %s", cudaGetErrorString(e), msg.c_str());
+            ctx->c_launches += 2;
+            ctx->c_gram += 1;
+        }
+        CUDA_OK(ctx, ld_count(w, ch, L.stream));
+        CUDA_OK(ctx, ld_sweep(w, ch, ctx->d_ld_keep, L.stream));
+        ctx->c_launches += 3;
+        if (listing) {
+            const int lo = ch.own_lo, nc = ch.nc;
+            CUDA_OK(ctx, cudaMemcpyAsync(row_total.data(), w.d_row_total + lo, (size_t)(nc - lo) * sizeof(int32_t),
+                                         cudaMemcpyDeviceToHost, L.stream));
+            CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+            start[lo] = listed;
+            for (int b = lo; b < nc; ++b) start[b + 1] = start[b] + row_total[b - lo];
+            CUDA_OK(ctx, cudaMemcpyAsync(w.d_row_start + lo, start.data() + lo, (size_t)(nc - lo) * sizeof(int64_t),
+                                         cudaMemcpyHostToDevice, L.stream));
+            const int64_t limit = std::min(start[nc], max_pairs);
+            auto row_end = [&](int bt) { return start[std::min(nc, std::max(lo, 32 * bt))]; };   // position after tile rows < bt
+            const int tiles_hi = (nc + 31) / 32;
+            for (int tlo = lo / 32; tlo < tiles_hi && row_end(tlo) < limit;) {
+                int thi = tlo + 1;   // as many row tiles as the scratch holds (one always fits, ld_buffers)
+                while (thi < tiles_hi && row_end(thi + 1) - row_end(tlo) <= w.cap && row_end(thi) < limit) ++thi;
+                const int64_t base = row_end(tlo), end = std::min(row_end(thi), limit), cnt = end - base;
+                if (cnt > 0) {
+                    CUDA_OK(ctx, ld_emit(w, ch, tlo, thi, base, end, L.stream));
+                    CUDA_OK(ctx, cudaMemcpyAsync(out_pairs + 2 * base, w.d_pairs, (size_t)cnt * 2 * sizeof(int64_t),
+                                                 cudaMemcpyDeviceToHost, L.stream));
+                    CUDA_OK(ctx, cudaMemcpyAsync(out_r2 + base, w.d_r2, (size_t)cnt * sizeof(double), cudaMemcpyDeviceToHost,
+                                                 L.stream));
+                    ctx->c_launches += 1;
+                    ctx->c_d2h += cnt * 24;
+                }
+                tlo = thi;
+            }
+            listed = start[nc];
+            listing = listed < max_pairs;
+        }
+        if (e_end == nv) break;
+        s = e_end - H;
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(keep, ctx->d_ld_keep, (size_t)nv, cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(n_pairs, w.d_total, sizeof(int64_t), cudaMemcpyDeviceToHost, L.stream));
+    ctx->c_d2h += nv + 8;
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     return VPCA_OK;
 }
 

@@ -105,6 +105,46 @@ cudaError_t encode_bits(const uint8_t* d_bits, int64_t stride, int64_t nv, int n
 cudaError_t encode_bed_planes(const uint8_t* d_rows, int64_t stride, int64_t nv, int n, void* d_x, int64_t panel,
                               cudaStream_t stream);
 
+// PLINK .bed rows -> the three int8 LD planes of a chunk of c variants (DESIGN.md 9) over samples [s0, s0 + len), panel
+// layout over 3c rows: row v the A1 count D, row c + v D^2, row 2c + v 1 if called (missing calls 0 in all three).  Row v of
+// the input is `pitch` bytes at d_rows + v * pitch holding samples s0 .. (its first `width` bytes are meaningful); rows
+// v >= nv and samples >= n are written as zero, and so is every cell up to the end of the last panel.
+cudaError_t encode_ld_planes(const uint8_t* d_rows, int64_t pitch, int64_t width, int nv, int c, int64_t s0, int64_t len,
+                             int n, void* d_x, int64_t panel, cudaStream_t stream);
+
+// ---- LD pruning from the 3c x 3c plane Gram of a chunk (ld.cu) -------------------------------------------------------
+constexpr int kLdMaxWindow = VPCA_LD_MAX_WINDOW;   // H: variants a window may reach back (vpca_ld_prune_bed)
+constexpr int kLdMaxChunk = 2 * kLdMaxWindow;   // C: variants per chunk (a multiple of 32)
+// One chunk: chunk rows [0, nc) are variants s0 + [0, nc), rows [own_lo, nc) are the ones it decides; wlo[v] is the global
+// window start of chunk row v.  Words: T = ceil(H / 32) + 1 per row; word w of row b holds the pairs (a, b) with a in
+// tile b / 32 - (T - 1) + w, bit a % 32.
+struct LdChunk {
+    const int32_t* G;      // 3c x 3c int32 plane Gram (lower triangle)
+    const int64_t* wlo;
+    int64_t s0;
+    int c, nc, own_lo, T;
+    double r2_max;
+};
+struct LdWork {
+    uint32_t* d_bits = nullptr;     // c x T in-LD bits
+    int32_t* d_seg = nullptr;       // c x T: pairs before word w in row b
+    int32_t* d_row_total = nullptr; // c: in-LD pairs of row b
+    int64_t* d_row_start = nullptr; // c: output position of the first pair of row b
+    int64_t* d_total = nullptr;     // in-LD pairs of the call so far
+    int64_t* d_pairs = nullptr;     // cap pairs: (i, j), then r2
+    double* d_r2 = nullptr;
+    int64_t cap = 0;                // pairs the scratch holds
+    int64_t cap_words = 0, cap_rows = 0;
+};
+// Pass 1: bits, per-word prefix, row totals (and their sum into *d_total) of the owned rows.  Never synchronises.
+cudaError_t ld_count(LdWork& w, const LdChunk& ch, cudaStream_t stream);
+// Keep-first sweep over the owned rows, in order: keep[s0 + b] = no kept a in b's window is in LD with b.  Reads keep of
+// the rows before own_lo (decided by the previous chunk).  Never synchronises.
+cudaError_t ld_sweep(LdWork& w, const LdChunk& ch, uint8_t* d_keep, cudaStream_t stream);
+// Pass 2: the in-LD pairs of row tiles [bt_lo, bt_hi) whose output position p lies in [base, end) go to scratch slot
+// p - base (needs w.d_row_start).  Never synchronises.
+cudaError_t ld_emit(LdWork& w, const LdChunk& ch, int bt_lo, int bt_hi, int64_t base, int64_t end, cudaStream_t stream);
+
 // ---- KING-robust kinship pairs from the 3n x 3n plane Gram (kinship.cu) ----------------------------------------------
 constexpr int kKinMaxN = 21845;   // 3n <= 65 535: the plane Gram stays below 2^32 cells
 // Device scratch of vpca_kinship_pairs, owned by the context and kept between calls.

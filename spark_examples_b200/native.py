@@ -52,10 +52,11 @@ EXPORTED_SYMBOLS = (
     "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan",
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
-    "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset",
+    "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
+LD_MAX_WINDOW = 4096          # vpca_ld_prune_bed: variants a window may reach back (VPCA_LD_MAX_WINDOW)
 
 
 class VpcaError(RuntimeError):
@@ -275,6 +276,8 @@ def load_library() -> ctypes.CDLL:
     L.vpca_kinship_bed.argtypes = [vp, vp, i64, i64]
     L.vpca_kinship_pairs.restype = ctypes.c_int
     L.vpca_kinship_pairs.argtypes = [vp, ctypes.c_double, i64, vp, vp, vp, ctypes.POINTER(i64)]
+    L.vpca_ld_prune_bed.restype = ctypes.c_int
+    L.vpca_ld_prune_bed.argtypes = [vp, vp, i64, i64, vp, ctypes.c_double, vp, i64, vp, vp, ctypes.POINTER(i64)]
     L.vpca_compute_pca_subset.restype = ctypes.c_int
     L.vpca_compute_pca_subset.argtypes = [vp, vp, i32, vp, vp, ctypes.POINTER(i32)]
     _lib = L
@@ -692,6 +695,34 @@ class NativePca:
             self._check(self._lib.vpca_kinship_pairs(self._h, float(min_kinship), p, _host_ptr(ids), _host_ptr(counts),
                                                      _host_ptr(kin), ctypes.byref(total)))
         return ids[:p], counts[:p], kin[:p]
+
+    # -- LD pruning of the variants (vpca.h, DESIGN.md 9) --------------------------------------------------------------
+    def ldPruneBed(self, rows: np.ndarray, window_lo, r2_max: float, max_pairs: int = 0):
+        """Keep-first LD pruning of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place, not copied) with
+        window_lo[j] the first variant of j's window -> (keep (V,) bool, pairs (P, 2) int64 of (i, j), r2 (P,) float64):
+        the first min(total, max_pairs) in-LD pairs in order of j, then i.  Synchronises."""
+        b = np.asarray(rows)
+        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
+            b = np.ascontiguousarray(b, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        nv = b.shape[0]
+        lo = np.ascontiguousarray(window_lo, dtype=np.int64).reshape(-1)
+        if len(lo) != nv:
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"window_lo must have {nv} entries")
+        keep = np.zeros(max(nv, 1), np.uint8)
+        p = max(int(max_pairs), 0)
+        pairs = np.zeros((max(p, 1), 2), np.int64)
+        r2 = np.zeros(max(p, 1), np.float64)
+        total = ctypes.c_int64(0)
+        empty = np.zeros(1, np.int64)          # a valid address for zero variants
+        rows_ptr = b.ctypes.data if b.size else _host_ptr(empty)
+        lo_ptr = lo.ctypes.data if lo.size else _host_ptr(empty)
+        self._check(self._lib.vpca_ld_prune_bed(self._h, rows_ptr, nv, b.shape[1], lo_ptr, float(r2_max), _host_ptr(keep),
+                                                p, _host_ptr(pairs) if p else None, _host_ptr(r2) if p else None,
+                                                ctypes.byref(total)))
+        got = min(int(total.value), p)
+        return keep[:nv] != 0, pairs[:got], r2[:got]
 
     def computePcaSubset(self, keep, k: int = 2):
         """PCs of the samples with keep[s] true, from the Gram of all of them (DESIGN.md 8) -> (vecs (n, k), evals (k,),

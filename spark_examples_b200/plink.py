@@ -121,10 +121,40 @@ def rows_to_calls(rows: np.ndarray, n_samples: int, counted: int = COUNT_A1):
     return off, idx
 
 
+def window_starts(bim: Sequence[BimRecord], kb: float) -> np.ndarray:
+    """(V,) int64 window_lo of LD pruning: the first variant i <= j on j's contig with pos_j - pos_i <= kb * 1000.
+    Raises ValueError unless the contigs are contiguous runs and the positions do not decrease within a contig."""
+    v = len(bim)
+    lo = np.zeros(v, np.int64)
+    pos = np.asarray([b.position for b in bim], np.int64)
+    seen = set()
+    r0 = 0
+    while r0 < v:
+        contig = bim[r0].contig
+        if contig in seen:
+            raise ValueError(f".bim is not sorted: contig {contig} comes back at variant {r0} ({bim[r0].id}, "
+                             f"{contig}:{bim[r0].position}) after other contigs")
+        seen.add(contig)
+        r1 = r0 + 1
+        while r1 < v and bim[r1].contig == contig:
+            r1 += 1
+        p = pos[r0:r1]
+        down = np.flatnonzero(np.diff(p) < 0)
+        if len(down):
+            j = r0 + int(down[0]) + 1
+            raise ValueError(f".bim is not sorted: variant {j} ({bim[j].id}, {contig}:{bim[j].position}) comes after "
+                             f"{contig}:{bim[j - 1].position}")
+        lo[r0:r1] = r0 + np.searchsorted(p, p - kb * 1000.0, side="left")
+        r0 = r1
+    return lo
+
+
 def write_fileset(prefix: str, dosage_a1: np.ndarray, fam: Sequence[Tuple[str, str]] | None = None,
-                  contig: str = "17", start: int = 41196311) -> None:
+                  contig: str = "17", start: int = 41196311, *, contigs: Sequence[str] | None = None,
+                  positions: Sequence[int] | None = None) -> None:
     """Write a fileset from an (N samples) x (V variants) array of A1 allele counts in {0, 1, 2} (-1 = missing);
-    fam = [(FID, IID)] (default ("synth", "S000000"), ...).  Used by the tests and to export the synthetic cohort."""
+    fam = [(FID, IID)] (default ("synth", "S000000"), ...).  Variant j sits on `contig` at start + j, or on contigs[j] at
+    positions[j] when those are given.  Used by the tests and to export the synthetic cohort."""
     d = np.asarray(dosage_a1)
     n, v = d.shape
     code = np.full((v, n), 1, np.uint8)                     # missing
@@ -143,7 +173,9 @@ def write_fileset(prefix: str, dosage_a1: np.ndarray, fam: Sequence[Tuple[str, s
         fh.write(packed.tobytes())
     with open(prefix + ".bim", "w", encoding="utf-8") as fh:
         for j in range(v):
-            fh.write(f"{contig}\trs{j + 1}\t0\t{start + j}\tA\tG\n")
+            c = contigs[j] if contigs is not None else contig
+            pos = int(positions[j]) if positions is not None else start + j
+            fh.write(f"{c}\trs{j + 1}\t0\t{pos}\tA\tG\n")
     with open(prefix + ".fam", "w", encoding="utf-8") as fh:
         for i in range(n):
             fid, iid = fam[i] if fam is not None else ("synth", f"S{i:06d}")

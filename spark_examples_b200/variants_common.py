@@ -56,9 +56,15 @@ class BedSlice:
     v0: int
     nv: int
     counted: int          # 1: carriers of A1, 2: carriers of A2
+    keep: Optional[np.ndarray] = None   # --ld-prune: (nv,) bool; the slice then stands for the kept rows only
 
     def rows(self) -> np.ndarray:
-        return self.bed.rows(self.v0, self.v0 + self.nv)
+        r = self.bed.rows(self.v0, self.v0 + self.nv)
+        return r if self.keep is None else r[self.keep]
+
+    @property
+    def n_rows(self) -> int:
+        return self.nv if self.keep is None else int(np.count_nonzero(self.keep))
 
 
 class VariantsDataset:

@@ -136,8 +136,8 @@ class CallsRdd:
         return rows
 
     def count(self) -> int:
-        return sum(p.nv if isinstance(p, (SyntheticSlice, BedSlice, ParquetSlice)) else len(p.offsets) - 1
-                   for p in self.partitions)
+        return sum(p.n_rows if isinstance(p, BedSlice) else p.nv if isinstance(p, (SyntheticSlice, ParquetSlice))
+                   else len(p.offsets) - 1 for p in self.partitions)
 
 
 class SimilarityMatrix:
@@ -421,6 +421,8 @@ class VariantsPcaDriver:
                 from . import plink
                 self._bim_cache[prefix] = plink.read_bim(prefix)
             bim = self._bim_cache[prefix][part.v0:part.v0 + part.nv]
+            if part.keep is not None:
+                bim = [b for b, k in zip(bim, part.keep.tolist()) if k]
             return np.asarray([_hash_words(bimKeyBytes(b)) for b in bim], np.uint64).reshape(-1, 2)
         if isinstance(part, CallsBatch) and part.keys is not None:
             return np.asarray(part.keys, np.uint64).reshape(-1, 2)
@@ -537,6 +539,24 @@ class VariantsPcaDriver:
         else:
             off, idx = _select_rows(*_partition_csr(part), sel)
             nat.projectCalls(off, idx, w, mean)
+
+    # -- LD pruning of the variants (beyond the reference; DESIGN.md 9) -------------------------------------------------
+    def ldPrune(self, callsets: CallsRdd, window_lo: np.ndarray) -> np.ndarray:
+        """--ld-prune R2: keep-first LD pruning of the whole fileset in one library call; every BedSlice then stands for
+        its kept rows only, so the Gram, the kinship counts and the loadings see the pruned variant set (what
+        `plink --extract P.prune.in` would give).  Returns the (V,) keep mask."""
+        from . import plink
+        r2, kb = self.conf.ldPrune(), self.conf.ldWindowKb()
+        slices = [p for p in callsets.partitions if isinstance(p, BedSlice)]
+        bed = slices[0].bed if slices else plink.BedFile(self.conf.bedPath(), n_samples=callsets.n_samples)
+        nat = self._native(callsets.n_samples)
+        keep, _, _ = nat.ldPruneBed(bed._map, window_lo, r2)
+        print(f"LD prune r2 > {r2!r} within {kb:g} kb: {int(keep.sum())} of {len(keep)} variants kept.")
+        if self.conf.outputPath.isDefined and self._rank == 0:
+            write_prune_lists(self.conf.outputPath(), plink.read_bim(self.conf.bedPath()), keep)
+        for p in slices:
+            p.keep = keep[p.v0:p.v0 + p.nv]
+        return keep
 
     # -- KING-robust kinship of the sample pairs (beyond the reference; DESIGN.md 7) --------------------------------------
     def writeKingTable(self, path: Optional[str] = None, min_kinship: Optional[float] = None):
@@ -666,6 +686,50 @@ def check_king_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
             raise ValueError(f"{flag} is limited to {native.KINSHIP_MAX_SAMPLES} samples; the cohort has {n_samples}")
 
 
+def check_ld_flags(conf: PcaConf, bim=None) -> Optional[np.ndarray]:
+    """Refuse --ld-prune / --ld-window-kb runs the LD path cannot serve, before any GPU work: without `bim` the flag
+    combinations, with the .bim records also their sort order and the window width.  Returns window_lo (with `bim`)."""
+    if conf.ldWindowKb.isSupplied and not conf.ldPrune.isDefined:
+        raise ValueError("--ld-window-kb needs --ld-prune")
+    if not conf.ldPrune.isDefined:
+        return None
+    r2, kb = conf.ldPrune(), conf.ldWindowKb()
+    if not (np.isfinite(r2) and 0.0 <= r2 < 1.0):
+        raise ValueError(f"--ld-prune takes an r2 threshold in [0, 1), not {r2!r}")
+    if not (np.isfinite(kb) and kb > 0):
+        raise ValueError(f"--ld-window-kb must be a positive number of kb, not {kb!r}")
+    if not conf.bedPath.isDefined:
+        raise ValueError("--ld-prune needs allele counts and positions: give a PLINK fileset with --bed-path")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("--ld-prune runs on one GPU; launch a single process (WORLD_SIZE=1)")
+    if conf.checkpointPath.isDefined:
+        raise ValueError("--ld-prune decides the variant set before the Gram; it cannot resume from --checkpoint-path")
+    if conf.projectLoadings.isDefined:
+        raise ValueError("--project-loadings must use the reference's variants; drop --ld-prune")
+    if bim is None:
+        return None
+    from . import plink
+    try:
+        lo = plink.window_starts(bim, kb)
+    except ValueError as e:
+        raise ValueError(f"--ld-prune needs a sorted .bim: {e}") from None
+    reach = np.arange(len(lo), dtype=np.int64) - lo
+    if len(reach) and reach.max() > native.LD_MAX_WINDOW:
+        j = int(np.flatnonzero(reach > native.LD_MAX_WINDOW)[0])
+        raise ValueError(f"--ld-window-kb {kb:g}: the window of variant {j} ({bim[j].id}, {bim[j].contig}:{bim[j].position}) "
+                         f"holds {int(reach[j])} earlier variants; at most {native.LD_MAX_WINDOW} are supported")
+    return lo
+
+
+def write_prune_lists(prefix: str, bim, keep: np.ndarray) -> None:
+    """PLINK's LD-pruning outputs: prefix.prune.in (the kept variants) and .prune.out (the pruned ones), the .bim variant
+    IDs one per line in file order."""
+    keep = np.asarray(keep, bool)
+    for suffix, sel in ((".prune.in", keep), (".prune.out", ~keep)):
+        with open(prefix + suffix, "w", encoding="utf-8") as fh:
+            fh.write("".join(f"{bim[j].id}\n" for j in np.flatnonzero(sel).tolist()))
+
+
 def check_king_cutoff_kept(kept: int, num_pc: int) -> None:
     """Refuse a --king-cutoff selection that leaves too few samples for the PCs asked for."""
     if kept < 2 or kept < num_pc:
@@ -771,6 +835,8 @@ def bimKeyBytes(b) -> bytes:
 
 
 def _partition_len(part) -> int:
+    if isinstance(part, BedSlice):
+        return part.n_rows
     return len(part.offsets) - 1 if isinstance(part, CallsBatch) else int(part.nv)
 
 
@@ -804,6 +870,7 @@ def main(args: Optional[Sequence[str]] = None):
     """VariantsPcaDriver.main (VariantsPca.scala:38-50)."""
     conf = PcaConf(list(sys.argv[1:] if args is None else args))
     check_king_flags(conf)
+    check_ld_flags(conf)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         import torch
         import torch.distributed as dist
@@ -811,9 +878,15 @@ def main(args: Optional[Sequence[str]] = None):
         dist.init_process_group("nccl")
     driver = VariantsPcaDriver(conf)
     check_king_flags(conf, len(driver.common.indexes))
+    window_lo = None
+    if conf.ldPrune.isDefined:
+        from . import plink
+        window_lo = check_ld_flags(conf, plink.read_bim(conf.bedPath()))
     data = driver.getData
     filtered = [driver.filterDataset(d) for d in data]
     callsRdd = driver.getCallsRdd(filtered)
+    if window_lo is not None:
+        driver.ldPrune(callsRdd, window_lo)             # the pruned set is the variant set of everything below
     if conf.projectLoadings.isDefined:
         if conf.saveLoadings.isDefined:
             raise ValueError("--project-loadings computes no principal components to save; drop --save-loadings")

@@ -388,6 +388,39 @@ int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, doubl
 int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const int64_t* window_lo,
                       double r2_max, uint8_t* keep, int64_t max_pairs, int64_t* out_pairs, double* out_r2,
                       int64_t* n_pairs);
+/* vpca_ld_prune_bed_masked: vpca_ld_prune_bed with eligible[j] in {0, 1} (nv bytes; NULL = all eligible, which is
+ *   vpca_ld_prune_bed bit for bit): keep[j] = 0 where eligible[j] = 0, and pairs are counted and listed only between
+ *   eligible variants.  keep and the pairs equal vpca_ld_prune_bed on the eligible rows alone, with their window_lo
+ *   recomputed (the first eligible variant at or after window_lo[j]), the pairs' indices staying those of all nv rows.
+ *   The window limit is still checked on the window_lo given.  VPCA_ERR_BAD_ARG also for an eligible byte above 1. */
+int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
+                             const int64_t* window_lo, const uint8_t* eligible, double r2_max, uint8_t* keep,
+                             int64_t max_pairs, int64_t* out_pairs, double* out_r2, int64_t* n_pairs);
+
+/* ---- variant quality control (beyond VariantsPca.scala: which variants go into S; DESIGN.md 10) ------------------------
+ * The three usual variant filters before an ancestry PCA -- minor-allele frequency, missing-call rate, Hardy-Weinberg
+ * equilibrium -- depend on four exact counts per variant, over all n_samples samples: HOM_A1 (code 00), HET (10), HOM_A2
+ * (11), MISSING (01).  With n = HOM_A1 + HET + HOM_A2 the called samples and r = 2 min(HOM_A1, HOM_A2) + HET the copies of
+ * the rarer allele, the HWE p-value is the exact test of Wigginton, Cutler & Abecasis (AJHG 76:887, 2005), in FP64:
+ *   the relative probability t(h) of h hets given r and n is 1 at m = floor(r (2n - r) / (2n)) (+1 when its parity differs
+ *   from r's), the mode or next to it; downward t(h - 2) = ((t(h) * h) * (h - 1)) / ((4 * (homr + 1)) * (homc + 1)), upward
+ *   t(h + 2) = (((t(h) * 4) * homr) * homc) / ((h + 2) * (h + 1)), with homr = (r - h) / 2, homc = n - h - homr at h;
+ *   each operation rounded once (no contraction).  A direction ends at its range end or at the first t that is exactly 0.
+ *   T = sum of t, S = sum of the t <= t(obs) * (1 + 2^-40), both summed m first, then downward, then upward;
+ *   p = min(S / T, 1), and p = 1 when r = 0 or n = 0.  A t(obs) that underflows to 0 gives p = 0 (true p below ~1e-300).
+ * vpca_variant_qc_bed: rows are PLINK 1 .bed rows (as vpca_accumulate_bed; bytes past ceil(n_samples / 4) and the padding
+ *   bits of the last byte are ignored); out_counts[4v ..] = HOM_A1, HET, HOM_A2, MISSING (exact, whatever the split of
+ *   the rows into calls); out_hwe_p (may be NULL) = the p-value of each row.
+ * vpca_hwe_exact: the same p-values from host counts in the layout above (MISSING ignored), for any n.
+ * Driver-side and synchronous.  Rows are staged in chunks of at most 64 MB and tested in batches of about 2^18 rows (at
+ * least one chunk), so device memory does not grow with nv: the chunk and 24 bytes per batch row are allocated on the
+ * first call and freed by vpca_destroy.  The PCA Gram, U, the kinship counts, the subset state and the LD state are left
+ * alone.
+ * VPCA_ERR_BAD_ARG, before any row is staged: rows / out_counts / counts / out_p NULL (nv > 0), nv < 0,
+ *   stride_bytes < ceil(n_samples / 4), negative counts or counts whose sum exceeds 2^31 - 1. */
+int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t* out_counts,
+                        double* out_hwe_p);
+int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out_p);
 
 /* ---- one process, all GPUs of the box (SURVEY 8b "process model") --------------------------------------------------
  * A vpca_pool is what `class VariantsPcaDriver` holds on a multi-GPU host: one vpca_ctx per GPU, wired with

@@ -120,4 +120,7 @@ class PcaConf(GenomicsConf):
                                                           # relatives projected onto them (PLINK 2's flag name)
             ("ldPrune", float, None, False),              # --bed-path runs: keep-first LD pruning, r2 > this within a window
             ("ldWindowKb", float, 500.0, False),          # the window of --ld-prune: same contig, positions <= this many kb apart
+            ("maf", float, None, False),                  # --bed-path runs: drop variants with minor-allele frequency < this
+            ("geno", float, None, False),                 # --bed-path runs: drop variants with missing-call rate > this
+            ("hwe", float, None, False),                  # --bed-path runs: drop variants with exact HWE p-value < this
         ]

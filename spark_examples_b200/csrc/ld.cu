@@ -31,7 +31,7 @@ struct PairOut {
 };
 
 // grid (T, row tiles): block (w, y) is row tile bt = bt_lo + y against column tile bt - (T - 1) + w
-template <bool EMIT>
+template <bool EMIT, bool MASKED>
 __global__ void __launch_bounds__(kTile * kWarps)
 ld_pairs_kernel(LdChunk ch, int bt_lo, uint32_t* __restrict__ bits, const int32_t* __restrict__ seg, PairOut out) {
     __shared__ int32_t t_sy[kTile][kTile + 1];    // [al][bl] = G[2c+a][b]
@@ -56,11 +56,12 @@ ld_pairs_kernel(LdChunk ch, int bt_lo, uint32_t* __restrict__ bits, const int32_
     }
     __syncthreads();
     const int a = a0 + lane;
+    const bool ea = !MASKED || (a < ch.nc && ch.elig[ch.s0 + a] != 0);
     for (int bl = warp; bl < kTile; bl += kWarps) {
         const int b = b0 + bl;
         bool sel = false;
         double r2 = 0.0;
-        if (b >= ch.own_lo && b < ch.nc && a < b && ch.s0 + a >= ch.wlo[b]) {
+        if (ea && b >= ch.own_lo && b < ch.nc && a < b && ch.s0 + a >= ch.wlo[b] && (!MASKED || ch.elig[ch.s0 + b] != 0)) {
             const int32_t* rb = G + (int64_t)b * R;
             const int32_t* rm = G + (2 * (int64_t)c + b) * R;
             const int64_t n = rm[2 * c + a], sx = rm[a], sxx = rm[c + a], sxy = rb[a];
@@ -120,7 +121,8 @@ __global__ void ld_row_scan_kernel(const uint32_t* __restrict__ bits, int32_t* _
 // the owned rows are decided in order.  A row without an in-LD partner is kept outright; a row with partners is kept iff
 // none of its in-LD bits meets a kept bit.  Bits of later rows never matter to a row's test (its bits only name a < b).
 // The bit words of 32 rows are contiguous: they are staged in shared memory with one coalesced pass, so the serial
-// per-row tests wait on shared memory only.
+// per-row tests wait on shared memory only.  MASKED: an ineligible row has no pairs and is never kept.
+template <bool MASKED>
 __global__ void __launch_bounds__(32) ld_sweep_kernel(LdChunk ch, const uint32_t* __restrict__ bits,
                                                       const int32_t* __restrict__ row_total, uint8_t* __restrict__ keep) {
     __shared__ uint32_t kb[kLdMaxChunk / kTile];
@@ -138,7 +140,8 @@ __global__ void __launch_bounds__(32) ld_sweep_kernel(LdChunk ch, const uint32_t
         const bool owned = r >= ch.own_lo && r < ch.nc;
         const uint32_t om = __ballot_sync(0xffffffffu, owned);
         uint32_t todo = __ballot_sync(0xffffffffu, owned && row_total[r] != 0);
-        uint32_t word = kb[wi] | (om & ~todo);
+        const uint32_t em = MASKED ? __ballot_sync(0xffffffffu, owned && ch.elig[ch.s0 + r] != 0) : om;
+        uint32_t word = kb[wi] | (em & ~todo);
         if (todo != 0u) {
             const uint32_t* src = bits + (int64_t)wi * kTile * T;
             for (int t = lane; t < kTile * T; t += 32) rb[t] = src[t];
@@ -166,8 +169,11 @@ cudaError_t ld_count(LdWork& w, const LdChunk& ch, cudaStream_t stream) {
     const int bt_lo = ch.own_lo / kTile, bt_hi = (ch.nc + kTile - 1) / kTile;
     if (bt_hi <= bt_lo) return cudaSuccess;
     PairOut none{};
-    ld_pairs_kernel<false><<<dim3((unsigned)ch.T, (unsigned)(bt_hi - bt_lo)), kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits,
-                                                                                                        nullptr, none);
+    const dim3 grid((unsigned)ch.T, (unsigned)(bt_hi - bt_lo));
+    if (ch.elig != nullptr)
+        ld_pairs_kernel<false, true><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, nullptr, none);
+    else
+        ld_pairs_kernel<false, false><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, nullptr, none);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const int rows = (bt_hi - bt_lo) * kTile, threads = 256;
@@ -177,15 +183,21 @@ cudaError_t ld_count(LdWork& w, const LdChunk& ch, cudaStream_t stream) {
 }
 
 cudaError_t ld_sweep(LdWork& w, const LdChunk& ch, uint8_t* d_keep, cudaStream_t stream) {
-    ld_sweep_kernel<<<1, 32, 0, stream>>>(ch, w.d_bits, w.d_row_total, d_keep);
+    if (ch.elig != nullptr)
+        ld_sweep_kernel<true><<<1, 32, 0, stream>>>(ch, w.d_bits, w.d_row_total, d_keep);
+    else
+        ld_sweep_kernel<false><<<1, 32, 0, stream>>>(ch, w.d_bits, w.d_row_total, d_keep);
     return cudaGetLastError();
 }
 
 cudaError_t ld_emit(LdWork& w, const LdChunk& ch, int bt_lo, int bt_hi, int64_t base, int64_t end, cudaStream_t stream) {
     if (bt_hi <= bt_lo) return cudaSuccess;
     PairOut out{w.d_pairs, w.d_r2, w.d_row_start, base, end};
-    ld_pairs_kernel<true><<<dim3((unsigned)ch.T, (unsigned)(bt_hi - bt_lo)), kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits,
-                                                                                                       w.d_seg, out);
+    const dim3 grid((unsigned)ch.T, (unsigned)(bt_hi - bt_lo));
+    if (ch.elig != nullptr)
+        ld_pairs_kernel<true, true><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, w.d_seg, out);
+    else
+        ld_pairs_kernel<true, false><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, w.d_seg, out);
     return cudaGetLastError();
 }
 

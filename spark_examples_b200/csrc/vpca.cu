@@ -91,7 +91,13 @@ struct vpca_ctx {
     uint8_t* d_ld_rows[2] = {nullptr, nullptr};
     int64_t* d_ld_wlo = nullptr;
     uint8_t* d_ld_keep = nullptr;
-    int64_t cap_ld_G = 0, cap_ld_x = 0, cap_ld_rows = 0, cap_ld_wlo = 0, cap_ld_keep = 0, cap_ld_words = 0;
+    uint8_t* d_ld_elig = nullptr;    // vpca_ld_prune_bed_masked: the eligible bytes of the call
+    int64_t cap_ld_G = 0, cap_ld_x = 0, cap_ld_rows = 0, cap_ld_wlo = 0, cap_ld_keep = 0, cap_ld_words = 0, cap_ld_elig = 0;
+    // variant QC (vpca_variant_qc_bed / vpca_hwe_exact): the raw rows, counts and p-values of one chunk; grow-only
+    uint8_t* d_qc_rows = nullptr;
+    int32_t* d_qc_counts = nullptr;
+    double* d_qc_p = nullptr;
+    int64_t cap_qc_rows = 0, cap_qc_counts = 0, cap_qc_p = 0;
     GramPlan ld_plan;
     LdWork ld;
 
@@ -685,7 +691,8 @@ int vpca_destroy(vpca_ctx* ctx) {
     kin_pair_free(ctx->kin_pairs);
     for (void* p : {(void*)ctx->d_ld_G, ctx->d_ld_x, (void*)ctx->d_ld_rows[0], (void*)ctx->d_ld_rows[1], (void*)ctx->d_ld_wlo,
                     (void*)ctx->d_ld_keep, (void*)ctx->ld.d_bits, (void*)ctx->ld.d_seg, (void*)ctx->ld.d_row_total,
-                    (void*)ctx->ld.d_row_start, (void*)ctx->ld.d_total, (void*)ctx->ld.d_pairs, (void*)ctx->ld.d_r2})
+                    (void*)ctx->ld.d_row_start, (void*)ctx->ld.d_total, (void*)ctx->ld.d_pairs, (void*)ctx->ld.d_r2,
+                    (void*)ctx->d_ld_elig, (void*)ctx->d_qc_rows, (void*)ctx->d_qc_counts, (void*)ctx->d_qc_p})
         cudaFree(p);
     gram_plan_free(ctx->ld_plan);
     gram_plan_free(ctx->plan);
@@ -1996,6 +2003,13 @@ cudaError_t ld_buffers(vpca_ctx* ctx, int64_t c, int T, int64_t x_bytes, int64_t
 int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const int64_t* window_lo,
                       double r2_max, uint8_t* keep, int64_t max_pairs, int64_t* out_pairs, double* out_r2,
                       int64_t* n_pairs) {
+    return vpca_ld_prune_bed_masked(ctx, rows, nv, stride_bytes, window_lo, nullptr, r2_max, keep, max_pairs, out_pairs,
+                                    out_r2, n_pairs);
+}
+
+int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
+                             const int64_t* window_lo, const uint8_t* eligible, double r2_max, uint8_t* keep,
+                             int64_t max_pairs, int64_t* out_pairs, double* out_r2, int64_t* n_pairs) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     const int n = ctx->n;
     if (rows == nullptr || window_lo == nullptr || keep == nullptr || n_pairs == nullptr || nv < 0 ||
@@ -2018,6 +2032,11 @@ int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t st
         return fail(ctx, VPCA_ERR_UNSUPPORTED, "vpca_ld_prune_bed: the window of variant %lld reaches back %lld variants; "
                     "the limit is %d", (long long)j, (long long)(j - window_lo[j]), kLdMaxWindow);
     }
+    if (eligible != nullptr)
+        for (int64_t j = 0; j < nv; ++j)
+            if (eligible[j] > 1)
+                return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_ld_prune_bed_masked: eligible[%lld] = %d must be 0 or 1",
+                            (long long)j, (int)eligible[j]);
     *n_pairs = 0;
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) return VPCA_OK;
@@ -2040,6 +2059,8 @@ int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t st
     LdWork& w = ctx->ld;
     {
         cudaError_t e = ld_buffers(ctx, c, T, R * piece, c * rp, nv);
+        if (e == cudaSuccess && eligible != nullptr)
+            e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_ld_elig), ctx->cap_ld_elig, nv, 1);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "LD pruning buffers for chunks of %lld variants: %s", (long long)c,
@@ -2047,6 +2068,10 @@ int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t st
         }
     }
     CUDA_OK(ctx, cudaMemsetAsync(w.d_total, 0, sizeof(int64_t), L.stream));
+    if (eligible != nullptr) {
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_elig, eligible, (size_t)nv, cudaMemcpyHostToDevice, L.stream));
+        ctx->c_h2d += nv;
+    }
     int64_t listed = 0;                   // pairs counted (and listed) before the current chunk while listing
     bool listing = max_pairs > 0;
     std::vector<int32_t> row_total((size_t)c);
@@ -2054,7 +2079,8 @@ int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t st
     int unit = 0;                         // staged pieces so far: selects the row buffer
     for (int64_t s = 0;;) {
         const int64_t e_end = std::min(s + c, nv);
-        LdChunk ch{ctx->d_ld_G, ctx->d_ld_wlo, s, (int)c, (int)(e_end - s), s == 0 ? 0 : (int)H, T, r2_max};
+        LdChunk ch{ctx->d_ld_G, ctx->d_ld_wlo, s, (int)c, (int)(e_end - s), s == 0 ? 0 : (int)H, T, r2_max,
+                   eligible != nullptr ? ctx->d_ld_elig : nullptr};
         CUDA_OK(ctx, cudaMemsetAsync(ctx->d_ld_G, 0, (size_t)(R * R) * sizeof(int32_t), L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_wlo, window_lo + s, (size_t)ch.nc * sizeof(int64_t), cudaMemcpyHostToDevice,
                                      L.stream));
@@ -2118,6 +2144,109 @@ int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t st
     CUDA_OK(ctx, cudaMemcpyAsync(keep, ctx->d_ld_keep, (size_t)nv, cudaMemcpyDeviceToHost, L.stream));
     CUDA_OK(ctx, cudaMemcpyAsync(n_pairs, w.d_total, sizeof(int64_t), cudaMemcpyDeviceToHost, L.stream));
     ctx->c_d2h += nv + 8;
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+// ---- variant QC (qc.cu, DESIGN.md 10) -----------------------------------------------------------------------------------
+// Driver-side and synchronous.  Rows are staged in chunks of at most kQcStageBytes on a lane's stream and counted; the
+// counts of whole chunks gather into batches of about kQcHweChunk rows, each tested with one HWE launch and copied back,
+// so that the HWE kernel fills the GPU even when a chunk holds a few thousand wide rows, and device memory stays bounded
+// whatever the number of variants.
+namespace {
+constexpr int64_t kQcStageBytes = 64ll << 20;   // raw .bed bytes per staged chunk
+constexpr int64_t kQcHweChunk = 1ll << 18;      // count rows per HWE launch (and per vpca_hwe_exact chunk)
+
+// grows the QC buffers to `row_bytes` staged bytes and `rows` count / p-value rows
+cudaError_t qc_buffers(vpca_ctx* ctx, int64_t row_bytes, int64_t rows) {
+    cudaError_t e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_qc_rows), ctx->cap_qc_rows, row_bytes, 1);
+    if (e == cudaSuccess) e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_qc_counts), ctx->cap_qc_counts, 4 * rows,
+                                            sizeof(int32_t));
+    if (e == cudaSuccess) e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_qc_p), ctx->cap_qc_p, rows, sizeof(double));
+    return e;
+}
+}   // namespace
+
+int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t* out_counts,
+                        double* out_hwe_p) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    const int n = ctx->n;
+    if (nv < 0 || (nv > 0 && (rows == nullptr || out_counts == nullptr)) || stride_bytes < (n + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_variant_qc_bed: bad argument (rows and out_counts must be set, "
+                    "stride_bytes >= ceil(n_samples / 4))");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int64_t step = std::max<int64_t>(1, std::min(nv, kQcStageBytes / stride_bytes));
+    const int64_t batch = std::min(nv, step * std::max<int64_t>(1, kQcHweChunk / step));   // whole chunks
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = qc_buffers(ctx, step * stride_bytes, batch);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "variant QC buffers for %lld rows of %lld bytes: %s", (long long)step,
+                        (long long)stride_bytes, cudaGetErrorString(e));
+        }
+    }
+    for (int64_t b0 = 0; b0 < nv; b0 += batch) {
+        const int64_t nb = std::min(batch, nv - b0);
+        for (int64_t v = b0; v < b0 + nb; v += step) {
+            const int64_t nvc = std::min(step, b0 + nb - v);
+            CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_rows, rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+                                         cudaMemcpyHostToDevice, L.stream));
+            ctx->c_h2d += nvc * stride_bytes;
+            CUDA_OK(ctx, qc_count(ctx->d_qc_rows, stride_bytes, (int)nvc, n, ctx->d_qc_counts + 4 * (v - b0), L.stream));
+            ctx->c_launches += 1;
+        }
+        CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 4 * b0, ctx->d_qc_counts, (size_t)(4 * nb) * sizeof(int32_t),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        ctx->c_d2h += 16 * nb;
+        if (out_hwe_p != nullptr) {
+            CUDA_OK(ctx, qc_hwe(ctx->d_qc_counts, (int)nb, ctx->d_qc_p, L.stream));
+            CUDA_OK(ctx, cudaMemcpyAsync(out_hwe_p + b0, ctx->d_qc_p, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost,
+                                         L.stream));
+            ctx->c_launches += 1;
+            ctx->c_d2h += 8 * nb;
+        }
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out_p) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    if (nv < 0 || (nv > 0 && (counts == nullptr || out_p == nullptr)))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_hwe_exact: bad argument (counts and out_p must be set)");
+    for (int64_t v = 0; v < nv; ++v) {
+        const int64_t a = counts[4 * v], h = counts[4 * v + 1], b = counts[4 * v + 2];
+        if (a < 0 || h < 0 || b < 0 || a + h + b > 2147483647ll)
+            return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_hwe_exact: counts of row %lld (%lld, %lld, %lld) must be non-negative "
+                        "with a sum below 2^31", (long long)v, (long long)a, (long long)h, (long long)b);
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int64_t step = std::min(nv, kQcHweChunk);
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = qc_buffers(ctx, 1, step);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "HWE buffers for %lld rows: %s", (long long)step, cudaGetErrorString(e));
+        }
+    }
+    for (int64_t v = 0; v < nv; v += step) {
+        const int64_t nvc = std::min(step, nv - v);
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_counts, counts + 4 * v, (size_t)(4 * nvc) * sizeof(int32_t),
+                                     cudaMemcpyHostToDevice, L.stream));
+        ctx->c_h2d += 16 * nvc;
+        CUDA_OK(ctx, qc_hwe(ctx->d_qc_counts, (int)nvc, ctx->d_qc_p, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_p + v, ctx->d_qc_p, (size_t)nvc * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
+        ctx->c_launches += 1;
+        ctx->c_d2h += 8 * nvc;
+    }
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     return VPCA_OK;
 }

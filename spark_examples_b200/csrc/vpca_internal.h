@@ -124,6 +124,7 @@ struct LdChunk {
     int64_t s0;
     int c, nc, own_lo, T;
     double r2_max;
+    const uint8_t* elig;   // vpca_ld_prune_bed_masked: eligible[v] of every variant v of the call; nullptr = all eligible
 };
 struct LdWork {
     uint32_t* d_bits = nullptr;     // c x T in-LD bits
@@ -144,6 +145,13 @@ cudaError_t ld_sweep(LdWork& w, const LdChunk& ch, uint8_t* d_keep, cudaStream_t
 // Pass 2: the in-LD pairs of row tiles [bt_lo, bt_hi) whose output position p lies in [base, end) go to scratch slot
 // p - base (needs w.d_row_start).  Never synchronises.
 cudaError_t ld_emit(LdWork& w, const LdChunk& ch, int bt_lo, int bt_hi, int64_t base, int64_t end, cudaStream_t stream);
+
+// ---- variant QC (qc.cu, DESIGN.md 10) ------------------------------------------------------------------------------
+// HOM_A1, HET, HOM_A2, MISSING of nv .bed rows of n samples, row v at d_rows + v * pitch, into d_counts[4v ..] (16-byte
+// aligned).  Bytes past ceil(n / 4) and the padding bits of the last byte are ignored.  Never synchronises.
+cudaError_t qc_count(const uint8_t* d_rows, int64_t pitch, int nv, int n, int32_t* d_counts, cudaStream_t stream);
+// The exact HWE p-value (vpca.h) of each of nv count rows (layout above, 16-byte aligned).  Never synchronises.
+cudaError_t qc_hwe(const int32_t* d_counts, int nv, double* d_p, cudaStream_t stream);
 
 // ---- KING-robust kinship pairs from the 3n x 3n plane Gram (kinship.cu) ----------------------------------------------
 constexpr int kKinMaxN = 21845;   // 3n <= 65 535: the plane Gram stays below 2^32 cells

@@ -53,6 +53,7 @@ EXPORTED_SYMBOLS = (
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
     "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
+    "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
@@ -278,6 +279,12 @@ def load_library() -> ctypes.CDLL:
     L.vpca_kinship_pairs.argtypes = [vp, ctypes.c_double, i64, vp, vp, vp, ctypes.POINTER(i64)]
     L.vpca_ld_prune_bed.restype = ctypes.c_int
     L.vpca_ld_prune_bed.argtypes = [vp, vp, i64, i64, vp, ctypes.c_double, vp, i64, vp, vp, ctypes.POINTER(i64)]
+    L.vpca_ld_prune_bed_masked.restype = ctypes.c_int
+    L.vpca_ld_prune_bed_masked.argtypes = [vp, vp, i64, i64, vp, vp, ctypes.c_double, vp, i64, vp, vp, ctypes.POINTER(i64)]
+    L.vpca_variant_qc_bed.restype = ctypes.c_int
+    L.vpca_variant_qc_bed.argtypes = [vp, vp, i64, i64, vp, vp]
+    L.vpca_hwe_exact.restype = ctypes.c_int
+    L.vpca_hwe_exact.argtypes = [vp, vp, i64, vp]
     L.vpca_compute_pca_subset.restype = ctypes.c_int
     L.vpca_compute_pca_subset.argtypes = [vp, vp, i32, vp, vp, ctypes.POINTER(i32)]
     _lib = L
@@ -697,10 +704,12 @@ class NativePca:
         return ids[:p], counts[:p], kin[:p]
 
     # -- LD pruning of the variants (vpca.h, DESIGN.md 9) --------------------------------------------------------------
-    def ldPruneBed(self, rows: np.ndarray, window_lo, r2_max: float, max_pairs: int = 0):
+    def ldPruneBed(self, rows: np.ndarray, window_lo, r2_max: float, max_pairs: int = 0, eligible=None):
         """Keep-first LD pruning of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place, not copied) with
         window_lo[j] the first variant of j's window -> (keep (V,) bool, pairs (P, 2) int64 of (i, j), r2 (P,) float64):
-        the first min(total, max_pairs) in-LD pairs in order of j, then i.  Synchronises."""
+        the first min(total, max_pairs) in-LD pairs in order of j, then i.  eligible ((V,) bool, e.g. the variant QC
+        mask): only eligible variants are paired or kept -- the result of pruning the eligible rows alone, indexed over
+        all V.  Synchronises."""
         b = np.asarray(rows)
         if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
             b = np.ascontiguousarray(b, dtype=np.uint8)
@@ -718,11 +727,48 @@ class NativePca:
         empty = np.zeros(1, np.int64)          # a valid address for zero variants
         rows_ptr = b.ctypes.data if b.size else _host_ptr(empty)
         lo_ptr = lo.ctypes.data if lo.size else _host_ptr(empty)
-        self._check(self._lib.vpca_ld_prune_bed(self._h, rows_ptr, nv, b.shape[1], lo_ptr, float(r2_max), _host_ptr(keep),
-                                                p, _host_ptr(pairs) if p else None, _host_ptr(r2) if p else None,
-                                                ctypes.byref(total)))
+        if eligible is None:
+            self._check(self._lib.vpca_ld_prune_bed(self._h, rows_ptr, nv, b.shape[1], lo_ptr, float(r2_max),
+                                                    _host_ptr(keep), p, _host_ptr(pairs) if p else None,
+                                                    _host_ptr(r2) if p else None, ctypes.byref(total)))
+        else:
+            el = np.ascontiguousarray(eligible, dtype=bool).reshape(-1)
+            if len(el) != nv:
+                raise VpcaError(VPCA_ERR_BAD_ARG, f"eligible must have {nv} entries")
+            el = np.concatenate([el.view(np.uint8), np.zeros(1, np.uint8)])   # a valid address for zero variants
+            self._check(self._lib.vpca_ld_prune_bed_masked(self._h, rows_ptr, nv, b.shape[1], lo_ptr, _host_ptr(el),
+                                                           float(r2_max), _host_ptr(keep), p,
+                                                           _host_ptr(pairs) if p else None,
+                                                           _host_ptr(r2) if p else None, ctypes.byref(total)))
         got = min(int(total.value), p)
         return keep[:nv] != 0, pairs[:got], r2[:got]
+
+    # -- variant QC (vpca.h, DESIGN.md 10) ---------------------------------------------------------------------------
+    def variantQcBed(self, rows: np.ndarray, hwe: bool = True):
+        """Genotype counts of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place, not copied) ->
+        (counts (V, 4) int32 of HOM_A1, HET, HOM_A2, MISSING; p (V,) float64 exact HWE p-values, or None without
+        `hwe`).  Synchronises."""
+        b = np.asarray(rows)
+        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
+            b = np.ascontiguousarray(b, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        nv = b.shape[0]
+        counts = np.zeros((max(nv, 1), 4), np.int32)
+        p = np.zeros(max(nv, 1), np.float64)
+        empty = np.zeros(1, np.uint8)
+        self._check(self._lib.vpca_variant_qc_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv, b.shape[1],
+                                                  _host_ptr(counts), _host_ptr(p) if hwe else None))
+        return counts[:nv], (p[:nv] if hwe else None)
+
+    def hweExact(self, counts) -> np.ndarray:
+        """Exact HWE p-values of (V, 4) int32 counts (HOM_A1, HET, HOM_A2, MISSING; MISSING ignored) -> (V,) float64."""
+        c = np.ascontiguousarray(counts, dtype=np.int32).reshape(-1, 4)
+        nv = c.shape[0]
+        c = np.concatenate([c, np.zeros((1, 4), np.int32)])   # a valid address for zero variants
+        p = np.zeros(nv + 1, np.float64)
+        self._check(self._lib.vpca_hwe_exact(self._h, _host_ptr(c), nv, _host_ptr(p)))
+        return p[:nv]
 
     def computePcaSubset(self, keep, k: int = 2):
         """PCs of the samples with keep[s] true, from the Gram of all of them (DESIGN.md 8) -> (vecs (n, k), evals (k,),

@@ -541,21 +541,49 @@ class VariantsPcaDriver:
             nat.projectCalls(off, idx, w, mean)
 
     # -- LD pruning of the variants (beyond the reference; DESIGN.md 9) -------------------------------------------------
-    def ldPrune(self, callsets: CallsRdd, window_lo: np.ndarray) -> np.ndarray:
+    def ldPrune(self, callsets: CallsRdd, window_lo: np.ndarray, eligible: Optional[np.ndarray] = None) -> np.ndarray:
         """--ld-prune R2: keep-first LD pruning of the whole fileset in one library call; every BedSlice then stands for
         its kept rows only, so the Gram, the kinship counts and the loadings see the pruned variant set (what
-        `plink --extract P.prune.in` would give).  Returns the (V,) keep mask."""
+        `plink --extract P.prune.in` would give).  eligible (the variant QC mask): prune only those variants, as PLINK
+        does after its filters; the others are neither kept nor listed.  Returns the (V,) keep mask."""
         from . import plink
         r2, kb = self.conf.ldPrune(), self.conf.ldWindowKb()
         slices = [p for p in callsets.partitions if isinstance(p, BedSlice)]
         bed = slices[0].bed if slices else plink.BedFile(self.conf.bedPath(), n_samples=callsets.n_samples)
         nat = self._native(callsets.n_samples)
-        keep, _, _ = nat.ldPruneBed(bed._map, window_lo, r2)
-        print(f"LD prune r2 > {r2!r} within {kb:g} kb: {int(keep.sum())} of {len(keep)} variants kept.")
+        if eligible is None:
+            keep, _, _ = nat.ldPruneBed(bed._map, window_lo, r2)
+        else:
+            keep, _, _ = nat.ldPruneBed(bed._map, window_lo, r2, eligible=eligible)
+        of = len(keep) if eligible is None else int(np.count_nonzero(eligible))
+        print(f"LD prune r2 > {r2!r} within {kb:g} kb: {int(keep.sum())} of {of} variants kept.")
         if self.conf.outputPath.isDefined and self._rank == 0:
-            write_prune_lists(self.conf.outputPath(), plink.read_bim(self.conf.bedPath()), keep)
+            write_prune_lists(self.conf.outputPath(), plink.read_bim(self.conf.bedPath()), keep, eligible)
         for p in slices:
             p.keep = keep[p.v0:p.v0 + p.nv]
+        return keep
+
+    # -- variant QC (beyond the reference; DESIGN.md 10) --------------------------------------------------------------
+    def variantQc(self, callsets: CallsRdd) -> np.ndarray:
+        """--maf / --geno / --hwe: genotype counts and exact HWE p-values of the whole fileset in one library call; every
+        BedSlice then stands for the variants that pass every filter given (what `plink --maf --geno --hwe --make-bed`
+        would leave).  Writes P.afreq, P.vmiss and P.hardy with --output-path.  Returns the (V,) keep mask."""
+        from . import plink
+        slices = [p for p in callsets.partitions if isinstance(p, BedSlice)]
+        bed = slices[0].bed if slices else plink.BedFile(self.conf.bedPath(), n_samples=callsets.n_samples)
+        nat = self._native(callsets.n_samples)
+        counts, p = nat.variantQcBed(bed._map)
+        limits = qc_limits(self.conf)
+        keep, removed_by = variant_qc_keep(counts, p, limits["--maf"], limits["--geno"], limits["--hwe"])
+        removed = ", ".join(f"{int(np.count_nonzero(removed_by == code))} by {flag} {limits[flag]!r}"
+                            for code, flag in enumerate(QC_FILTERS, 1) if limits[flag] is not None)
+        print(f"Variant QC: {int(keep.sum())} of {len(keep)} variants kept ({removed} removed).")
+        if self.conf.outputPath.isDefined and self._rank == 0:
+            write_qc_reports(self.conf.outputPath(), plink.read_bim(self.conf.bedPath()), counts, p)
+        if not keep.any():
+            raise ValueError(f"variant QC keeps none of the {len(keep)} variants ({removed}): relax --maf / --geno / --hwe")
+        for s in slices:
+            s.keep = keep[s.v0:s.v0 + s.nv]
         return keep
 
     # -- KING-robust kinship of the sample pairs (beyond the reference; DESIGN.md 7) --------------------------------------
@@ -721,13 +749,103 @@ def check_ld_flags(conf: PcaConf, bim=None) -> Optional[np.ndarray]:
     return lo
 
 
-def write_prune_lists(prefix: str, bim, keep: np.ndarray) -> None:
+def write_prune_lists(prefix: str, bim, keep: np.ndarray, eligible: Optional[np.ndarray] = None) -> None:
     """PLINK's LD-pruning outputs: prefix.prune.in (the kept variants) and .prune.out (the pruned ones), the .bim variant
-    IDs one per line in file order."""
+    IDs one per line in file order; with `eligible` (the variant QC mask) only eligible variants are listed."""
     keep = np.asarray(keep, bool)
-    for suffix, sel in ((".prune.in", keep), (".prune.out", ~keep)):
+    pruned = ~keep if eligible is None else np.asarray(eligible, bool) & ~keep
+    for suffix, sel in ((".prune.in", keep), (".prune.out", pruned)):
         with open(prefix + suffix, "w", encoding="utf-8") as fh:
             fh.write("".join(f"{bim[j].id}\n" for j in np.flatnonzero(sel).tolist()))
+
+
+QC_FILTERS = ("--geno", "--hwe", "--maf")   # PLINK's order: a removed variant is attributed to the first it fails
+QC_RANGES = {"--maf": 0.5, "--geno": 1.0, "--hwe": 1.0}
+
+
+def qc_limits(conf: PcaConf) -> Dict[str, Optional[float]]:
+    """{flag: threshold or None} of the variant QC flags."""
+    return {"--maf": conf.maf.get, "--geno": conf.geno.get, "--hwe": conf.hwe.get}
+
+
+def check_qc_flags(conf: PcaConf) -> None:
+    """Refuse --maf / --geno / --hwe runs the variant QC path cannot serve, before any GPU work."""
+    given = [(flag, v) for flag, v in qc_limits(conf).items() if v is not None]
+    if not given:
+        return
+    for flag, v in given:
+        if not (np.isfinite(v) and 0.0 <= v <= QC_RANGES[flag]):
+            raise ValueError(f"{flag} takes a value in [0, {QC_RANGES[flag]:g}], not {v!r}")
+    flags = " / ".join(flag for flag, _ in given)
+    if not conf.bedPath.isDefined:
+        raise ValueError(f"{flags} counts genotypes: give a PLINK fileset with --bed-path")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError(f"{flags} runs on one GPU; launch a single process (WORLD_SIZE=1)")
+    if conf.checkpointPath.isDefined:
+        raise ValueError(f"{flags} decides the variant set before the Gram; it cannot resume from --checkpoint-path")
+    if conf.projectLoadings.isDefined:
+        raise ValueError(f"--project-loadings must use the reference's variants; drop {flags}")
+
+
+def _allele_freqs(counts: np.ndarray):
+    """(n called, A1 frequency f = (2 HOM_A1 + HET) / 2n, one rounded division; NaN when n = 0) of (V, 4) counts."""
+    c = np.asarray(counts, np.int64).reshape(-1, 4)
+    n = c[:, 0] + c[:, 1] + c[:, 2]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        f = (2 * c[:, 0] + c[:, 1]).astype(np.float64) / (2 * n).astype(np.float64)
+    return n, f
+
+
+def variant_qc_keep(counts, p, maf: Optional[float], geno: Optional[float], hwe: Optional[float]):
+    """(keep (V,) bool, removed_by (V,) int8) of (V, 4) counts (HOM_A1, HET, HOM_A2, MISSING) and HWE p-values (may be
+    None without --hwe).  keep is the intersection of the filters given: --maf removes n = 0 or min(f, 1 - f) < maf,
+    --geno removes MISSING / N > geno, --hwe removes p < hwe.  removed_by is 0 for a kept variant, else 1 + the index in
+    QC_FILTERS of the first filter it fails."""
+    c = np.asarray(counts, np.int64).reshape(-1, 4)
+    n, f = _allele_freqs(c)
+    fails = []
+    if geno is not None:
+        total = (n + c[:, 3]).astype(np.float64)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            fails.append(c[:, 3].astype(np.float64) / total > geno)
+    else:
+        fails.append(np.zeros(len(c), bool))
+    fails.append(np.asarray(p, np.float64) < hwe if hwe is not None else np.zeros(len(c), bool))
+    if maf is not None:
+        with np.errstate(invalid="ignore"):
+            fails.append((n == 0) | (np.minimum(f, 1.0 - f) < maf))
+    else:
+        fails.append(np.zeros(len(c), bool))
+    removed_by = np.zeros(len(c), np.int8)
+    for code in (3, 2, 1):                          # the first filter failed wins
+        removed_by[fails[code - 1]] = code
+    return removed_by == 0, removed_by
+
+
+def write_qc_reports(prefix: str, bim, counts, p) -> None:
+    """PLINK 2's variant QC reports of every variant, tab-separated, in .bim order, doubles as the shortest text that
+    reads back as the same double: prefix.afreq (A2 as REF, A1 as ALT, ALT_FREQS = the A1 frequency, OBS_CT = 2n),
+    .vmiss (MISSING_CT, OBS_CT = N, F_MISS = MISSING_CT / N) and .hardy (O(HET_A1) = HET / n, E(HET_A1) = (2 f) (1 - f),
+    P the exact HWE p-value)."""
+    c = np.asarray(counts, np.int64).reshape(-1, 4)
+    n, f = _allele_freqs(c)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        total = n + c[:, 3]
+        fmiss = c[:, 3].astype(np.float64) / total.astype(np.float64)
+        o_het = c[:, 1].astype(np.float64) / n.astype(np.float64)
+        e_het = (2.0 * f) * (1.0 - f)
+    rows = list(zip(bim, c.tolist(), n.tolist(), f.tolist(), total.tolist(), fmiss.tolist(), o_het.tolist(),
+                    e_het.tolist(), np.asarray(p, np.float64).tolist()))
+    with open(prefix + ".afreq", "w", encoding="utf-8") as fh:
+        fh.write("#CHROM\tID\tREF\tALT\tALT_FREQS\tOBS_CT\n")
+        fh.write("".join(f"{b.contig}\t{b.id}\t{b.a2}\t{b.a1}\t{fr!r}\t{2 * nn}\n" for b, _, nn, fr, *_ in rows))
+    with open(prefix + ".vmiss", "w", encoding="utf-8") as fh:
+        fh.write("#CHROM\tID\tMISSING_CT\tOBS_CT\tF_MISS\n")
+        fh.write("".join(f"{b.contig}\t{b.id}\t{cc[3]}\t{t}\t{fm!r}\n" for b, cc, _, _, t, fm, *_ in rows))
+    with open(prefix + ".hardy", "w", encoding="utf-8") as fh:
+        fh.write("#CHROM\tID\tA1\tAX\tHOM_A1_CT\tHET_A1_CT\tTWO_AX_CT\tO(HET_A1)\tE(HET_A1)\tP\n")
+        fh.write("".join(f"{b.contig}\t{b.id}\t{b.a1}\t{b.a2}\t{cc[0]}\t{cc[1]}\t{cc[2]}\t{o!r}\t{e!r}\t{pp!r}\n"
+                         for b, cc, _, _, _, _, o, e, pp in rows))
 
 
 def check_king_cutoff_kept(kept: int, num_pc: int) -> None:
@@ -871,6 +989,7 @@ def main(args: Optional[Sequence[str]] = None):
     conf = PcaConf(list(sys.argv[1:] if args is None else args))
     check_king_flags(conf)
     check_ld_flags(conf)
+    check_qc_flags(conf)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         import torch
         import torch.distributed as dist
@@ -885,8 +1004,11 @@ def main(args: Optional[Sequence[str]] = None):
     data = driver.getData
     filtered = [driver.filterDataset(d) for d in data]
     callsRdd = driver.getCallsRdd(filtered)
+    qc_keep = None
+    if any(v is not None for v in qc_limits(conf).values()):
+        qc_keep = driver.variantQc(callsRdd)            # the QC-passing set is the variant set of everything below
     if window_lo is not None:
-        driver.ldPrune(callsRdd, window_lo)             # the pruned set is the variant set of everything below
+        driver.ldPrune(callsRdd, window_lo, qc_keep)    # the pruned set is the variant set of everything below
     if conf.projectLoadings.isDefined:
         if conf.saveLoadings.isDefined:
             raise ValueError("--project-loadings computes no principal components to save; drop --save-loadings")

@@ -422,6 +422,29 @@ int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
                         double* out_hwe_p);
 int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out_p);
 
+/* ---- sample quality control (beyond VariantsPca.scala: which samples go into S; DESIGN.md 11) -------------------------
+ * --keep / --remove / --mind decide the samples of a run before its context exists: the per-sample missing-call counts
+ * over every row of a fileset, then the rows repacked to the kept samples, which a plain run reads as its fileset.
+ * n_samples is the rows' own sample count; the context supplies only its device, a lane and scratch buffers (its own
+ * n_samples plays no part), so the driver can run these before it knows the size of the run's context.  Rows are PLINK 1
+ * .bed rows (as vpca_accumulate_bed; bytes past ceil(n_samples / 4) and the padding bits of the last byte are ignored).
+ * vpca_sample_missing_bed: out_missing[s] = the rows where sample s has code 01 (exact int32 sums, whatever the split of
+ *   the rows into calls); all n_samples entries are overwritten, with zeros when nv = 0.
+ * vpca_subset_bed_samples: out row v (at out_rows + v * out_stride) = the codes of samples keep_idx[0 .. m) of row v, in
+ *   that order, packed as a .bed row of m samples: the padding bits of its last byte are 0, as PLINK writes them, so the
+ *   bytes equal those of a fileset of the kept samples.  Bytes of an out row past ceil(m / 4) are not written.
+ * Driver-side and synchronous.  Rows are staged in chunks of at most 64 MB, so device memory does not grow with nv or
+ *   n_samples; the subset pass double-buffers its chunks and overlaps the upload of chunk i + 1 with the download of
+ *   chunk i.  The buffers are allocated on the first call and freed by vpca_destroy.  The PCA Gram, U, the kinship counts,
+ *   the subset state, the LD state and the variant QC buffers are left alone.
+ * VPCA_ERR_BAD_ARG, before any row is staged and with the outputs untouched: a NULL rows / out_missing / keep_idx /
+ *   out_rows when nv > 0, nv < 0, n_samples < 1, stride_bytes < ceil(n_samples / 4), m < 1, keep_idx not strictly
+ *   increasing or outside [0, n_samples), out_stride < ceil(m / 4).  VPCA_ERR_OVERFLOW: nv > 2^31 - 1 for the counts. */
+int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t n_samples,
+                            int32_t* out_missing /* n_samples entries, overwritten */);
+int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t n_samples,
+                            const int32_t* keep_idx, int32_t m, uint8_t* out_rows, int64_t out_stride);
+
 /* ---- one process, all GPUs of the box (SURVEY 8b "process model") --------------------------------------------------
  * A vpca_pool is what `class VariantsPcaDriver` holds on a multi-GPU host: one vpca_ctx per GPU, wired with
  * vpca_gram_set_peers_local in VPCA_PEER_OWNER_ROWS mode (VPCA_PEER_REPLICATE when n_samples < 64 x n_gpus).  Spark

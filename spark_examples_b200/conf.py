@@ -123,4 +123,7 @@ class PcaConf(GenomicsConf):
             ("maf", float, None, False),                  # --bed-path runs: drop variants with minor-allele frequency < this
             ("geno", float, None, False),                 # --bed-path runs: drop variants with missing-call rate > this
             ("hwe", float, None, False),                  # --bed-path runs: drop variants with exact HWE p-value < this
+            ("keep", str, None, False),                   # --bed-path runs: analyse only the samples listed in this ID file
+            ("remove", str, None, False),                 # --bed-path runs: leave out the samples listed in this ID file
+            ("mind", float, None, False),                 # --bed-path runs: drop samples with missing-call rate > this
         ]

@@ -21,6 +21,7 @@
 #include <functional>
 #include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "vpca_internal.h"
@@ -98,6 +99,15 @@ struct vpca_ctx {
     int32_t* d_qc_counts = nullptr;
     double* d_qc_p = nullptr;
     int64_t cap_qc_rows = 0, cap_qc_counts = 0, cap_qc_p = 0;
+    // sample QC (vpca_sample_missing_bed / vpca_subset_bed_samples): double-buffered raw and repacked rows of one chunk, the
+    // per-sample counts, the kept indices, and a stream and events of their own for the D2H copies; grow-only
+    uint8_t* d_sm_rows[2] = {nullptr, nullptr};
+    uint8_t* d_sm_out[2] = {nullptr, nullptr};
+    int32_t* d_sm_miss = nullptr;
+    int32_t* d_sm_idx = nullptr;
+    int64_t cap_sm_rows[2] = {0, 0}, cap_sm_out[2] = {0, 0}, cap_sm_miss = 0, cap_sm_idx = 0;
+    cudaStream_t sm_d2h_stream = nullptr;
+    cudaEvent_t sm_ev_copy[2] = {nullptr, nullptr}, sm_ev_kern[2] = {nullptr, nullptr};
     GramPlan ld_plan;
     LdWork ld;
 
@@ -692,8 +702,13 @@ int vpca_destroy(vpca_ctx* ctx) {
     for (void* p : {(void*)ctx->d_ld_G, ctx->d_ld_x, (void*)ctx->d_ld_rows[0], (void*)ctx->d_ld_rows[1], (void*)ctx->d_ld_wlo,
                     (void*)ctx->d_ld_keep, (void*)ctx->ld.d_bits, (void*)ctx->ld.d_seg, (void*)ctx->ld.d_row_total,
                     (void*)ctx->ld.d_row_start, (void*)ctx->ld.d_total, (void*)ctx->ld.d_pairs, (void*)ctx->ld.d_r2,
-                    (void*)ctx->d_ld_elig, (void*)ctx->d_qc_rows, (void*)ctx->d_qc_counts, (void*)ctx->d_qc_p})
+                    (void*)ctx->d_ld_elig, (void*)ctx->d_qc_rows, (void*)ctx->d_qc_counts, (void*)ctx->d_qc_p,
+                    (void*)ctx->d_sm_rows[0], (void*)ctx->d_sm_rows[1], (void*)ctx->d_sm_out[0], (void*)ctx->d_sm_out[1],
+                    (void*)ctx->d_sm_miss, (void*)ctx->d_sm_idx})
         cudaFree(p);
+    for (cudaEvent_t ev : {ctx->sm_ev_copy[0], ctx->sm_ev_copy[1], ctx->sm_ev_kern[0], ctx->sm_ev_kern[1]})
+        if (ev) cudaEventDestroy(ev);
+    if (ctx->sm_d2h_stream) cudaStreamDestroy(ctx->sm_d2h_stream);
     gram_plan_free(ctx->ld_plan);
     gram_plan_free(ctx->plan);
     for (cudaEvent_t ev : {ctx->ev_t0, ctx->ev_t1, ctx->ev_e0, ctx->ev_e1})
@@ -2248,6 +2263,207 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
         ctx->c_d2h += 8 * nvc;
     }
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+// ---- sample QC (samples.cu, DESIGN.md 11) -------------------------------------------------------------------------------
+// Driver-side and synchronous, on rows of their own sample count: the context lends its device, a lane and scratch.  Rows
+// are staged in chunks of at most kSmStageBytes.  The subset pass copies both ways: chunk i + 1 goes up on the lane's copy
+// stream while a helper thread brings chunk i down on a stream of its own, so that the two copies (pageable, hence each
+// blocking the thread that issues it) run at once on the two copy engines.
+namespace {
+constexpr int64_t kSmStageBytes = 64ll << 20;   // raw .bed bytes per staged chunk
+
+// the checks both calls share; 0 when the arguments are good
+int sample_rows_args(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
+                     int32_t n_samples) {
+    if (nv < 0 || (nv > 0 && rows == nullptr))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (nv = %lld must be >= 0, rows set when nv > 0)", fn,
+                    (long long)nv);
+    if (n_samples < 1 || stride_bytes < ((int64_t)n_samples + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (n_samples = %d must be >= 1, stride_bytes = %lld >= "
+                    "ceil(n_samples / 4))", fn, (int)n_samples, (long long)stride_bytes);
+    return VPCA_OK;
+}
+
+cudaError_t sm_grow(void* p, int64_t& cap, int64_t need, size_t elem) {
+    return ld_grow_bytes(reinterpret_cast<void**>(p), cap, need, elem);
+}
+
+// The D2H side of vpca_subset_bed_samples: copies chunk i down once the main thread has launched its kernel, and
+// reports each finished copy, which frees the chunk's two buffers for chunk i + 2.
+struct SubsetDownloader {
+    std::mutex mu;
+    std::condition_variable cv;
+    int64_t launched = 0, copied = 0;   // chunks whose kernel is enqueued / whose rows are on the host
+    bool stop = false;
+    cudaError_t err = cudaSuccess;
+    std::thread th;
+
+    void launched_chunk(int64_t i) {
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            launched = i + 1;
+        }
+        cv.notify_all();
+    }
+    // blocks until `count` chunks are on the host; false on a copy error
+    bool wait_copied(int64_t count) {
+        std::unique_lock<std::mutex> lk(mu);
+        cv.wait(lk, [&] { return copied >= count || err != cudaSuccess; });
+        return err == cudaSuccess;
+    }
+    ~SubsetDownloader() {
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            stop = true;
+        }
+        cv.notify_all();
+        if (th.joinable()) th.join();
+    }
+};
+}   // namespace
+
+int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t n_samples,
+                            int32_t* out_missing) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    if (int rc = sample_rows_args(ctx, "vpca_sample_missing_bed", rows, nv, stride_bytes, n_samples)) return rc;
+    if (nv > 0 && out_missing == nullptr)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_sample_missing_bed: out_missing is NULL");
+    if (nv > 2147483647ll)
+        return fail(ctx, VPCA_ERR_OVERFLOW, "vpca_sample_missing_bed: %lld rows could overflow an int32 count",
+                    (long long)nv);
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) {
+        if (out_missing != nullptr) memset(out_missing, 0, (size_t)n_samples * sizeof(int32_t));
+        return VPCA_OK;
+    }
+    const int64_t step = std::max<int64_t>(1, std::min(nv, kSmStageBytes / stride_bytes));
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = sm_grow(&ctx->d_sm_rows[0], ctx->cap_sm_rows[0], step * stride_bytes, 1);
+        if (e == cudaSuccess) e = sm_grow(&ctx->d_sm_miss, ctx->cap_sm_miss, n_samples, sizeof(int32_t));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "sample QC buffers for %lld rows of %lld bytes: %s", (long long)step,
+                        (long long)stride_bytes, cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->d_sm_miss, 0, (size_t)n_samples * sizeof(int32_t), L.stream));
+    for (int64_t v = 0; v < nv; v += step) {
+        const int64_t nvc = std::min(step, nv - v);
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[0], rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+                                     cudaMemcpyHostToDevice, L.stream));
+        ctx->c_h2d += nvc * stride_bytes;
+        CUDA_OK(ctx, sample_missing(ctx->d_sm_rows[0], stride_bytes, (int)nvc, n_samples, ctx->d_sm_miss, L.stream));
+        ctx->c_launches += 1;
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(out_missing, ctx->d_sm_miss, (size_t)n_samples * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                                 L.stream));
+    ctx->c_d2h += 4 * (int64_t)n_samples;
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t n_samples,
+                            const int32_t* keep_idx, int32_t m, uint8_t* out_rows, int64_t out_stride) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    if (int rc = sample_rows_args(ctx, "vpca_subset_bed_samples", rows, nv, stride_bytes, n_samples)) return rc;
+    if (nv > 0 && (keep_idx == nullptr || out_rows == nullptr))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_subset_bed_samples: keep_idx and out_rows must be set");
+    if (m < 1 || out_stride < ((int64_t)m + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_subset_bed_samples: bad argument (m = %d must be >= 1, out_stride = %lld "
+                    ">= ceil(m / 4))", (int)m, (long long)out_stride);
+    if (keep_idx != nullptr)
+        for (int32_t j = 0; j < m; ++j)
+            if (keep_idx[j] < 0 || keep_idx[j] >= n_samples || (j > 0 && keep_idx[j] <= keep_idx[j - 1]))
+                return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_subset_bed_samples: keep_idx[%d] = %d must be in [0, %d) and "
+                            "above the entry before it", (int)j, (int)keep_idx[j], (int)n_samples);
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int64_t mb = ((int64_t)m + 3) / 4;
+    const int64_t step = std::max<int64_t>(1, std::min(nv, kSmStageBytes / stride_bytes));
+    const int64_t chunks = (nv + step - 1) / step;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = cudaSuccess;
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
+            e = sm_grow(&ctx->d_sm_rows[b], ctx->cap_sm_rows[b], step * stride_bytes, 1);
+            if (e == cudaSuccess) e = sm_grow(&ctx->d_sm_out[b], ctx->cap_sm_out[b], step * mb, 1);
+            if (e == cudaSuccess && ctx->sm_ev_copy[b] == nullptr)
+                e = cudaEventCreateWithFlags(&ctx->sm_ev_copy[b], cudaEventDisableTiming);
+            if (e == cudaSuccess && ctx->sm_ev_kern[b] == nullptr)
+                e = cudaEventCreateWithFlags(&ctx->sm_ev_kern[b], cudaEventDisableTiming);
+        }
+        if (e == cudaSuccess) e = sm_grow(&ctx->d_sm_idx, ctx->cap_sm_idx, m, sizeof(int32_t));
+        if (e == cudaSuccess && ctx->sm_d2h_stream == nullptr)
+            e = cudaStreamCreateWithFlags(&ctx->sm_d2h_stream, cudaStreamNonBlocking);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "sample subset buffers for %lld rows of %lld bytes: %s", (long long)step,
+                        (long long)stride_bytes, cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_idx, keep_idx, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, L.stream));
+    ctx->c_h2d += 4 * (int64_t)m;
+    SubsetDownloader down;
+    const int device = ctx->cfg.device;
+    down.th = std::thread([&down, ctx, device, chunks, step, nv, mb, out_rows, out_stride] {
+        cudaError_t e = cudaSetDevice(device);
+        for (int64_t i = 0; i < chunks && e == cudaSuccess; ++i) {
+            {
+                std::unique_lock<std::mutex> lk(down.mu);
+                down.cv.wait(lk, [&] { return down.launched > i || down.stop; });
+                if (down.launched <= i) return;
+            }
+            const int b = (int)(i & 1);
+            const int64_t v = i * step, nvc = std::min(step, nv - v);
+            e = cudaStreamWaitEvent(ctx->sm_d2h_stream, ctx->sm_ev_kern[b], 0);
+            if (e == cudaSuccess)
+                e = out_stride == mb
+                        ? cudaMemcpyAsync(out_rows + (size_t)(v * mb), ctx->d_sm_out[b], (size_t)(nvc * mb),
+                                          cudaMemcpyDeviceToHost, ctx->sm_d2h_stream)
+                        : cudaMemcpy2DAsync(out_rows + (size_t)(v * out_stride), (size_t)out_stride, ctx->d_sm_out[b],
+                                            (size_t)mb, (size_t)mb, (size_t)nvc, cudaMemcpyDeviceToHost, ctx->sm_d2h_stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->sm_d2h_stream);
+            {
+                std::lock_guard<std::mutex> lk(down.mu);
+                if (e == cudaSuccess)
+                    down.copied = i + 1;
+                else
+                    down.err = e;
+            }
+            down.cv.notify_all();
+        }
+        if (e != cudaSuccess) {   // cudaSetDevice failed before the first chunk
+            std::lock_guard<std::mutex> lk(down.mu);
+            down.err = e;
+            down.cv.notify_all();
+        }
+    });
+    for (int64_t i = 0; i < chunks; ++i) {
+        const int b = (int)(i & 1);
+        const int64_t v = i * step, nvc = std::min(step, nv - v);
+        if (!down.wait_copied(i - 1)) break;   // chunk i - 2, the last user of buffers b, is on the host
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[b], rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+                                     cudaMemcpyHostToDevice, L.copy_stream));
+        CUDA_OK(ctx, cudaEventRecord(ctx->sm_ev_copy[b], L.copy_stream));
+        ctx->c_h2d += nvc * stride_bytes;
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, ctx->sm_ev_copy[b], 0));
+        CUDA_OK(ctx, subset_samples(ctx->d_sm_rows[b], stride_bytes, (int)nvc, ctx->d_sm_idx, m, ctx->d_sm_out[b], mb,
+                                    L.stream));
+        CUDA_OK(ctx, cudaEventRecord(ctx->sm_ev_kern[b], L.stream));
+        ctx->c_launches += 1;
+        down.launched_chunk(i);
+    }
+    if (!down.wait_copied(chunks))
+        return fail(ctx, VPCA_ERR_CUDA, "vpca_subset_bed_samples: device-to-host copy failed: %s",
+                    cudaGetErrorString(down.err));
+    ctx->c_d2h += nv * mb;
     return VPCA_OK;
 }
 

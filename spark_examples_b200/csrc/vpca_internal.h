@@ -153,6 +153,16 @@ cudaError_t qc_count(const uint8_t* d_rows, int64_t pitch, int nv, int n, int32_
 // The exact HWE p-value (vpca.h) of each of nv count rows (layout above, 16-byte aligned).  Never synchronises.
 cudaError_t qc_hwe(const int32_t* d_counts, int nv, double* d_p, cudaStream_t stream);
 
+// ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
+// Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to
+// d_missing[0 .. n) with integer atomics.  Bytes past ceil(n / 4) and the padding bits of the last byte are ignored.
+// Never synchronises.
+cudaError_t sample_missing(const uint8_t* d_rows, int64_t pitch, int nv, int n, int32_t* d_missing, cudaStream_t stream);
+// Out row v (at d_out + v * out_pitch, ceil(m / 4) bytes written, padding bits 0) = the codes of samples d_keep_idx[0 .. m)
+// of source row v (at d_rows + v * pitch).  Never synchronises.
+cudaError_t subset_samples(const uint8_t* d_rows, int64_t pitch, int nv, const int32_t* d_keep_idx, int m, uint8_t* d_out,
+                           int64_t out_pitch, cudaStream_t stream);
+
 // ---- KING-robust kinship pairs from the 3n x 3n plane Gram (kinship.cu) ----------------------------------------------
 constexpr int kKinMaxN = 21845;   // 3n <= 65 535: the plane Gram stays below 2^32 cells
 // Device scratch of vpca_kinship_pairs, owned by the context and kept between calls.

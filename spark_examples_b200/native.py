@@ -53,7 +53,8 @@ EXPORTED_SYMBOLS = (
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
     "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
-    "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact",
+    "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact", "vpca_sample_missing_bed",
+    "vpca_subset_bed_samples",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
@@ -285,6 +286,10 @@ def load_library() -> ctypes.CDLL:
     L.vpca_variant_qc_bed.argtypes = [vp, vp, i64, i64, vp, vp]
     L.vpca_hwe_exact.restype = ctypes.c_int
     L.vpca_hwe_exact.argtypes = [vp, vp, i64, vp]
+    L.vpca_sample_missing_bed.restype = ctypes.c_int
+    L.vpca_sample_missing_bed.argtypes = [vp, vp, i64, i64, i32, vp]
+    L.vpca_subset_bed_samples.restype = ctypes.c_int
+    L.vpca_subset_bed_samples.argtypes = [vp, vp, i64, i64, i32, vp, i32, vp, i64]
     L.vpca_compute_pca_subset.restype = ctypes.c_int
     L.vpca_compute_pca_subset.argtypes = [vp, vp, i32, vp, vp, ctypes.POINTER(i32)]
     _lib = L
@@ -769,6 +774,41 @@ class NativePca:
         p = np.zeros(nv + 1, np.float64)
         self._check(self._lib.vpca_hwe_exact(self._h, _host_ptr(c), nv, _host_ptr(p)))
         return p[:nv]
+
+    # -- sample QC (vpca.h, DESIGN.md 11) ----------------------------------------------------------------------------
+    @staticmethod
+    def _bed_rows(rows) -> np.ndarray:
+        b = np.asarray(rows)
+        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
+            b = np.ascontiguousarray(b, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        return b
+
+    def sampleMissingBed(self, rows: np.ndarray, n_samples: int) -> np.ndarray:
+        """Missing calls of each of the n_samples samples of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in
+        place, not copied) -> (n_samples,) int32.  The rows need not have this context's sample count.  Synchronises."""
+        b = self._bed_rows(rows)
+        out = np.zeros(max(int(n_samples), 1), np.int32)
+        empty = np.zeros(1, np.uint8)
+        self._check(self._lib.vpca_sample_missing_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), b.shape[0],
+                                                      b.shape[1], int(n_samples), _host_ptr(out)))
+        return out[:int(n_samples)]
+
+    def subsetBedSamples(self, rows: np.ndarray, n_samples: int, keep) -> np.ndarray:
+        """PLINK .bed rows of n_samples samples ((V, stride) uint8; a .bed memmap is read in place, not copied) repacked to
+        the samples keep (strictly increasing indices) -> (V, ceil(M / 4)) uint8, the rows of a fileset of those samples.
+        The rows need not have this context's sample count.  Synchronises."""
+        b = self._bed_rows(rows)
+        idx = np.ascontiguousarray(keep, dtype=np.int32).reshape(-1)
+        m = len(idx)
+        mb = (m + 3) // 4
+        out = np.empty((b.shape[0], mb), np.uint8)
+        empty = np.zeros(1, np.uint8)
+        self._check(self._lib.vpca_subset_bed_samples(
+            self._h, b.ctypes.data if b.size else _host_ptr(empty), b.shape[0], b.shape[1], int(n_samples),
+            _host_ptr(idx) if m else None, m, out.ctypes.data if out.size else _host_ptr(empty), mb))
+        return out
 
     def computePcaSubset(self, keep, k: int = 2):
         """PCs of the samples with keep[s] true, from the Gram of all of them (DESIGN.md 8) -> (vecs (n, k), evals (k,),

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 from pathlib import Path
-from typing import List, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -96,6 +96,78 @@ class BedFile:
 
     def rows(self, v0: int, v1: int) -> np.ndarray:
         return np.ascontiguousarray(self._map[v0:v1])
+
+
+def read_id_file(path: str) -> List[Tuple[Optional[str], str]]:
+    """[(FID or None, IID)] of a sample ID file (--keep / --remove): whitespace-separated, blank lines ignored, a first line
+    that starts with '#' is a header; a line gives FID IID as its first two tokens, or a bare IID as its only token.  This
+    reads PLINK 2's `#FID IID` lists, such as .king.cutoff.in.id and .mindrem.id."""
+    out: List[Tuple[Optional[str], str]] = []
+    first = True
+    with open(path, "r", encoding="utf-8") as fh:
+        for line in fh:
+            tok = line.split()
+            if not tok:
+                continue
+            if first and tok[0].startswith("#"):
+                first = False
+                continue
+            first = False
+            out.append((tok[0], tok[1]) if len(tok) >= 2 else (None, tok[0]))
+    return out
+
+
+def match_sample_ids(fam_ids: Sequence[Tuple[str, str]], ids: Sequence[Tuple[Optional[str], str]], path: str = "ID file"):
+    """(listed (N,) bool over the .fam samples, IDs that match no sample) of read_id_file's entries.  A bare IID matches
+    the sample with that IID; it is refused (ValueError) when several families hold that IID."""
+    pair = {fi: k for k, fi in enumerate(fam_ids)}
+    by_iid: dict = {}
+    for k, (_, iid) in enumerate(fam_ids):
+        by_iid.setdefault(iid, []).append(k)
+    listed = np.zeros(len(fam_ids), bool)
+    unmatched = 0
+    for fid, iid in ids:
+        if fid is None:
+            ks = by_iid.get(iid, [])
+            if len(ks) > 1:
+                fams = ", ".join(fam_ids[k][0] for k in ks)
+                raise ValueError(f"{path}: the bare IID {iid} is ambiguous: it occurs in families {fams}; give FID IID")
+            k = ks[0] if ks else None
+        else:
+            k = pair.get((fid, iid))
+        if k is None:
+            unmatched += 1
+        else:
+            listed[k] = True
+    return listed, unmatched
+
+
+class SampleSubset:
+    """The .bed rows of a fileset repacked to some of its samples (NativePca.subsetBedSamples), held in host memory, with
+    the interface the driver reads from a BedFile; the prefix, and with it the .bim, stays the fileset's."""
+
+    def __init__(self, bed: BedFile, keep_idx: np.ndarray, rows: np.ndarray):
+        self.prefix = bed.prefix
+        self.keep_idx = np.asarray(keep_idx, np.int64)
+        self.n_samples = len(self.keep_idx)
+        self.stride = (self.n_samples + 3) // 4
+        self.n_variants = bed.n_variants
+        if rows.shape != (self.n_variants, self.stride):
+            raise ValueError(f"subset rows have shape {rows.shape}, not ({self.n_variants}, {self.stride})")
+        self._map = rows
+
+    def rows(self, v0: int, v1: int) -> np.ndarray:
+        return np.ascontiguousarray(self._map[v0:v1])
+
+
+@dataclass
+class SampleSet:
+    """The samples a --bed-path run analyses (--keep / --remove / --mind): the kept .fam entries in file order and the
+    rows to read -- the fileset's own BedFile when every sample is kept, else a SampleSubset."""
+    keep: np.ndarray                       # (N,) bool over the .fam samples
+    callsets: List[Tuple[str, str]]        # read_fam entries of the kept samples
+    fam_ids: List[Tuple[str, str]]         # read_fam_ids entries of the kept samples
+    bed: object                            # BedFile | SampleSubset
 
 
 def decode_rows(rows: np.ndarray, n_samples: int, counted: int = COUNT_A1) -> np.ndarray:

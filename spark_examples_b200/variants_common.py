@@ -83,10 +83,11 @@ class VariantsDataset:
 
 
 class VariantsCommon:
-    """VariantsCommon.scala:33.  `indexes`/`names` as at :38-50, `data` as at :52-66."""
+    """VariantsCommon.scala:33.  `indexes`/`names` as at :38-50, `data` as at :52-66.  samples (plink.SampleSet, --bed-path
+    only): the samples chosen by --keep / --remove / --mind, which stand for the whole .fam."""
 
     def __init__(self, conf: PcaConf, sc=None, callsets: Optional[Sequence[Tuple[str, str]]] = None,
-                 datasets: Optional[Sequence[Sequence[Variant]]] = None):
+                 datasets: Optional[Sequence[Sequence[Variant]]] = None, samples=None):
         self.conf = conf
         self.ioStats: Optional[Dict[str, int]] = None
         per_part = conf.variantsPerPartition()
@@ -123,8 +124,12 @@ class VariantsCommon:
         elif conf.bedPath.isDefined:                               # additive: PLINK fileset on disk
             from . import plink
             counted = {"A1": plink.COUNT_A1, "A2": plink.COUNT_A2}[conf.bedCountedAllele().upper()]
-            self._set_callsets(plink.read_fam(conf.bedPath()))
-            bed = plink.BedFile(conf.bedPath(), n_samples=len(self.indexes))
+            if samples is not None:                                # --keep / --remove / --mind: the kept samples
+                self._set_callsets(samples.callsets)
+                bed = samples.bed
+            else:
+                self._set_callsets(plink.read_fam(conf.bedPath()))
+                bed = plink.BedFile(conf.bedPath(), n_samples=len(self.indexes))
             slices = [BedSlice(bed, v0, min(per_part, bed.n_variants - v0), counted)
                       for v0 in range(0, bed.n_variants, per_part)]
             self.data = [VariantsDataset(slices, "bed")]

@@ -174,8 +174,11 @@ class VariantsPcaDriver:
     def __init__(self, conf: PcaConf, ctx=None, common: Optional[VariantsCommon] = None):
         self.conf = conf
         self.applicationName = type(self).__name__
-        self.common = common if common is not None else VariantsCommon(conf, ctx)
         self._rank, self._world = vdist.rank_world()
+        self.samples = None   # plink.SampleSet of --keep / --remove / --mind: every .fam read and fileset goes through it
+        if common is None and sample_flags_given(conf):
+            self.samples = self.selectSamples()
+        self.common = common if common is not None else VariantsCommon(conf, ctx, samples=self.samples)
         self._nat: Optional[native.NativePca] = None
         self._gram_tensor = None
         self._torch_stream = None
@@ -365,8 +368,7 @@ class VariantsPcaDriver:
         check_king_cutoff_kept(m, numPc)
         print(f"KING cutoff {cutoff!r}: {m} of {rowCount} samples kept, {rowCount - m} projected.")
         if self.conf.outputPath.isDefined and self._rank == 0:
-            from . import plink
-            write_king_cutoff_ids(self.conf.outputPath(), plink.read_fam_ids(self.conf.bedPath()), keep)
+            write_king_cutoff_ids(self.conf.outputPath(), self._famIds(), keep)
         vecs, evals, nonZeroRows = nat.computePcaSubset(keep, numPc)
         print(f"Non zero rows in matrix: {nonZeroRows} / {m}.")                  # :208, of the kept samples' matrix
         self.pcaSamples = m
@@ -549,7 +551,7 @@ class VariantsPcaDriver:
         from . import plink
         r2, kb = self.conf.ldPrune(), self.conf.ldWindowKb()
         slices = [p for p in callsets.partitions if isinstance(p, BedSlice)]
-        bed = slices[0].bed if slices else plink.BedFile(self.conf.bedPath(), n_samples=callsets.n_samples)
+        bed = slices[0].bed if slices else self._bedFile(callsets.n_samples)
         nat = self._native(callsets.n_samples)
         if eligible is None:
             keep, _, _ = nat.ldPruneBed(bed._map, window_lo, r2)
@@ -570,7 +572,7 @@ class VariantsPcaDriver:
         would leave).  Writes P.afreq, P.vmiss and P.hardy with --output-path.  Returns the (V,) keep mask."""
         from . import plink
         slices = [p for p in callsets.partitions if isinstance(p, BedSlice)]
-        bed = slices[0].bed if slices else plink.BedFile(self.conf.bedPath(), n_samples=callsets.n_samples)
+        bed = slices[0].bed if slices else self._bedFile(callsets.n_samples)
         nat = self._native(callsets.n_samples)
         counts, p = nat.variantQcBed(bed._map)
         limits = qc_limits(self.conf)
@@ -586,6 +588,65 @@ class VariantsPcaDriver:
             s.keep = keep[s.v0:s.v0 + s.nv]
         return keep
 
+    # -- sample QC (beyond the reference; DESIGN.md 11) ----------------------------------------------------------------
+    def selectSamples(self):
+        """--keep / --remove / --mind: decide the samples of this --bed-path run before its context exists -> plink.SampleSet.
+        The ID lists are matched on the host; --mind counts every sample's missing calls over all variants, and the rows
+        are repacked to the kept samples, both on a short-lived 2-sample context (_sampleQcNative).  Every step below then
+        sees a fileset of the kept samples only.  Prints the `Sample QC` line; writes P.smiss and P.mindrem.id with --mind
+        and --output-path."""
+        from . import plink
+        conf, path = self.conf, self.conf.bedPath()
+        callsets, fam_ids = plink.read_fam(path), plink.read_fam_ids(path)
+        n = len(callsets)
+        bed = plink.BedFile(path, n_samples=n)
+        listed = {}
+        for flag, opt in (("--keep", conf.keep), ("--remove", conf.remove)):
+            if opt.isDefined:
+                listed[flag], unmatched = plink.match_sample_ids(fam_ids, plink.read_id_file(opt()), f"{flag} {opt()}")
+                if unmatched:
+                    print(f"{flag} {opt()}: {unmatched} IDs match no sample.")
+        keep, removed_by = sample_qc_keep(n, listed.get("--keep"), listed.get("--remove"))
+        mind = conf.mind.get
+        nat = None
+        try:
+            if mind is not None:
+                nat = self._sampleQcNative()
+                missing = np.asarray(nat.sampleMissingBed(bed._map, n), np.int64)
+                left = keep.copy()
+                keep, removed_by = sample_qc_keep(n, listed.get("--keep"), listed.get("--remove"), missing,
+                                                  bed.n_variants, mind)
+                if conf.outputPath.isDefined and self._rank == 0:
+                    write_sample_qc_reports(conf.outputPath(), fam_ids, left, missing, bed.n_variants, removed_by == 3)
+            m = int(keep.sum())
+            given = {"--keep": "--keep" in listed, "--remove": "--remove" in listed, "--mind": mind is not None}
+            removed = ", ".join(f"{int(np.count_nonzero(removed_by == code))} by {flag}" + (f" {mind!r}" if code == 3 else "")
+                                for code, flag in enumerate(SAMPLE_FILTERS, 1) if given[flag])
+            print(f"Sample QC: {m} of {n} samples kept ({removed} removed).")
+            check_sample_kept(m, n, conf.numPc())
+            check_king_flags(conf, m)                   # the kinship limit applies to the kept samples
+            if m == n:
+                return plink.SampleSet(keep, callsets, fam_ids, bed)   # the fileset as it is
+            kept = np.flatnonzero(keep)
+            if nat is None:
+                nat = self._sampleQcNative()
+            rows = nat.subsetBedSamples(bed._map, n, kept)
+        finally:
+            if nat is not None:
+                nat.close()
+        return plink.SampleSet(keep, [callsets[k] for k in kept.tolist()], [fam_ids[k] for k in kept.tolist()],
+                               plink.SampleSubset(bed, kept, rows))
+
+    def _famIds(self) -> List[Tuple[str, str]]:
+        """(FID, IID) of the samples of this run, in matrix order."""
+        from . import plink
+        return self.samples.fam_ids if self.samples is not None else plink.read_fam_ids(self.conf.bedPath())
+
+    def _bedFile(self, n: int):
+        """The fileset of this run's samples: its rows are what the Gram reads."""
+        from . import plink
+        return self.samples.bed if self.samples is not None else plink.BedFile(self.conf.bedPath(), n_samples=n)
+
     # -- KING-robust kinship of the sample pairs (beyond the reference; DESIGN.md 7) --------------------------------------
     def writeKingTable(self, path: Optional[str] = None, min_kinship: Optional[float] = None):
         """After getSimilarityMatrix of a --bed-path run with --make-king-table: rank 0 writes the pairs (filtered by
@@ -595,9 +656,8 @@ class VariantsPcaDriver:
         path = path if path is not None else self.conf.makeKingTable()
         if min_kinship is None:
             min_kinship = self.conf.kingTableFilter() if self.conf.kingTableFilter.isDefined else float("-inf")
-        from . import plink
         ids, counts, kin = self._nat.kinshipPairs(min_kinship)
-        write_king_table(path, plink.read_fam_ids(self.conf.bedPath()), ids, counts, kin)
+        write_king_table(path, self._famIds(), ids, counts, kin)
 
     def reportIoStats(self):                                                     # :281
         self.common.reportIoStats()
@@ -613,10 +673,18 @@ class VariantsPcaDriver:
             self._nat = None
 
     # -- GPU plumbing --------------------------------------------------------------------------------------------
+    def _device(self) -> int:
+        return self.conf.gpuDevice() if self.conf.gpuDevice.isDefined else int(os.environ.get("LOCAL_RANK", "0"))
+
+    def _sampleQcNative(self) -> native.NativePca:
+        """The short-lived context of the sample QC calls, which read rows of any sample count: 2 samples (a few bytes of
+        Gram), closed before the run's M-sample context and its M x M Gram exist."""
+        return native.NativePca(2, device=self._device())
+
     def _native(self, n: int) -> native.NativePca:
         if self._nat is not None:
             return self._nat
-        device = self.conf.gpuDevice() if self.conf.gpuDevice.isDefined else int(os.environ.get("LOCAL_RANK", "0"))
+        device = self._device()
         dtype = {"int8": native.DTYPE_I8, "i8": native.DTYPE_I8, "bf16": native.DTYPE_BF16}[self.conf.gpuDtype()]
         stream = d_gram = 0
         try:
@@ -848,6 +916,78 @@ def write_qc_reports(prefix: str, bim, counts, p) -> None:
                          for b, cc, _, _, _, _, o, e, pp in rows))
 
 
+SAMPLE_FILTERS = ("--keep", "--remove", "--mind")   # a removed sample is attributed to the first that removes it
+
+
+def sample_flags_given(conf: PcaConf) -> bool:
+    return conf.keep.isDefined or conf.remove.isDefined or conf.mind.isDefined
+
+
+def check_sample_flags(conf: PcaConf) -> None:
+    """Refuse --keep / --remove / --mind runs the sample QC path cannot serve, before any GPU work.  An ID file that cannot
+    be read is refused here; a bare IID that several families hold, when the .fam is matched (still before GPU work)."""
+    given = [flag for flag, opt in zip(SAMPLE_FILTERS, (conf.keep, conf.remove, conf.mind)) if opt.isDefined]
+    if not given:
+        return
+    if conf.mind.isDefined and not (np.isfinite(conf.mind()) and 0.0 <= conf.mind() <= 1.0):
+        raise ValueError(f"--mind takes a value in [0, 1], not {conf.mind()!r}")
+    flags = " / ".join(given)
+    if not conf.bedPath.isDefined:
+        raise ValueError(f"{flags} selects samples of a PLINK fileset: give --bed-path")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError(f"{flags} runs on one GPU; launch a single process (WORLD_SIZE=1)")
+    if conf.checkpointPath.isDefined:
+        raise ValueError(f"{flags} decides the samples before the Gram, and a checkpoint does not record them; drop "
+                         "--checkpoint-path")
+    from . import plink
+    for flag, opt in (("--keep", conf.keep), ("--remove", conf.remove)):
+        if opt.isDefined:
+            try:
+                plink.read_id_file(opt())
+            except (OSError, UnicodeDecodeError) as e:
+                raise ValueError(f"{flag} {opt()}: cannot read the ID file ({e})") from None
+
+
+def sample_qc_keep(n: int, listed_keep=None, listed_remove=None, missing=None, n_variants: int = 0,
+                   mind: Optional[float] = None):
+    """(keep (N,) bool, removed_by (N,) int8) of the sample filters given: --keep keeps only listed_keep, --remove drops
+    listed_remove, --mind drops F_MISS = MISSING_CT / V > mind (one rounded division; V = 0 removes nothing).  removed_by
+    is 0 for a kept sample, else 1 + the index in SAMPLE_FILTERS of the first filter that removes it."""
+    removed_by = np.zeros(n, np.int8)
+    if listed_keep is not None:
+        removed_by[~np.asarray(listed_keep, bool)] = 1
+    if listed_remove is not None:
+        removed_by[(removed_by == 0) & np.asarray(listed_remove, bool)] = 2
+    if mind is not None:
+        with np.errstate(invalid="ignore", divide="ignore"):
+            fmiss = np.asarray(missing, np.int64).astype(np.float64) / np.float64(n_variants)
+        removed_by[(removed_by == 0) & (fmiss > mind)] = 3
+    return removed_by == 0, removed_by
+
+
+def check_sample_kept(kept: int, n: int, num_pc: int) -> None:
+    """Refuse a sample selection that leaves too few samples for the PCs asked for."""
+    if kept < 2 or kept < num_pc:
+        raise ValueError(f"sample QC keeps {kept} of {n} samples: at least max(2, --num-pc = {num_pc}) are needed")
+
+
+def write_sample_qc_reports(prefix: str, fam: Sequence[Tuple[str, str]], left: np.ndarray, missing: np.ndarray,
+                            n_variants: int, mind_removed: np.ndarray) -> None:
+    """--mind's outputs: prefix.smiss (PLINK 2's columns, tab-separated: one line per sample left by --keep / --remove, in
+    .fam order; OBS_CT = V, F_MISS = MISSING_CT / V as the shortest text that reads back as the same double) and
+    prefix.mindrem.id (`#FID<TAB>IID`, the samples --mind removed; written even when empty)."""
+    miss = np.asarray(missing, np.int64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        fmiss = miss.astype(np.float64) / np.float64(n_variants)
+    with open(prefix + ".smiss", "w", encoding="utf-8") as fh:
+        fh.write("#FID\tIID\tMISSING_CT\tOBS_CT\tF_MISS\n")
+        fh.write("".join(f"{fam[s][0]}\t{fam[s][1]}\t{int(miss[s])}\t{n_variants}\t{float(fmiss[s])!r}\n"
+                         for s in np.flatnonzero(left).tolist()))
+    with open(prefix + ".mindrem.id", "w", encoding="utf-8") as fh:
+        fh.write("#FID\tIID\n")
+        fh.write("".join(f"{fam[s][0]}\t{fam[s][1]}\n" for s in np.flatnonzero(mind_removed).tolist()))
+
+
 def check_king_cutoff_kept(kept: int, num_pc: int) -> None:
     """Refuse a --king-cutoff selection that leaves too few samples for the PCs asked for."""
     if kept < 2 or kept < num_pc:
@@ -987,6 +1127,7 @@ def _select_rows(off: np.ndarray, idx: np.ndarray, sel: np.ndarray):
 def main(args: Optional[Sequence[str]] = None):
     """VariantsPcaDriver.main (VariantsPca.scala:38-50)."""
     conf = PcaConf(list(sys.argv[1:] if args is None else args))
+    check_sample_flags(conf)
     check_king_flags(conf)
     check_ld_flags(conf)
     check_qc_flags(conf)

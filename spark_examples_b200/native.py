@@ -479,8 +479,9 @@ class NativePca:
         self._check(self._lib.vpca_abort(self._h, int(partition_id)))
 
     def accumulateDense(self, x: np.ndarray, nv: Optional[int] = None):
-        """Host dense tile, shape (n, nv), int8 (or uint16 bf16 bits); for DTYPE_E2M1 packed uint8 of shape
-        (n, ld / 2) with ld % 128 == 0, `nv` valid cells per row and zero cells after them."""
+        """Host dense tile, shape (n, ld), int8 (or uint16 bf16 bits), of which the first `nv` columns (default: all)
+        are cells; for DTYPE_E2M1 packed uint8 of shape (n, ld / 2) with ld % 128 == 0, `nv` valid cells per row and
+        zero cells after them up to a multiple of 128."""
         x = np.asarray(x)
         if self.elem_bits == 4:
             if x.dtype != np.uint8 or x.ndim != 2 or x.shape[0] != self.n or (x.shape[1] * 2) % 128:
@@ -491,10 +492,11 @@ class NativePca:
             return
         want = np.int8 if self.elem_bits == 8 else np.uint16
         if x.dtype != want or x.ndim != 2 or x.shape[0] != self.n:
-            raise VpcaError(VPCA_ERR_BAD_ARG, f"dense tile must be ({self.n}, nv) {np.dtype(want).name}")
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"dense tile must be ({self.n}, ld) {np.dtype(want).name}")
         if not x.flags.c_contiguous:
             x = np.ascontiguousarray(x)
-        self._check(self._lib.vpca_accumulate_dense(self._h, _host_ptr(x), x.shape[1], x.shape[1], 0))
+        ld = x.shape[1]
+        self._check(self._lib.vpca_accumulate_dense(self._h, _host_ptr(x), ld if nv is None else int(nv), ld, 0))
 
     def accumulateDenseDevice(self, d_ptr: int, nv: int, ld: int):
         self._check(self._lib.vpca_accumulate_dense(self._h, d_ptr, int(nv), int(ld), 1))

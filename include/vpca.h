@@ -536,7 +536,8 @@ int vpca_debug_lanczos_profile(vpca_ctx* ctx, int64_t* out, int32_t max_steps);
  *   the group's first input row.  sample_idx holds the calls that survive `_.hasVariation` (:164), already mapped to
  *   [0, n_samples).  The result stays on the device inside the context until the next vpca_join_rows / vpca_reset;
  *   *out_rows / *out_nnz report its size.  Driver-side step (the reference's join is a shuffle stage that precedes the
- *   mapPartitions tasks): one join at a time per context.
+ *   mapPartitions tasks): one join at a time per context.  Every argument check runs on the host before anything is
+ *   copied: a call refused with VPCA_ERR_BAD_ARG keeps the previous result, a call that fails later drops it.
  * vpca_join_fetch: copies the retained result to the host (out_offsets: out_rows + 1, out_idx: out_nnz entries).
  * vpca_accumulate_joined: encodes the retained rows and accumulates them into the staging Gram of partition_id, exactly
  *   like vpca_accumulate_calls would for the same rows (commit / abort as usual); no host round trip of the joined rows. */

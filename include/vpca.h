@@ -575,6 +575,16 @@ int vpca_debug_band_tiles(int32_t n_samples, int32_t cta_group, int32_t row0, in
  * (cudaOccupancyMaxActiveClusters); negative vpca_status on error. */
 int vpca_debug_max_clusters(int32_t device, int32_t cluster_size);
 int vpca_debug_plan(const int32_t* tiles, int32_t num_tiles, int32_t workers, int32_t kb_window, int32_t* out, int32_t max_pieces);
+/* Host-only: every (tile, k-range) piece each of `workers` workers replays in one launch of kb_total k-blocks, in launch
+ * order, under the schedule the Gram kernel takes for a whole-cohort context of n_samples (tiles as vpca_debug_tiles)
+ * with windows of kb_window k-blocks and the initial split -- 6 int32 per piece {worker, tile, first k-block, end k-block,
+ * first (the accumulator starts from zero), flush (the accumulator is added into S after it)}.  front_frac >= 0 sets the
+ * split point s = floor(front_frac * kb_total) of the front/tail schedule (taken when workers / 2 < tiles < workers:
+ * worker t < tiles owns tile t for k-blocks [0, s), the others split the tiles x [s, kb_total)); < 0: its initial
+ * tiles / workers.  info (2 int32): {schedule: 0 whole-tile waves, 1 resident, 2 front/tail; s, or kb_total for the
+ * others}.  Returns the piece count (may exceed max_pieces), or VPCA_ERR_STATE when a worker's accumulators would not fit. */
+int vpca_debug_schedule(int32_t n_samples, int32_t cta_group, int32_t exact, int32_t workers, int32_t kb_window,
+                        int32_t kb_total, double front_frac, int32_t* out, int32_t max_pieces, int32_t* info);
 
 #ifdef __cplusplus
 }

@@ -33,6 +33,9 @@
 //     worker a piece of a single tile (N = 2504: 55 tiles, 66 pairs) that piece is the same in every window and the
 //     accumulator is flushed once at the end of the launch; otherwise (large N) it is whole-tile waves + a stream-K tail
 //     whose pieces are flushed one after the other;
+//   * with more tiles than half the workers but fewer than all of them (N = 2504: 55 tiles, 66 pairs) that split would
+//     leave some workers a whole tile in every window: there each tile has a front worker that multiplies it over the
+//     k-blocks [0, s), and the remaining workers share the tiles over [s, K) (front/tail schedule, see Sched);
 //   * the split of a window over the workers is speed-weighted from launch to launch (rebalance_kernel, repair_split);
 //   * the flush packs two cells into one 64-bit red (no carry between the halves: counts are non-negative, sums < 2^31).
 // Integer atomics make the result independent of the order of the flushes: S is bit-exact.
@@ -119,6 +122,8 @@ struct GramArgs {
     int* win_done;     // win_done[w] = number of workers whose producer has issued every load of window w
     long long* prof;   // optional per-CTA timestamps (globaltimer ns): start, first MMA, MMA done, end
     const double* cum; // cum[w] = fraction of every window's units owned by workers < w (cum[0] = 0, cum[W] = 1)
+    int front_tiles;   // > 0: the front/tail schedule (see Sched), with this many tiles (= front workers)
+    const double* front_frac;   // front/tail schedule: the front ends at k-block front_split(*front_frac, kb_total)
     int col_limit;     // accumulator columns of one worker (kAccCols)
     int acc_stride;    // unused by the register accumulator (Seg.col of the large-N schedule)
     int row_limit;     // rows of S at or beyond this one are never written (n, or the end of an owner-computes band)
@@ -245,40 +250,83 @@ __host__ __device__ inline bool repair_split(const TileDesc* tiles, int num_tile
     return true;
 }
 
+// The front/tail schedule applies when W / 2 < T < W (T tiles, W workers): an equal split of every window would give some
+// workers a whole tile and the others a sliver, so the critical path would be a whole tile in every window.
+__host__ __device__ inline bool front_tail_applies(int num_tiles, int workers) {
+    return 2 * num_tiles > workers && num_tiles < workers;
+}
+
+// Its split point s: the front covers k-blocks [0, s), the tail [s, kb_total).
+__host__ __device__ inline int front_split(double frac, int kb_total) {
+    const double f = frac < 0.0 ? 0.0 : (frac > 1.0 ? 1.0 : frac);
+    const int s = (int)(f * (double)kb_total);
+    return s < kb_total ? s : kb_total;
+}
+
 // Every role of a worker (TMA producer, MMA issuer, epilogue) replays the same deterministic schedule.
 //   resident (every worker's accumulators fit its budget):  window-synchronous stream-K -- the worker owns the same pieces
 //               (tile, k-range) in every window, so its accumulator stays in registers for the whole launch;
+//   front/tail (resident, W / 2 < T < W): front worker t < T owns tile t for k-blocks [0, s) and walks the windows like
+//               the resident schedule (one flush); the W - T tail workers split the region T tiles x [s, kb_total),
+//               tile-major, into contiguous equal shares, and flush every piece when it completes.  The tail stays out
+//               of the window pacing (Seg.win = -1).  s moves from launch to launch (rebalance_front_kernel);
 //   otherwise:  full tiles in waves (wave i = tiles [i W, (i+1) W), one per worker, whole K) -- the tile list is ordered
 //               so that a wave is a compact 2-D block of S and shares few row panels of X -- then the leftover
 //               tiles are split stream-K style over all workers; accumulators double-buffered against the epilogue.
+// Host-callable so that vpca_debug_schedule replays exactly what the kernel runs.
 struct Sched {
     SegPlan plan;
     long long u_begin, u_end, u;
-    int kbw, nwin, kb_total, resident, win, seg_i, nflush, acc_stride;
+    int kbw, nwin, kb_total, kb_end, resident, win, seg_i, nflush, acc_stride;
     int worker, workers, num_tiles, wave, full_waves, tail_first;
+    int tail, kb_split;   // front/tail schedule: this worker is in the tail; the split point s
     const TileDesc* tiles;
 
-    __device__ void init(const GramArgs& a, int w) {
+    // false if the worker's resident pieces do not fit its accumulator (the kernel then traps)
+    __host__ __device__ bool init(const GramArgs& a, int w) {
         kbw = a.kb_window;
         kb_total = a.kb_total;
+        kb_end = kb_total;
         resident = a.resident;
         acc_stride = a.acc_stride;
         worker = w;
         workers = a.num_workers;
         num_tiles = a.num_tiles;
         tiles = a.tiles;
-        nwin = (kb_total + kbw - 1) / kbw;
         win = 0;
         seg_i = 0;
         nflush = 0;
         wave = 0;
-        if (resident) {
+        tail = 0;
+        kb_split = kb_total;
+        u_begin = u_end = 0;
+        if (a.front_tiles > 0) {
+            kb_split = front_split(*a.front_frac, kb_total);
+            if (worker < a.front_tiles) {   // one piece of a whole tile's width in every window of [0, s)
+                kb_end = kb_split;
+                plan.n = 1;
+                plan.tile[0] = worker;
+                plan.lo[0] = 0;
+                plan.hi[0] = kbw;
+                plan.col[0] = 0;
+                plan.cols = tiles[worker].acc_cols;
+                plan.overflow = 0;
+            } else {                        // units of the tail: tile-major, kb_total - s per tile
+                tail = 1;
+                const long long units = (long long)a.front_tiles * (kb_total - kb_split);
+                const int tw = workers - a.front_tiles, j = worker - a.front_tiles;
+                u_begin = units * j / tw;
+                u_end = units * (j + 1) / tw;
+                plan.n = 0;
+            }
+        } else if (resident) {
             const long long uw = (long long)a.total_weight * kbw;
             // speed-weighted split (equal shares until the first launches have been timed, see rebalance_kernel)
             u_begin = (long long)((double)uw * a.cum[worker]);
             u_end = (worker + 1 == a.num_workers) ? uw : (long long)((double)uw * a.cum[worker + 1]);
             plan_segments(tiles, num_tiles, 0, u_begin, u_end, kbw, plan);
             if (plan.overflow || plan.cols > a.col_limit) {   // overlapping accumulators would corrupt S silently
+#ifdef __CUDA_ARCH__
                 if (a.err != nullptr && threadIdx.x == 0) {
                     a.err[0] = 9;
                     a.err[1] = (int)blockIdx.x;
@@ -287,6 +335,9 @@ struct Sched {
                     __threadfence_system();
                 }
                 __trap();
+#else
+                return false;
+#endif
             }
         } else {
             full_waves = a.num_full / workers;
@@ -297,11 +348,18 @@ struct Sched {
             u_end = tail_units * (worker + 1) / workers;
             plan.n = 0;
         }
+        nwin = (kb_end + kbw - 1) / kbw;
         u = u_begin;
+        return true;
     }
-    __device__ void fill(Seg& s, int t) const {
+    __host__ __device__ void fill(Seg& s, int t) const {
+#ifdef __CUDA_ARCH__
         const int4 lo = __ldg(reinterpret_cast<const int4*>(tiles + t));
         const int4 hi = __ldg(reinterpret_cast<const int4*>(tiles + t) + 1);
+#else
+        const int4 lo = reinterpret_cast<const int4*>(tiles + t)[0];
+        const int4 hi = reinterpret_cast<const int4*>(tiles + t)[1];
+#endif
         s.tile = t;
         s.rowA0 = lo.x;
         s.rowA1 = lo.y;
@@ -309,7 +367,25 @@ struct Sched {
         s.n_eff = lo.w;
         s.flags = hi.y;
     }
-    __device__ bool next(Seg& s) {
+    __host__ __device__ bool next(Seg& s) {
+        if (tail) {   // one piece at a time: [u, end of its tile or of the share), flushed when it completes
+            if (u >= u_end) return false;
+            const int span = kb_total - kb_split;
+            const int t = (int)(u / span);
+            const long long e = u_end < (long long)(t + 1) * span ? u_end : (long long)(t + 1) * span;
+            fill(s, t);
+            s.kb0 = kb_split + (int)(u - (long long)t * span);
+            s.kb1 = kb_split + (int)(e - (long long)t * span);
+            s.win = -1;
+            s.last_in_win = 0;
+            s.first = 1;
+            s.flush = 1;
+            s.col = 0;
+            s.slot = 0;
+            s.use = 0;
+            u = e;
+            return true;
+        }
         if (!resident) {
             s.win = 0;
             s.last_in_win = 0;
@@ -356,9 +432,9 @@ struct Sched {
         const int i = seg_i++;
         fill(s, plan.tile[i]);
         const int base = win * kbw;
-        const int cnt = min(kbw, kb_total - base);
-        s.kb0 = base + min(plan.lo[i], cnt);
-        s.kb1 = base + min(plan.hi[i], cnt);
+        const int cnt = kbw < kb_end - base ? kbw : kb_end - base;
+        s.kb0 = base + (plan.lo[i] < cnt ? plan.lo[i] : cnt);
+        s.kb1 = base + (plan.hi[i] < cnt ? plan.hi[i] : cnt);
         s.win = win;
         s.last_in_win = (seg_i == plan.n);
         s.col = plan.col[i];
@@ -802,6 +878,47 @@ __global__ void rebalance_kernel(const long long* __restrict__ prof, double* __r
     if (w == 0) *gen += 1;
 }
 
+// The front/tail schedule's counterpart: moves the split point s so that the slowest front worker (s k-blocks, one
+// flush) and the slowest tail worker (T (K - s) / (W - T) k-blocks, a flush per piece, its own L2 traffic) finish
+// together.  Each side's time is taken as proportional to its k-blocks, so the fixed point is where both finish
+// together, whatever the tail's flushes cost.  *frac stays within [lo, hi].
+__global__ void rebalance_front_kernel(const long long* __restrict__ prof, double* __restrict__ frac, int front, int workers,
+                                       int cta_group, int kb_total, double gain, double lo, double hi, long long min_ns,
+                                       int* __restrict__ gen) {
+    __shared__ long long tmax[2][32];
+    const int w = threadIdx.x;
+    long long t = 0;
+    if (w < workers) t = prof[(size_t)w * cta_group * 4 + 2] - prof[(size_t)w * cta_group * 4 + 0];
+    const int side = w < front ? 0 : 1;
+    // per-side max: a warp's lanes may straddle the two sides, so reduce each side with the other side's lanes at 0
+    long long m0 = side == 0 ? t : 0, m1 = side == 1 ? t : 0;
+    for (int o = 16; o > 0; o >>= 1) {
+        m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+        m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+    }
+    if ((w & 31) == 0) {
+        tmax[0][w >> 5] = m0;
+        tmax[1][w >> 5] = m1;
+    }
+    __syncthreads();
+    if (w != 0) return;
+    long long tf = 0, tt = 0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) {
+        tf = max(tf, tmax[0][i]);
+        tt = max(tt, tmax[1][i]);
+    }
+    const double f = *frac;
+    const int s = front_split(f, kb_total);
+    if (s <= 0 || s >= kb_total) return;                  // one side did no work: nothing to compare
+    if (tf < min_ns || tt < min_ns) return;                // too short to time
+    if (llabs(tf - tt) < (max(tf, tt) >> 8)) return;       // balanced to within 0.4 %: keep s (hysteresis against noise)
+    const double a = (double)tf / (double)s, b = (double)tt / (double)(kb_total - s);   // ns per k-block of each side
+    const double target = b / (a + b);                     // a s = b (K - s)
+    const double nf = fmin(fmax((1.0 - gain) * f + gain * target, lo), hi);
+    *frac = nf;
+    *gen += 1;
+}
+
 __global__ void symmetrize_kernel(int32_t* __restrict__ S, int n) {
     // block (bx >= by): read lower tile (bx, by), write it transposed into the upper tile (by, bx)
     __shared__ int32_t tile[32][33];
@@ -1015,7 +1132,7 @@ std::map<SplitKey, std::vector<double>> g_splits;
 static void remember_split(GramPlan& plan) {
     if (plan.d_cum == nullptr || plan.cum_workers <= 0 || !plan.adaptive) return;
     if (plan.own_hi > plan.own_lo && plan.num_peers <= 1) return;   // a band's tile list is not the cohort's
-    std::vector<double> cum((size_t)plan.cum_workers + 1);
+    std::vector<double> cum((size_t)plan.cum_workers + 2);   // the split and the front/tail split point
     if (cudaMemcpy(cum.data(), plan.d_cum, cum.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
         cudaGetLastError();
         return;
@@ -1182,6 +1299,25 @@ static cudaError_t build_tiles(GramPlan& plan, int n, bool exact, int BN, int ro
     return e;
 }
 
+// Whether a launch takes the front/tail schedule, and its split point as a fraction of K: initially T / W, the balance
+// when a k-block costs the same on both sides; the adaptation keeps it within half the distance to either end.
+// Owner-computes bands keep the within-window split.
+struct FrontRange {
+    bool on = false;
+    double init = 0.0, lo = 0.0, hi = 0.0;
+};
+
+static FrontRange front_range(int num_tiles, int workers, bool banded) {
+    FrontRange r;
+    r.on = !banded && front_tail_applies(num_tiles, workers);
+    if (r.on) {
+        r.init = (double)num_tiles / (double)workers;
+        r.lo = 0.5 * r.init;
+        r.hi = r.init + 0.5 * (1.0 - r.init);
+    }
+    return r;
+}
+
 // Resident schedule (accumulators stay in registers for the whole launch) iff the equal split of a window of `kbw`
 // k-blocks, after the same repair the rebalancer applies (a worker stops at the edge of a tile whose accumulator would not
 // fit any more), lets every worker keep its pieces in its accumulator budget.  `cum` receives that initial split
@@ -1254,6 +1390,56 @@ int gram_debug_repair(const int32_t* tiles8, int num_tiles, int workers, int kbw
             if (cnt < max_pieces) {
                 int32_t* o = out + (size_t)cnt * 6;
                 o[0] = w; o[1] = p.tile[i]; o[2] = p.lo[i]; o[3] = p.hi[i]; o[4] = p.col[i]; o[5] = p.cols;
+            }
+    }
+    return cnt;
+}
+
+// Host-only: every piece each worker of a launch replays, in launch order, under the schedule gram_accumulate picks for a
+// whole-cohort context (no band) with the initial split.  frac >= 0 sets the front/tail split point instead of T / W.
+// info: {schedule (0 waves, 1 resident, 2 front/tail), split point s (kb_total unless front/tail)}.
+int gram_debug_schedule(int n, int cta_group, int exact, int workers, int kbw, int kb_total, double frac, int32_t* out,
+                        int max_pieces, int32_t* info) {
+    GramPlan plan;
+    plan.cta_group = cta_group == 1 ? 1 : 2;
+    std::vector<TileDesc> tiles;
+    int num_full = 0;
+    make_tiles(n, plan.cta_group, exact != 0, kUmmaN, 0, n, true, tiles, &num_full);
+    plan.h_tiles.assign(reinterpret_cast<const int32_t*>(tiles.data()), reinterpret_cast<const int32_t*>(tiles.data() + tiles.size()));
+    plan.num_tiles = (int)tiles.size();
+    plan.num_full = num_full;
+    plan.total_weight = tiles.back().wstart + (tiles.back().n_eff >> 4);
+    kbw = std::min(kbw, kb_total);
+    std::vector<double> cum;
+    const FrontRange front = front_range(plan.num_tiles, workers, false);
+    GramArgs a{};
+    a.tiles = tiles.data();
+    a.n = n;
+    a.num_tiles = plan.num_tiles;
+    a.num_full = num_full;
+    a.total_weight = plan.total_weight;
+    a.kb_total = kb_total;
+    a.num_workers = workers;
+    a.col_limit = plan.tiles_col_limit;
+    a.resident = front.on || (plan.num_tiles <= 4 * workers && initial_split(plan, workers, kbw, cum)) ? 1 : 0;
+    a.kb_window = a.resident ? kbw : kb_total;
+    a.cum = cum.data();
+    const double f = frac >= 0.0 ? frac : front.init;
+    if (front.on) {
+        a.front_tiles = plan.num_tiles;
+        a.front_frac = &f;
+    }
+    info[0] = front.on ? 2 : a.resident;
+    info[1] = front.on ? front_split(f, kb_total) : kb_total;
+    int cnt = 0;
+    for (int w = 0; w < workers; ++w) {
+        Sched sc;
+        if (!sc.init(a, w)) return -1 - w;
+        Seg s;
+        for (; sc.next(s); ++cnt)
+            if (cnt < max_pieces) {
+                int32_t* o = out + (size_t)cnt * 6;
+                o[0] = w; o[1] = s.tile; o[2] = s.kb0; o[3] = s.kb1; o[4] = s.first; o[5] = s.flush;
             }
     }
     return cnt;
@@ -1391,6 +1577,7 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
     args.col_limit = plan.tiles_col_limit;
     args.row_limit = row_hi;
     args.red64 = plan.red64 ? 1 : 0;
+    FrontRange front;
     {
         int kbw = plan.kb_window;
         if (kbw <= 0 && panel > 0) kbw = args.kb_per_panel;   // one L2 window per panel
@@ -1400,14 +1587,22 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
             kbw = (int)std::max<long long>(8, std::min<long long>(4096, target / ((long long)n * kKBytes)));
         }
         kbw = std::min(kbw, args.kb_total);
-        // cheap upper bound first (a worker with less than a tile's worth of work can touch few tiles), then the exact test
         std::vector<double> cum0;
-        args.resident = (plan.num_tiles <= 4 * workers && initial_split(plan, workers, kbw, cum0)) ? 1 : 0;
+        front = front_range(plan.num_tiles, workers, banded);
+        if (front.on) {
+            args.resident = 1;
+            cum0.assign((size_t)workers + 1, 0.0);   // the within-window split is not used
+        } else {
+            // cheap upper bound first (a worker with less than a tile's worth of work can touch few tiles), then the exact test
+            args.resident = (plan.num_tiles <= 4 * workers && initial_split(plan, workers, kbw, cum0)) ? 1 : 0;
+        }
+        double frac0 = front.init;
         int dev = 0;
         cudaGetDevice(&dev);
         args.kb_window = args.resident ? kbw : args.kb_total;
-        // the device-side split (speed-weighted by rebalance_kernel from launch to launch) starts from the repaired
-        // equal split; it is only meaningful for one (workers, tile list, window length)
+        // the device-side split (speed-weighted by rebalance_kernel, or the front/tail split point moved by
+        // rebalance_front_kernel, from launch to launch) starts from the repaired equal split / the initial split point;
+        // it is only meaningful for one (workers, tile list, window length)
         if (args.resident && (plan.d_cum == nullptr || plan.cum_workers != workers || plan.cum_tiles != plan.num_tiles ||
                               plan.cum_kbw != kbw || plan.cum_for_n != n || plan.cum_elem != elem_bits)) {
             remember_split(plan);
@@ -1416,18 +1611,24 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
                 auto it = g_splits.find(SplitKey{dev, n, plan.num_tiles, kbw, workers, elem_bits});
                 if (it != g_splits.end()) {
                     std::vector<double> learned = it->second;
-                    const TileDesc* tiles = reinterpret_cast<const TileDesc*>(plan.h_tiles.data());
-                    std::vector<long long> need((size_t)workers + 1);
-                    if (repair_split(tiles, plan.num_tiles, workers, (long long)plan.total_weight * kbw, kbw, plan.tiles_col_limit,
-                                     learned.data(), need.data()))
-                        cum0 = learned;
+                    if (front.on) {
+                        const double f = learned.size() > (size_t)workers + 1 ? learned[(size_t)workers + 1] : -1.0;
+                        if (f >= front.lo && f <= front.hi) frac0 = f;
+                    } else {
+                        const TileDesc* tiles = reinterpret_cast<const TileDesc*>(plan.h_tiles.data());
+                        std::vector<long long> need((size_t)workers + 1);
+                        learned.resize((size_t)workers + 1);
+                        if (repair_split(tiles, plan.num_tiles, workers, (long long)plan.total_weight * kbw, kbw,
+                                         plan.tiles_col_limit, learned.data(), need.data()))
+                            cum0 = learned;
+                    }
                 }
             }
             if (plan.d_cum) cudaFree(plan.d_cum);
             plan.d_cum = nullptr;
             cudaError_t e = cudaMalloc(&plan.d_cum, (size_t)(workers + 2) * sizeof(double) + sizeof(int));
             if (e != cudaSuccess) return e;
-            cum0.push_back(0.0);                                   // [workers + 1]: unused
+            cum0.push_back(frac0);                                 // [workers + 1]: the front/tail split point (fraction of K)
             cum0.push_back(0.0);                                   // [workers + 2]: the update counter (int)
             e = cudaMemcpyAsync(plan.d_cum, cum0.data(), (size_t)(workers + 2) * sizeof(double) + sizeof(int),
                                 cudaMemcpyHostToDevice, stream);   // pageable source: staged before the call returns
@@ -1444,9 +1645,14 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
     const int nwin = (args.kb_total + args.kb_window - 1) / args.kb_window;
     const long long uw = (long long)args.total_weight * args.kb_window;
     args.active_workers = (int)std::min<long long>(workers, uw);
+    if (front.on) {   // only the front workers take part in the window pacing
+        args.front_tiles = plan.num_tiles;
+        args.front_frac = plan.d_cum + workers + 1;
+        args.active_workers = plan.num_tiles;
+    }
     args.sync_lead = (args.resident && nwin <= GramPlan::kMaxWindows) ? plan.sync_lead : 0;
     args.win_done = plan.d_win_done;
-    const bool adapt = plan.adaptive && args.resident && workers <= 1024 && args.active_workers == workers;
+    const bool adapt = plan.adaptive && args.resident && workers <= 1024 && (front.on || args.active_workers == workers);
     args.prof = (plan.profile || adapt) ? plan.d_prof : nullptr;
     args.cum = plan.d_cum;
     if (args.sync_lead > 0) {
@@ -1463,7 +1669,12 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
         le = kind == 0 ? launch<1, 0>(tmap, args, grid, stream)
                        : (kind == 1 ? launch<1, 1>(tmap, args, grid, stream) : launch<1, 2>(tmap, args, grid, stream));
     if (le != cudaSuccess) return le;
-    if (adapt) {
+    if (adapt && front.on) {
+        rebalance_front_kernel<<<1, (workers + 31) / 32 * 32, 0, stream>>>(
+            plan.d_prof, plan.d_cum + workers + 1, plan.num_tiles, workers, cgp, args.kb_total, plan.gain, front.lo, front.hi,
+            300000, reinterpret_cast<int*>(plan.d_cum + workers + 2));
+        le = cudaGetLastError();
+    } else if (adapt) {
         // shares move towards the measured speeds, at most 35 % above the mean; a split under which some worker's
         // accumulators would not fit its budget is rejected by the kernel itself
         rebalance_kernel<<<1, 1024, 0, stream>>>(plan.d_prof, plan.d_cum, workers, cgp, plan.gain, 1.35, 300000,
@@ -1487,7 +1698,7 @@ cudaError_t gram_preload_kernels(cudaStream_t stream) {
 #define VPCA_LOAD(k) if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k)
     VPCA_LOAD((gram_kernel<1, 0>)); VPCA_LOAD((gram_kernel<1, 1>)); VPCA_LOAD((gram_kernel<1, 2>));
     VPCA_LOAD((gram_kernel<2, 0>)); VPCA_LOAD((gram_kernel<2, 1>)); VPCA_LOAD((gram_kernel<2, 2>));
-    VPCA_LOAD(rebalance_kernel); VPCA_LOAD(symmetrize_kernel); VPCA_LOAD(add_i32_kernel); VPCA_LOAD(add_i32_peers_kernel);
+    VPCA_LOAD(rebalance_kernel); VPCA_LOAD(rebalance_front_kernel); VPCA_LOAD(symmetrize_kernel); VPCA_LOAD(add_i32_kernel); VPCA_LOAD(add_i32_peers_kernel);
     VPCA_LOAD(add_i32_owner_kernel); VPCA_LOAD(gather_rows_kernel); VPCA_LOAD(push_rows_kernel); VPCA_LOAD(peer_barrier_kernel);
 #undef VPCA_LOAD
     if (e != cudaSuccess) return e;

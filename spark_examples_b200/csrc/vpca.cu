@@ -2729,6 +2729,16 @@ int vpca_debug_plan(const int32_t* tiles, int32_t num_tiles, int32_t workers, in
     return rc;
 }
 
+int vpca_debug_schedule(int32_t n_samples, int32_t cta_group, int32_t exact, int32_t workers, int32_t kb_window,
+                        int32_t kb_total, double front_frac, int32_t* out, int32_t max_pieces, int32_t* info) {
+    if (n_samples < 2 || workers < 1 || workers > 1024 || kb_window < 1 || kb_total < 1 || !(front_frac <= 1.0) ||
+        info == nullptr || max_pieces < 0 || (out == nullptr && max_pieces > 0))
+        return fail(nullptr, VPCA_ERR_BAD_ARG, "vpca_debug_schedule: bad argument");
+    const int rc = gram_debug_schedule(n_samples, cta_group, exact, workers, kb_window, kb_total, front_frac, out, max_pieces, info);
+    if (rc < 0) return fail(nullptr, VPCA_ERR_STATE, "vpca_debug_schedule: the accumulators of a worker do not fit its budget");
+    return rc;
+}
+
 int vpca_debug_rebalance(const int32_t* tiles, int32_t num_tiles, int32_t workers, int32_t kb_window, int32_t col_limit,
                          double* cum, int32_t* out, int32_t max_pieces) {
     if (tiles == nullptr || num_tiles < 1 || workers < 1 || kb_window < 1 || cum == nullptr || col_limit < 32 ||

@@ -84,6 +84,8 @@ int gram_debug_max_clusters(int cluster_size);
 int gram_debug_band_tiles(int n, int cta_group, int row_lo, int row_hi, int32_t* out, int max_tiles);
 int gram_debug_tiles(int n, int cta_group, int exact, int32_t* out, int max_tiles);
 int gram_debug_plan(const int32_t* tiles8, int num_tiles, int workers, int kbw, int32_t* out, int max_pieces);
+int gram_debug_schedule(int n, int cta_group, int exact, int workers, int kbw, int kb_total, double frac, int32_t* out,
+                        int max_pieces, int32_t* info);
 int gram_debug_repair(const int32_t* tiles8, int num_tiles, int workers, int kbw, int col_limit, double* cum, int32_t* out,
                       int max_pieces);
 

@@ -49,7 +49,7 @@ EXPORTED_SYMBOLS = (
     "vpca_pool_create", "vpca_pool_destroy", "vpca_pool_size", "vpca_pool_ctx", "vpca_pool_last_error", "vpca_pool_reset",
     "vpca_pool_accumulate_calls", "vpca_pool_accumulate_calls_u16", "vpca_pool_accumulate_bits", "vpca_pool_accumulate_bed",
     "vpca_pool_commit", "vpca_pool_abort", "vpca_pool_reduce_and_finalize", "vpca_pool_get_gram", "vpca_pool_compute_pca",
-    "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan",
+    "vpca_pool_get_stats", "vpca_debug_tiles", "vpca_debug_plan", "vpca_debug_schedule",
     "vpca_loadings_calls", "vpca_loadings_bed", "vpca_loadings_panels", "vpca_project_begin", "vpca_project_calls",
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
     "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
@@ -224,6 +224,8 @@ def load_library() -> ctypes.CDLL:
     L.vpca_debug_tiles.argtypes = [i32, i32, i32, vp, i32]
     L.vpca_debug_plan.restype = ctypes.c_int
     L.vpca_debug_plan.argtypes = [vp, i32, i32, i32, vp, i32]
+    L.vpca_debug_schedule.restype = ctypes.c_int
+    L.vpca_debug_schedule.argtypes = [i32, i32, i32, i32, i32, i32, ctypes.c_double, vp, i32, vp]
     L.vpca_debug_lanczos_profile.restype = ctypes.c_int
     L.vpca_debug_lanczos_profile.argtypes = [vp, vp, i32]
     L.vpca_debug_rebalance.restype = ctypes.c_int
@@ -849,6 +851,22 @@ def debugPlan(tiles: np.ndarray, workers: int, kb_window: int) -> np.ndarray:
     if cnt < 0:
         raise VpcaError(VPCA_ERR_STATE, L.vpca_last_error(None).decode("utf-8", "replace"))
     return out[:cnt]
+
+
+def debugSchedule(n_samples: int, cta_group: int, exact: bool, workers: int, kb_window: int, kb_total: int,
+                  front_frac: float = -1.0):
+    """Every piece each worker replays in one launch (vpca_debug_schedule): returns ((pieces, 6) int32 {worker, tile,
+    kb_lo, kb_hi, first, flush} in launch order, schedule (0 waves, 1 resident, 2 front/tail), split point s)."""
+    L = load_library()
+    info = np.zeros(2, dtype=np.int32)
+    args = (int(n_samples), int(cta_group), 1 if exact else 0, int(workers), int(kb_window), int(kb_total),
+            float(front_frac))
+    cnt = L.vpca_debug_schedule(*args, None, 0, _host_ptr(info))
+    if cnt < 0:
+        raise VpcaError(cnt, L.vpca_last_error(None).decode("utf-8", "replace"))
+    out = np.zeros((cnt, 6), dtype=np.int32)
+    L.vpca_debug_schedule(*args, _host_ptr(out), cnt, _host_ptr(info))
+    return out, int(info[0]), int(info[1])
 
 
 def debugBandTiles(n_samples: int, cta_group: int, row0: int, rows: int) -> np.ndarray:

@@ -9,7 +9,7 @@
 //   N >= 512 (default): Lanczos with full reorthogonalisation for the top k pairs only -- as ONE persistent cooperative
 //               kernel per 16-step chunk that reads the int32 Gram S itself and applies the centring to the vector
 //               (lz_persist_kernel below) while its shared-memory working set fits one block (N <= 10 752 on 132 SMs);
-//               past that the five-kernel CUDA-graph form on the FP64 matrix C;
+//               past that the band solver's Lanczos (band_eig_topk) with the whole Gram as its one band;
 //   small N, VPCA_EIG=direct, and the fallback of the Krylov solver:
 //               1. Householder tridiagonalisation  C = Q T Q^T           (N steps, 1-2 kernels per step, not blocked)
 //               2. k largest eigenvalues of T by Sturm-count multisection (parallel over shifts)
@@ -667,10 +667,10 @@ __global__ void __launch_bounds__(512) backtransform_kernel(const double* __rest
 // above, on m instead of N) give Ritz values theta and vectors z = V y whose residual is |beta_m y_m|.  One step
 // costs one pass over C (50 MB from L2 at N = 2504) instead of the N steps the reduction needs, and population
 // structure separates the top of the spectrum, so a few dozen steps reach |beta_m y_m| <= 1e-12 ||T||.
-// Graph form (past N = 10 752 on 132 SMs, where the persistent kernel's shared memory no longer fits a block, and
-// VPCA_LZ_PERSIST=0): five launches per step (matvec | V^T w | w -= V h | V^T w | w -= V h), step index and stop flag in
-// device memory so that kLzChunk steps replay from one CUDA graph; the host looks at the residual after a replay.
-// Persistent form (default): see lz_persist_kernel further down.
+// Persistent form (default): see lz_persist_kernel further down.  Past N = 10 752 on 132 SMs, where its shared memory no
+// longer fits a block, and with VPCA_LZ_PERSIST=0, the whole Gram is solved by the band solver (band_eig_topk) on one
+// band: nine launches per step, step index and stop flag in device memory; the host looks at the residual after a chunk.
+// Both forms follow the same convergence policy (LzPolicy).
 // Anything unusual -- breakdown, slow convergence, a larger eigenvalue found by the deflated re-run that guards
 // against a missed copy of a multiple eigenvalue -- falls back to the direct reduction, which remains the
 // reference-grade path.  Every reduction has a fixed order: the result is run-to-run deterministic.
@@ -681,7 +681,41 @@ constexpr int kLzVerify = 8;      // steps of the deflated re-run (persistent fo
                                   // theta_k when a copy of a larger eigenvalue was missed, not to converge
 constexpr int kLzMaxIter = 320;   // give up (-> direct solver) beyond this
 constexpr int kLzCap = kLzMaxIter + 64;   // columns of V: main run, or k locked vectors + one verification chunk
+constexpr double kLzTol = 1e-12;   // converged: max_c |beta_m y_m,c| <= kLzTol ||T||
 // st[0] = step j, st[1] = flag (0 run, 1 converged, 2 breakdown, 3 missed eigenvalue), st[2] = ticket, st[3] = step cap
+
+// The convergence policy of both host-driven Lanczos loops (the persistent form of lanczos_topk and band_eig_topk): the
+// step budget, the chunks after which the residual is tested, and when a residual still above kLzTol is given up on.
+struct LzPolicy {
+    int max_iter = kLzMaxIter;   // st[3] of the main run
+    int max_chunks = 0;
+    int m_prev = 0;
+    double rho_prev = 0.0;
+
+    explicit LzPolicy(int n) {
+        if (const char* mi = getenv("VPCA_EIG_MAXIT")) max_iter = std::max(kLzChunk, std::min(kLzMaxIter, atoi(mi)));
+        max_chunks = std::min(max_iter, n - 1) / kLzChunk;
+    }
+    // Whether the residual is tested after `chunk` chunks: after every chunk up to 64 steps, then after every other one.
+    // Fewer steps than wanted pairs (k > 16): T has no k Ritz pairs, and the residual of the missing ones is noise that
+    // would only feed the convergence-rate forecast below.
+    bool test_after(int chunk, int k) const {
+        if (chunk * kLzChunk < k) return false;
+        return chunk <= 4 || (chunk & 1) == 0 || chunk == max_chunks;
+    }
+    // After a test at m steps that neither converged nor broke down: false when residual rho will not reach kLzTol
+    // within the step budget.
+    bool keep_going(int m, double rho) {
+        if (m >= 96 && rho > 1e-3) return false;   // no separated top of the spectrum: hopeless within kLzMaxIter
+        if (m_prev >= 32 && rho < rho_prev) {
+            const double rate = std::log(rho_prev / rho) / (m - m_prev);
+            if (m + 1.5 * std::log(rho / kLzTol) / rate > max_iter + 2 * kLzChunk) return false;
+        }
+        rho_prev = rho;
+        m_prev = m;
+        return true;
+    }
+};
 
 __device__ __forceinline__ double lz_uniform(unsigned long long i, unsigned long long salt) {
     unsigned long long z = (i + 1) * 0x9E3779B97F4A7C15ull + salt;   // splitmix64
@@ -705,51 +739,8 @@ __global__ void lz_init_kernel(double* __restrict__ w, int n, unsigned long long
     if (threadIdx.x == 0) part[blockIdx.x] = s;
 }
 
-// Step j, phase 1: beta_j = ||w_in|| (from the partial sums), v_j = w_in / beta_j -> V[:, j], w_out = C v_j.
-// 4 rows per 256-thread block, two warps per row, 8 independent loads in flight per lane.
-__global__ void __launch_bounds__(256) lz_matvec_kernel(const double* __restrict__ C, int n, double* __restrict__ V,
-                                                        double* __restrict__ wbuf, const double* __restrict__ part,
-                                                        int npart, double* __restrict__ beta, int* __restrict__ st) {
-    __shared__ double half[8];
-    const int j = st[0];
-    if (st[1] != 0 || j >= st[3]) return;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    double s = 0.0;
-    for (int p = lane; p < npart; p += 32) s += part[p];
-    s = warp_sum(s);
-    const double nrm = sqrt(s);
-    if (!(nrm > 0.0) || !(nrm <= DBL_MAX)) {   // exact breakdown or non-finite: every block sees the same value
-        if (blockIdx.x == 0 && threadIdx.x == 0) st[1] = 2;
-        return;
-    }
-    const double inv = 1.0 / nrm;
-    const double* __restrict__ win = wbuf + (size_t)(j & 1) * n;
-    double* __restrict__ wout = wbuf + (size_t)((j + 1) & 1) * n;
-    const int row = blockIdx.x * 4 + (wid >> 1);
-    double acc = 0.0;
-    if (row < n) {
-        const double* __restrict__ c = C + (size_t)row * n;
-        double a[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-        for (int t0 = (wid & 1) * 32 + lane; t0 < n; t0 += 8 * 64) {
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {   // predicated, so the 8 loads of the ragged last round still issue together
-                const int t = t0 + u * 64;
-                if (t < n) a[u] += c[t] * win[t];
-            }
-        }
-        acc = ((a[0] + a[1]) + (a[2] + a[3])) + ((a[4] + a[5]) + (a[6] + a[7]));
-    }
-    acc = warp_sum(acc);
-    if (lane == 0) half[wid] = acc;
-    __syncthreads();
-    if (row < n && (wid & 1) == 0 && lane == 0) {
-        wout[row] = (half[wid] + half[wid + 1]) * inv;
-        V[(size_t)j * n + row] = win[row] * inv;
-        if (row == 0) beta[j] = nrm;
-    }
-}
-
-// Phases 2 and 4: h[q] = V[:, q] . w for q <= j.  One block per column (blocks beyond j return).
+// Each of a band-solver step's two Gram-Schmidt passes, part 1: h[q] = V[:, q] . w for q <= j.  One block per column
+// (blocks beyond j return).
 __global__ void __launch_bounds__(128) lz_dots_kernel(const double* __restrict__ V, int n,
                                                       const double* __restrict__ wbuf, double* __restrict__ h,
                                                       const int* __restrict__ st) {
@@ -772,7 +763,7 @@ __global__ void __launch_bounds__(128) lz_dots_kernel(const double* __restrict__
     if (threadIdx.x == 0) h[q] = sum;
 }
 
-// Phases 3 and 5: w -= V[:, 0..j] h.  32 rows per block, the columns split over the 8 warps.  The second pass also
+// Part 2 of each pass: w -= V[:, 0..j] h.  32 rows per block, the columns split over the 8 warps.  The second pass also
 // leaves the partial sums of ||w||^2 for the next step and, through a ticket, advances the step counter once every
 // block has read it.  alpha_j = h_j (first pass) + its correction (second pass).
 __global__ void __launch_bounds__(256) lz_update_kernel(const double* __restrict__ V, int n, double* __restrict__ wbuf,
@@ -870,7 +861,7 @@ __global__ void lz_verify_kernel(const double* __restrict__ theta, int k, const 
 
 
 // ------------------------------------------------- Lanczos, persistent form (while its shared memory fits one block)
-// The five launches of a step (and the 80 of a 16-step chunk) become ONE cooperative launch per chunk: 1024 threads on
+// A step's mat-vec and two Gram-Schmidt passes, for all 16 steps of a chunk, are ONE cooperative launch: 1024 threads on
 // every SM, block b owns the rows [b R, (b + 1) R) of everything (R = ceil(n / blocks)), and a step is three phases
 // separated by grid-wide barriers (an atomic counter in L2, ~1-2 us each instead of a kernel boundary):
 //   A  every block stages the whole w_in in shared memory (computing ||w_in||, sum(w_in) and rowmean . w_in on the way,
@@ -1383,10 +1374,11 @@ __global__ void lz_lock_kernel(double* __restrict__ VT, int n, int cap, const do
     for (int c = 0; c < k; ++c) VT[(size_t)i * cap + c] = Z[(size_t)c * n + i];
 }
 
-// ------------------------------------------------- Lanczos on a Gram held as row bands (vpca_compute_pca_bands)
-// The five-kernel Lanczos above with its mat-vec sharded over the contexts that hold the bands.  Rank q stores rows
-// [row0, row0 + rows) of S, of which only the cells j <= i are meaningful (the upper part of a band-only allocation is not
-// the transpose and is never read).  Its partial product covers what those cells give:
+// ------------------------------------------------- Lanczos on a Gram held as row bands (vpca_compute_pca_bands, and
+// vpca_compute_pca past the persistent form's fit, on one band)
+// Lanczos with lz_dots / lz_update for the Gram-Schmidt and the mat-vec sharded over the contexts that hold the bands.
+// Rank q stores rows [row0, row0 + rows) of S, of which only the cells j <= i are meaningful (the upper part of a
+// band-only allocation is not the transpose and is never read).  Its partial product covers what those cells give:
 //   y_i += sum_{j <= i} S_ij v_j  (its rows)        y_j += S_ij v_i  for j < i  (the transpose, columns [0, row0 + rows))
 // Every stored cell is read once per step and feeds both FMAs.  The band's lower part is cut into kBandTR x kBandTC tiles;
 // a tile writes one row partial per row and one column partial per column into scratch, and band_reduce_kernel adds them
@@ -1632,7 +1624,8 @@ void eig_free(EigWork& w) {
     cudaFree(w.d_evecs); cudaFree(w.d_lu); cudaFree(w.d_nz); cudaFree(w.d_step);
     cudaFree(w.d_V); cudaFree(w.d_lzw); cudaFree(w.d_lzs); cudaFree(w.d_lzst); cudaFree(w.d_lzbar); cudaFree(w.d_lzprof); cudaFree(w.d_lzG);
     if (w.graph_exec != nullptr) cudaGraphExecDestroy(w.graph_exec);
-    if (w.lz_graph != nullptr) cudaGraphExecDestroy(w.lz_graph);
+    band_eig_free(w.band_eig);
+    band_part_free(w.band_part);
     w = EigWork{};
 }
 
@@ -1647,7 +1640,7 @@ cudaError_t center_gram(EigWork& w, const int32_t* d_S, cudaStream_t stream, boo
 }
 
 // C = S - rowMean - colMean + matrixMean as an FP64 matrix (VariantsPca.scala:216-221): what vpca_get_centered returns and
-// what the direct reduction and the five-kernel Lanczos read.  The persistent Lanczos never needs it (50 MB at N = 2504).
+// what the direct reduction reads.  Neither Lanczos form needs it (50 MB at N = 2504).
 cudaError_t center_matrix(EigWork& w, cudaStream_t stream) {
     if (w.c_valid) return cudaSuccess;
     const int n = w.n;
@@ -1666,7 +1659,7 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     const int kmax = w.kmax;
     cudaError_t e;
 #define VPCA_TRY(x) if ((e = (x)) != cudaSuccess) return e
-    if (w.d_V == nullptr) {
+    if (w.lz_blocks < 0) {
         // persistent form: one 1024-thread block per SM, launched cooperatively (all blocks co-resident), with as much
         // dynamic shared memory as the device grants one block beside the kernel's static arrays
         int dev = 0, sms = 0, coop = 0, optin = 0;
@@ -1680,7 +1673,36 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
         const char* lp = getenv("VPCA_LZ_PERSIST");
         w.lz_blocks = (coop != 0 && sms > 0 && !(lp != nullptr && atoi(lp) == 0)) ? sms : 0;
     }
-    const size_t small_doubles = 5 * (size_t)kLzCap + (size_t)kLzCap * kmax + 16 + 4 + 16 + (size_t)npart +
+    // the persistent kernel's shared-memory layout (lz_persist_kernel): two length-n vectors plus per-block buffers that
+    // grow with rows_per = n / SMs -- 222 448 bytes at N = 10 752 on 132 SMs, past the 227 KB a block may use soon after
+    const int rows_per = w.lz_blocks > 0 ? (n + w.lz_blocks - 1) / w.lz_blocks : 0;
+    const size_t base_smem =
+        ((((size_t)n + 1) & ~(size_t)1) + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1) +
+         ((((size_t)rows_per * ((n + kLzSeg - 1) / kLzSeg)) + 1) & ~(size_t)1) + (size_t)rows_per * kLzVtCols + (((size_t)n + 1) & ~(size_t)1) +
+         (size_t)kLzVtCols * kLzVtCols + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1)) * sizeof(double);
+    // persistent form (one cooperative launch per chunk) whenever that layout fits; otherwise, and with VPCA_LZ_PERSIST=0,
+    // the band solver with the whole Gram as its one band (reads S, no FP64 matrix)
+    if (w.lz_blocks == 0 || base_smem > w.lz_smem_max) {
+        BandPart& p = w.band_part;
+        VPCA_TRY(cudaGetDevice(&p.device));
+        p.stream = stream;
+        p.d_S = w.d_S;
+        p.n = n;
+        p.row0 = 0;
+        p.rows = n;
+        BandPart* parts[1] = {&p};
+        int outcome = 0;
+        VPCA_TRY(band_eig_topk(w.band_eig, parts, 1, kmax, k, launches, &outcome));
+        w.last_iters = w.band_eig.last_iters;
+        if (outcome != 0) return cudaSuccess;
+        VPCA_TRY(cudaMemcpyAsync(w.d_evals, w.band_eig.d_evals, k * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+        VPCA_TRY(cudaMemcpyAsync(w.d_evecs, w.band_eig.d_evecs, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice,
+                                 stream));
+        *used = true;
+        return cudaSuccess;
+    }
+
+    const size_t small_doubles = 3 * (size_t)kLzCap + (size_t)kLzCap * kmax + 16 + 4 + 16 + (size_t)npart +
                                  2 * (size_t)w.lz_blocks * kLzCap;
     if (w.d_V == nullptr) {
         VPCA_TRY(cudaMalloc(&w.d_V, (size_t)n * kLzCap * sizeof(double)));
@@ -1698,41 +1720,21 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     }
     double* alpha = w.d_lzs;
     double* beta = alpha + kLzCap;
-    double* h1 = beta + kLzCap;
-    double* h2 = h1 + kLzCap;
-    double* e2 = h2 + kLzCap;
+    double* e2 = beta + kLzCap;
     double* Y = e2 + kLzCap;
     double* theta2 = Y + (size_t)kLzCap * kmax;
     double* res = theta2 + 16;
     double* scal2 = res + 4;
     double* part = scal2 + 16;
-    int64_t nl = 0;
-    const int upd_blocks = npart, mv_blocks = (n + 3) / 4;
     double* hpart = part + npart;
-    // the persistent kernel's shared-memory layout (lz_persist_kernel): two length-n vectors plus per-block buffers that
-    // grow with rows_per = n / SMs -- 222 448 bytes at N = 10 752 on 132 SMs, past the 227 KB a block may use soon after
-    const int rows_per = w.lz_blocks > 0 ? (n + w.lz_blocks - 1) / w.lz_blocks : 0;
-    const size_t base_smem =
-        ((((size_t)n + 1) & ~(size_t)1) + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1) +
-         ((((size_t)rows_per * ((n + kLzSeg - 1) / kLzSeg)) + 1) & ~(size_t)1) + (size_t)rows_per * kLzVtCols + (((size_t)n + 1) & ~(size_t)1) +
-         (size_t)kLzVtCols * kLzVtCols + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1)) * sizeof(double);
-    // persistent form (one cooperative launch per chunk) whenever that layout fits; otherwise, and with VPCA_LZ_PERSIST=0,
-    // the five-kernel graph form, which needs only the FP64 matrix C
-    const bool persist = w.lz_blocks > 0 && base_smem <= w.lz_smem_max;
+    int64_t nl = 0;
     // what is left of the block's shared memory holds rows of S
-    int rows_smem = 0;
-    if (persist) {
-        const size_t row_bytes = (size_t)((n + 3) & ~3) * sizeof(int32_t);
-        rows_smem = (int)std::min<size_t>((size_t)rows_per, (w.lz_smem_max - base_smem) / row_bytes);
-        if (const char* sr = getenv("VPCA_LZ_SROWS"); sr != nullptr) rows_smem = std::min(rows_smem, std::max(0, atoi(sr)));
-    }
-    const size_t persist_smem = base_smem + (size_t)rows_smem * ((n + 3) & ~3) * sizeof(int32_t);
-    if (persist) VPCA_TRY(cudaFuncSetAttribute(lz_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)persist_smem));
+    const size_t row_bytes = (size_t)((n + 3) & ~3) * sizeof(int32_t);
+    int rows_smem = (int)std::min<size_t>((size_t)rows_per, (w.lz_smem_max - base_smem) / row_bytes);
+    if (const char* sr = getenv("VPCA_LZ_SROWS"); sr != nullptr) rows_smem = std::min(rows_smem, std::max(0, atoi(sr)));
+    const size_t persist_smem = base_smem + (size_t)rows_smem * row_bytes;
+    VPCA_TRY(cudaFuncSetAttribute(lz_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)persist_smem));
     auto run_chunk = [&](int pre, const int* gate = nullptr) -> cudaError_t {
-        if (!persist) {
-            nl += 5 * kLzChunk;
-            return cudaGraphLaunch(w.lz_graph, stream);
-        }
         cudaError_t ce = cudaMemsetAsync(w.d_lzbar, 0, sizeof(unsigned), stream);
         if (ce != cudaSuccess) return ce;
         LzArgs a{};
@@ -1760,53 +1762,27 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
         return cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(lz_persist_kernel), dim3((unsigned)w.lz_blocks),
                                            dim3(kLzThreads), params, persist_smem, stream);
     };
-
-    if (!persist) VPCA_TRY(center_matrix(w, stream));   // the five-kernel form reads the FP64 matrix
-    if (!persist && w.lz_graph == nullptr) {
-        cudaGraph_t graph = nullptr;
-        VPCA_TRY(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-        for (int g = 0; g < kLzChunk; ++g) {
-            lz_matvec_kernel<<<mv_blocks, 256, 0, stream>>>(w.d_C, n, w.d_V, w.d_lzw, part, npart, beta, w.d_lzst);
-            lz_dots_kernel<<<kLzCap, 128, 0, stream>>>(w.d_V, n, w.d_lzw, h1, w.d_lzst);
-            lz_update_kernel<<<upd_blocks, 256, 0, stream>>>(w.d_V, n, w.d_lzw, h1, alpha, part, w.d_lzst, 1);
-            lz_dots_kernel<<<kLzCap, 128, 0, stream>>>(w.d_V, n, w.d_lzw, h2, w.d_lzst);
-            lz_update_kernel<<<upd_blocks, 256, 0, stream>>>(w.d_V, n, w.d_lzw, h2, alpha, part, w.d_lzst, 2);
-        }
-        VPCA_TRY(cudaStreamEndCapture(stream, &graph));
-        e = cudaGraphInstantiate(&w.lz_graph, graph, 0);
-        cudaGraphDestroy(graph);
-        if (e != cudaSuccess) return e;
-    }
     VPCA_TRY(cudaFuncSetAttribute(invit_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
 
-    const double tol = 1e-12;
-    int max_iter = kLzMaxIter;
-    if (const char* mi = getenv("VPCA_EIG_MAXIT")) max_iter = std::max(kLzChunk, std::min(kLzMaxIter, atoi(mi)));
-    int hst[8] = {0, 0, 0, max_iter, 0, 0, 0, 0};
+    LzPolicy policy(n);
+    int hst[8] = {0, 0, 0, policy.max_iter, 0, 0, 0, 0};
     double hres[2] = {0.0, 0.0};
-    const int vsteps = persist ? kLzVerify : kLzChunk;
     const char* spe = getenv("VPCA_LZ_SPECULATE");
-    const bool speculate = persist && k + kLzChunk < n && !(spe != nullptr && atoi(spe) == 0);
+    const bool speculate = k + kLzChunk < n && !(spe != nullptr && atoi(spe) == 0);
     VPCA_TRY(cudaMemcpyAsync(w.d_lzst, hst, sizeof(hst), cudaMemcpyHostToDevice, stream));
     lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw, n, 0x5eedULL, part);
     nl += 1;
-    int m = 0, m_prev = 0;
+    int m = 0;
     bool converged = false;
-    double rho_prev = 0.0;
-    const int max_chunks = std::min(max_iter, n - 1) / kLzChunk;
-    for (int chunk = 1; chunk <= max_chunks; ++chunk) {
+    for (int chunk = 1; chunk <= policy.max_chunks; ++chunk) {
         VPCA_TRY(run_chunk(0));
         m = chunk * kLzChunk;
-        // fewer steps than wanted pairs (k > 16): T has no k Ritz pairs, and the residual of the missing ones is noise
-        // that would only feed the convergence-rate forecast below
-        if (m < k) continue;
-        // look at the residual after every replay up to 64 steps, then after every other one
-        if (chunk > 4 && (chunk & 1) && chunk != max_chunks) continue;
+        if (!policy.test_after(chunk, k)) continue;
         bisect_kernel<<<k, 256, 0, stream>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
         // a tridiagonal matrix of a few dozen rows: one warp (its block-wide reductions then cost no barrier latency)
         invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), stream>>>(alpha, beta + 1, m, k, w.d_evals, w.d_scal,
                                                                                 w.d_lu, Y);
-        lz_check_kernel<<<1, 32, 0, stream>>>(part, persist ? 1 : npart, Y, m, k, w.d_scal, w.d_lzst, res, tol);
+        lz_check_kernel<<<1, 32, 0, stream>>>(part, 1, Y, m, k, w.d_scal, w.d_lzst, res, kLzTol);
         nl += 3;
         const bool spec = speculate && chunk == 1;
         if (spec) {
@@ -1815,13 +1791,13 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
             // synchronises once per solve; had the test failed, every gated kernel returns at once and the main run
             // goes on below with its state untouched.
             const int* gate = w.d_lzst + 4;
-            lz_gate_kernel<<<1, 1, 0, stream>>>(w.d_lzst, k, vsteps);
+            lz_gate_kernel<<<1, 1, 0, stream>>>(w.d_lzst, k, kLzVerify);
             lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V, n, kLzCap, Y, m, k, w.d_evecs, gate);
             lz_finish_kernel<<<k, 512, 0, stream>>>(w.d_evecs, n, gate);
             lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V, n, kLzCap, w.d_evecs, k, gate);
             lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw + (size_t)(k & 1) * n, n, 0xfaceULL, part, gate);
             VPCA_TRY(run_chunk(1, gate));
-            bisect_kernel<<<1, 256, 0, stream>>>(alpha + k, beta + k + 1, vsteps, e2, theta2, scal2, gate);
+            bisect_kernel<<<1, 256, 0, stream>>>(alpha + k, beta + k + 1, kLzVerify, e2, theta2, scal2, gate);
             lz_verify_kernel<<<1, 1, 0, stream>>>(w.d_evals, k, theta2, w.d_scal, w.d_lzst, gate);
             nl += 7;
         }
@@ -1840,14 +1816,7 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
             break;
         }
         if (hst[1] != 0) break;   // breakdown
-        const double rho = hres[0];
-        if (m >= 96 && rho > 1e-3) break;   // no separated top of the spectrum: hopeless within kLzMaxIter
-        if (m_prev >= 32 && rho < rho_prev) {
-            const double rate = std::log(rho_prev / rho) / (m - m_prev);
-            if (m + 1.5 * std::log(rho / tol) / rate > max_iter + 2 * kLzChunk) break;
-        }
-        rho_prev = rho;
-        m_prev = m;
+        if (!policy.keep_going(m, hres[0])) break;
     }
     w.last_iters = m;
     if (launches) *launches += nl;
@@ -1855,8 +1824,7 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     nl = 0;
 
     // Ritz vectors, unit norm, sign rule
-    if (persist) lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V, n, kLzCap, Y, m, k, w.d_evecs);
-    else lz_ritz_kernel<<<dim3(npart, k), 256, 0, stream>>>(w.d_V, n, Y, m, w.d_evecs);
+    lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V, n, kLzCap, Y, m, k, w.d_evecs);
     lz_finish_kernel<<<k, 512, 0, stream>>>(w.d_evecs, n);
     nl += 2;
 
@@ -1864,26 +1832,13 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     // lock the k Ritz vectors as the first k basis columns and run one more chunk from a fresh start vector that is
     // orthogonal to them.  Its top Ritz value is a lower bound of the largest eigenvalue of the deflated operator.
     if (k + kLzChunk < n) {
-        if (persist) {
-            lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V, n, kLzCap, w.d_evecs, k);
-            int vst[4] = {k, 0, 0, k + vsteps};
-            VPCA_TRY(cudaMemcpyAsync(w.d_lzst, vst, sizeof(vst), cudaMemcpyHostToDevice, stream));
-            lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw + (size_t)(k & 1) * n, n, 0xfaceULL, part);
-            nl += 2;
-            VPCA_TRY(run_chunk(1));   // orthogonalises the start vector against the locked columns, then kLzChunk steps
-        } else {
-            VPCA_TRY(cudaMemcpyAsync(w.d_V, w.d_evecs, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice, stream));
-            int vst[4] = {k - 1, 0, 0, k + kLzChunk};
-            VPCA_TRY(cudaMemcpyAsync(w.d_lzst, vst, sizeof(vst), cudaMemcpyHostToDevice, stream));
-            lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw + (size_t)(k & 1) * n, n, 0xfaceULL, part);
-            lz_dots_kernel<<<kLzCap, 128, 0, stream>>>(w.d_V, n, w.d_lzw, h1, w.d_lzst);
-            lz_update_kernel<<<upd_blocks, 256, 0, stream>>>(w.d_V, n, w.d_lzw, h1, alpha, part, w.d_lzst, 1);
-            lz_dots_kernel<<<kLzCap, 128, 0, stream>>>(w.d_V, n, w.d_lzw, h2, w.d_lzst);
-            lz_update_kernel<<<upd_blocks, 256, 0, stream>>>(w.d_V, n, w.d_lzw, h2, alpha, part, w.d_lzst, 2);
-            nl += 5;
-            VPCA_TRY(run_chunk(0));
-        }
-        bisect_kernel<<<1, 256, 0, stream>>>(alpha + k, beta + k + 1, vsteps, e2, theta2, scal2);
+        lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V, n, kLzCap, w.d_evecs, k);
+        int vst[4] = {k, 0, 0, k + kLzVerify};
+        VPCA_TRY(cudaMemcpyAsync(w.d_lzst, vst, sizeof(vst), cudaMemcpyHostToDevice, stream));
+        lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw + (size_t)(k & 1) * n, n, 0xfaceULL, part);
+        nl += 2;
+        VPCA_TRY(run_chunk(1));   // orthogonalises the start vector against the locked columns, then kLzChunk steps
+        bisect_kernel<<<1, 256, 0, stream>>>(alpha + k, beta + k + 1, kLzVerify, e2, theta2, scal2);
         lz_verify_kernel<<<1, 1, 0, stream>>>(w.d_evals, k, theta2, w.d_scal, w.d_lzst);
         nl += 2;
         VPCA_TRY(cudaMemcpyAsync(hst, w.d_lzst, sizeof(hst), cudaMemcpyDeviceToHost, stream));
@@ -2116,7 +2071,7 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
         return cudaSuccess;
     };
     // One Lanczos step: normalise on rank 0, v_j to every rank, the sharded product, the partials back in rank order,
-    // centring, then both Gram-Schmidt passes with the five-kernel form's kernels.  No host synchronisation.
+    // centring, then both Gram-Schmidt passes (lz_dots / lz_update).  No host synchronisation.
     auto step = [&]() -> cudaError_t {
         cudaError_t ce;
         band_norm_kernel<<<1, 1024, 0, s0>>>(part, npart, w.d_w, w.d_rbar, n, beta, sc, w.d_st);
@@ -2140,29 +2095,24 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     matrix_mean_kernel<<<1, 1024, 0, s0>>>(w.d_rowsum, n, w.d_scal, w.d_nz);
     nl += 2;
 
-    // ---- main run: the convergence test and its step budget are those of lanczos_topk's five-kernel form
-    const double tol = 1e-12;
-    int max_iter = kLzMaxIter;
-    if (const char* mi = getenv("VPCA_EIG_MAXIT")) max_iter = std::max(kLzChunk, std::min(kLzMaxIter, atoi(mi)));
-    int hst[8] = {0, 0, 0, max_iter, 0, 0, 0, 0};
+    // ---- main run: the convergence policy is that of lanczos_topk's persistent form
+    LzPolicy policy(n);
+    int hst[8] = {0, 0, 0, policy.max_iter, 0, 0, 0, 0};
     double hres[2] = {0.0, 0.0};
     VPCA_TRY(cudaMemcpyAsync(w.d_st, hst, sizeof(hst), cudaMemcpyHostToDevice, s0));
     lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w, n, 0x5eedULL, part);
     nl += 1;
-    int m = 0, m_prev = 0;
+    int m = 0;
     bool converged = false;
-    double rho_prev = 0.0;
-    const int max_chunks = std::min(max_iter, n - 1) / kLzChunk;
     *outcome = 4;
-    for (int chunk = 1; chunk <= max_chunks; ++chunk) {
+    for (int chunk = 1; chunk <= policy.max_chunks; ++chunk) {
         for (int g = 0; g < kLzChunk; ++g) VPCA_TRY(step());
         m = chunk * kLzChunk;
-        if (m < k) continue;   // as in lanczos_topk: no k Ritz pairs yet
-        if (chunk > 4 && (chunk & 1) && chunk != max_chunks) continue;
+        if (!policy.test_after(chunk, k)) continue;
         bisect_kernel<<<k, 256, 0, s0>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
         invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), s0>>>(alpha, beta + 1, m, k, w.d_evals,
                                                                                            w.d_scal, w.d_lu, Y);
-        lz_check_kernel<<<1, 32, 0, s0>>>(part, npart, Y, m, k, w.d_scal, w.d_st, res, tol);
+        lz_check_kernel<<<1, 32, 0, s0>>>(part, npart, Y, m, k, w.d_scal, w.d_st, res, kLzTol);
         nl += 3;
         VPCA_TRY(cudaMemcpyAsync(hst, w.d_st, sizeof(hst), cudaMemcpyDeviceToHost, s0));
         VPCA_TRY(cudaMemcpyAsync(hres, res, sizeof(hres), cudaMemcpyDeviceToHost, s0));
@@ -2175,14 +2125,7 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
             *outcome = 2;
             break;
         }
-        const double rho = hres[0];
-        if (m >= 96 && rho > 1e-3) break;   // no separated top of the spectrum: hopeless within kLzMaxIter
-        if (m_prev >= 32 && rho < rho_prev) {
-            const double rate = std::log(rho_prev / rho) / (m - m_prev);
-            if (m + 1.5 * std::log(rho / tol) / rate > max_iter + 2 * kLzChunk) break;
-        }
-        rho_prev = rho;
-        m_prev = m;
+        if (!policy.keep_going(m, hres[0])) break;
     }
     w.last_iters = m;
     if (launches) *launches += nl;
@@ -2193,7 +2136,7 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     lz_ritz_kernel<<<dim3(npart, k), 256, 0, s0>>>(w.d_V, n, Y, m, w.d_evecs);
     lz_finish_kernel<<<k, 512, 0, s0>>>(w.d_evecs, n);
     nl += 2;
-    // ---- deflated verification run (as in the five-kernel form): the k Ritz vectors become the first k basis columns, a
+    // ---- deflated verification run: the k Ritz vectors become the first k basis columns, a
     // fresh start vector is made orthogonal to them and one chunk runs; a Ritz value above theta_k means a missed eigenvalue
     if (k + kLzChunk < n) {
         VPCA_TRY(cudaMemcpyAsync(w.d_V, w.d_evecs, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice, s0));

@@ -219,54 +219,10 @@ cudaError_t join_rows(JoinWork& w, int mode, int variant_set_count, int64_t n_le
                       int64_t* out_rows, int64_t* out_nnz, int64_t* launches);
 void join_free(JoinWork& w);
 
-// ---- centering + eigensolve (eig.cu) ---------------------------------------------------------------
-struct EigWork {
-    int n = 0;
-    double* d_C = nullptr;     // n x n centered matrix, overwritten by the tridiagonalisation
-    double* d_rowsum = nullptr;
-    double* d_v = nullptr;     // Householder vector of the current step (n)
-    double* d_w = nullptr;     // w vector of the current step (n)
-    double* d_p = nullptr;     // p = tau A v (n)
-    double* d_diag = nullptr;  // n
-    double* d_off = nullptr;   // n
-    double* d_tau = nullptr;   // n
-    double* d_scal = nullptr;  // small scalar scratch
-    double* d_evals = nullptr; // k
-    double* d_evecs = nullptr; // n x k (column-major)
-    double* d_lu = nullptr;    // 8 n scratch for inverse iteration
-    int* d_nz = nullptr;
-    int* d_step = nullptr;               // {next step, step of the pending trailing update}
-    cudaGraphExec_t graph_exec = nullptr; // kGraphSteps tridiagonalisation steps, replayed n / kGraphSteps times
-    int graph_n = 0;
-    bool graph_fused = false;
-    int kmax = 0;
-    // Lanczos workspace (allocated on the first Lanczos solve)
-    double* d_V = nullptr;      // n x kLzCap orthonormal basis, column-major
-    double* d_lzw = nullptr;    // 2 n: w ping-pong
-    double* d_lzs = nullptr;    // alpha | beta | h | h2 | e2 | Y | theta2 | res | scal2 | part
-    int* d_lzst = nullptr;      // {step, flag, ticket, step cap}
-    unsigned* d_lzbar = nullptr;   // grid barrier counter of the persistent Lanczos kernel
-    double* d_lzG = nullptr;       // kLzCap x kLzCap: V^T V of the Lanczos basis (one-reduction Gram-Schmidt)
-    long long* d_lzprof = nullptr; // VPCA_LZ_PROF=1: phase timestamps of block 0 (first 64 steps)
-    bool c_valid = false;       // d_C holds the centred matrix of the last center_gram()
-    int lz_blocks = 0;          // blocks of the persistent kernel (= SMs; 0: cooperative launch unavailable or VPCA_LZ_PERSIST=0)
-    size_t lz_smem_max = 0;     // dynamic shared memory a block of the persistent kernel may take (opt-in limit - static)
-    const int32_t* d_S = nullptr;   // the (symmetrised) int32 Gram the last center_gram() read
-    cudaGraphExec_t lz_graph = nullptr;   // kLzChunk Lanczos steps
-    int last_method = 0;        // 1 direct, 2 Lanczos, 3 Lanczos abandoned -> direct
-    int last_iters = 0;         // Lanczos steps of the last solve
-    int mode = 0;               // 0 auto, 1 direct, 2 Lanczos whenever n allows
-};
-cudaError_t eig_alloc(EigWork& w, int n, int kmax);
-void eig_free(EigWork& w);
-// row sums + matrix mean always; the FP64 matrix C only when `materialise` (or later, on demand, through center_matrix)
-cudaError_t center_gram(EigWork& w, const int32_t* d_S, cudaStream_t stream, bool materialise);
-cudaError_t center_matrix(EigWork& w, cudaStream_t stream);
-cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches);
-
 // ---- top-k of a Gram held as row bands across contexts (eig.cu, vpca_compute_pca_bands) ------------------------------
 // One rank's share: its band of S (rows [row0, row0 + rows), lower-triangle cells meaningful) and the buffers of its part
-// of the sharded mat-vec, all on the rank's device.  Owned by the rank's context, kept between solves.
+// of the sharded mat-vec, all on the rank's device.  Owned by the rank's context (or by an EigWork for its one-band
+// solves), kept between solves.
 struct BandPart {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -301,6 +257,55 @@ struct BandEigWork {
     int last_iters = 0;
 };
 void band_eig_free(BandEigWork& w);
+
+// ---- centering + eigensolve (eig.cu) ---------------------------------------------------------------
+struct EigWork {
+    int n = 0;
+    double* d_C = nullptr;     // n x n centered matrix, overwritten by the tridiagonalisation
+    double* d_rowsum = nullptr;
+    double* d_v = nullptr;     // Householder vector of the current step (n)
+    double* d_w = nullptr;     // w vector of the current step (n)
+    double* d_p = nullptr;     // p = tau A v (n)
+    double* d_diag = nullptr;  // n
+    double* d_off = nullptr;   // n
+    double* d_tau = nullptr;   // n
+    double* d_scal = nullptr;  // small scalar scratch
+    double* d_evals = nullptr; // k
+    double* d_evecs = nullptr; // n x k (column-major)
+    double* d_lu = nullptr;    // 8 n scratch for inverse iteration
+    int* d_nz = nullptr;
+    int* d_step = nullptr;               // {next step, step of the pending trailing update}
+    cudaGraphExec_t graph_exec = nullptr; // kGraphSteps tridiagonalisation steps, replayed n / kGraphSteps times
+    int graph_n = 0;
+    bool graph_fused = false;
+    int kmax = 0;
+    // persistent Lanczos workspace (allocated on the first solve in that form)
+    double* d_V = nullptr;      // n x kLzCap orthonormal basis, column-major
+    double* d_lzw = nullptr;    // 2 n: w ping-pong
+    double* d_lzs = nullptr;    // alpha | beta | e2 | Y | theta2 | res | scal2 | part | hpart
+    int* d_lzst = nullptr;      // {step, flag, ticket, step cap}
+    unsigned* d_lzbar = nullptr;   // grid barrier counter of the persistent Lanczos kernel
+    double* d_lzG = nullptr;       // kLzCap x kLzCap: V^T V of the Lanczos basis (one-reduction Gram-Schmidt)
+    long long* d_lzprof = nullptr; // VPCA_LZ_PROF=1: phase timestamps of block 0 (first 64 steps)
+    bool c_valid = false;       // d_C holds the centred matrix of the last center_gram()
+    int lz_blocks = -1;         // blocks of the persistent kernel (= SMs; 0: cooperative launch unavailable or
+                                // VPCA_LZ_PERSIST=0; -1: not queried yet, at the first Lanczos solve)
+    size_t lz_smem_max = 0;     // dynamic shared memory a block of the persistent kernel may take (opt-in limit - static)
+    const int32_t* d_S = nullptr;   // the (symmetrised) int32 Gram the last center_gram() read
+    BandEigWork band_eig;       // Lanczos where the persistent form does not run: the band solver, the whole Gram as one
+    BandPart band_part;         // band
+    int last_method = 0;        // 1 direct, 2 Lanczos, 3 Lanczos abandoned -> direct
+    int last_iters = 0;         // Lanczos steps of the last solve
+    int mode = 0;               // 0 auto, 1 direct, 2 Lanczos whenever n allows
+};
+cudaError_t eig_alloc(EigWork& w, int n, int kmax);
+void eig_free(EigWork& w);
+// row sums + matrix mean always; the FP64 matrix C only when `materialise` (or later, on demand, through center_matrix)
+cudaError_t center_gram(EigWork& w, const int32_t* d_S, cudaStream_t stream, bool materialise);
+cudaError_t center_matrix(EigWork& w, cudaStream_t stream);
+cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches);
+
+// Lanczos on the bands of `world` ranks (vpca_compute_pca_bands; eig_topk past the persistent form's fit, on one band).
 // outcome: 0 converged (d_evals / d_evecs / d_nz hold the answer), 2 breakdown, 3 a missed eigenvalue found by the
 // deflated verification run, 4 no convergence within the step budget.  Synchronises rank 0's stream at every convergence
 // test; the bands are only read.

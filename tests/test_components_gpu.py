@@ -8,15 +8,15 @@ as a bad premise, not as a solver bug.
 What depends on k (csrc/eig.cu): bisect_kernel<<<k>>>, the Gram-Schmidt over earlier columns in invit_kernel, the max
 over k columns in lz_check_kernel, lz_ritz_kernel / lz_ritz_rm_kernel, lz_finish_kernel<<<k>>>, lz_lock_kernel,
 backtransform_kernel<<<k>>>, and the deflated verification run that starts at column k (persistent: k .. k + 8, where
-k + 8 > 32 reads the locked columns past the kLzVtCols shared-memory mirror from global memory; graph form and band
-solver: k - 1 .. k + 16).  vpca_compute_pca takes 1 <= k <= min(N, max(num_pc, 16)); k > 16 needs num_pc >= k.  Every
+k + 8 > 32 reads the locked columns past the kLzVtCols shared-memory mirror from global memory; band solver, also on
+one band: k - 1 .. k + 16).  vpca_compute_pca takes 1 <= k <= min(N, max(num_pc, 16)); k > 16 needs num_pc >= k.  Every
 case proves its path from eig_method and the call's launch count."""
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
-from eig_ref import (P, Reference, assert_direct, assert_graph, assert_persistent, band_contexts, check_agree,
+from eig_ref import (P, Reference, assert_direct, assert_one_band, assert_persistent, band_contexts, check_agree,
                      check_pairs, close_all, compute_pca, compute_pca_bands, gram_context, panel_buffer,
                      structured_cells, synth_cells)
 
@@ -81,22 +81,23 @@ def test_persistent_lanczos_past_16_components(cohorts, k):
     check_pairs(ref, s.vecs, s.evals, s.nz, k)
 
 
-# ------------------------------------------------------------------------------------------ graph-form Lanczos
+# ------------------------------------------------------------------------------------------- one-band Lanczos
 @pytest.mark.parametrize("k,pops", [(16, 20), (33, 40)], ids=["k16", "k33"])
-def test_graph_lanczos_forced_along_k(cohorts, k, pops):
-    """Graph-form Lanczos forced with VPCA_LZ_PERSIST=0 at N = 2504; its deflated run covers columns k - 1 .. k + 16."""
+def test_one_band_lanczos_forced_along_k(cohorts, k, pops):
+    """One-band Lanczos (the band solver on the whole Gram) forced with VPCA_LZ_PERSIST=0 at N = 2504; its deflated run
+    covers columns k - 1 .. k + 16."""
     n, nv = 2504, 8192
     buf, ref = cohorts(n, nv, pops)
     premise(ref, k)
     with gram_context(n, buf, nv, k) as nat:
         s = compute_pca(nat, k, {"VPCA_LZ_PERSIST": "0"})
-    report(f"graph n={n} k={k}", s)
-    assert_graph(s)
+    report(f"one-band n={n} k={k}", s)
+    assert_one_band(s)
     check_pairs(ref, s.vecs, s.evals, s.nz, k)
 
 
-def test_graph_lanczos_by_size_16_components(cohorts):
-    """Graph-form Lanczos chosen by the solver (N = 12 000 is past the persistent form's shared-memory fit), k = 16."""
+def test_one_band_lanczos_by_size_16_components(cohorts):
+    """One-band Lanczos chosen by the solver (N = 12 000 is past the persistent form's shared-memory fit), k = 16."""
     import torch
     n, nv, k = 12_000, 8192, 16
     free, _ = torch.cuda.mem_get_info()
@@ -106,8 +107,8 @@ def test_graph_lanczos_by_size_16_components(cohorts):
     premise(ref, k)
     with gram_context(n, buf, nv, k) as nat:
         s = compute_pca(nat, k)
-    report(f"graph n={n} k={k}", s)
-    assert_graph(s)
+    report(f"one-band n={n} k={k}", s)
+    assert_one_band(s)
     check_pairs(ref, s.vecs, s.evals, s.nz, k)
 
 

@@ -7,13 +7,14 @@
                task list  N % 4 == 0 otherwise (5632, 10 000, 10 752, ...)
                scalar     N % 4 != 0
       rows of S kept in shared memory as far as they fit, the rest read from L2 (VPCA_LZ_SROWS caps them)
-  graph-form Lanczos (five kernels per step on the FP64 matrix C): past that fit (~10 750 on 132 SMs), VPCA_LZ_PERSIST=0
+  one-band Lanczos (the band solver of vpca_compute_pca_bands with the whole Gram as its one band, nine kernels per step
+      on the int32 S): past that fit (~10 750 on 132 SMs), VPCA_LZ_PERSIST=0
   direct reduction: fused step kernel up to N = 3072, two kernels above (or VPCA_EIG_TWO_KERNELS); inverse iteration
       out of shared memory up to N = 3200, out of global memory above
   Lanczos that gives up hands over to the direct reduction (eig_method 3)
 
 Each test names the path it exercises and proves that it ran: `eig_method`, and -- both Lanczos forms report 2 -- the
-`kernel_launches` delta of the call: the persistent form needs fewer launches than steps, the graph form at least five
+`kernel_launches` delta of the call: the persistent form needs fewer launches than steps, the one-band form at least nine
 per step, the direct reduction 64 (fused) or 128 (two kernels) per 64-step graph replay.
 
 Reference: the cohort is the synthetic generator's cells X (N x nv, 0/1) and the Gram kernel builds S = X X^T from them
@@ -23,7 +24,7 @@ cost O(N nv) without forming C."""
 import numpy as np
 import pytest
 
-from eig_ref import (P, Reference, assert_direct, assert_graph, assert_persistent, band_contexts, bands_from_edges,
+from eig_ref import (P, Reference, assert_direct, assert_one_band, assert_persistent, band_contexts, bands_from_edges,
                      check_agree, check_pairs, close_all, compute_pca, compute_pca_bands, gram_context, solve,
                      synth_cells)
 
@@ -44,8 +45,9 @@ def need_free_hbm(gib):
         pytest.skip(f"needs {gib:.0f} GB of free HBM")
 
 
-def graph_form_gib(n):
-    """S (int32) + C (FP64) + the Krylov basis + the reference's cells, with room to spare"""
+def past_fit_gib(n):
+    """S (int32) + C (FP64, which eig_alloc allocates whatever the solver) + the Krylov basis + the reference's cells, with
+    room to spare"""
     return 1.3 * (12 * n * n + 8 * 400 * n + 24 * n * NV) / 2 ** 30 + 1
 
 
@@ -107,35 +109,45 @@ def test_persistent_lanczos_switches(env):
     check_agree(switched, default, K, ref)
 
 
-# ------------------------------------------------------------------------------------------- 2. graph-form Lanczos
+# ------------------------------------------------------------------------------------------- 2. one-band Lanczos
+def assert_same_bits(a, b):
+    assert np.array_equal(a.vecs, b.vecs) and np.array_equal(a.evals, b.evals) and a.nz == b.nz, (a, b)
+
+
 @pytest.mark.parametrize("n", [1092, 2503])
 def test_graph_lanczos_forced(n):
-    """Graph-form Lanczos (lz_matvec_kernel on the FP64 C, lz_dots / lz_update, lz_ritz_kernel, and the column-major
-    deflated verification run) forced with VPCA_LZ_PERSIST=0, against the persistent form and the reference."""
+    """One-band Lanczos (the band solver on the whole Gram: band_tile_kernel on the int32 S, lz_dots / lz_update,
+    lz_ritz_kernel, and the column-major deflated verification run) forced with VPCA_LZ_PERSIST=0: bit for bit
+    vpca_compute_pca_bands on the same context, and against the persistent form and the reference."""
     buf, X = synth_cells(n, NV)
     ref = Reference(X, K)
-    graph, persistent = solve(n, buf, NV, K, {"VPCA_LZ_PERSIST": "0"}), solve(n, buf, NV, K)
-    assert_graph(graph)
+    with gram_context(n, buf, NV, K) as nat:
+        one_band = compute_pca(nat, K, {"VPCA_LZ_PERSIST": "0"})
+        bands = compute_pca_bands([nat], K)
+    persistent = solve(n, buf, NV, K)
+    assert_one_band(one_band)
+    assert bands.method == 4, bands
     assert_persistent(persistent)
-    check_pairs(ref, graph.vecs, graph.evals, graph.nz, K)
-    check_agree(graph, persistent, K, ref)
+    check_pairs(ref, one_band.vecs, one_band.evals, one_band.nz, K)
+    assert_same_bits(one_band, bands)
+    check_agree(one_band, persistent, K, ref)
 
 
 @pytest.mark.parametrize("n", ["past_fit", 12_000, 16_384, 16_385, 20_000])
 def test_graph_lanczos_past_the_persistent_fit(n):
-    """Graph-form Lanczos chosen by the solver itself: from the first N whose persistent working set no longer fits a
+    """One-band Lanczos chosen by the solver itself: from the first N whose persistent working set no longer fits a
     block of shared memory (10 753 on 132 SMs) on, where the persistent kernel cannot be launched."""
     n = resolve(n)
-    need_free_hbm(graph_form_gib(n))
+    need_free_hbm(past_fit_gib(n))
     buf, X = synth_cells(n, NV)
     s = solve(n, buf, NV, K)
-    assert_graph(s)
+    assert_one_band(s)
     check_pairs(Reference(X, K), s.vecs, s.evals, s.nz, K)
 
 
 def test_graph_lanczos_at_the_sample_limit():
-    """Graph-form Lanczos at N = 65 535, vpca_compute_pca's limit: S is 17 GB, C 34 GB, and center_kernel's grid is
-    exactly 65 535 rows high.  k = 2 on the structured cohort converges without a hand-over to the direct solver."""
+    """One-band Lanczos at N = 65 535, vpca_compute_pca's limit: S is 17 GB, and C (34 GB) is allocated but not built.
+    k = 2 on the structured cohort converges without a hand-over to the direct solver."""
     import torch
     n, nv, k = 65_535, 2048, 2
     need_free_hbm(60)
@@ -143,7 +155,7 @@ def test_graph_lanczos_at_the_sample_limit():
     with gram_context(n, buf, nv, k) as nat:
         s = compute_pca(nat, k)
     torch.cuda.empty_cache()
-    assert_graph(s)
+    assert_one_band(s)
     check_pairs(Reference(X, k), s.vecs, s.evals, s.nz, k)
 
 
@@ -245,19 +257,19 @@ def test_band_solver_world_16():
     check_agree(bands, solve(n, buf, NV, K), K, ref)
 
 
-# ------------------------------------------------------------------------------------ 6. cross-solver agreement
+# ----------------------------------------------------------------- 6. vpca_compute_pca past the fit is the band solver
 @pytest.mark.parametrize("n", [12_000, 20_000])
 def test_graph_lanczos_and_band_solver_agree(n):
-    """Two independent mat-vecs of the same Gram past the persistent fit: the graph-form Lanczos on the FP64 C
-    (vpca_compute_pca) and the band solver on the int32 lower triangle (vpca_compute_pca_bands, world 1)."""
-    need_free_hbm(graph_form_gib(n))
+    """Past the persistent fit vpca_compute_pca solves the whole Gram as one band of the band solver: bit for bit what
+    vpca_compute_pca_bands (world 1) gives on the same context."""
+    need_free_hbm(past_fit_gib(n))
     buf, X = synth_cells(n, NV)
     ref = Reference(X, K)
     with gram_context(n, buf, NV, K) as nat:
-        graph = compute_pca(nat, K)
+        one_band = compute_pca(nat, K)
         bands = compute_pca_bands([nat], K)
-    assert_graph(graph)
+    assert_one_band(one_band)
     assert bands.method == 4, bands
-    for s in (graph, bands):
+    for s in (one_band, bands):
         check_pairs(ref, s.vecs, s.evals, s.nz, K)
-    check_agree(graph, bands, K, ref)
+    assert_same_bits(one_band, bands)

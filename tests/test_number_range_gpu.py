@@ -571,15 +571,15 @@ def _assert_scaled(base, scaled, factor, what):
 @pytest.mark.parametrize("path,env", [("direct-fused", {"VPCA_EIG": "direct"}),
                                       ("direct-two-kernels", {"VPCA_EIG": "direct", "VPCA_EIG_TWO_KERNELS": "1"}),
                                       ("persistent-lanczos", {}),
-                                      ("graph-lanczos", {"VPCA_LZ_PERSIST": "0"}),
+                                      ("one-band-lanczos", {"VPCA_LZ_PERSIST": "0"}),
                                       ("bands", None)])
 def test_eigensolver_scale_invariance(path, env):
     """The same cohort's cells times 2^5 (int8 cells 0/32, max_multiplicity 32) and its Gram times 2^16 (setGram) give
     bit-identical vectors and eigenvalues exactly 4^5 and 2^16 times as large on every solver path, and each solve
     passes the FP64 reference."""
     import torch
-    from eig_ref import (Reference, assert_direct, assert_graph, assert_persistent, check_pairs, close_all, compute_pca,
-                         compute_pca_bands, synth_cells)
+    from eig_ref import (Reference, assert_direct, assert_one_band, assert_persistent, check_pairs, close_all,
+                         compute_pca, compute_pca_bands, synth_cells)
     n, nv, k = 1092, 4096, 4
     buf, X = synth_cells(n, nv)
     buf_scaled = buf * SCALE
@@ -614,7 +614,7 @@ def test_eigensolver_scale_invariance(path, env):
             solves["gram"] = compute_pca(nat, k, env)
         ran_as_named = {"direct-fused": lambda s: assert_direct(s, n, fused=True),
                         "direct-two-kernels": lambda s: assert_direct(s, n, fused=False),
-                        "persistent-lanczos": assert_persistent, "graph-lanczos": assert_graph}[path]
+                        "persistent-lanczos": assert_persistent, "one-band-lanczos": assert_one_band}[path]
         for s in solves.values():
             ran_as_named(s)
     for name, r in (("base", ref), ("cells", ref_scaled), ("gram_base", ref)):

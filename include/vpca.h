@@ -518,6 +518,10 @@ int vpca_debug_gram_profile(vpca_ctx* ctx, int64_t* out, int32_t max_ctas);
  * for steps 0..31 (each slot holds the last launch that ran that step index); returns the number of steps written or a
  * negative vpca_status. */
 int vpca_debug_lanczos_profile(vpca_ctx* ctx, int64_t* out, int32_t max_steps);
+/* Host-only diagnostic: the bytes of device memory every context of the process holds right now (their Grams, staging
+ * and solver workspaces; not caller-owned Grams or pinned host memory).  vpca_destroy brings it back to what it was
+ * before the context was created. */
+int64_t vpca_debug_device_bytes(void);
 
 /* ---- Multi-dataset keying on the device (SURVEY 8 f-3) ------------------------------------------------------------
  * The 2-dataset and N-dataset branches of VariantsPcaDriver.getCallsRdd (VariantsPca.scala:153-168) key every variant by

@@ -1596,33 +1596,28 @@ __global__ void band_combine_kernel(const double* __restrict__ slots, int n, int
 }  // namespace
 
 cudaError_t eig_alloc(EigWork& w, int n, int kmax) {
+    const int64_t n1 = n;
+    cudaError_t e = w.d_C.ensure(n1 * n);
+    if (e == cudaSuccess) e = w.d_rowsum.ensure(n1);
+    if (e == cudaSuccess) e = w.d_v.ensure(2 * n1);   // vprev / vcur ping-pong
+    if (e == cudaSuccess) e = w.d_w.ensure(n1);
+    if (e == cudaSuccess) e = w.d_p.ensure(2 * n1);   // p ping-pong (fused step kernel)
+    if (e == cudaSuccess) e = w.d_diag.ensure(n1);
+    if (e == cudaSuccess) e = w.d_off.ensure(2 * n1);   // e and e^2
+    if (e == cudaSuccess) e = w.d_tau.ensure(n1);
+    if (e == cudaSuccess) e = w.d_scal.ensure(16);
+    if (e == cudaSuccess) e = w.d_evals.ensure(kmax);
+    if (e == cudaSuccess) e = w.d_evecs.ensure(n1 * kmax);
+    if (e == cudaSuccess) e = w.d_lu.ensure(8 * n1);
+    if (e == cudaSuccess) e = w.d_nz.ensure(1);
+    if (e == cudaSuccess) e = w.d_step.ensure(4);   // {next, current step, ticket counter, -}
+    if (e != cudaSuccess) return e;
     w.n = n;
     w.kmax = kmax;
-    cudaError_t e;
-#define VPCA_TRY(x) if ((e = (x)) != cudaSuccess) return e
-    VPCA_TRY(cudaMalloc(&w.d_C, (size_t)n * n * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_rowsum, (size_t)n * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_v, 2 * (size_t)n * sizeof(double)));   // vprev / vcur ping-pong
-    VPCA_TRY(cudaMalloc(&w.d_w, (size_t)n * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_p, 2 * (size_t)n * sizeof(double)));   // p ping-pong (fused step kernel)
-    VPCA_TRY(cudaMalloc(&w.d_diag, (size_t)n * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_off, 2 * (size_t)n * sizeof(double)));   // e and e^2
-    VPCA_TRY(cudaMalloc(&w.d_tau, (size_t)n * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_scal, 16 * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_evals, (size_t)kmax * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_evecs, (size_t)n * kmax * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_lu, 8 * (size_t)n * sizeof(double)));
-    VPCA_TRY(cudaMalloc(&w.d_nz, sizeof(int)));
-    VPCA_TRY(cudaMalloc(&w.d_step, 4 * sizeof(int)));   // {next, current step, ticket counter, -}
-#undef VPCA_TRY
     return cudaSuccess;
 }
 
 void eig_free(EigWork& w) {
-    cudaFree(w.d_C); cudaFree(w.d_rowsum); cudaFree(w.d_v); cudaFree(w.d_w); cudaFree(w.d_p);
-    cudaFree(w.d_diag); cudaFree(w.d_off); cudaFree(w.d_tau); cudaFree(w.d_scal); cudaFree(w.d_evals);
-    cudaFree(w.d_evecs); cudaFree(w.d_lu); cudaFree(w.d_nz); cudaFree(w.d_step);
-    cudaFree(w.d_V); cudaFree(w.d_lzw); cudaFree(w.d_lzs); cudaFree(w.d_lzst); cudaFree(w.d_lzbar); cudaFree(w.d_lzprof); cudaFree(w.d_lzG);
     if (w.graph_exec != nullptr) cudaGraphExecDestroy(w.graph_exec);
     band_eig_free(w.band_eig);
     band_part_free(w.band_part);
@@ -1632,8 +1627,8 @@ void eig_free(EigWork& w) {
 cudaError_t center_gram(EigWork& w, const int32_t* d_S, cudaStream_t stream, bool materialise) {
     const int n = w.n;
     w.d_S = d_S;   // the persistent Lanczos applies the centring to vectors and reads the int32 Gram itself
-    rowsum_kernel<<<(n + 7) / 8, 256, 0, stream>>>(d_S, n, w.d_rowsum);
-    matrix_mean_kernel<<<1, 1024, 0, stream>>>(w.d_rowsum, n, w.d_scal, w.d_nz);
+    rowsum_kernel<<<(n + 7) / 8, 256, 0, stream>>>(d_S, n, w.d_rowsum.get());
+    matrix_mean_kernel<<<1, 1024, 0, stream>>>(w.d_rowsum.get(), n, w.d_scal.get(), w.d_nz.get());
     w.c_valid = false;
     if (materialise) return center_matrix(w, stream);
     return cudaGetLastError();
@@ -1645,7 +1640,7 @@ cudaError_t center_matrix(EigWork& w, cudaStream_t stream) {
     if (w.c_valid) return cudaSuccess;
     const int n = w.n;
     const int bx = (n + 1023) / 1024 < 1 ? 1 : (n + 1023) / 1024;
-    center_kernel<<<dim3(bx, n), 256, 0, stream>>>(w.d_S, w.d_rowsum, w.d_scal, n, w.d_C);
+    center_kernel<<<dim3(bx, n), 256, 0, stream>>>(w.d_S, w.d_rowsum.get(), w.d_scal.get(), n, w.d_C.get());
     w.c_valid = true;
     return cudaGetLastError();
 }
@@ -1695,8 +1690,8 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
         VPCA_TRY(band_eig_topk(w.band_eig, parts, 1, kmax, k, launches, &outcome));
         w.last_iters = w.band_eig.last_iters;
         if (outcome != 0) return cudaSuccess;
-        VPCA_TRY(cudaMemcpyAsync(w.d_evals, w.band_eig.d_evals, k * sizeof(double), cudaMemcpyDeviceToDevice, stream));
-        VPCA_TRY(cudaMemcpyAsync(w.d_evecs, w.band_eig.d_evecs, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice,
+        VPCA_TRY(cudaMemcpyAsync(w.d_evals.get(), w.band_eig.d_evals.get(), k * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+        VPCA_TRY(cudaMemcpyAsync(w.d_evecs.get(), w.band_eig.d_evecs.get(), (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice,
                                  stream));
         *used = true;
         return cudaSuccess;
@@ -1704,21 +1699,21 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
 
     const size_t small_doubles = 3 * (size_t)kLzCap + (size_t)kLzCap * kmax + 16 + 4 + 16 + (size_t)npart +
                                  2 * (size_t)w.lz_blocks * kLzCap;
-    if (w.d_V == nullptr) {
-        VPCA_TRY(cudaMalloc(&w.d_V, (size_t)n * kLzCap * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_lzw, 2 * (size_t)n * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_lzs, small_doubles * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_lzst, 8 * sizeof(int)));
-        VPCA_TRY(cudaMemset(w.d_lzst, 0, 8 * sizeof(int)));
-        VPCA_TRY(cudaMalloc(&w.d_lzbar, sizeof(unsigned)));
-        VPCA_TRY(cudaMalloc(&w.d_lzG, (size_t)kLzCap * kLzCap * sizeof(double)));
-        VPCA_TRY(cudaMemset(w.d_lzG, 0, (size_t)kLzCap * kLzCap * sizeof(double)));
+    if (w.d_V.get() == nullptr) {   // d_V is allocated last: null until the whole workspace is in place
+        VPCA_TRY(w.d_lzw.ensure(2 * (int64_t)n));
+        VPCA_TRY(w.d_lzs.ensure((int64_t)small_doubles));
+        VPCA_TRY(w.d_lzst.ensure(8));
+        VPCA_TRY(cudaMemset(w.d_lzst.get(), 0, 8 * sizeof(int)));
+        VPCA_TRY(w.d_lzbar.ensure(1));
+        VPCA_TRY(w.d_lzG.ensure((int64_t)kLzCap * kLzCap));
+        VPCA_TRY(cudaMemset(w.d_lzG.get(), 0, (size_t)kLzCap * kLzCap * sizeof(double)));
         if (const char* pf = getenv("VPCA_LZ_PROF"); pf != nullptr && atoi(pf) != 0) {
-            VPCA_TRY(cudaMalloc(&w.d_lzprof, 64 * 4 * sizeof(long long)));
-            VPCA_TRY(cudaMemset(w.d_lzprof, 0, 64 * 4 * sizeof(long long)));
+            VPCA_TRY(w.d_lzprof.ensure(64 * 4));
+            VPCA_TRY(cudaMemset(w.d_lzprof.get(), 0, 64 * 4 * sizeof(long long)));
         }
+        VPCA_TRY(w.d_V.ensure((int64_t)n * kLzCap));
     }
-    double* alpha = w.d_lzs;
+    double* alpha = w.d_lzs.get();
     double* beta = alpha + kLzCap;
     double* e2 = beta + kLzCap;
     double* Y = e2 + kLzCap;
@@ -1735,28 +1730,28 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     const size_t persist_smem = base_smem + (size_t)rows_smem * row_bytes;
     VPCA_TRY(cudaFuncSetAttribute(lz_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)persist_smem));
     auto run_chunk = [&](int pre, const int* gate = nullptr) -> cudaError_t {
-        cudaError_t ce = cudaMemsetAsync(w.d_lzbar, 0, sizeof(unsigned), stream);
+        cudaError_t ce = cudaMemsetAsync(w.d_lzbar.get(), 0, sizeof(unsigned), stream);
         if (ce != cudaSuccess) return ce;
         LzArgs a{};
         a.S = w.d_S;
-        a.rowsum = w.d_rowsum;
-        a.scal = w.d_scal;
-        a.VT = w.d_V;
-        a.wbuf = w.d_lzw;
+        a.rowsum = w.d_rowsum.get();
+        a.scal = w.d_scal.get();
+        a.VT = w.d_V.get();
+        a.wbuf = w.d_lzw.get();
         a.alpha = alpha;
         a.beta = beta;
         a.hpart = hpart;
-        a.G = w.d_lzG;
+        a.G = w.d_lzG.get();
         a.part = part;
-        a.st = w.d_lzst;
-        a.bar = w.d_lzbar;
+        a.st = w.d_lzst.get();
+        a.bar = w.d_lzbar.get();
         a.n = n;
         a.cap = kLzCap;
         a.nsteps = kLzChunk;
         a.pre = pre;
         a.gate = gate;
         a.rows_smem = rows_smem;
-        a.prof = w.d_lzprof;
+        a.prof = w.d_lzprof.get();
         void* params[] = {&a};
         nl += 1;
         return cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(lz_persist_kernel), dim3((unsigned)w.lz_blocks),
@@ -1769,8 +1764,8 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     double hres[2] = {0.0, 0.0};
     const char* spe = getenv("VPCA_LZ_SPECULATE");
     const bool speculate = k + kLzChunk < n && !(spe != nullptr && atoi(spe) == 0);
-    VPCA_TRY(cudaMemcpyAsync(w.d_lzst, hst, sizeof(hst), cudaMemcpyHostToDevice, stream));
-    lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw, n, 0x5eedULL, part);
+    VPCA_TRY(cudaMemcpyAsync(w.d_lzst.get(), hst, sizeof(hst), cudaMemcpyHostToDevice, stream));
+    lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw.get(), n, 0x5eedULL, part);
     nl += 1;
     int m = 0;
     bool converged = false;
@@ -1778,11 +1773,11 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
         VPCA_TRY(run_chunk(0));
         m = chunk * kLzChunk;
         if (!policy.test_after(chunk, k)) continue;
-        bisect_kernel<<<k, 256, 0, stream>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
+        bisect_kernel<<<k, 256, 0, stream>>>(alpha, beta + 1, m, e2, w.d_evals.get(), w.d_scal.get());
         // a tridiagonal matrix of a few dozen rows: one warp (its block-wide reductions then cost no barrier latency)
-        invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), stream>>>(alpha, beta + 1, m, k, w.d_evals, w.d_scal,
-                                                                                w.d_lu, Y);
-        lz_check_kernel<<<1, 32, 0, stream>>>(part, 1, Y, m, k, w.d_scal, w.d_lzst, res, kLzTol);
+        invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), stream>>>(alpha, beta + 1, m, k, w.d_evals.get(), w.d_scal.get(),
+                                                                                w.d_lu.get(), Y);
+        lz_check_kernel<<<1, 32, 0, stream>>>(part, 1, Y, m, k, w.d_scal.get(), w.d_lzst.get(), res, kLzTol);
         nl += 3;
         const bool spec = speculate && chunk == 1;
         if (spec) {
@@ -1790,18 +1785,18 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
             // locking them, the deflated re-run and its verdict -- is enqueued NOW behind a one-thread gate, so the host
             // synchronises once per solve; had the test failed, every gated kernel returns at once and the main run
             // goes on below with its state untouched.
-            const int* gate = w.d_lzst + 4;
-            lz_gate_kernel<<<1, 1, 0, stream>>>(w.d_lzst, k, kLzVerify);
-            lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V, n, kLzCap, Y, m, k, w.d_evecs, gate);
-            lz_finish_kernel<<<k, 512, 0, stream>>>(w.d_evecs, n, gate);
-            lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V, n, kLzCap, w.d_evecs, k, gate);
-            lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw + (size_t)(k & 1) * n, n, 0xfaceULL, part, gate);
+            const int* gate = w.d_lzst.get() + 4;
+            lz_gate_kernel<<<1, 1, 0, stream>>>(w.d_lzst.get(), k, kLzVerify);
+            lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V.get(), n, kLzCap, Y, m, k, w.d_evecs.get(), gate);
+            lz_finish_kernel<<<k, 512, 0, stream>>>(w.d_evecs.get(), n, gate);
+            lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V.get(), n, kLzCap, w.d_evecs.get(), k, gate);
+            lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw.get() + (size_t)(k & 1) * n, n, 0xfaceULL, part, gate);
             VPCA_TRY(run_chunk(1, gate));
             bisect_kernel<<<1, 256, 0, stream>>>(alpha + k, beta + k + 1, kLzVerify, e2, theta2, scal2, gate);
-            lz_verify_kernel<<<1, 1, 0, stream>>>(w.d_evals, k, theta2, w.d_scal, w.d_lzst, gate);
+            lz_verify_kernel<<<1, 1, 0, stream>>>(w.d_evals.get(), k, theta2, w.d_scal.get(), w.d_lzst.get(), gate);
             nl += 7;
         }
-        VPCA_TRY(cudaMemcpyAsync(hst, w.d_lzst, sizeof(hst), cudaMemcpyDeviceToHost, stream));
+        VPCA_TRY(cudaMemcpyAsync(hst, w.d_lzst.get(), sizeof(hst), cudaMemcpyDeviceToHost, stream));
         VPCA_TRY(cudaMemcpyAsync(hres, res, sizeof(hres), cudaMemcpyDeviceToHost, stream));
         VPCA_TRY(cudaStreamSynchronize(stream));
         if (spec && hst[4] == 1) {   // converged at the first test; the re-run has delivered its verdict in st[1]
@@ -1824,24 +1819,24 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
     nl = 0;
 
     // Ritz vectors, unit norm, sign rule
-    lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V, n, kLzCap, Y, m, k, w.d_evecs);
-    lz_finish_kernel<<<k, 512, 0, stream>>>(w.d_evecs, n);
+    lz_ritz_rm_kernel<<<(n + 7) / 8, 256, 0, stream>>>(w.d_V.get(), n, kLzCap, Y, m, k, w.d_evecs.get());
+    lz_finish_kernel<<<k, 512, 0, stream>>>(w.d_evecs.get(), n);
     nl += 2;
 
     // Guard against a missed copy of a multiple eigenvalue (a single Krylov sequence sees one vector per eigenspace):
     // lock the k Ritz vectors as the first k basis columns and run one more chunk from a fresh start vector that is
     // orthogonal to them.  Its top Ritz value is a lower bound of the largest eigenvalue of the deflated operator.
     if (k + kLzChunk < n) {
-        lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V, n, kLzCap, w.d_evecs, k);
+        lz_lock_kernel<<<(n + 255) / 256, 256, 0, stream>>>(w.d_V.get(), n, kLzCap, w.d_evecs.get(), k);
         int vst[4] = {k, 0, 0, k + kLzVerify};
-        VPCA_TRY(cudaMemcpyAsync(w.d_lzst, vst, sizeof(vst), cudaMemcpyHostToDevice, stream));
-        lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw + (size_t)(k & 1) * n, n, 0xfaceULL, part);
+        VPCA_TRY(cudaMemcpyAsync(w.d_lzst.get(), vst, sizeof(vst), cudaMemcpyHostToDevice, stream));
+        lz_init_kernel<<<npart, 32, 0, stream>>>(w.d_lzw.get() + (size_t)(k & 1) * n, n, 0xfaceULL, part);
         nl += 2;
         VPCA_TRY(run_chunk(1));   // orthogonalises the start vector against the locked columns, then kLzChunk steps
         bisect_kernel<<<1, 256, 0, stream>>>(alpha + k, beta + k + 1, kLzVerify, e2, theta2, scal2);
-        lz_verify_kernel<<<1, 1, 0, stream>>>(w.d_evals, k, theta2, w.d_scal, w.d_lzst);
+        lz_verify_kernel<<<1, 1, 0, stream>>>(w.d_evals.get(), k, theta2, w.d_scal.get(), w.d_lzst.get());
         nl += 2;
-        VPCA_TRY(cudaMemcpyAsync(hst, w.d_lzst, sizeof(hst), cudaMemcpyDeviceToHost, stream));
+        VPCA_TRY(cudaMemcpyAsync(hst, w.d_lzst.get(), sizeof(hst), cudaMemcpyDeviceToHost, stream));
         VPCA_TRY(cudaStreamSynchronize(stream));
         if (launches) *launches += nl;
         if (hst[1] != 1) return cudaGetLastError();
@@ -1871,14 +1866,14 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
     cudaError_t e = center_matrix(w, stream);   // the reduction works on (and overwrites) the FP64 matrix
     if (e != cudaSuccess) return e;
     w.c_valid = false;
-    e = cudaMemsetAsync(w.d_v, 0, 2 * (size_t)n * sizeof(double), stream);
+    e = cudaMemsetAsync(w.d_v.get(), 0, 2 * (size_t)n * sizeof(double), stream);
     if (e != cudaSuccess) return e;
-    cudaMemsetAsync(w.d_w, 0, (size_t)n * sizeof(double), stream);
-    cudaMemsetAsync(w.d_p, 0, 2 * (size_t)n * sizeof(double), stream);
-    cudaMemsetAsync(w.d_tau, 0, (size_t)n * sizeof(double), stream);
-    cudaMemsetAsync(w.d_off, 0, 2 * (size_t)n * sizeof(double), stream);
+    cudaMemsetAsync(w.d_w.get(), 0, (size_t)n * sizeof(double), stream);
+    cudaMemsetAsync(w.d_p.get(), 0, 2 * (size_t)n * sizeof(double), stream);
+    cudaMemsetAsync(w.d_tau.get(), 0, (size_t)n * sizeof(double), stream);
+    cudaMemsetAsync(w.d_off.get(), 0, 2 * (size_t)n * sizeof(double), stream);
     int64_t nl = 0;
-    cudaMemsetAsync(w.d_step, 0, 4 * sizeof(int), stream);
+    cudaMemsetAsync(w.d_step.get(), 0, 4 * sizeof(int), stream);
     // The step loop is replayed from ONE CUDA graph of kGraphSteps identical launches: the step index lives in device
     // memory, so no launch has step-dependent arguments; launches past the last step return at once.
     constexpr int kGraphSteps = 64;
@@ -1903,12 +1898,12 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
         if (e != cudaSuccess) return e;
         for (int g = 0; g < kGraphSteps; ++g) {
             if (fused) {
-                tridiag_fused_kernel<<<fused_blocks, 512, fused_smem, stream>>>(w.d_C, n, w.d_step, w.d_v, w.d_p, w.d_diag,
-                                                                                w.d_off, w.d_tau);
+                tridiag_fused_kernel<<<fused_blocks, 512, fused_smem, stream>>>(w.d_C.get(), n, w.d_step.get(), w.d_v.get(), w.d_p.get(), w.d_diag.get(),
+                                                                                w.d_off.get(), w.d_tau.get());
             } else {
-                tridiag_small_kernel<<<1, kSmallThreads, 0, stream>>>(w.d_C, n, w.d_step, w.d_v, w.d_p, w.d_w, w.d_diag,
-                                                                      w.d_off, w.d_tau, w.d_scal);
-                tridiag_big_kernel<<<big_blocks, 128, 0, stream>>>(w.d_C, n, w.d_step, w.d_v, w.d_w, w.d_tau, w.d_p);
+                tridiag_small_kernel<<<1, kSmallThreads, 0, stream>>>(w.d_C.get(), n, w.d_step.get(), w.d_v.get(), w.d_p.get(), w.d_w.get(), w.d_diag.get(),
+                                                                      w.d_off.get(), w.d_tau.get(), w.d_scal.get());
+                tridiag_big_kernel<<<big_blocks, 128, 0, stream>>>(w.d_C.get(), n, w.d_step.get(), w.d_v.get(), w.d_w.get(), w.d_tau.get(), w.d_p.get());
             }
         }
         e = cudaStreamEndCapture(stream, &graph);
@@ -1924,17 +1919,17 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
         if (e != cudaSuccess) return e;
         nl += (fused ? 1 : 2) * kGraphSteps;
     }
-    bisect_kernel<<<k, 256, 0, stream>>>(w.d_diag, w.d_off, n, w.d_off + n, w.d_evals, w.d_scal);
+    bisect_kernel<<<k, 256, 0, stream>>>(w.d_diag.get(), w.d_off.get(), n, w.d_off.get() + n, w.d_evals.get(), w.d_scal.get());
     const size_t invit_smem = 8 * (size_t)n * sizeof(double);
     if (invit_smem <= 200 * 1024) {
         e = cudaFuncSetAttribute(invit_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         if (e != cudaSuccess) return e;   // (per device: not cached)
-        invit_kernel<true><<<1, 256, invit_smem, stream>>>(w.d_diag, w.d_off, n, k, w.d_evals, w.d_scal, w.d_lu,
-                                                           w.d_evecs);
+        invit_kernel<true><<<1, 256, invit_smem, stream>>>(w.d_diag.get(), w.d_off.get(), n, k, w.d_evals.get(), w.d_scal.get(), w.d_lu.get(),
+                                                           w.d_evecs.get());
     } else {
-        invit_kernel<false><<<1, 256, 0, stream>>>(w.d_diag, w.d_off, n, k, w.d_evals, w.d_scal, w.d_lu, w.d_evecs);
+        invit_kernel<false><<<1, 256, 0, stream>>>(w.d_diag.get(), w.d_off.get(), n, k, w.d_evals.get(), w.d_scal.get(), w.d_lu.get(), w.d_evecs.get());
     }
-    backtransform_kernel<<<k, 512, 0, stream>>>(w.d_C, n, w.d_tau, w.d_evecs);
+    backtransform_kernel<<<k, 512, 0, stream>>>(w.d_C.get(), n, w.d_tau.get(), w.d_evecs.get());
     nl += 3;
     if (launches) *launches += nl;
     return cudaGetLastError();
@@ -1942,14 +1937,11 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
 
 // ------------------------------------------------------------------------------------------- band Lanczos, host side
 void band_part_free(BandPart& p) {
-    cudaFree(p.d_v); cudaFree(p.d_y); cudaFree(p.d_scratch);
     if (p.ev_done != nullptr) cudaEventDestroy(p.ev_done);
     p = BandPart{};
 }
 
 void band_eig_free(BandEigWork& w) {
-    cudaFree(w.d_V); cudaFree(w.d_w); cudaFree(w.d_small); cudaFree(w.d_slots); cudaFree(w.d_rowsum); cudaFree(w.d_rbar);
-    cudaFree(w.d_scal); cudaFree(w.d_evals); cudaFree(w.d_evecs); cudaFree(w.d_lu); cudaFree(w.d_nz); cudaFree(w.d_st);
     if (w.ev_v != nullptr) cudaEventDestroy(w.ev_v);
     w = BandEigWork{};
 }
@@ -1962,16 +1954,16 @@ constexpr size_t kBandSmallFixed = 5 * (size_t)kLzCap + 16 + 4 + 16 + 4;   // + 
 // row partials and ceil(rows / kBandTR) x (row0 + rows) column partials.
 cudaError_t band_part_prepare(BandPart& p) {
     if (p.alloc_n == p.n && p.alloc_row0 == p.row0 && p.alloc_rows == p.rows) return cudaSuccess;
-    cudaFree(p.d_v); cudaFree(p.d_y); cudaFree(p.d_scratch);
-    p.d_v = p.d_y = p.d_scratch = nullptr;
+    p.d_v.reset();
+    p.d_y.reset();
+    p.d_scratch.reset();
     p.alloc_n = 0;
-    const size_t ncols = (size_t)p.row0 + p.rows;
-    const size_t ntc = (ncols + kBandTC - 1) / kBandTC, ntr = ((size_t)p.rows + kBandTR - 1) / kBandTR;
-    p.scratch_doubles = ntc * p.rows + ntr * ncols;
+    const int64_t ncols = (int64_t)p.row0 + p.rows;
+    const int64_t ntc = (ncols + kBandTC - 1) / kBandTC, ntr = ((int64_t)p.rows + kBandTR - 1) / kBandTR;
     cudaError_t e;
-    if ((e = cudaMalloc(&p.d_v, (size_t)p.n * sizeof(double))) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&p.d_y, ncols * sizeof(double))) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&p.d_scratch, p.scratch_doubles * sizeof(double))) != cudaSuccess) return e;
+    if ((e = p.d_v.ensure(p.n)) != cudaSuccess) return e;
+    if ((e = p.d_y.ensure(ncols)) != cudaSuccess) return e;
+    if ((e = p.d_scratch.ensure(ntc * p.rows + ntr * ncols)) != cudaSuccess) return e;
     if (p.ev_done == nullptr && (e = cudaEventCreateWithFlags(&p.ev_done, cudaEventDisableTiming)) != cudaSuccess) return e;
     p.alloc_n = p.n;
     p.alloc_row0 = p.row0;
@@ -1984,7 +1976,7 @@ template <typename T>
 cudaError_t band_product(const BandPart& p, const double* v, T* y) {
     const int ncols = p.row0 + p.rows;
     const dim3 grid((unsigned)((ncols + kBandTC - 1) / kBandTC), (unsigned)((p.rows + kBandTR - 1) / kBandTR));
-    T* rowp = reinterpret_cast<T*>(p.d_scratch);
+    T* rowp = reinterpret_cast<T*>(p.d_scratch.get());
     T* colp = rowp + (size_t)grid.x * p.rows;
     const bool vec = (p.n & 3) == 0 && (reinterpret_cast<uintptr_t>(p.d_S) & 15) == 0;
     if (vec) band_tile_kernel<T, true><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
@@ -2006,24 +1998,24 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
 #define VPCA_TRY(x) if ((e = (x)) != cudaSuccess) return e
     // ---- workspace: rank 0's solver state, every rank's share
     VPCA_TRY(cudaSetDevice(dev0));
-    if (w.d_V == nullptr || w.n != n || w.kmax != kmax) {
-        band_eig_free(w);
-        w.n = n;
-        w.kmax = kmax;
-        VPCA_TRY(cudaMalloc(&w.d_V, (size_t)n * kLzCap * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_w, 2 * (size_t)n * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_small, (kBandSmallFixed + (size_t)kLzCap * kmax + npart) * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_slots, 16 * (size_t)n * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_rowsum, (size_t)n * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_rbar, (size_t)n * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_scal, 16 * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_evals, (size_t)kmax * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_evecs, (size_t)n * kmax * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_lu, 8 * (size_t)kLzCap * sizeof(double)));
-        VPCA_TRY(cudaMalloc(&w.d_nz, sizeof(int)));
-        VPCA_TRY(cudaMalloc(&w.d_st, 8 * sizeof(int)));
+    if (w.d_V.get() == nullptr || w.n != n || w.kmax != kmax) {
+        band_eig_free(w);   // a new geometry: every buffer is allocated afresh
+        VPCA_TRY(w.d_V.ensure((int64_t)n * kLzCap));
+        VPCA_TRY(w.d_w.ensure(2 * (int64_t)n));
+        VPCA_TRY(w.d_small.ensure((int64_t)(kBandSmallFixed + (size_t)kLzCap * kmax + npart)));
+        VPCA_TRY(w.d_slots.ensure(16 * (int64_t)n));
+        VPCA_TRY(w.d_rowsum.ensure(n));
+        VPCA_TRY(w.d_rbar.ensure(n));
+        VPCA_TRY(w.d_scal.ensure(16));
+        VPCA_TRY(w.d_evals.ensure(kmax));
+        VPCA_TRY(w.d_evecs.ensure((int64_t)n * kmax));
+        VPCA_TRY(w.d_lu.ensure(8 * (int64_t)kLzCap));
+        VPCA_TRY(w.d_nz.ensure(1));
+        VPCA_TRY(w.d_st.ensure(8));
         VPCA_TRY(cudaEventCreateWithFlags(&w.ev_v, cudaEventDisableTiming));
-        VPCA_TRY(cudaMemset(w.d_small, 0, (kBandSmallFixed + (size_t)kLzCap * kmax + npart) * sizeof(double)));
+        VPCA_TRY(cudaMemset(w.d_small.get(), 0, (kBandSmallFixed + (size_t)kLzCap * kmax + npart) * sizeof(double)));
+        w.n = n;   // set once the workspace is complete, so that a failed call allocates it again
+        w.kmax = kmax;
     }
     for (int q = 0; q < world; ++q) {
         VPCA_TRY(cudaSetDevice(parts[q]->device));
@@ -2031,7 +2023,7 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     }
     VPCA_TRY(cudaSetDevice(dev0));
     VPCA_TRY(cudaFuncSetAttribute(invit_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    double* alpha = w.d_small;
+    double* alpha = w.d_small.get();
     double* beta = alpha + kLzCap;
     double* h1 = beta + kLzCap;
     double* h2 = h1 + kLzCap;
@@ -2055,16 +2047,16 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
             if ((ce = cudaSetDevice(p.device)) != cudaSuccess) return ce;
             if ((ce = cudaStreamWaitEvent(p.stream, w.ev_v, 0)) != cudaSuccess) return ce;   // rank 0 is done with slot q
             if (v != nullptr &&
-                (ce = cudaMemcpyPeerAsync(p.d_v, p.device, v, dev0, (size_t)n * sizeof(double), p.stream)) != cudaSuccess)
+                (ce = cudaMemcpyPeerAsync(p.d_v.get(), p.device, v, dev0, (size_t)n * sizeof(double), p.stream)) != cudaSuccess)
                 return ce;
-            if ((ce = band_product<T>(p, p.d_v, reinterpret_cast<T*>(p.d_y))) != cudaSuccess) return ce;
-            if ((ce = cudaMemcpyPeerAsync(w.d_slots + (size_t)q * n, dev0, p.d_y, p.device,
+            if ((ce = band_product<T>(p, p.d_v.get(), reinterpret_cast<T*>(p.d_y.get()))) != cudaSuccess) return ce;
+            if ((ce = cudaMemcpyPeerAsync(w.d_slots.get() + (size_t)q * n, dev0, p.d_y.get(), p.device,
                                           (size_t)(p.row0 + p.rows) * sizeof(double), p.stream)) != cudaSuccess) return ce;
             if ((ce = cudaEventRecord(p.ev_done, p.stream)) != cudaSuccess) return ce;
             nl += 2;
         }
         if ((ce = cudaSetDevice(dev0)) != cudaSuccess) return ce;
-        if ((ce = band_product<T>(p0, v, reinterpret_cast<T*>(w.d_slots))) != cudaSuccess) return ce;
+        if ((ce = band_product<T>(p0, v, reinterpret_cast<T*>(w.d_slots.get()))) != cudaSuccess) return ce;
         for (int q = 1; q < world; ++q)
             if ((ce = cudaStreamWaitEvent(s0, parts[q]->ev_done, 0)) != cudaSuccess) return ce;
         nl += 2;
@@ -2074,15 +2066,15 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     // centring, then both Gram-Schmidt passes (lz_dots / lz_update).  No host synchronisation.
     auto step = [&]() -> cudaError_t {
         cudaError_t ce;
-        band_norm_kernel<<<1, 1024, 0, s0>>>(part, npart, w.d_w, w.d_rbar, n, beta, sc, w.d_st);
-        band_scale_kernel<<<(n + 255) / 256, 256, 0, s0>>>(w.d_w, n, sc, w.d_V, p0.d_v, w.d_st);
+        band_norm_kernel<<<1, 1024, 0, s0>>>(part, npart, w.d_w.get(), w.d_rbar.get(), n, beta, sc, w.d_st.get());
+        band_scale_kernel<<<(n + 255) / 256, 256, 0, s0>>>(w.d_w.get(), n, sc, w.d_V.get(), p0.d_v.get(), w.d_st.get());
         if (world > 1 && (ce = cudaEventRecord(w.ev_v, s0)) != cudaSuccess) return ce;
-        if ((ce = gather((double*)nullptr, p0.d_v)) != cudaSuccess) return ce;
-        band_combine_kernel<<<(n + 255) / 256, 256, 0, s0>>>(w.d_slots, n, world, be, w.d_rbar, sc, w.d_scal, w.d_w, w.d_st);
-        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h1, w.d_st);
-        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h1, alpha, part, w.d_st, 1);
-        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h2, w.d_st);
-        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h2, alpha, part, w.d_st, 2);
+        if ((ce = gather((double*)nullptr, p0.d_v.get())) != cudaSuccess) return ce;
+        band_combine_kernel<<<(n + 255) / 256, 256, 0, s0>>>(w.d_slots.get(), n, world, be, w.d_rbar.get(), sc, w.d_scal.get(), w.d_w.get(), w.d_st.get());
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h1, w.d_st.get());
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h1, alpha, part, w.d_st.get(), 1);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h2, w.d_st.get());
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h2, alpha, part, w.d_st.get(), 2);
         nl += 7;
         return cudaGetLastError();
     };
@@ -2090,17 +2082,17 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     // ---- row sums (exact, int64), matrixMean and non_zero_rows (VariantsPca.scala:206-211)
     if (world > 1) VPCA_TRY(cudaEventRecord(w.ev_v, s0));   // the ranks write rank 0's slots after its earlier work
     VPCA_TRY(gather((long long*)nullptr, nullptr));
-    band_rowsum_kernel<<<(n + 255) / 256, 256, 0, s0>>>(reinterpret_cast<const long long*>(w.d_slots), n, world, be,
-                                                         w.d_rowsum, w.d_rbar);
-    matrix_mean_kernel<<<1, 1024, 0, s0>>>(w.d_rowsum, n, w.d_scal, w.d_nz);
+    band_rowsum_kernel<<<(n + 255) / 256, 256, 0, s0>>>(reinterpret_cast<const long long*>(w.d_slots.get()), n, world, be,
+                                                         w.d_rowsum.get(), w.d_rbar.get());
+    matrix_mean_kernel<<<1, 1024, 0, s0>>>(w.d_rowsum.get(), n, w.d_scal.get(), w.d_nz.get());
     nl += 2;
 
     // ---- main run: the convergence policy is that of lanczos_topk's persistent form
     LzPolicy policy(n);
     int hst[8] = {0, 0, 0, policy.max_iter, 0, 0, 0, 0};
     double hres[2] = {0.0, 0.0};
-    VPCA_TRY(cudaMemcpyAsync(w.d_st, hst, sizeof(hst), cudaMemcpyHostToDevice, s0));
-    lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w, n, 0x5eedULL, part);
+    VPCA_TRY(cudaMemcpyAsync(w.d_st.get(), hst, sizeof(hst), cudaMemcpyHostToDevice, s0));
+    lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w.get(), n, 0x5eedULL, part);
     nl += 1;
     int m = 0;
     bool converged = false;
@@ -2109,12 +2101,12 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
         for (int g = 0; g < kLzChunk; ++g) VPCA_TRY(step());
         m = chunk * kLzChunk;
         if (!policy.test_after(chunk, k)) continue;
-        bisect_kernel<<<k, 256, 0, s0>>>(alpha, beta + 1, m, e2, w.d_evals, w.d_scal);
-        invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), s0>>>(alpha, beta + 1, m, k, w.d_evals,
-                                                                                           w.d_scal, w.d_lu, Y);
-        lz_check_kernel<<<1, 32, 0, s0>>>(part, npart, Y, m, k, w.d_scal, w.d_st, res, kLzTol);
+        bisect_kernel<<<k, 256, 0, s0>>>(alpha, beta + 1, m, e2, w.d_evals.get(), w.d_scal.get());
+        invit_kernel<true><<<1, m <= 128 ? 32 : 256, 8 * (size_t)m * sizeof(double), s0>>>(alpha, beta + 1, m, k, w.d_evals.get(),
+                                                                                           w.d_scal.get(), w.d_lu.get(), Y);
+        lz_check_kernel<<<1, 32, 0, s0>>>(part, npart, Y, m, k, w.d_scal.get(), w.d_st.get(), res, kLzTol);
         nl += 3;
-        VPCA_TRY(cudaMemcpyAsync(hst, w.d_st, sizeof(hst), cudaMemcpyDeviceToHost, s0));
+        VPCA_TRY(cudaMemcpyAsync(hst, w.d_st.get(), sizeof(hst), cudaMemcpyDeviceToHost, s0));
         VPCA_TRY(cudaMemcpyAsync(hres, res, sizeof(hres), cudaMemcpyDeviceToHost, s0));
         VPCA_TRY(cudaStreamSynchronize(s0));
         if (hst[1] == 1) {
@@ -2133,26 +2125,26 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
     if (!converged) return cudaGetLastError();
 
     // ---- Ritz vectors, unit norm, sign rule
-    lz_ritz_kernel<<<dim3(npart, k), 256, 0, s0>>>(w.d_V, n, Y, m, w.d_evecs);
-    lz_finish_kernel<<<k, 512, 0, s0>>>(w.d_evecs, n);
+    lz_ritz_kernel<<<dim3(npart, k), 256, 0, s0>>>(w.d_V.get(), n, Y, m, w.d_evecs.get());
+    lz_finish_kernel<<<k, 512, 0, s0>>>(w.d_evecs.get(), n);
     nl += 2;
     // ---- deflated verification run: the k Ritz vectors become the first k basis columns, a
     // fresh start vector is made orthogonal to them and one chunk runs; a Ritz value above theta_k means a missed eigenvalue
     if (k + kLzChunk < n) {
-        VPCA_TRY(cudaMemcpyAsync(w.d_V, w.d_evecs, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice, s0));
+        VPCA_TRY(cudaMemcpyAsync(w.d_V.get(), w.d_evecs.get(), (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice, s0));
         int vst[4] = {k - 1, 0, 0, k + kLzChunk};
-        VPCA_TRY(cudaMemcpyAsync(w.d_st, vst, sizeof(vst), cudaMemcpyHostToDevice, s0));
-        lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w + (size_t)(k & 1) * n, n, 0xfaceULL, part);
-        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h1, w.d_st);
-        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h1, alpha, part, w.d_st, 1);
-        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V, n, w.d_w, h2, w.d_st);
-        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V, n, w.d_w, h2, alpha, part, w.d_st, 2);
+        VPCA_TRY(cudaMemcpyAsync(w.d_st.get(), vst, sizeof(vst), cudaMemcpyHostToDevice, s0));
+        lz_init_kernel<<<npart, 32, 0, s0>>>(w.d_w.get() + (size_t)(k & 1) * n, n, 0xfaceULL, part);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h1, w.d_st.get());
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h1, alpha, part, w.d_st.get(), 1);
+        lz_dots_kernel<<<kLzCap, 128, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h2, w.d_st.get());
+        lz_update_kernel<<<npart, 256, 0, s0>>>(w.d_V.get(), n, w.d_w.get(), h2, alpha, part, w.d_st.get(), 2);
         nl += 5;
         for (int g = 0; g < kLzChunk; ++g) VPCA_TRY(step());
         bisect_kernel<<<1, 256, 0, s0>>>(alpha + k, beta + k + 1, kLzChunk, e2, theta2, scal2);
-        lz_verify_kernel<<<1, 1, 0, s0>>>(w.d_evals, k, theta2, w.d_scal, w.d_st);
+        lz_verify_kernel<<<1, 1, 0, s0>>>(w.d_evals.get(), k, theta2, w.d_scal.get(), w.d_st.get());
         nl += 2;
-        VPCA_TRY(cudaMemcpyAsync(hst, w.d_st, sizeof(hst), cudaMemcpyDeviceToHost, s0));
+        VPCA_TRY(cudaMemcpyAsync(hst, w.d_st.get(), sizeof(hst), cudaMemcpyDeviceToHost, s0));
         VPCA_TRY(cudaStreamSynchronize(s0));
         if (launches) *launches += nl;
         if (hst[1] != 1) {

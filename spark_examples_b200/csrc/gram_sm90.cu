@@ -1130,10 +1130,10 @@ std::map<SplitKey, std::vector<double>> g_splits;
 }  // namespace
 
 static void remember_split(GramPlan& plan) {
-    if (plan.d_cum == nullptr || plan.cum_workers <= 0 || !plan.adaptive) return;
+    if (plan.d_cum.get() == nullptr || plan.cum_workers <= 0 || !plan.adaptive) return;
     if (plan.own_hi > plan.own_lo && plan.num_peers <= 1) return;   // a band's tile list is not the cohort's
     std::vector<double> cum((size_t)plan.cum_workers + 2);   // the split and the front/tail split point
-    if (cudaMemcpy(cum.data(), plan.d_cum, cum.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
+    if (cudaMemcpy(cum.data(), plan.d_cum.get(), cum.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
         cudaGetLastError();
         return;
     }
@@ -1143,24 +1143,16 @@ static void remember_split(GramPlan& plan) {
 
 void gram_plan_free(GramPlan& plan) {
     remember_split(plan);
-    if (plan.d_tiles) cudaFree(plan.d_tiles);
     plan.h_tiles.clear();
     if (plan.d_err) cudaFreeHost(plan.d_err);
-    if (plan.d_win_done) cudaFree(plan.d_win_done);
-    if (plan.d_prof) cudaFree(plan.d_prof);
-    if (plan.d_cum) cudaFree(plan.d_cum);
-    plan.d_cum = nullptr;
-    plan.d_win_done = nullptr;
-    plan.d_prof = nullptr;
-    plan.d_tiles = nullptr;
     plan.d_err = nullptr;
     plan.tiles_for_n = -1;
 }
 
 int gram_read_profile(GramPlan& plan, long long* out, int max_ctas) {
-    if (plan.d_prof == nullptr) return 0;
+    if (plan.d_prof.get() == nullptr) return 0;
     const int ctas = std::min(max_ctas, std::min(1024, plan.num_sms));
-    if (cudaMemcpy(out, plan.d_prof, (size_t)ctas * 4 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
+    if (cudaMemcpy(out, plan.d_prof.get(), (size_t)ctas * 4 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
     return ctas;
 }
 
@@ -1278,11 +1270,10 @@ static cudaError_t build_tiles(GramPlan& plan, int n, bool exact, int BN, int ro
     std::vector<TileDesc> tiles;
     int num_full = 0;
     make_tiles(n, plan.cta_group, exact, BN, row_lo, row_hi, plan.self_b, tiles, &num_full);
-    if (plan.d_tiles) cudaFree(plan.d_tiles);
-    plan.d_tiles = nullptr;
-    cudaError_t e = cudaMalloc(&plan.d_tiles, tiles.size() * sizeof(TileDesc));
+    plan.d_tiles.reset();
+    cudaError_t e = plan.d_tiles.ensure((int64_t)(tiles.size() * sizeof(TileDesc)));
     if (e != cudaSuccess) return e;
-    e = cudaMemcpyAsync(plan.d_tiles, tiles.data(), tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice, stream);
+    e = cudaMemcpyAsync(plan.d_tiles.get(), tiles.data(), tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice, stream);
     if (e != cudaSuccess) return e;
     e = cudaStreamSynchronize(stream);   // `tiles` is a stack vector
     plan.h_tiles.assign(reinterpret_cast<const int32_t*>(tiles.data()),
@@ -1476,14 +1467,11 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
         const char* ex = getenv("VPCA_EXACT_COVER");
         if (ex != nullptr) plan.exact_cover = atoi(ex) != 0;
     }
-    if (plan.d_win_done == nullptr) {
-        cudaError_t e = cudaMalloc(&plan.d_win_done, GramPlan::kMaxWindows * sizeof(int));
+    if (cudaError_t e = plan.d_win_done.ensure(GramPlan::kMaxWindows); e != cudaSuccess) return e;
+    if ((plan.profile || plan.adaptive) && plan.d_prof.get() == nullptr) {
+        cudaError_t e = plan.d_prof.ensure(1024 * 4);
         if (e != cudaSuccess) return e;
-    }
-    if ((plan.profile || plan.adaptive) && plan.d_prof == nullptr) {
-        cudaError_t e = cudaMalloc(&plan.d_prof, 1024 * 4 * sizeof(long long));
-        if (e != cudaSuccess) return e;
-        e = cudaMemsetAsync(plan.d_prof, 0, 1024 * 4 * sizeof(long long), stream);
+        e = cudaMemsetAsync(plan.d_prof.get(), 0, 1024 * 4 * sizeof(long long), stream);
         if (e != cudaSuccess) return e;
     }
     if (plan.d_err == nullptr) {
@@ -1563,7 +1551,7 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
     for (int d = 0; d < kMaxPeers; ++d) args.peer[d] = d < plan.num_peers ? plan.peer_S[d] : nullptr;
     args.peer_mode = plan.peer_mode;
     for (int d = 0; d < kMaxPeers; ++d) args.own_end[d] = plan.own_end[d];
-    args.tiles = static_cast<const TileDesc*>(plan.d_tiles);
+    args.tiles = reinterpret_cast<const TileDesc*>(plan.d_tiles.get());
     cudaHostGetDevicePointer(reinterpret_cast<void**>(&args.err), plan.d_err, 0);
     args.n = n;
     args.num_tiles = plan.num_tiles;
@@ -1603,7 +1591,7 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
         // the device-side split (speed-weighted by rebalance_kernel, or the front/tail split point moved by
         // rebalance_front_kernel, from launch to launch) starts from the repaired equal split / the initial split point;
         // it is only meaningful for one (workers, tile list, window length)
-        if (args.resident && (plan.d_cum == nullptr || plan.cum_workers != workers || plan.cum_tiles != plan.num_tiles ||
+        if (args.resident && (plan.d_cum.get() == nullptr || plan.cum_workers != workers || plan.cum_tiles != plan.num_tiles ||
                               plan.cum_kbw != kbw || plan.cum_for_n != n || plan.cum_elem != elem_bits)) {
             remember_split(plan);
             if (plan.adaptive && !banded) {   // a split learned earlier on this device for the same schedule, if it still fits the accumulator budget
@@ -1624,13 +1612,12 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
                     }
                 }
             }
-            if (plan.d_cum) cudaFree(plan.d_cum);
-            plan.d_cum = nullptr;
-            cudaError_t e = cudaMalloc(&plan.d_cum, (size_t)(workers + 2) * sizeof(double) + sizeof(int));
+            plan.d_cum.reset();
+            cudaError_t e = plan.d_cum.ensure((int64_t)(workers + 2) * sizeof(double) + sizeof(int));
             if (e != cudaSuccess) return e;
             cum0.push_back(frac0);                                 // [workers + 1]: the front/tail split point (fraction of K)
             cum0.push_back(0.0);                                   // [workers + 2]: the update counter (int)
-            e = cudaMemcpyAsync(plan.d_cum, cum0.data(), (size_t)(workers + 2) * sizeof(double) + sizeof(int),
+            e = cudaMemcpyAsync(plan.d_cum.get(), cum0.data(), (size_t)(workers + 2) * sizeof(double) + sizeof(int),
                                 cudaMemcpyHostToDevice, stream);   // pageable source: staged before the call returns
             if (e != cudaSuccess) return e;
             plan.cum_workers = workers;
@@ -1642,21 +1629,22 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
         }
     }
     plan.last_resident = args.resident;
+    double* cum = reinterpret_cast<double*>(plan.d_cum.get());   // the split (see GramPlan::d_cum)
     const int nwin = (args.kb_total + args.kb_window - 1) / args.kb_window;
     const long long uw = (long long)args.total_weight * args.kb_window;
     args.active_workers = (int)std::min<long long>(workers, uw);
     if (front.on) {   // only the front workers take part in the window pacing
         args.front_tiles = plan.num_tiles;
-        args.front_frac = plan.d_cum + workers + 1;
+        args.front_frac = cum + workers + 1;
         args.active_workers = plan.num_tiles;
     }
     args.sync_lead = (args.resident && nwin <= GramPlan::kMaxWindows) ? plan.sync_lead : 0;
-    args.win_done = plan.d_win_done;
+    args.win_done = plan.d_win_done.get();
     const bool adapt = plan.adaptive && args.resident && workers <= 1024 && (front.on || args.active_workers == workers);
-    args.prof = (plan.profile || adapt) ? plan.d_prof : nullptr;
-    args.cum = plan.d_cum;
+    args.prof = (plan.profile || adapt) ? plan.d_prof.get() : nullptr;
+    args.cum = cum;
     if (args.sync_lead > 0) {
-        cudaError_t e = cudaMemsetAsync(plan.d_win_done, 0, (size_t)nwin * sizeof(int), stream);
+        cudaError_t e = cudaMemsetAsync(plan.d_win_done.get(), 0, (size_t)nwin * sizeof(int), stream);
         if (e != cudaSuccess) return e;
     }
 
@@ -1671,14 +1659,14 @@ cudaError_t gram_accumulate(GramPlan& plan, const void* d_x, int elem_bits, int 
     if (le != cudaSuccess) return le;
     if (adapt && front.on) {
         rebalance_front_kernel<<<1, (workers + 31) / 32 * 32, 0, stream>>>(
-            plan.d_prof, plan.d_cum + workers + 1, plan.num_tiles, workers, cgp, args.kb_total, plan.gain, front.lo, front.hi,
-            300000, reinterpret_cast<int*>(plan.d_cum + workers + 2));
+            plan.d_prof.get(), cum + workers + 1, plan.num_tiles, workers, cgp, args.kb_total, plan.gain, front.lo, front.hi,
+            300000, reinterpret_cast<int*>(cum + workers + 2));
         le = cudaGetLastError();
     } else if (adapt) {
         // shares move towards the measured speeds, at most 35 % above the mean; a split under which some worker's
         // accumulators would not fit its budget is rejected by the kernel itself
-        rebalance_kernel<<<1, 1024, 0, stream>>>(plan.d_prof, plan.d_cum, workers, cgp, plan.gain, 1.35, 300000,
-                                                 reinterpret_cast<int*>(plan.d_cum + workers + 2), static_cast<const TileDesc*>(plan.d_tiles), plan.num_tiles,
+        rebalance_kernel<<<1, 1024, 0, stream>>>(plan.d_prof.get(), cum, workers, cgp, plan.gain, 1.35, 300000,
+                                                 reinterpret_cast<int*>(cum + workers + 2), reinterpret_cast<const TileDesc*>(plan.d_tiles.get()), plan.num_tiles,
                                                  plan.total_weight, args.kb_window, plan.tiles_col_limit);
         le = cudaGetLastError();
     }

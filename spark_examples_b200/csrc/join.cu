@@ -17,6 +17,7 @@
 // left row, then right row), so the joined rows are reproducible and equal to the host implementation's.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 
 #include "vpca_internal.h"
@@ -279,41 +280,35 @@ cudaError_t hash_keys(const uint8_t* d_payload, const int64_t* d_off, int64_t nk
 }
 
 void join_free(JoinWork& w) {
-    cudaFree(w.d_hash); cudaFree(w.d_table); cudaFree(w.d_rows); cudaFree(w.d_len); cudaFree(w.d_row_base);
-    cudaFree(w.d_nnz_base); cudaFree(w.d_leader); cudaFree(w.d_prefix); cudaFree(w.d_block); cudaFree(w.d_totals);
-    cudaFree(w.d_out_off); cudaFree(w.d_out_idx);
-    cudaFree(w.d_payload); cudaFree(w.d_key_off); cudaFree(w.d_off); cudaFree(w.d_idx);
     if (w.h_totals) cudaFreeHost(w.h_totals);
     w = JoinWork{};
 }
 
-// Sizes the per-row workspace for `nrows` rows (grow-only).
+// Sizes the per-row workspace for `nrows` rows (grow-only).  d_rows is emptied first and grows last, so its capacity is
+// the rows every buffer holds: after a failed call it is 0 and the next call reserves again.
 static cudaError_t join_reserve(JoinWork& w, int64_t nrows) {
-    if (nrows <= w.cap_rows && w.d_hash != nullptr) return cudaSuccess;
-    const int64_t cap = nrows + nrows / 4 + 1024;
-    cudaFree(w.d_hash); cudaFree(w.d_table); cudaFree(w.d_rows); cudaFree(w.d_len); cudaFree(w.d_row_base);
-    cudaFree(w.d_nnz_base); cudaFree(w.d_leader); cudaFree(w.d_prefix); cudaFree(w.d_block);
-    w.d_hash = nullptr; w.d_table = nullptr; w.d_rows = w.d_len = w.d_row_base = w.d_nnz_base = w.d_prefix = w.d_block = nullptr;
-    w.d_leader = nullptr;
-    w.cap_rows = 0;
+    if (nrows <= w.d_rows.capacity()) return cudaSuccess;
+    const int64_t cap = with_slack(nrows);
     uint64_t slots = 1024;
     while (slots < 2 * (uint64_t)cap) slots <<= 1;
+    w.d_rows.reset();
+    w.d_table.reset();   // the table and the scan scratch are sized for `cap` rows: reallocated whenever the rows grow
+    w.d_block.reset();
     cudaError_t e;
 #define VPCA_TRY(x) if ((e = (x)) != cudaSuccess) return e
-    VPCA_TRY(cudaMalloc(&w.d_hash, (size_t)cap * 16));
-    VPCA_TRY(cudaMalloc(&w.d_table, (size_t)slots * sizeof(int32_t)));
-    VPCA_TRY(cudaMalloc(&w.d_rows, (size_t)cap * 8));
-    VPCA_TRY(cudaMalloc(&w.d_len, (size_t)cap * 8));
-    VPCA_TRY(cudaMalloc(&w.d_row_base, (size_t)cap * 8));
-    VPCA_TRY(cudaMalloc(&w.d_nnz_base, (size_t)cap * 8));
-    VPCA_TRY(cudaMalloc(&w.d_leader, (size_t)cap * 4));
-    VPCA_TRY(cudaMalloc(&w.d_prefix, (size_t)cap * 8));
-    VPCA_TRY(cudaMalloc(&w.d_block, (size_t)((cap + kScanBlock - 1) / kScanBlock + 1) * 8));
-    if (w.d_totals == nullptr) VPCA_TRY(cudaMalloc(&w.d_totals, 2 * sizeof(int64_t)));
-    if (w.h_totals == nullptr) VPCA_TRY(cudaHostAlloc(&w.h_totals, 2 * sizeof(int64_t), cudaHostAllocPortable));
-#undef VPCA_TRY
-    w.cap_rows = cap;
+    VPCA_TRY(w.d_hash.ensure(2 * nrows, 2 * cap));
+    VPCA_TRY(w.d_table.ensure((int64_t)slots));
     w.table_slots = slots;
+    VPCA_TRY(w.d_len.ensure(nrows, cap));
+    VPCA_TRY(w.d_row_base.ensure(nrows, cap));
+    VPCA_TRY(w.d_nnz_base.ensure(nrows, cap));
+    VPCA_TRY(w.d_leader.ensure(nrows, cap));
+    VPCA_TRY(w.d_prefix.ensure(nrows, cap));
+    VPCA_TRY(w.d_block.ensure((cap + kScanBlock - 1) / kScanBlock + 1));
+    VPCA_TRY(w.d_totals.ensure(2));
+    if (w.h_totals == nullptr) VPCA_TRY(cudaHostAlloc(&w.h_totals, 2 * sizeof(int64_t), cudaHostAllocPortable));
+    VPCA_TRY(w.d_rows.ensure(nrows, cap));
+#undef VPCA_TRY
     return cudaSuccess;
 }
 
@@ -329,44 +324,31 @@ cudaError_t join_rows(JoinWork& w, int mode, int variant_set_count, int64_t n_le
     if (nrows > 0) {
         const unsigned gb = (unsigned)((nrows + 255) / 256);
         const uint32_t mask = (uint32_t)(w.table_slots - 1);
-        hash_keys_kernel<<<gb, 256, 0, stream>>>(d_payload, d_key_off, nrows, w.d_hash);
-        fill_i32_kernel<<<1184, 256, 0, stream>>>(w.d_table, (int64_t)w.table_slots, -1);
-        insert_kernel<<<gb, 256, 0, stream>>>(w.d_hash, nrows, w.d_table, mask);
-        analyze_kernel<<<gb, 256, 0, stream>>>(w.d_hash, d_off, nrows, n_left, mode, variant_set_count, w.d_table, mask, w.d_rows,
-                                               w.d_len, w.d_leader, w.d_prefix);
-        if ((e = exclusive_scan(w.d_rows, nrows, w.d_row_base, w.d_block, w.d_totals, stream)) != cudaSuccess) return e;
-        if ((e = exclusive_scan(w.d_len, nrows, w.d_nnz_base, w.d_block, w.d_totals + 1, stream)) != cudaSuccess) return e;
+        hash_keys_kernel<<<gb, 256, 0, stream>>>(d_payload, d_key_off, nrows, w.d_hash.get());
+        fill_i32_kernel<<<1184, 256, 0, stream>>>(w.d_table.get(), (int64_t)w.table_slots, -1);
+        insert_kernel<<<gb, 256, 0, stream>>>(w.d_hash.get(), nrows, w.d_table.get(), mask);
+        analyze_kernel<<<gb, 256, 0, stream>>>(w.d_hash.get(), d_off, nrows, n_left, mode, variant_set_count, w.d_table.get(), mask, w.d_rows.get(),
+                                               w.d_len.get(), w.d_leader.get(), w.d_prefix.get());
+        if ((e = exclusive_scan(w.d_rows.get(), nrows, w.d_row_base.get(), w.d_block.get(), w.d_totals.get(), stream)) != cudaSuccess) return e;
+        if ((e = exclusive_scan(w.d_len.get(), nrows, w.d_nnz_base.get(), w.d_block.get(), w.d_totals.get() + 1, stream)) != cudaSuccess) return e;
         if (launches) *launches += 4 + 6;
-        if ((e = cudaMemcpyAsync(w.h_totals, w.d_totals, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+        if ((e = cudaMemcpyAsync(w.h_totals, w.d_totals.get(), 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
         if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
         *out_rows = w.h_totals[0];
         *out_nnz = w.h_totals[1];
     }
-    if (*out_rows + 1 > w.cap_out_rows) {
-        cudaFree(w.d_out_off);
-        w.d_out_off = nullptr;
-        w.cap_out_rows = 0;
-        const int64_t cap = *out_rows + *out_rows / 4 + 1024;
-        if ((e = cudaMalloc(&w.d_out_off, (size_t)cap * 8)) != cudaSuccess) return e;
-        w.cap_out_rows = cap;
-    }
-    if (*out_nnz > w.cap_out_nnz || w.d_out_idx == nullptr) {
-        cudaFree(w.d_out_idx);
-        w.d_out_idx = nullptr;
-        w.cap_out_nnz = 0;
-        const int64_t cap = *out_nnz + *out_nnz / 4 + 1024;
-        if ((e = cudaMalloc(&w.d_out_idx, (size_t)cap * 4)) != cudaSuccess) return e;
-        w.cap_out_nnz = cap;
-    }
+    if ((e = w.d_out_off.ensure(*out_rows + 1, with_slack(*out_rows))) != cudaSuccess) return e;
+    // never left null, even after a join without calls
+    if ((e = w.d_out_idx.ensure(std::max<int64_t>(*out_nnz, 1), with_slack(*out_nnz))) != cudaSuccess) return e;
     if (nrows > 0) {
         const uint32_t mask = (uint32_t)(w.table_slots - 1);
-        emit_kernel<<<(unsigned)((nrows + 7) / 8), 256, 0, stream>>>(w.d_hash, d_off, d_idx, nrows, n_left, mode, w.d_table, mask,
-                                                                      w.d_row_base, w.d_nnz_base, w.d_leader, w.d_prefix,
-                                                                      w.d_out_off, w.d_out_idx);
-        set_i64_kernel<<<1, 1, 0, stream>>>(w.d_out_off, w.d_totals, w.d_totals + 1);
+        emit_kernel<<<(unsigned)((nrows + 7) / 8), 256, 0, stream>>>(w.d_hash.get(), d_off, d_idx, nrows, n_left, mode, w.d_table.get(), mask,
+                                                                      w.d_row_base.get(), w.d_nnz_base.get(), w.d_leader.get(), w.d_prefix.get(),
+                                                                      w.d_out_off.get(), w.d_out_idx.get());
+        set_i64_kernel<<<1, 1, 0, stream>>>(w.d_out_off.get(), w.d_totals.get(), w.d_totals.get() + 1);
         if (launches) *launches += 2;
     } else {
-        if ((e = cudaMemsetAsync(w.d_out_off, 0, 8, stream)) != cudaSuccess) return e;
+        if ((e = cudaMemsetAsync(w.d_out_off.get(), 0, 8, stream)) != cudaSuccess) return e;
     }
     return cudaGetLastError();
 }

@@ -136,32 +136,20 @@ __global__ void kin_row_scan_kernel(int32_t* __restrict__ seg, int32_t* __restri
 
 }  // namespace
 
-void kin_pair_free(KinPairWork& w) {
-    for (void* p : {(void*)w.d_seg, (void*)w.d_row_total, (void*)w.d_row_start, (void*)w.d_ids, (void*)w.d_counts,
-                    (void*)w.d_kin})
-        cudaFree(p);
-    w = KinPairWork{};
-}
-
 cudaError_t kin_pair_alloc(KinPairWork& w, int n) {
     if (w.n == n) return cudaSuccess;
-    kin_pair_free(w);
+    w = KinPairWork{};   // a new sample count: every buffer is allocated afresh
     const int tiles = (n + kTile - 1) / kTile;
     // a tile row (32 rows b) holds fewer than 32 n pairs: one always fits the scratch
     const int64_t cap = std::max<int64_t>(int64_t(1) << 21, (int64_t)kTile * n);
-    cudaError_t e = cudaMalloc(&w.d_seg, (size_t)n * tiles * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&w.d_row_total, (size_t)n * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&w.d_row_start, (size_t)n * sizeof(int64_t));
-    if (e == cudaSuccess) e = cudaMalloc(&w.d_ids, (size_t)cap * 2 * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&w.d_counts, (size_t)cap * 5 * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&w.d_kin, (size_t)cap * sizeof(double));
-    if (e != cudaSuccess) {
-        kin_pair_free(w);
-        return e;
-    }
-    w.n = n;
-    w.cap = cap;
-    return cudaSuccess;
+    cudaError_t e = w.d_seg.ensure((int64_t)n * tiles);
+    if (e == cudaSuccess) e = w.d_row_total.ensure(n);
+    if (e == cudaSuccess) e = w.d_row_start.ensure(n);
+    if (e == cudaSuccess) e = w.d_ids.ensure(cap * 2);
+    if (e == cudaSuccess) e = w.d_counts.ensure(cap * 5);
+    if (e == cudaSuccess) e = w.d_kin.ensure(cap);
+    if (e == cudaSuccess) w.n = n;
+    return e;
 }
 
 cudaError_t kin_count(KinPairWork& w, const int32_t* d_G, int n, double min_kinship, bool select_all, cudaStream_t stream) {
@@ -169,11 +157,11 @@ cudaError_t kin_count(KinPairWork& w, const int32_t* d_G, int n, double min_kins
     const int64_t num_tiles = (int64_t)tiles * (tiles + 1) / 2;
     PairOut none{};
     kin_pairs_kernel<false><<<(unsigned)num_tiles, kTile * kWarps, 0, stream>>>(d_G, n, tiles, 0, min_kinship,
-                                                                               select_all ? 1 : 0, w.d_seg, none);
+                                                                               select_all ? 1 : 0, w.d_seg.get(), none);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const int threads = 256;
-    kin_row_scan_kernel<<<(unsigned)(((int64_t)n * 32 + threads - 1) / threads), threads, 0, stream>>>(w.d_seg, w.d_row_total,
+    kin_row_scan_kernel<<<(unsigned)(((int64_t)n * 32 + threads - 1) / threads), threads, 0, stream>>>(w.d_seg.get(), w.d_row_total.get(),
                                                                                                       n, tiles);
     return cudaGetLastError();
 }
@@ -183,9 +171,9 @@ cudaError_t kin_emit(KinPairWork& w, const int32_t* d_G, int n, double min_kinsh
     const int tiles = (n + kTile - 1) / kTile;
     const int64_t t0 = (int64_t)bt_lo * (bt_lo + 1) / 2, t1 = (int64_t)bt_hi * (bt_hi + 1) / 2;
     if (t1 <= t0) return cudaSuccess;
-    PairOut out{w.d_ids, w.d_counts, w.d_kin, w.d_row_start, base, end};
+    PairOut out{w.d_ids.get(), w.d_counts.get(), w.d_kin.get(), w.d_row_start.get(), base, end};
     kin_pairs_kernel<true><<<(unsigned)(t1 - t0), kTile * kWarps, 0, stream>>>(d_G, n, tiles, t0, min_kinship,
-                                                                              select_all ? 1 : 0, w.d_seg, out);
+                                                                              select_all ? 1 : 0, w.d_seg.get(), out);
     return cudaGetLastError();
 }
 

@@ -171,33 +171,33 @@ cudaError_t ld_count(LdWork& w, const LdChunk& ch, cudaStream_t stream) {
     PairOut none{};
     const dim3 grid((unsigned)ch.T, (unsigned)(bt_hi - bt_lo));
     if (ch.elig != nullptr)
-        ld_pairs_kernel<false, true><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, nullptr, none);
+        ld_pairs_kernel<false, true><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits.get(), nullptr, none);
     else
-        ld_pairs_kernel<false, false><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, nullptr, none);
+        ld_pairs_kernel<false, false><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits.get(), nullptr, none);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const int rows = (bt_hi - bt_lo) * kTile, threads = 256;
     ld_row_scan_kernel<<<(unsigned)(((int64_t)rows * 32 + threads - 1) / threads), threads, 0, stream>>>(
-        w.d_bits, w.d_seg, w.d_row_total, reinterpret_cast<unsigned long long*>(w.d_total), bt_lo * kTile, rows, ch.T);
+        w.d_bits.get(), w.d_seg.get(), w.d_row_total.get(), reinterpret_cast<unsigned long long*>(w.d_total.get()), bt_lo * kTile, rows, ch.T);
     return cudaGetLastError();
 }
 
 cudaError_t ld_sweep(LdWork& w, const LdChunk& ch, uint8_t* d_keep, cudaStream_t stream) {
     if (ch.elig != nullptr)
-        ld_sweep_kernel<true><<<1, 32, 0, stream>>>(ch, w.d_bits, w.d_row_total, d_keep);
+        ld_sweep_kernel<true><<<1, 32, 0, stream>>>(ch, w.d_bits.get(), w.d_row_total.get(), d_keep);
     else
-        ld_sweep_kernel<false><<<1, 32, 0, stream>>>(ch, w.d_bits, w.d_row_total, d_keep);
+        ld_sweep_kernel<false><<<1, 32, 0, stream>>>(ch, w.d_bits.get(), w.d_row_total.get(), d_keep);
     return cudaGetLastError();
 }
 
 cudaError_t ld_emit(LdWork& w, const LdChunk& ch, int bt_lo, int bt_hi, int64_t base, int64_t end, cudaStream_t stream) {
     if (bt_hi <= bt_lo) return cudaSuccess;
-    PairOut out{w.d_pairs, w.d_r2, w.d_row_start, base, end};
+    PairOut out{w.d_pairs.get(), w.d_r2.get(), w.d_row_start.get(), base, end};
     const dim3 grid((unsigned)ch.T, (unsigned)(bt_hi - bt_lo));
     if (ch.elig != nullptr)
-        ld_pairs_kernel<true, true><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, w.d_seg, out);
+        ld_pairs_kernel<true, true><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits.get(), w.d_seg.get(), out);
     else
-        ld_pairs_kernel<true, false><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits, w.d_seg, out);
+        ld_pairs_kernel<true, false><<<grid, kTile * kWarps, 0, stream>>>(ch, bt_lo, w.d_bits.get(), w.d_seg.get(), out);
     return cudaGetLastError();
 }
 

@@ -42,8 +42,8 @@ struct vpca_ctx {
     int num_pc = 2;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int32_t* d_S = nullptr;
-    bool own_S = false;
+    int32_t* d_S = nullptr;          // the Gram: cfg.d_gram, or owned_S
+    DeviceBuffer<int32_t> owned_S;   // a library-owned Gram, with the barrier flags of the peer-reduce mode after it
     int band_row0 = 0, band_rows = 0;   // rows of the Gram this context stores (band_rows == n: all of them)
     bool finalized = false;
     bool pca_done = false;
@@ -57,55 +57,49 @@ struct vpca_ctx {
     int pca_k = 0;        // k of the last solve whose U / eigenvalues are still valid on the device (0: none)
     const double* d_U = nullptr;     // that U (n x min(pca_k, 16), column-major): eig.d_evecs after vpca_compute_pca;
                                      // band_eig.d_evecs or d_band_U after vpca_compute_pca_bands
-    double* d_band_U = nullptr;      // n x 16: this rank's copy of U from a band solve driven by another context
+    DeviceBuffer<double> d_band_U;   // n x 16: this rank's copy of U from a band solve driven by another context
     // vpca_compute_pca_subset: a solver of its own for the m kept samples (ctx->eig is never touched), their m x m Gram,
     // U scattered to n x 16 with zero rows for the removed samples (d_U points here after a subset solve, which is what
     // makes the loadings apply d_sub_keep), the n x k output, the sample lists and the keep bytes
     EigWork sub_eig;
-    int32_t* d_sub_S = nullptr;
-    int64_t cap_sub_S = 0;
-    double* d_sub_U = nullptr;
-    double* d_sub_vecs = nullptr;    // n x max(num_pc, 16) (the first k columns used)
-    double* d_sub_t = nullptr;       // max(num_pc, 16): sum_j rho_j u_c[j]
-    int32_t* d_sub_idx = nullptr;    // n: kept samples, then removed ones, each in increasing order
-    uint8_t* d_sub_keep = nullptr;   // n: 1 for kept samples
+    DeviceBuffer<int32_t> d_sub_S;
+    DeviceBuffer<double> d_sub_U;
+    DeviceBuffer<double> d_sub_vecs;    // n x max(num_pc, 16) (the first k columns used)
+    DeviceBuffer<double> d_sub_t;       // max(num_pc, 16): sum_j rho_j u_c[j]
+    DeviceBuffer<int32_t> d_sub_idx;    // n: kept samples, then removed ones, each in increasing order
+    DeviceBuffer<uint8_t> d_sub_keep;   // n: 1 for kept samples
     int proj_k = 0;       // k of the projection begun by vpca_project_begin (0: none in progress)
-    double* d_proj_acc = nullptr;    // n x kProjLd partial projection sums (project.cu)
-    double* d_proj_part = nullptr;   // per-panel partial sums of one launch
-    int64_t cap_proj_part = 0;
-    double* d_lp_w = nullptr;        // host-input loadings / projection: one chunk of w (loadings out, projection in)
-    double* d_lp_mean = nullptr;     // and of the means (projection)
-    int32_t* d_lp_count = nullptr;   // and of the carrier counts (loadings)
-    int64_t cap_lp_w = 0, cap_lp_mean = 0, cap_lp_count = 0;
+    DeviceBuffer<double> d_proj_acc;    // n x kProjLd partial projection sums (project.cu)
+    DeviceBuffer<double> d_proj_part;   // per-panel partial sums of one launch
+    DeviceBuffer<double> d_lp_w;        // host-input loadings / projection: one chunk of w (loadings out, projection in)
+    DeviceBuffer<double> d_lp_mean;     // and of the means (projection)
+    DeviceBuffer<int32_t> d_lp_count;   // and of the carrier counts (loadings)
     // kinship (vpca_kinship_bed / _pairs): the 3n x 3n int32 Gram of the indicator planes, allocated on the first call, with
     // a Gram schedule and plane staging of its own (the PCA Gram's tiles and stream-K split are never touched)
-    int32_t* d_kin = nullptr;
+    DeviceBuffer<int32_t> d_kin;
     GramPlan kin_plan;
-    void* d_kin_x[2] = {nullptr, nullptr};
+    DeviceBuffer<uint8_t> d_kin_x[2];
     int64_t kin_chunk = 0, kin_panel = 0;   // rows per staged chunk, variants per panel of the 3n-row plane tile
     int64_t kin_variants = 0;               // rows added since creation / the last vpca_reset
     KinPairWork kin_pairs;
     // LD pruning (vpca_ld_prune_bed): the 3c x 3c plane Gram of one chunk, its plane tile, double-buffered raw rows, the
     // chunk's window starts, the pair scratch and the keep bytes; all grow-only, with a Gram schedule of their own
-    int32_t* d_ld_G = nullptr;
-    void* d_ld_x = nullptr;
-    uint8_t* d_ld_rows[2] = {nullptr, nullptr};
-    int64_t* d_ld_wlo = nullptr;
-    uint8_t* d_ld_keep = nullptr;
-    uint8_t* d_ld_elig = nullptr;    // vpca_ld_prune_bed_masked: the eligible bytes of the call
-    int64_t cap_ld_G = 0, cap_ld_x = 0, cap_ld_rows = 0, cap_ld_wlo = 0, cap_ld_keep = 0, cap_ld_words = 0, cap_ld_elig = 0;
+    DeviceBuffer<int32_t> d_ld_G;
+    DeviceBuffer<uint8_t> d_ld_x;
+    DeviceBuffer<uint8_t> d_ld_rows[2];
+    DeviceBuffer<int64_t> d_ld_wlo;
+    DeviceBuffer<uint8_t> d_ld_keep;
+    DeviceBuffer<uint8_t> d_ld_elig;    // vpca_ld_prune_bed_masked: the eligible bytes of the call
     // variant QC (vpca_variant_qc_bed / vpca_hwe_exact): the raw rows, counts and p-values of one chunk; grow-only
-    uint8_t* d_qc_rows = nullptr;
-    int32_t* d_qc_counts = nullptr;
-    double* d_qc_p = nullptr;
-    int64_t cap_qc_rows = 0, cap_qc_counts = 0, cap_qc_p = 0;
+    DeviceBuffer<uint8_t> d_qc_rows;
+    DeviceBuffer<int32_t> d_qc_counts;
+    DeviceBuffer<double> d_qc_p;
     // sample QC (vpca_sample_missing_bed / vpca_subset_bed_samples): double-buffered raw and repacked rows of one chunk, the
     // per-sample counts, the kept indices, and a stream and events of their own for the D2H copies; grow-only
-    uint8_t* d_sm_rows[2] = {nullptr, nullptr};
-    uint8_t* d_sm_out[2] = {nullptr, nullptr};
-    int32_t* d_sm_miss = nullptr;
-    int32_t* d_sm_idx = nullptr;
-    int64_t cap_sm_rows[2] = {0, 0}, cap_sm_out[2] = {0, 0}, cap_sm_miss = 0, cap_sm_idx = 0;
+    DeviceBuffer<uint8_t> d_sm_rows[2];
+    DeviceBuffer<uint8_t> d_sm_out[2];
+    DeviceBuffer<int32_t> d_sm_miss;
+    DeviceBuffer<int32_t> d_sm_idx;
     cudaStream_t sm_d2h_stream = nullptr;
     cudaEvent_t sm_ev_copy[2] = {nullptr, nullptr}, sm_ev_kern[2] = {nullptr, nullptr};
     GramPlan ld_plan;
@@ -113,7 +107,7 @@ struct vpca_ctx {
 
     struct Slot {
         int64_t pid = -1;
-        int32_t* d_S = nullptr;
+        DeviceBuffer<int32_t> d_S;
         bool used = false;
         bool busy = false;             // a call of the owning task is in flight
         bool fresh = false;            // still to be zeroed by its first batch
@@ -127,13 +121,13 @@ struct vpca_ctx {
     // a running kernel, so they are per stream).
     struct Lane {
         cudaStream_t stream = nullptr, copy_stream = nullptr;
-        int64_t* d_off[2] = {nullptr, nullptr};
-        int32_t* d_idx[2] = {nullptr, nullptr};
-        void* d_x[2] = {nullptr, nullptr};
+        DeviceBuffer<int64_t> d_off[2];
+        DeviceBuffer<int32_t> d_idx[2];
+        DeviceBuffer<uint8_t> d_x[2];
         cudaEvent_t ev_copy[2] = {nullptr, nullptr};
         cudaEvent_t ev_done[2] = {nullptr, nullptr};
         cudaEvent_t ev_order = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
-        int* d_flags = nullptr;
+        DeviceBuffer<int> d_flags;
         int* h_flags = nullptr;
         GramPlan plan;
         bool ready = false, busy = false;
@@ -196,14 +190,8 @@ void free_lane(vpca_ctx::Lane& L) {
     if (L.stream) cudaStreamSynchronize(L.stream);
     if (L.copy_stream) cudaStreamSynchronize(L.copy_stream);
     for (int b = 0; b < 2; ++b) {
-        cudaFree(L.d_off[b]);
-        cudaFree(L.d_idx[b]);
-        cudaFree(L.d_x[b]);
         if (L.ev_copy[b]) cudaEventDestroy(L.ev_copy[b]);
         if (L.ev_done[b]) cudaEventDestroy(L.ev_done[b]);
-        L.d_off[b] = nullptr;
-        L.d_idx[b] = nullptr;
-        L.d_x[b] = nullptr;
         L.ev_copy[b] = L.ev_done[b] = nullptr;
     }
     for (cudaEvent_t* ev : {&L.ev_order, &L.ev_t0, &L.ev_t1})
@@ -211,8 +199,6 @@ void free_lane(vpca_ctx::Lane& L) {
             cudaEventDestroy(*ev);
             *ev = nullptr;
         }
-    cudaFree(L.d_flags);
-    L.d_flags = nullptr;
     if (L.h_flags) cudaFreeHost(L.h_flags);
     L.h_flags = nullptr;
     gram_plan_free(L.plan);
@@ -259,8 +245,8 @@ void staging_geometry(vpca_ctx* ctx) {
     ctx->chunk_nnz = cz;
 }
 
-// Allocates the lane's streams and staging buffers on first use; on any failure everything is released again, so a
-// later call retries from scratch instead of running on half a lane.
+// Allocates the lane's streams and staging buffers on first use; on any failure the streams and events are released
+// again, so a later call retries instead of running on half a lane.
 int ensure_lane(vpca_ctx* ctx, vpca_ctx::Lane& L) {
     if (L.ready) return VPCA_OK;
     const int n = ctx->n, bits = ctx->elem_bits;
@@ -268,16 +254,16 @@ int ensure_lane(vpca_ctx* ctx, vpca_ctx::Lane& L) {
     cudaError_t e = cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&L.copy_stream, cudaStreamNonBlocking);
     for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-        e = cudaMalloc(&L.d_off[b], (size_t)(cv + 1) * sizeof(int64_t));
-        if (e == cudaSuccess) e = cudaMalloc(&L.d_idx[b], (size_t)cz * sizeof(int32_t));
-        if (e == cudaSuccess) e = cudaMalloc(&L.d_x[b], (size_t)n * (size_t)cv * bits / 8);
+        e = L.d_off[b].ensure(cv + 1);
+        if (e == cudaSuccess) e = L.d_idx[b].ensure(cz);
+        if (e == cudaSuccess) e = L.d_x[b].ensure((int64_t)n * cv * bits / 8);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&L.ev_copy[b], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&L.ev_done[b], cudaEventDisableTiming);
     }
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&L.ev_order, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreate(&L.ev_t0);
     if (e == cudaSuccess) e = cudaEventCreate(&L.ev_t1);
-    if (e == cudaSuccess) e = cudaMalloc(&L.d_flags, sizeof(int));
+    if (e == cudaSuccess) e = L.d_flags.ensure(1);
     if (e == cudaSuccess) e = cudaHostAlloc(&L.h_flags, sizeof(int), cudaHostAllocPortable);
     if (e != cudaSuccess) {
         free_lane(L);
@@ -365,15 +351,11 @@ vpca_ctx::Slot* find_slot(vpca_ctx* ctx, int64_t pid, bool create, int* rc) {
     if (!create) return nullptr;
     for (auto& s : ctx->slots)
         if (!s.used) {
-            if (s.d_S == nullptr) {
-                cudaError_t e = cudaMalloc(&s.d_S, (size_t)ctx->n * ctx->n * sizeof(int32_t));
-                if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.ev_free, cudaEventDisableTiming);
-                if (e != cudaSuccess) {
-                    cudaFree(s.d_S);
-                    s.d_S = nullptr;
-                    *rc = fail(ctx, VPCA_ERR_NOMEM, "cudaMalloc of a partition Gram failed: %s", cudaGetErrorString(e));
-                    return nullptr;
-                }
+            cudaError_t e = s.d_S.ensure((int64_t)ctx->n * ctx->n);
+            if (e == cudaSuccess && s.ev_free == nullptr) e = cudaEventCreateWithFlags(&s.ev_free, cudaEventDisableTiming);
+            if (e != cudaSuccess) {
+                *rc = fail(ctx, VPCA_ERR_NOMEM, "cudaMalloc of a partition Gram failed: %s", cudaGetErrorString(e));
+                return nullptr;
             }
             s.used = true;
             s.fresh = true;
@@ -412,7 +394,7 @@ struct CallScope {
             slot->busy = true;
             fresh = slot->fresh;
             slot->fresh = false;
-            target = slot->d_S;
+            target = slot->d_S.get();
             ctx->inflight_variants += nv;   // reserved now, so that concurrent tasks cannot jointly pass the bound
         } else if (ctx->band_rows != ctx->n) {
             return fail(ctx, VPCA_ERR_STATE, "a band-only Gram takes device-resident input (vpca_accumulate_panels / "
@@ -447,7 +429,7 @@ struct CallScope {
 int prepare_slot(vpca_ctx* ctx, vpca_ctx::Lane& L, CallScope& sc) {
     if (sc.slot == nullptr || !sc.fresh) return VPCA_OK;
     CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, sc.slot->ev_free, 0));
-    CUDA_OK(ctx, cudaMemsetAsync(sc.slot->d_S, 0, (size_t)ctx->n * ctx->n * sizeof(int32_t), L.stream));
+    CUDA_OK(ctx, cudaMemsetAsync(sc.slot->d_S.get(), 0, (size_t)ctx->n * ctx->n * sizeof(int32_t), L.stream));
     return VPCA_OK;
 }
 
@@ -475,7 +457,7 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
     for (int64_t q = 0; q < nv; ++q)
         if (offsets[q + 1] < offsets[q]) return fail(ctx, VPCA_ERR_BAD_ARG, "offsets must be non-decreasing (row %lld)", (long long)q);
     *L.h_flags = 0;
-    CUDA_OK(ctx, cudaMemsetAsync(L.d_flags, 0, sizeof(int), L.stream));
+    CUDA_OK(ctx, cudaMemsetAsync(L.d_flags.get(), 0, sizeof(int), L.stream));
     int64_t v = 0;
     int chunk = 0;
     while (v < nv) {
@@ -496,17 +478,17 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
         const int b = chunk & 1;
         // the copy stream may overwrite buffer b only after the kernels that read it have run
         CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-        CUDA_OK(ctx, cudaMemcpyAsync(L.d_off[b], offsets + v, (size_t)(nvc + 1) * sizeof(int64_t), cudaMemcpyHostToDevice,
+        CUDA_OK(ctx, cudaMemcpyAsync(L.d_off[b].get(), offsets + v, (size_t)(nvc + 1) * sizeof(int64_t), cudaMemcpyHostToDevice,
                                      L.copy_stream));
         if (nnz > 0)
-            CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b], static_cast<const char*>(sample_idx) + (size_t)offsets[v] * idx_bytes,
+            CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b].get(), static_cast<const char*>(sample_idx) + (size_t)offsets[v] * idx_bytes,
                                          (size_t)nnz * idx_bytes, cudaMemcpyHostToDevice, L.copy_stream));
         CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
         ctx->c_h2d += (nvc + 1) * 8 + nnz * idx_bytes;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
         const int64_t P = ctx->panel;
-        CUDA_OK(ctx, encode_calls(L.d_off[b], offsets[v], L.d_idx[b], idx_bytes, nvc, ctx->n, bits, ctx->max_mult, L.d_x[b], P, P,
-                                  L.d_flags, L.stream));
+        CUDA_OK(ctx, encode_calls(L.d_off[b].get(), offsets[v], L.d_idx[b].get(), idx_bytes, nvc, ctx->n, bits, ctx->max_mult, L.d_x[b].get(), P, P,
+                                  L.d_flags.get(), L.stream));
         ctx->c_launches += 2;
         int rc = consume(L, b, v, nvc);
         if (rc != VPCA_OK) return rc;
@@ -514,7 +496,7 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
         v = vend;
         ++chunk;
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, L.d_flags, sizeof(int), cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, L.d_flags.get(), sizeof(int), cudaMemcpyDeviceToHost, L.stream));
     // the caller's buffers are read asynchronously: do not return before every copy has completed
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     if (gram && nv > 0) lane_gram_time(ctx, L);
@@ -544,13 +526,13 @@ int process_packed(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* bits, int64_
         const int64_t nvc = std::min(step, nv - v);
         const int b = chunk & 1;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b], bits + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
+        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b].get(), bits + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
                                      cudaMemcpyHostToDevice, L.copy_stream));
         CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
         ctx->c_h2d += nvc * stride_bytes;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, encode_bits(reinterpret_cast<const uint8_t*>(L.d_idx[b]), stride_bytes, nvc, ctx->n, ctx->elem_bits,
-                                 L.d_x[b], P, P, code, L.stream));
+        CUDA_OK(ctx, encode_bits(reinterpret_cast<const uint8_t*>(L.d_idx[b].get()), stride_bytes, nvc, ctx->n, ctx->elem_bits,
+                                 L.d_x[b].get(), P, P, code, L.stream));
         ctx->c_launches += 1;
         int r = consume(L, b, v, nvc);
         if (r != VPCA_OK) return r;
@@ -558,18 +540,6 @@ int process_packed(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* bits, int64_
     }
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     return VPCA_OK;
-}
-
-template <typename T>
-static cudaError_t grow_buffer(T** p, int64_t* cap, int64_t need) {
-    if (need <= *cap && *p != nullptr) return cudaSuccess;
-    cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    const int64_t c = need + need / 4 + 1024;
-    cudaError_t e = cudaMalloc(p, (size_t)c * sizeof(T));
-    if (e == cudaSuccess) *cap = c;
-    return e;
 }
 
 }  // namespace
@@ -650,8 +620,8 @@ int vpca_create(const vpca_config* cfg, vpca_ctx** out) {
         if (cfg->d_gram != nullptr) {
             ctx->d_S = static_cast<int32_t*>(cfg->d_gram);
         } else {
-            e = cudaMalloc(&ctx->d_S, (gram_cells + 64) * sizeof(int32_t));   // + barrier flags of the peer-reduce mode
-            ctx->own_S = true;
+            e = ctx->owned_S.ensure((int64_t)gram_cells + 64);   // + barrier flags of the peer-reduce mode
+            ctx->d_S = ctx->owned_S.get();
             if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_S + gram_cells, 0, 64 * sizeof(int32_t), ctx->stream);
         }
     }
@@ -678,34 +648,17 @@ int vpca_destroy(vpca_ctx* ctx) {
     cudaSetDevice(ctx->cfg.device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (auto& L : ctx->lanes) free_lane(L);
-    for (auto& s : ctx->slots) {
-        cudaFree(s.d_S);
+    for (auto& s : ctx->slots)
         if (s.ev_free) cudaEventDestroy(s.ev_free);
-    }
     if (ctx->plan.peers_ipc)
         for (int d = 0; d < ctx->plan.num_peers; ++d)
             if (d != ctx->plan.peer_rank && ctx->plan.peer_S[d] != nullptr) cudaIpcCloseMemHandle(ctx->plan.peer_base[d]);
-    if (ctx->own_S) cudaFree(ctx->d_S);
     if (ctx->eig_ready) eig_free(ctx->eig);
     band_eig_free(ctx->band_eig);
     band_part_free(ctx->band_part);
-    for (void* p : {(void*)ctx->d_proj_acc, (void*)ctx->d_proj_part, (void*)ctx->d_lp_w, (void*)ctx->d_lp_mean,
-                    (void*)ctx->d_lp_count, (void*)ctx->d_band_U, (void*)ctx->d_sub_S, (void*)ctx->d_sub_U,
-                    (void*)ctx->d_sub_vecs, (void*)ctx->d_sub_t, (void*)ctx->d_sub_idx, (void*)ctx->d_sub_keep})
-        cudaFree(p);
     if (ctx->sub_eig.n != 0) eig_free(ctx->sub_eig);
     join_free(ctx->join);
-    cudaFree(ctx->d_kin);
-    for (void* p : ctx->d_kin_x) cudaFree(p);
     gram_plan_free(ctx->kin_plan);
-    kin_pair_free(ctx->kin_pairs);
-    for (void* p : {(void*)ctx->d_ld_G, ctx->d_ld_x, (void*)ctx->d_ld_rows[0], (void*)ctx->d_ld_rows[1], (void*)ctx->d_ld_wlo,
-                    (void*)ctx->d_ld_keep, (void*)ctx->ld.d_bits, (void*)ctx->ld.d_seg, (void*)ctx->ld.d_row_total,
-                    (void*)ctx->ld.d_row_start, (void*)ctx->ld.d_total, (void*)ctx->ld.d_pairs, (void*)ctx->ld.d_r2,
-                    (void*)ctx->d_ld_elig, (void*)ctx->d_qc_rows, (void*)ctx->d_qc_counts, (void*)ctx->d_qc_p,
-                    (void*)ctx->d_sm_rows[0], (void*)ctx->d_sm_rows[1], (void*)ctx->d_sm_out[0], (void*)ctx->d_sm_out[1],
-                    (void*)ctx->d_sm_miss, (void*)ctx->d_sm_idx})
-        cudaFree(p);
     for (cudaEvent_t ev : {ctx->sm_ev_copy[0], ctx->sm_ev_copy[1], ctx->sm_ev_kern[0], ctx->sm_ev_kern[1]})
         if (ev) cudaEventDestroy(ev);
     if (ctx->sm_d2h_stream) cudaStreamDestroy(ctx->sm_d2h_stream);
@@ -714,7 +667,7 @@ int vpca_destroy(vpca_ctx* ctx) {
     for (cudaEvent_t ev : {ctx->ev_t0, ctx->ev_t1, ctx->ev_e0, ctx->ev_e1})
         if (ev) cudaEventDestroy(ev);
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;   // frees every device buffer, on the device selected above
     return VPCA_OK;
 }
 
@@ -733,8 +686,8 @@ int vpca_reset(vpca_ctx* ctx) {
         if (L.busy) return fail(ctx, VPCA_ERR_STATE, "vpca_reset while an accumulate call is in flight");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     CUDA_OK(ctx, cudaMemsetAsync(ctx->d_S, 0, (size_t)ctx->band_rows * ctx->n * sizeof(int32_t), ctx->stream));
-    if (ctx->d_kin != nullptr)
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin, 0, (size_t)9 * ctx->n * ctx->n * sizeof(int32_t), ctx->stream));
+    if (ctx->d_kin.get() != nullptr)
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin.get(), 0, (size_t)9 * ctx->n * ctx->n * sizeof(int32_t), ctx->stream));
     ctx->kin_variants = 0;
     for (auto& s : ctx->slots) s.used = false;
     ctx->finalized = false;
@@ -765,7 +718,7 @@ int vpca_encode_calls(vpca_ctx* ctx, const int64_t* offsets, const int32_t* samp
         for (int64_t pv = 0; pv < nvc; pv += P) {
             const int64_t wv = std::min(P, nvc - pv);
             CUDA_OK(ctx, cudaMemcpy2DAsync(static_cast<char*>(out) + (size_t)(v + pv) * bits / 8, (size_t)ld * bits / 8,
-                                           static_cast<const char*>(L.d_x[b]) + (size_t)(pv / P) * ctx->n * P * bits / 8,
+                                           L.d_x[b].get() + (size_t)(pv / P) * ctx->n * P * bits / 8,
                                            (size_t)P * bits / 8, (size_t)(wv * bits + 7) / 8, (size_t)ctx->n,
                                            cudaMemcpyDeviceToHost, L.stream));
         }
@@ -794,7 +747,7 @@ static int accumulate_calls_impl(vpca_ctx* ctx, int64_t partition_id, const int6
         rc = lg.rc;
         if (rc == VPCA_OK) rc = prepare_slot(ctx, *lg.lane, sc);
         auto gram = [&](vpca_ctx::Lane& L, int b, int64_t, int64_t nvc) -> int {
-            return launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b], nvc, ctx->panel, ctx->panel, sc.target);
+            return launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b].get(), nvc, ctx->panel, ctx->panel, sc.target);
         };
         if (rc == VPCA_OK) rc = process_calls(ctx, *lg.lane, offsets, sample_idx, idx_bytes, nv, gram, true);
     }
@@ -832,7 +785,7 @@ static int accumulate_packed(vpca_ctx* ctx, int64_t partition_id, const uint8_t*
         int r = prepare_slot(ctx, L, sc);
         if (r != VPCA_OK) return r;
         auto gram = [&](vpca_ctx::Lane& L2, int b, int64_t, int64_t nvc) -> int {
-            return launch_gram(ctx, L2.plan, L2.stream, L2.ev_t0, L2.ev_t1, L2.d_x[b], nvc, ctx->panel, ctx->panel, sc.target);
+            return launch_gram(ctx, L2.plan, L2.stream, L2.ev_t0, L2.ev_t1, L2.d_x[b].get(), nvc, ctx->panel, ctx->panel, sc.target);
         };
         r = process_packed(ctx, L, bits, nv, stride_bytes, code, gram);
         if (r != VPCA_OK) return r;
@@ -870,22 +823,20 @@ int vpca_hash_keys(vpca_ctx* ctx, const uint8_t* payload, const int64_t* key_off
     const int64_t bytes = key_offsets[nkeys] - key_offsets[0];
     if (bytes > 0 && payload == nullptr) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_hash_keys: payload is NULL");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    uint8_t* d_pay = nullptr;
-    int64_t* d_koff = nullptr;
-    uint64_t* d_out = nullptr;
-    cudaError_t e = cudaMalloc(&d_pay, (size_t)bytes + 16);
-    if (e == cudaSuccess) e = cudaMalloc(&d_koff, (size_t)(nkeys + 1) * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&d_out, (size_t)nkeys * 16);
+    DeviceBuffer<uint8_t> d_pay;
+    DeviceBuffer<int64_t> d_koff;
+    DeviceBuffer<uint64_t> d_out;
+    cudaError_t e = d_pay.ensure(bytes + 16);
+    if (e == cudaSuccess) e = d_koff.ensure(nkeys + 1);
+    if (e == cudaSuccess) e = d_out.ensure(2 * nkeys);
     if (e == cudaSuccess && bytes > 0)
-        e = cudaMemcpyAsync(d_pay, payload + key_offsets[0], (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_koff, key_offsets, (size_t)(nkeys + 1) * 8, cudaMemcpyHostToDevice, ctx->stream);
+        e = cudaMemcpyAsync(d_pay.get(), payload + key_offsets[0], (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(d_koff.get(), key_offsets, (size_t)(nkeys + 1) * 8, cudaMemcpyHostToDevice, ctx->stream);
     // the device copy starts at the first key: shift the base pointer instead of rebasing the offsets
-    if (e == cudaSuccess) e = hash_keys(d_pay - key_offsets[0], d_koff, nkeys, d_out, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, (size_t)nkeys * 16, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = hash_keys(d_pay.get() - key_offsets[0], d_koff.get(), nkeys, d_out.get(), ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out.get(), (size_t)nkeys * 16, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_pay);
-    cudaFree(d_koff);
-    cudaFree(d_out);
     if (e != cudaSuccess) return fail(ctx, VPCA_ERR_CUDA, "vpca_hash_keys: %s", cudaGetErrorString(e));
     ctx->c_launches += 1;
     ctx->c_h2d += bytes + (nkeys + 1) * 8;
@@ -915,29 +866,21 @@ int vpca_join_rows(vpca_ctx* ctx, int32_t mode, int32_t variant_set_count, int64
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     JoinWork& w = ctx->join;
     w.out_rows = -1;
-    CUDA_OK(ctx, grow_buffer(&w.d_payload, &w.cap_payload, kbytes + 16));
-    if (nrows + 1 > w.cap_in_rows || w.d_key_off == nullptr || w.d_off == nullptr) {
-        cudaFree(w.d_key_off);
-        cudaFree(w.d_off);
-        w.d_key_off = w.d_off = nullptr;
-        w.cap_in_rows = 0;
-        const int64_t c = nrows + nrows / 4 + 1024;
-        CUDA_OK(ctx, cudaMalloc(&w.d_key_off, (size_t)c * 8));
-        CUDA_OK(ctx, cudaMalloc(&w.d_off, (size_t)c * 8));
-        w.cap_in_rows = c;
-    }
-    CUDA_OK(ctx, grow_buffer(&w.d_idx, &w.cap_in_nnz, nnz + 1));
+    CUDA_OK(ctx, w.d_payload.ensure(kbytes + 16, with_slack(kbytes + 16)));
+    CUDA_OK(ctx, w.d_key_off.ensure(nrows + 1, with_slack(nrows)));
+    CUDA_OK(ctx, w.d_off.ensure(nrows + 1, with_slack(nrows)));
+    CUDA_OK(ctx, w.d_idx.ensure(nnz + 1, with_slack(nnz + 1)));
     if (kbytes > 0)
-        CUDA_OK(ctx, cudaMemcpyAsync(w.d_payload, key_payload + key_offsets[0], (size_t)kbytes, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(w.d_key_off, key_offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(w.d_off, offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(w.d_payload.get(), key_payload + key_offsets[0], (size_t)kbytes, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(w.d_key_off.get(), key_offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(w.d_off.get(), offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
     if (nnz > 0)
-        CUDA_OK(ctx, cudaMemcpyAsync(w.d_idx, sample_idx + offsets[0], (size_t)nnz * 4, cudaMemcpyHostToDevice, ctx->stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(w.d_idx.get(), sample_idx + offsets[0], (size_t)nnz * 4, cudaMemcpyHostToDevice, ctx->stream));
     ctx->c_h2d += kbytes + 2 * (nrows + 1) * 8 + nnz * 4;
     int64_t launches = 0, rows = 0, calls = 0;
     // the device copies start at the first key / first call: shift the base pointers instead of rebasing the offsets
-    cudaError_t e = join_rows(w, mode, variant_set_count, n_left, w.d_payload - key_offsets[0], w.d_key_off, w.d_off,
-                              w.d_idx - offsets[0], nrows, ctx->stream, &rows, &calls, &launches);
+    cudaError_t e = join_rows(w, mode, variant_set_count, n_left, w.d_payload.get() - key_offsets[0], w.d_key_off.get(), w.d_off.get(),
+                              w.d_idx.get() - offsets[0], nrows, ctx->stream, &rows, &calls, &launches);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);   // the caller's buffers were read asynchronously
     ctx->c_launches += launches;
     if (e != cudaSuccess)
@@ -956,9 +899,9 @@ int vpca_join_fetch(vpca_ctx* ctx, int64_t* out_offsets, int32_t* out_idx) {
     if (w.out_rows < 0) return fail(ctx, VPCA_ERR_STATE, "no joined rows: call vpca_join_rows first");
     if (w.out_nnz > 0 && out_idx == nullptr) return fail(ctx, VPCA_ERR_BAD_ARG, "out_idx is NULL");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    CUDA_OK(ctx, cudaMemcpyAsync(out_offsets, w.d_out_off, (size_t)(w.out_rows + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(out_offsets, w.d_out_off.get(), (size_t)(w.out_rows + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     if (w.out_nnz > 0)
-        CUDA_OK(ctx, cudaMemcpyAsync(out_idx, w.d_out_idx, (size_t)w.out_nnz * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_idx, w.d_out_idx.get(), (size_t)w.out_nnz * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->c_d2h += (w.out_rows + 1) * 8 + w.out_nnz * 4;
     return VPCA_OK;
@@ -992,20 +935,20 @@ int vpca_accumulate_joined(vpca_ctx* ctx, int64_t partition_id) {
         int r = prepare_slot(ctx, L, sc);
         if (r != VPCA_OK) return r;
         *L.h_flags = 0;
-        CUDA_OK(ctx, cudaMemsetAsync(L.d_flags, 0, sizeof(int), L.stream));
+        CUDA_OK(ctx, cudaMemsetAsync(L.d_flags.get(), 0, sizeof(int), L.stream));
         const int64_t P = ctx->panel;
         int chunk = 0;
         for (int64_t v = 0; v < nv; v += ctx->chunk_variants, ++chunk) {
             const int64_t nvc = std::min(ctx->chunk_variants, nv - v);
             const int b = chunk & 1;
             // the joined CSR is device-resident: rows [v, v + nvc) are encoded straight from it (absolute offsets, base 0)
-            CUDA_OK(ctx, encode_calls(w.d_out_off + v, 0, w.d_out_idx, 4, nvc, ctx->n, ctx->elem_bits, ctx->max_mult, L.d_x[b],
-                                      P, P, L.d_flags, L.stream));
+            CUDA_OK(ctx, encode_calls(w.d_out_off.get() + v, 0, w.d_out_idx.get(), 4, nvc, ctx->n, ctx->elem_bits, ctx->max_mult, L.d_x[b].get(),
+                                      P, P, L.d_flags.get(), L.stream));
             ctx->c_launches += 2;
-            r = launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b], nvc, P, P, sc.target);
+            r = launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b].get(), nvc, P, P, sc.target);
             if (r != VPCA_OK) return r;
         }
-        CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, L.d_flags, sizeof(int), cudaMemcpyDeviceToHost, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, L.d_flags.get(), sizeof(int), cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
         lane_gram_time(ctx, L);
         if (*L.h_flags & 1)
@@ -1037,11 +980,11 @@ int vpca_commit(vpca_ctx* ctx, int64_t partition_id) {
     if (s->nv > 0) {
         // every accumulate call of the partition synchronised its lane before returning: the staging Gram is complete
         if (ctx->plan.num_peers > 1 && ctx->plan.peer_mode == 1)
-            CUDA_OK(ctx, gram_add_owners(ctx->plan, s->d_S, ctx->n, ctx->stream));
+            CUDA_OK(ctx, gram_add_owners(ctx->plan, s->d_S.get(), ctx->n, ctx->stream));
         else if (ctx->plan.num_peers > 1)
-            CUDA_OK(ctx, gram_add_peers(ctx->plan, s->d_S, (int64_t)ctx->n * ctx->n, ctx->stream));
+            CUDA_OK(ctx, gram_add_peers(ctx->plan, s->d_S.get(), (int64_t)ctx->n * ctx->n, ctx->stream));
         else   // an owner-computes band staged only its own rows, at the band Gram's own offsets
-            CUDA_OK(ctx, gram_add(ctx->d_S, s->d_S, (int64_t)ctx->band_rows * ctx->n, ctx->stream));
+            CUDA_OK(ctx, gram_add(ctx->d_S, s->d_S.get(), (int64_t)ctx->band_rows * ctx->n, ctx->stream));
         CUDA_OK(ctx, cudaEventRecord(s->ev_free, ctx->stream));
         ctx->c_launches += 1;
     }
@@ -1104,11 +1047,11 @@ int vpca_accumulate_dense(vpca_ctx* ctx, const void* x, int64_t nv, int64_t ld, 
             // the caller's row-major tile -> panel layout, one 2-D copy per panel; a partial last panel is zeroed first
             const int64_t P = ctx->panel;
             if ((nvc % P) != 0)
-                CUDA_OK(ctx, cudaMemsetAsync(static_cast<char*>(L.d_x[b]) + (size_t)(nvc / P) * ctx->n * P * bits / 8, 0,
+                CUDA_OK(ctx, cudaMemsetAsync(L.d_x[b].get() + (size_t)(nvc / P) * ctx->n * P * bits / 8, 0,
                                              (size_t)ctx->n * P * bits / 8, L.copy_stream));
             for (int64_t pv = 0; pv < nvc; pv += P) {
                 const int64_t wv = std::min(P, nvc - pv);
-                CUDA_OK(ctx, cudaMemcpy2DAsync(static_cast<char*>(L.d_x[b]) + (size_t)(pv / P) * ctx->n * P * bits / 8,
+                CUDA_OK(ctx, cudaMemcpy2DAsync(L.d_x[b].get() + (size_t)(pv / P) * ctx->n * P * bits / 8,
                                                (size_t)P * bits / 8, static_cast<const char*>(x) + (size_t)(v + pv) * bits / 8,
                                                (size_t)ld * bits / 8, (size_t)(wv * bits + 7) / 8, (size_t)ctx->n,
                                                cudaMemcpyHostToDevice, L.copy_stream));
@@ -1116,7 +1059,7 @@ int vpca_accumulate_dense(vpca_ctx* ctx, const void* x, int64_t nv, int64_t ld, 
             CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
             ctx->c_h2d += (nvc * bits + 7) / 8 * (int64_t)ctx->n;
             CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-            int r = launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b], nvc, P, P, ctx->d_S);
+            int r = launch_gram(ctx, L.plan, L.stream, L.ev_t0, L.ev_t1, L.d_x[b].get(), nvc, P, P, ctx->d_S);
             if (r != VPCA_OK) return r;
             CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
         }
@@ -1282,10 +1225,7 @@ int64_t vpca_variant_count(vpca_ctx* ctx) {
 static int run_center(vpca_ctx* ctx, bool materialise) {
     if (!ctx->eig_ready) {
         cudaError_t e = eig_alloc(ctx->eig, ctx->n, std::max(ctx->num_pc, 16));
-        if (e != cudaSuccess) {
-            eig_free(ctx->eig);
-            return fail(ctx, VPCA_ERR_NOMEM, "eigensolver workspace: %s", cudaGetErrorString(e));
-        }
+        if (e != cudaSuccess) return fail(ctx, VPCA_ERR_NOMEM, "eigensolver workspace: %s", cudaGetErrorString(e));
         ctx->eig_ready = true;
     }
     CUDA_OK(ctx, center_gram(ctx->eig, ctx->d_S, ctx->stream, materialise));
@@ -1320,16 +1260,16 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
     ctx->st.eig_iterations = ctx->eig.last_iters;
     ctx->eig_timed = true;
     const size_t nb = (size_t)ctx->n * k * sizeof(double);
-    CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->eig.d_evecs, nb, cudaMemcpyDeviceToHost, ctx->stream));
-    if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, ctx->eig.d_evals, k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->eig.d_evecs.get(), nb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, ctx->eig.d_evals.get(), k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     int nz = 0;
-    CUDA_OK(ctx, cudaMemcpyAsync(&nz, ctx->eig.d_nz, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(&nz, ctx->eig.d_nz.get(), sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     if (non_zero_rows) *non_zero_rows = nz;
     ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
     ctx->pca_done = true;
     ctx->pca_k = k;
-    ctx->d_U = ctx->eig.d_evecs;
+    ctx->d_U = ctx->eig.d_evecs.get();
     return VPCA_OK;
 }
 
@@ -1342,7 +1282,7 @@ int vpca_get_centered(vpca_ctx* ctx, double* out) {
     int rc = run_center(ctx, true);   // the eigensolve overwrites C, so recompute it
     if (rc != VPCA_OK) return rc;
     const size_t bytes = (size_t)ctx->n * ctx->n * sizeof(double);
-    CUDA_OK(ctx, cudaMemcpyAsync(out, ctx->eig.d_C, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(out, ctx->eig.d_C.get(), bytes, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->c_d2h += (int64_t)bytes;
     ctx->pca_done = false;
@@ -1356,8 +1296,8 @@ int vpca_get_tridiagonal(vpca_ctx* ctx, double* diag, double* offdiag) {
     if (ctx->eig.last_method == 2)
         return fail(ctx, VPCA_ERR_STATE, "the last solve used Lanczos and did not tridiagonalise C (set VPCA_EIG=direct)");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    CUDA_OK(ctx, cudaMemcpyAsync(diag, ctx->eig.d_diag, (size_t)ctx->n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(offdiag, ctx->eig.d_off, (size_t)(ctx->n - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(diag, ctx->eig.d_diag.get(), (size_t)ctx->n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(offdiag, ctx->eig.d_off.get(), (size_t)(ctx->n - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     return VPCA_OK;
 }
@@ -1392,47 +1332,37 @@ int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, doubl
     ctx->pca_k = 0;   // U is overwritten from here on
     ctx->pca_done = false;   // the tridiagonal form of ctx->eig does not belong to this solve
     if (ctx->sub_eig.n != m) {
-        if (ctx->sub_eig.n != 0) eig_free(ctx->sub_eig);
+        eig_free(ctx->sub_eig);   // a new subset size: the whole workspace is allocated afresh
         const cudaError_t e = eig_alloc(ctx->sub_eig, m, kmax);
-        if (e != cudaSuccess) {
-            eig_free(ctx->sub_eig);
-            return fail(ctx, VPCA_ERR_NOMEM, "subset eigensolver workspace: %s", cudaGetErrorString(e));
-        }
+        if (e != cudaSuccess) return fail(ctx, VPCA_ERR_NOMEM, "subset eigensolver workspace: %s", cudaGetErrorString(e));
     }
-    if (ctx->d_sub_U == nullptr) {
+    {
         // U keeps the 16 columns the loadings read; the output and t take every component a solve may ask for
-        cudaError_t e = cudaMalloc(&ctx->d_sub_U, (size_t)n * 16 * sizeof(double));
-        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_vecs, (size_t)n * kmax * sizeof(double));
-        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_t, (size_t)kmax * sizeof(double));
-        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_idx, (size_t)n * sizeof(int32_t));
-        if (e == cudaSuccess) e = cudaMalloc(&ctx->d_sub_keep, (size_t)n);
-        if (e != cudaSuccess) {
-            for (void* p : {(void*)ctx->d_sub_U, (void*)ctx->d_sub_vecs, (void*)ctx->d_sub_t, (void*)ctx->d_sub_idx})
-                cudaFree(p);
-            ctx->d_sub_U = ctx->d_sub_vecs = ctx->d_sub_t = nullptr;
-            ctx->d_sub_idx = nullptr;
-            ctx->d_sub_keep = nullptr;
-            return fail(ctx, VPCA_ERR_NOMEM, "subset buffers: %s", cudaGetErrorString(e));
-        }
+        cudaError_t e = ctx->d_sub_U.ensure((int64_t)n * 16);
+        if (e == cudaSuccess) e = ctx->d_sub_vecs.ensure((int64_t)n * kmax);
+        if (e == cudaSuccess) e = ctx->d_sub_t.ensure(kmax);
+        if (e == cudaSuccess) e = ctx->d_sub_idx.ensure(n);
+        if (e == cudaSuccess) e = ctx->d_sub_keep.ensure(n);
+        if (e != cudaSuccess) return fail(ctx, VPCA_ERR_NOMEM, "subset buffers: %s", cudaGetErrorString(e));
     }
-    CUDA_OK(ctx, grow_buffer(&ctx->d_sub_S, &ctx->cap_sub_S, (int64_t)m * m));
+    CUDA_OK(ctx, ctx->d_sub_S.ensure((int64_t)m * m, with_slack((int64_t)m * m)));
     std::vector<uint8_t> keep01(n);
     for (int s = 0; s < n; ++s) keep01[s] = keep[s] != 0;
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_e0, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sub_idx, idx.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sub_keep, keep01.data(), (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sub_idx.get(), idx.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sub_keep.get(), keep01.data(), (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
     ctx->c_h2d += (int64_t)n * 5;
-    CUDA_OK(ctx, subset_gather(ctx->d_S, n, ctx->d_sub_idx, m, ctx->d_sub_S, ctx->stream));
+    CUDA_OK(ctx, subset_gather(ctx->d_S, n, ctx->d_sub_idx.get(), m, ctx->d_sub_S.get(), ctx->stream));
     EigWork& w = ctx->sub_eig;
-    CUDA_OK(ctx, center_gram(w, ctx->d_sub_S, ctx->stream, false));
+    CUDA_OK(ctx, center_gram(w, ctx->d_sub_S.get(), ctx->stream, false));
     {   // VPCA_EIG as for vpca_compute_pca
         const char* em = getenv("VPCA_EIG");
         w.mode = (em != nullptr && strcmp(em, "direct") == 0) ? 1 : (em != nullptr && strcmp(em, "lanczos") == 0) ? 2 : 0;
     }
     int64_t launches = 3;
     CUDA_OK(ctx, eig_topk(w, k, ctx->stream, &launches));
-    CUDA_OK(ctx, subset_place(ctx->d_S, n, ctx->d_sub_idx, m, w.d_evecs, w.d_evals, w.d_rowsum, k, ctx->d_sub_U,
-                              ctx->d_sub_vecs, ctx->d_sub_t, ctx->stream));
+    CUDA_OK(ctx, subset_place(ctx->d_S, n, ctx->d_sub_idx.get(), m, w.d_evecs.get(), w.d_evals.get(), w.d_rowsum.get(), k, ctx->d_sub_U.get(),
+                              ctx->d_sub_vecs.get(), ctx->d_sub_t.get(), ctx->stream));
     launches += m < n ? 3 : 1;
     ctx->c_launches += launches;
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_e1, ctx->stream));
@@ -1440,15 +1370,15 @@ int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, doubl
     ctx->st.eig_iterations = w.last_iters;
     ctx->eig_timed = true;
     const size_t nb = (size_t)n * k * sizeof(double);
-    CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->d_sub_vecs, nb, cudaMemcpyDeviceToHost, ctx->stream));
-    if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, w.d_evals, k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->d_sub_vecs.get(), nb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, w.d_evals.get(), k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     int nz = 0;
-    CUDA_OK(ctx, cudaMemcpyAsync(&nz, w.d_nz, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(&nz, w.d_nz.get(), sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     if (non_zero_rows) *non_zero_rows = nz;
     ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
     ctx->pca_k = k;
-    ctx->d_U = ctx->d_sub_U;
+    ctx->d_U = ctx->d_sub_U.get();
     return VPCA_OK;
 }
 
@@ -1523,25 +1453,20 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
                     "fallback", c0->band_eig.last_iters, why);
     }
     const size_t nb = (size_t)n * k * sizeof(double);
-    CUDA_OK(c0, cudaMemcpyAsync(vecs, c0->band_eig.d_evecs, nb, cudaMemcpyDeviceToHost, c0->stream));
-    if (evals) CUDA_OK(c0, cudaMemcpyAsync(evals, c0->band_eig.d_evals, k * sizeof(double), cudaMemcpyDeviceToHost, c0->stream));
+    CUDA_OK(c0, cudaMemcpyAsync(vecs, c0->band_eig.d_evecs.get(), nb, cudaMemcpyDeviceToHost, c0->stream));
+    if (evals) CUDA_OK(c0, cudaMemcpyAsync(evals, c0->band_eig.d_evals.get(), k * sizeof(double), cudaMemcpyDeviceToHost, c0->stream));
     int nz = 0;
-    CUDA_OK(c0, cudaMemcpyAsync(&nz, c0->band_eig.d_nz, sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
+    CUDA_OK(c0, cudaMemcpyAsync(&nz, c0->band_eig.d_nz.get(), sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
     // U for the loadings on every rank: rank 0 reads its solver's vectors, every other rank gets a copy of the first
     // min(k, 16) columns on its own device, in stream order after the solve (ev_e1), as v_j travels during it
     const int kc = std::min(k, 16);
     for (int r = 1; r < world; ++r) {
         vpca_ctx* c = ctxs[r];
         CUDA_OK(c0, cudaSetDevice(c->cfg.device));
-        if (c->d_band_U == nullptr) {
-            const cudaError_t ae = cudaMalloc(&c->d_band_U, (size_t)n * 16 * sizeof(double));
-            if (ae != cudaSuccess) {
-                c->d_band_U = nullptr;
-                return fail(c0, VPCA_ERR_NOMEM, "ctxs[%d]: U for the loadings: %s", r, cudaGetErrorString(ae));
-            }
-        }
+        if (const cudaError_t ae = c->d_band_U.ensure((int64_t)n * 16); ae != cudaSuccess)
+            return fail(c0, VPCA_ERR_NOMEM, "ctxs[%d]: U for the loadings: %s", r, cudaGetErrorString(ae));
         CUDA_OK(c0, cudaStreamWaitEvent(c->stream, c0->ev_e1, 0));
-        CUDA_OK(c0, cudaMemcpyPeerAsync(c->d_band_U, c->cfg.device, c0->band_eig.d_evecs, c0->cfg.device,
+        CUDA_OK(c0, cudaMemcpyPeerAsync(c->d_band_U.get(), c->cfg.device, c0->band_eig.d_evecs.get(), c0->cfg.device,
                                         (size_t)n * kc * sizeof(double), c->stream));
     }
     for (int r = 1; r < world; ++r) {   // the source is rank 0's solver state, which the next solve overwrites
@@ -1554,7 +1479,7 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
     c0->c_d2h += (int64_t)nb + (evals ? k * 8 : 0) + 4;
     for (int r = 0; r < world; ++r) {
         ctxs[r]->pca_k = k;
-        ctxs[r]->d_U = r == 0 ? c0->band_eig.d_evecs : ctxs[r]->d_band_U;
+        ctxs[r]->d_U = r == 0 ? c0->band_eig.d_evecs.get() : ctxs[r]->d_band_U.get();
     }
     return VPCA_OK;
 }
@@ -1576,7 +1501,7 @@ static int loadings_check(vpca_ctx* ctx, int32_t k, const double** U, const uint
                     "set_gram / load_partial_gram / finalize_gram");
     if (k > ctx->pca_k) return fail(ctx, VPCA_ERR_BAD_ARG, "loadings of %d components, the last solve computed %d", k, ctx->pca_k);
     *U = ctx->d_U;
-    *keep = ctx->d_U == ctx->d_sub_U ? ctx->d_sub_keep : nullptr;
+    *keep = ctx->d_U == ctx->d_sub_U.get() ? ctx->d_sub_keep.get() : nullptr;
     return VPCA_OK;
 }
 
@@ -1590,21 +1515,21 @@ static int project_check(vpca_ctx* ctx) {   // caller holds ctx->mu
 // lane's stream (the single buffer is reused in stream order), then the projection kernels add into the accumulator.
 static int project_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, const double* w, const double* mean) {
     const int k = ctx->proj_k;
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_lp_w, w + v * k, (size_t)nvc * k * sizeof(double), cudaMemcpyHostToDevice, L.stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_lp_mean, mean + v, (size_t)nvc * sizeof(double), cudaMemcpyHostToDevice, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_lp_w.get(), w + v * k, (size_t)nvc * k * sizeof(double), cudaMemcpyHostToDevice, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_lp_mean.get(), mean + v, (size_t)nvc * sizeof(double), cudaMemcpyHostToDevice, L.stream));
     ctx->c_h2d += nvc * (k + 1) * (int64_t)sizeof(double);
-    CUDA_OK(ctx, project_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, ctx->d_lp_w, ctx->d_lp_mean, k,
-                                ctx->d_proj_part, ctx->d_proj_acc, kProjLd, L.stream));
+    CUDA_OK(ctx, project_launch(L.d_x[b].get(), ctx->elem_bits, ctx->n, nvc, ctx->panel, ctx->d_lp_w.get(), ctx->d_lp_mean.get(), k,
+                                ctx->d_proj_part.get(), ctx->d_proj_acc.get(), kProjLd, L.stream));
     ctx->c_launches += 2;
     return VPCA_OK;
 }
 
 static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, int64_t nvc, const double* U,
                           const uint8_t* keep, int k, double* out_w, int32_t* out_count) {
-    CUDA_OK(ctx, loadings_launch(L.d_x[b], ctx->elem_bits, ctx->n, nvc, ctx->panel, U, k, ctx->d_lp_w,
-                                 ctx->d_lp_count, keep, L.stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_lp_w, (size_t)nvc * k * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(out_count + v, ctx->d_lp_count, (size_t)nvc * sizeof(int32_t), cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, loadings_launch(L.d_x[b].get(), ctx->elem_bits, ctx->n, nvc, ctx->panel, U, k, ctx->d_lp_w.get(),
+                                 ctx->d_lp_count.get(), keep, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_lp_w.get(), (size_t)nvc * k * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(out_count + v, ctx->d_lp_count.get(), (size_t)nvc * sizeof(int32_t), cudaMemcpyDeviceToHost, L.stream));
     ctx->c_launches += 1;
     ctx->c_d2h += nvc * (k * (int64_t)sizeof(double) + 4);
     return VPCA_OK;
@@ -1613,12 +1538,13 @@ static int loadings_chunk(vpca_ctx* ctx, vpca_ctx::Lane& L, int b, int64_t v, in
 // chunk buffers for host-input loadings (project == false) or projection; after LaneGuard (it fixes chunk_variants)
 static int lp_buffers(vpca_ctx* ctx, int k, bool project) {
     const int64_t cv = ctx->chunk_variants;
-    CUDA_OK(ctx, grow_buffer(&ctx->d_lp_w, &ctx->cap_lp_w, cv * k));
+    CUDA_OK(ctx, ctx->d_lp_w.ensure(cv * k, with_slack(cv * k)));
     if (project) {
-        CUDA_OK(ctx, grow_buffer(&ctx->d_lp_mean, &ctx->cap_lp_mean, cv));
-        CUDA_OK(ctx, grow_buffer(&ctx->d_proj_part, &ctx->cap_proj_part, project_scratch_doubles(ctx->n, cv, ctx->panel, k)));
+        const int64_t part = project_scratch_doubles(ctx->n, cv, ctx->panel, k);
+        CUDA_OK(ctx, ctx->d_lp_mean.ensure(cv, with_slack(cv)));
+        CUDA_OK(ctx, ctx->d_proj_part.ensure(part, with_slack(part)));
     } else {
-        CUDA_OK(ctx, grow_buffer(&ctx->d_lp_count, &ctx->cap_lp_count, cv));
+        CUDA_OK(ctx, ctx->d_lp_count.ensure(cv, with_slack(cv)));
     }
     return VPCA_OK;
 }
@@ -1697,8 +1623,8 @@ int vpca_project_begin(vpca_ctx* ctx, int32_t k) {
     if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_UNSUPPORTED, "projection needs a context that stores the whole Gram");
     if (k < 1 || k > 16) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_begin: k=%d out of range [1, 16]", k);
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    if (ctx->d_proj_acc == nullptr) CUDA_OK(ctx, cudaMalloc(&ctx->d_proj_acc, (size_t)ctx->n * kProjLd * sizeof(double)));
-    CUDA_OK(ctx, cudaMemsetAsync(ctx->d_proj_acc, 0, (size_t)ctx->n * kProjLd * sizeof(double), ctx->stream));
+    CUDA_OK(ctx, ctx->d_proj_acc.ensure((int64_t)ctx->n * kProjLd));
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->d_proj_acc.get(), 0, (size_t)ctx->n * kProjLd * sizeof(double), ctx->stream));
     ctx->proj_k = k;
     return VPCA_OK;
 }
@@ -1758,13 +1684,13 @@ int vpca_project_panels(vpca_ctx* ctx, const void* d_x, int64_t nv, int64_t pane
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) return VPCA_OK;
     const int64_t need = project_scratch_doubles(ctx->n, nv, panel_variants, ctx->proj_k);
-    if (need > ctx->cap_proj_part) {
+    if (need > ctx->d_proj_part.capacity()) {
         // the scratch may still be read by an earlier launch on this stream
         CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-        CUDA_OK(ctx, grow_buffer(&ctx->d_proj_part, &ctx->cap_proj_part, need));
+        CUDA_OK(ctx, ctx->d_proj_part.ensure(need, with_slack(need)));
     }
-    CUDA_OK(ctx, project_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, d_w, d_mean, ctx->proj_k, ctx->d_proj_part,
-                                ctx->d_proj_acc, kProjLd, ctx->stream));
+    CUDA_OK(ctx, project_launch(d_x, ctx->elem_bits, ctx->n, nv, panel_variants, d_w, d_mean, ctx->proj_k, ctx->d_proj_part.get(),
+                                ctx->d_proj_acc.get(), kProjLd, ctx->stream));
     ctx->c_launches += 2;
     return VPCA_OK;
 }
@@ -1778,7 +1704,7 @@ int vpca_project_get(vpca_ctx* ctx, const double* evals, double* out) {
     const int k = ctx->proj_k, n = ctx->n;
     std::vector<double> acc((size_t)n * kProjLd);
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    CUDA_OK(ctx, cudaMemcpyAsync(acc.data(), ctx->d_proj_acc, acc.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(acc.data(), ctx->d_proj_acc.get(), acc.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->c_d2h += (int64_t)(acc.size() * sizeof(double));
     for (int c = 0; c < k; ++c)
@@ -1805,24 +1731,19 @@ static int kinship_buffers(vpca_ctx* ctx, vpca_ctx::Lane& L) {
         ctx->kin_panel = std::min<int64_t>(ctx->panel, p);
         ctx->kin_chunk = std::max<int64_t>(ctx->kin_panel, (budget / R / ctx->kin_panel) * ctx->kin_panel);
         for (int b = 0; b < 2; ++b) {
-            cudaError_t e = cudaMalloc(&ctx->d_kin_x[b], (size_t)R * ctx->kin_chunk);
+            cudaError_t e = ctx->d_kin_x[b].ensure(R * ctx->kin_chunk);
             if (e != cudaSuccess) {
-                cudaFree(ctx->d_kin_x[0]);
-                ctx->d_kin_x[0] = ctx->d_kin_x[1] = nullptr;
                 ctx->kin_panel = ctx->kin_chunk = 0;
                 return fail(ctx, VPCA_ERR_NOMEM, "kinship plane staging: %s", cudaGetErrorString(e));
             }
         }
     }
-    if (ctx->d_kin == nullptr) {
-        const size_t bytes = (size_t)R * R * sizeof(int32_t);
-        cudaError_t e = cudaMalloc(&ctx->d_kin, bytes);
-        if (e != cudaSuccess) {
-            ctx->d_kin = nullptr;
+    if (ctx->d_kin.get() == nullptr) {
+        cudaError_t e = ctx->d_kin.ensure(R * R);
+        if (e != cudaSuccess)
             return fail(ctx, VPCA_ERR_NOMEM, "kinship Gram of %lld x %lld int32: %s", (long long)R, (long long)R,
                         cudaGetErrorString(e));
-        }
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin, 0, bytes, L.stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin.get(), 0, (size_t)R * R * sizeof(int32_t), L.stream));
     }
     return VPCA_OK;
 }
@@ -1856,15 +1777,15 @@ int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t str
         const int64_t nvc = std::min(step, nv - v);
         const int b = chunk & 1;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b], rows + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
+        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b].get(), rows + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
                                      cudaMemcpyHostToDevice, L.copy_stream));
         CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
         ctx->c_h2d += nvc * stride_bytes;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, encode_bed_planes(reinterpret_cast<const uint8_t*>(L.d_idx[b]), stride_bytes, nvc, n, ctx->d_kin_x[b], P,
+        CUDA_OK(ctx, encode_bed_planes(reinterpret_cast<const uint8_t*>(L.d_idx[b].get()), stride_bytes, nvc, n, ctx->d_kin_x[b].get(), P,
                                        L.stream));
         std::string msg;
-        cudaError_t e = gram_accumulate(ctx->kin_plan, ctx->d_kin_x[b], 8, (int)R, nvc, P, P, ctx->d_kin, L.stream, &msg);
+        cudaError_t e = gram_accumulate(ctx->kin_plan, ctx->d_kin_x[b].get(), 8, (int)R, nvc, P, P, ctx->d_kin.get(), L.stream, &msg);
         if (e != cudaSuccess)
             return fail(ctx, VPCA_ERR_CUDA, "kinship Gram launch failed: %s %s [the kinship counts may hold a partial "
                         "batch, call vpca_reset]", cudaGetErrorString(e), msg.c_str());
@@ -1897,9 +1818,9 @@ int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int
     KinPairWork& w = ctx->kin_pairs;
     cudaError_t e = kin_pair_alloc(w, n);
     if (e != cudaSuccess) return fail(ctx, VPCA_ERR_NOMEM, "kinship pair scratch: %s", cudaGetErrorString(e));
-    CUDA_OK(ctx, kin_count(w, ctx->d_kin, n, min_kinship, all, ctx->stream));
+    CUDA_OK(ctx, kin_count(w, ctx->d_kin.get(), n, min_kinship, all, ctx->stream));
     std::vector<int32_t> row_total(n);
-    CUDA_OK(ctx, cudaMemcpyAsync(row_total.data(), w.d_row_total, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost,
+    CUDA_OK(ctx, cudaMemcpyAsync(row_total.data(), w.d_row_total.get(), (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost,
                                  ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->c_launches += 2;
@@ -1908,20 +1829,20 @@ int vpca_kinship_pairs(vpca_ctx* ctx, double min_kinship, int64_t max_pairs, int
     *n_pairs = start[n];
     const int64_t limit = std::min(start[n], max_pairs);
     if (limit == 0) return VPCA_OK;
-    CUDA_OK(ctx, cudaMemcpyAsync(w.d_row_start, start.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(w.d_row_start.get(), start.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
     ctx->c_h2d += (int64_t)n * 8;
     auto row_end = [&](int bt) { return start[std::min(n, 32 * bt)]; };   // position after tile rows [0, bt)
     for (int lo = 0; lo < tile_rows && row_end(lo) < limit;) {
         int hi = lo + 1;   // as many tile rows as the scratch holds (one always fits, kin_pair_alloc)
-        while (hi < tile_rows && row_end(hi + 1) - row_end(lo) <= w.cap && row_end(hi) < limit) ++hi;
+        while (hi < tile_rows && row_end(hi + 1) - row_end(lo) <= w.d_kin.capacity() && row_end(hi) < limit) ++hi;
         const int64_t base = row_end(lo), end = std::min(row_end(hi), limit), cnt = end - base;
         if (cnt > 0) {
-            CUDA_OK(ctx, kin_emit(w, ctx->d_kin, n, min_kinship, all, lo, hi, base, end, ctx->stream));
-            CUDA_OK(ctx, cudaMemcpyAsync(out_ids + 2 * base, w.d_ids, (size_t)cnt * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost,
+            CUDA_OK(ctx, kin_emit(w, ctx->d_kin.get(), n, min_kinship, all, lo, hi, base, end, ctx->stream));
+            CUDA_OK(ctx, cudaMemcpyAsync(out_ids + 2 * base, w.d_ids.get(), (size_t)cnt * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost,
                                          ctx->stream));
-            CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 5 * base, w.d_counts, (size_t)cnt * 5 * sizeof(int32_t),
+            CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 5 * base, w.d_counts.get(), (size_t)cnt * 5 * sizeof(int32_t),
                                          cudaMemcpyDeviceToHost, ctx->stream));
-            CUDA_OK(ctx, cudaMemcpyAsync(out_kinship + base, w.d_kin, (size_t)cnt * sizeof(double), cudaMemcpyDeviceToHost,
+            CUDA_OK(ctx, cudaMemcpyAsync(out_kinship + base, w.d_kin.get(), (size_t)cnt * sizeof(double), cudaMemcpyDeviceToHost,
                                          ctx->stream));
             ctx->c_launches += 1;
             ctx->c_d2h += cnt * 36;
@@ -1942,77 +1863,32 @@ constexpr int64_t kLdMaxPiece = 32768;            // samples per staged piece
 constexpr int64_t kLdPlaneBudget = 256ll << 20;   // bytes of the plane tile of one piece
 constexpr int64_t kLdWindowBytes = 16ll << 20;    // bytes of one panel of the plane tile (the Gram kernel's L2 window)
 
-// (re)allocates *p for `need` elements of `elem` bytes unless it already holds `cap` >= need
-cudaError_t ld_grow_bytes(void** p, int64_t& cap, int64_t need, size_t elem) {
-    if (need <= cap) return cudaSuccess;
-    cudaFree(*p);
-    *p = nullptr;
-    cap = 0;
-    cudaError_t e = cudaMalloc(p, (size_t)need * elem);
-    if (e == cudaSuccess) cap = need;
-    return e;
-}
-#define ld_grow(ptr, cap, need) ld_grow_bytes(reinterpret_cast<void**>(&(ptr)), (cap), (need), sizeof(*(ptr)))
-
 // Grows every buffer of one call: the 3c x 3c Gram, the plane tile (x_bytes), two row buffers (row_bytes each), the window
 // starts and the row arrays (c), the bit words (c T), a pair scratch that holds a whole row tile (32 rows of at most 32 T
 // pairs) and the keep bytes (nv).
 cudaError_t ld_buffers(vpca_ctx* ctx, int64_t c, int T, int64_t x_bytes, int64_t row_bytes, int64_t nv) {
     LdWork& w = ctx->ld;
-    cudaError_t e = ld_grow(ctx->d_ld_G, ctx->cap_ld_G, 9 * c * c);
-    if (e == cudaSuccess) {
-        e = ld_grow_bytes(&ctx->d_ld_x, ctx->cap_ld_x, x_bytes, 1);
-    }
-    if (e == cudaSuccess && row_bytes > ctx->cap_ld_rows) {
-        int64_t c0 = 0, c1 = 0;
-        cudaFree(ctx->d_ld_rows[0]);
-        cudaFree(ctx->d_ld_rows[1]);
-        ctx->d_ld_rows[0] = ctx->d_ld_rows[1] = nullptr;
-        ctx->cap_ld_rows = 0;
-        e = ld_grow(ctx->d_ld_rows[0], c0, row_bytes);
-        if (e == cudaSuccess) e = ld_grow(ctx->d_ld_rows[1], c1, row_bytes);
-        if (e == cudaSuccess) ctx->cap_ld_rows = row_bytes;
-    }
-    if (e == cudaSuccess) e = ld_grow(ctx->d_ld_wlo, ctx->cap_ld_wlo, c);
-    if (e == cudaSuccess) e = ld_grow(ctx->d_ld_keep, ctx->cap_ld_keep, nv);
-    if (e == cudaSuccess && c * T > w.cap_words) {
-        int64_t cb = 0, cs = 0;
-        cudaFree(w.d_bits);
-        cudaFree(w.d_seg);
-        w.d_bits = nullptr;
-        w.d_seg = nullptr;
-        w.cap_words = 0;
-        e = ld_grow(w.d_bits, cb, c * T);
-        if (e == cudaSuccess) e = ld_grow(w.d_seg, cs, c * T);
-        if (e == cudaSuccess) w.cap_words = c * T;
-    }
-    if (e == cudaSuccess && c > w.cap_rows) {
-        int64_t ct = 0, cs = 0;
-        cudaFree(w.d_row_total);
-        cudaFree(w.d_row_start);
-        w.d_row_total = nullptr;
-        w.d_row_start = nullptr;
-        w.cap_rows = 0;
-        e = ld_grow(w.d_row_total, ct, c);
-        if (e == cudaSuccess) e = ld_grow(w.d_row_start, cs, c);
-        if (e == cudaSuccess) w.cap_rows = c;
-    }
     const int64_t pairs = std::max<int64_t>(int64_t(1) << 20, 1024 * (int64_t)T);
-    if (e == cudaSuccess && pairs > w.cap) {
-        int64_t cp = 0, cr = 0;
-        cudaFree(w.d_pairs);
-        cudaFree(w.d_r2);
-        w.d_pairs = nullptr;
-        w.d_r2 = nullptr;
-        w.cap = 0;
-        e = ld_grow(w.d_pairs, cp, 2 * pairs);
-        if (e == cudaSuccess) e = ld_grow(w.d_r2, cr, pairs);
-        if (e == cudaSuccess) w.cap = pairs;
+    cudaError_t e = ctx->d_ld_G.ensure(9 * c * c);
+    if (e == cudaSuccess) e = ctx->d_ld_x.ensure(x_bytes);
+    if (e == cudaSuccess) e = ctx->d_ld_rows[0].ensure(row_bytes);
+    if (e == cudaSuccess) e = ctx->d_ld_rows[1].ensure(row_bytes);
+    if (e == cudaSuccess) e = ctx->d_ld_wlo.ensure(c);
+    if (e == cudaSuccess) e = ctx->d_ld_keep.ensure(nv);
+    if (e == cudaSuccess) e = w.d_bits.ensure(c * T);
+    if (e == cudaSuccess) e = w.d_seg.ensure(c * T);
+    if (e == cudaSuccess) e = w.d_row_total.ensure(c);
+    if (e == cudaSuccess) e = w.d_row_start.ensure(c);
+    if (pairs > w.d_r2.capacity() || 2 * pairs > w.d_pairs.capacity()) {
+        // the pair scratch holds d_r2.capacity() pairs in both buffers: they are reallocated together
+        w.d_pairs.reset();
+        w.d_r2.reset();
     }
-    if (e == cudaSuccess && w.d_total == nullptr) e = cudaMalloc(&w.d_total, sizeof(int64_t));
+    if (e == cudaSuccess) e = w.d_pairs.ensure(2 * pairs);
+    if (e == cudaSuccess) e = w.d_r2.ensure(pairs);
+    if (e == cudaSuccess) e = w.d_total.ensure(1);
     return e;
 }
-#undef ld_grow
 }   // namespace
 
 int vpca_ld_prune_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const int64_t* window_lo,
@@ -2074,17 +1950,16 @@ int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int
     LdWork& w = ctx->ld;
     {
         cudaError_t e = ld_buffers(ctx, c, T, R * piece, c * rp, nv);
-        if (e == cudaSuccess && eligible != nullptr)
-            e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_ld_elig), ctx->cap_ld_elig, nv, 1);
+        if (e == cudaSuccess && eligible != nullptr) e = ctx->d_ld_elig.ensure(nv);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "LD pruning buffers for chunks of %lld variants: %s", (long long)c,
                         cudaGetErrorString(e));
         }
     }
-    CUDA_OK(ctx, cudaMemsetAsync(w.d_total, 0, sizeof(int64_t), L.stream));
+    CUDA_OK(ctx, cudaMemsetAsync(w.d_total.get(), 0, sizeof(int64_t), L.stream));
     if (eligible != nullptr) {
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_elig, eligible, (size_t)nv, cudaMemcpyHostToDevice, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_elig.get(), eligible, (size_t)nv, cudaMemcpyHostToDevice, L.stream));
         ctx->c_h2d += nv;
     }
     int64_t listed = 0;                   // pairs counted (and listed) before the current chunk while listing
@@ -2094,10 +1969,10 @@ int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int
     int unit = 0;                         // staged pieces so far: selects the row buffer
     for (int64_t s = 0;;) {
         const int64_t e_end = std::min(s + c, nv);
-        LdChunk ch{ctx->d_ld_G, ctx->d_ld_wlo, s, (int)c, (int)(e_end - s), s == 0 ? 0 : (int)H, T, r2_max,
-                   eligible != nullptr ? ctx->d_ld_elig : nullptr};
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_ld_G, 0, (size_t)(R * R) * sizeof(int32_t), L.stream));
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_wlo, window_lo + s, (size_t)ch.nc * sizeof(int64_t), cudaMemcpyHostToDevice,
+        LdChunk ch{ctx->d_ld_G.get(), ctx->d_ld_wlo.get(), s, (int)c, (int)(e_end - s), s == 0 ? 0 : (int)H, T, r2_max,
+                   eligible != nullptr ? ctx->d_ld_elig.get() : nullptr};
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_ld_G.get(), 0, (size_t)(R * R) * sizeof(int32_t), L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_ld_wlo.get(), window_lo + s, (size_t)ch.nc * sizeof(int64_t), cudaMemcpyHostToDevice,
                                      L.stream));
         ctx->c_h2d += ch.nc * 8;
         for (int64_t s0 = 0; s0 < n; s0 += piece, ++unit) {
@@ -2105,45 +1980,45 @@ int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int
             const int64_t width = std::min(rp, row_bytes - s0 / 4);
             const int b = unit & 1;
             CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-            CUDA_OK(ctx, cudaMemcpy2DAsync(ctx->d_ld_rows[b], (size_t)rp, rows + (size_t)s * stride_bytes + s0 / 4,
+            CUDA_OK(ctx, cudaMemcpy2DAsync(ctx->d_ld_rows[b].get(), (size_t)rp, rows + (size_t)s * stride_bytes + s0 / 4,
                                            (size_t)stride_bytes, (size_t)width, (size_t)ch.nc, cudaMemcpyHostToDevice,
                                            L.copy_stream));
             CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
             ctx->c_h2d += width * ch.nc;
             CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-            CUDA_OK(ctx, encode_ld_planes(ctx->d_ld_rows[b], rp, width, ch.nc, (int)c, s0, len, n, ctx->d_ld_x, P, L.stream));
+            CUDA_OK(ctx, encode_ld_planes(ctx->d_ld_rows[b].get(), rp, width, ch.nc, (int)c, s0, len, n, ctx->d_ld_x.get(), P, L.stream));
             CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));   // the row buffer is free again
             std::string msg;
-            cudaError_t e = gram_accumulate(ctx->ld_plan, ctx->d_ld_x, 8, (int)R, len, P, P, ctx->d_ld_G, L.stream, &msg);
+            cudaError_t e = gram_accumulate(ctx->ld_plan, ctx->d_ld_x.get(), 8, (int)R, len, P, P, ctx->d_ld_G.get(), L.stream, &msg);
             if (e != cudaSuccess)
                 return fail(ctx, VPCA_ERR_CUDA, "LD plane Gram launch failed: %s %s", cudaGetErrorString(e), msg.c_str());
             ctx->c_launches += 2;
             ctx->c_gram += 1;
         }
         CUDA_OK(ctx, ld_count(w, ch, L.stream));
-        CUDA_OK(ctx, ld_sweep(w, ch, ctx->d_ld_keep, L.stream));
+        CUDA_OK(ctx, ld_sweep(w, ch, ctx->d_ld_keep.get(), L.stream));
         ctx->c_launches += 3;
         if (listing) {
             const int lo = ch.own_lo, nc = ch.nc;
-            CUDA_OK(ctx, cudaMemcpyAsync(row_total.data(), w.d_row_total + lo, (size_t)(nc - lo) * sizeof(int32_t),
+            CUDA_OK(ctx, cudaMemcpyAsync(row_total.data(), w.d_row_total.get() + lo, (size_t)(nc - lo) * sizeof(int32_t),
                                          cudaMemcpyDeviceToHost, L.stream));
             CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
             start[lo] = listed;
             for (int b = lo; b < nc; ++b) start[b + 1] = start[b] + row_total[b - lo];
-            CUDA_OK(ctx, cudaMemcpyAsync(w.d_row_start + lo, start.data() + lo, (size_t)(nc - lo) * sizeof(int64_t),
+            CUDA_OK(ctx, cudaMemcpyAsync(w.d_row_start.get() + lo, start.data() + lo, (size_t)(nc - lo) * sizeof(int64_t),
                                          cudaMemcpyHostToDevice, L.stream));
             const int64_t limit = std::min(start[nc], max_pairs);
             auto row_end = [&](int bt) { return start[std::min(nc, std::max(lo, 32 * bt))]; };   // position after tile rows < bt
             const int tiles_hi = (nc + 31) / 32;
             for (int tlo = lo / 32; tlo < tiles_hi && row_end(tlo) < limit;) {
                 int thi = tlo + 1;   // as many row tiles as the scratch holds (one always fits, ld_buffers)
-                while (thi < tiles_hi && row_end(thi + 1) - row_end(tlo) <= w.cap && row_end(thi) < limit) ++thi;
+                while (thi < tiles_hi && row_end(thi + 1) - row_end(tlo) <= w.d_r2.capacity() && row_end(thi) < limit) ++thi;
                 const int64_t base = row_end(tlo), end = std::min(row_end(thi), limit), cnt = end - base;
                 if (cnt > 0) {
                     CUDA_OK(ctx, ld_emit(w, ch, tlo, thi, base, end, L.stream));
-                    CUDA_OK(ctx, cudaMemcpyAsync(out_pairs + 2 * base, w.d_pairs, (size_t)cnt * 2 * sizeof(int64_t),
+                    CUDA_OK(ctx, cudaMemcpyAsync(out_pairs + 2 * base, w.d_pairs.get(), (size_t)cnt * 2 * sizeof(int64_t),
                                                  cudaMemcpyDeviceToHost, L.stream));
-                    CUDA_OK(ctx, cudaMemcpyAsync(out_r2 + base, w.d_r2, (size_t)cnt * sizeof(double), cudaMemcpyDeviceToHost,
+                    CUDA_OK(ctx, cudaMemcpyAsync(out_r2 + base, w.d_r2.get(), (size_t)cnt * sizeof(double), cudaMemcpyDeviceToHost,
                                                  L.stream));
                     ctx->c_launches += 1;
                     ctx->c_d2h += cnt * 24;
@@ -2156,8 +2031,8 @@ int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int
         if (e_end == nv) break;
         s = e_end - H;
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(keep, ctx->d_ld_keep, (size_t)nv, cudaMemcpyDeviceToHost, L.stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(n_pairs, w.d_total, sizeof(int64_t), cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(keep, ctx->d_ld_keep.get(), (size_t)nv, cudaMemcpyDeviceToHost, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(n_pairs, w.d_total.get(), sizeof(int64_t), cudaMemcpyDeviceToHost, L.stream));
     ctx->c_d2h += nv + 8;
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     return VPCA_OK;
@@ -2174,10 +2049,9 @@ constexpr int64_t kQcHweChunk = 1ll << 18;      // count rows per HWE launch (an
 
 // grows the QC buffers to `row_bytes` staged bytes and `rows` count / p-value rows
 cudaError_t qc_buffers(vpca_ctx* ctx, int64_t row_bytes, int64_t rows) {
-    cudaError_t e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_qc_rows), ctx->cap_qc_rows, row_bytes, 1);
-    if (e == cudaSuccess) e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_qc_counts), ctx->cap_qc_counts, 4 * rows,
-                                            sizeof(int32_t));
-    if (e == cudaSuccess) e = ld_grow_bytes(reinterpret_cast<void**>(&ctx->d_qc_p), ctx->cap_qc_p, rows, sizeof(double));
+    cudaError_t e = ctx->d_qc_rows.ensure(row_bytes);
+    if (e == cudaSuccess) e = ctx->d_qc_counts.ensure(4 * rows);
+    if (e == cudaSuccess) e = ctx->d_qc_p.ensure(rows);
     return e;
 }
 }   // namespace
@@ -2208,18 +2082,18 @@ int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
         const int64_t nb = std::min(batch, nv - b0);
         for (int64_t v = b0; v < b0 + nb; v += step) {
             const int64_t nvc = std::min(step, b0 + nb - v);
-            CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_rows, rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+            CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_rows.get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
                                          cudaMemcpyHostToDevice, L.stream));
             ctx->c_h2d += nvc * stride_bytes;
-            CUDA_OK(ctx, qc_count(ctx->d_qc_rows, stride_bytes, (int)nvc, n, ctx->d_qc_counts + 4 * (v - b0), L.stream));
+            CUDA_OK(ctx, qc_count(ctx->d_qc_rows.get(), stride_bytes, (int)nvc, n, ctx->d_qc_counts.get() + 4 * (v - b0), L.stream));
             ctx->c_launches += 1;
         }
-        CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 4 * b0, ctx->d_qc_counts, (size_t)(4 * nb) * sizeof(int32_t),
+        CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 4 * b0, ctx->d_qc_counts.get(), (size_t)(4 * nb) * sizeof(int32_t),
                                      cudaMemcpyDeviceToHost, L.stream));
         ctx->c_d2h += 16 * nb;
         if (out_hwe_p != nullptr) {
-            CUDA_OK(ctx, qc_hwe(ctx->d_qc_counts, (int)nb, ctx->d_qc_p, L.stream));
-            CUDA_OK(ctx, cudaMemcpyAsync(out_hwe_p + b0, ctx->d_qc_p, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost,
+            CUDA_OK(ctx, qc_hwe(ctx->d_qc_counts.get(), (int)nb, ctx->d_qc_p.get(), L.stream));
+            CUDA_OK(ctx, cudaMemcpyAsync(out_hwe_p + b0, ctx->d_qc_p.get(), (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost,
                                          L.stream));
             ctx->c_launches += 1;
             ctx->c_d2h += 8 * nb;
@@ -2254,11 +2128,11 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
     }
     for (int64_t v = 0; v < nv; v += step) {
         const int64_t nvc = std::min(step, nv - v);
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_counts, counts + 4 * v, (size_t)(4 * nvc) * sizeof(int32_t),
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_counts.get(), counts + 4 * v, (size_t)(4 * nvc) * sizeof(int32_t),
                                      cudaMemcpyHostToDevice, L.stream));
         ctx->c_h2d += 16 * nvc;
-        CUDA_OK(ctx, qc_hwe(ctx->d_qc_counts, (int)nvc, ctx->d_qc_p, L.stream));
-        CUDA_OK(ctx, cudaMemcpyAsync(out_p + v, ctx->d_qc_p, (size_t)nvc * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
+        CUDA_OK(ctx, qc_hwe(ctx->d_qc_counts.get(), (int)nvc, ctx->d_qc_p.get(), L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_p + v, ctx->d_qc_p.get(), (size_t)nvc * sizeof(double), cudaMemcpyDeviceToHost, L.stream));
         ctx->c_launches += 1;
         ctx->c_d2h += 8 * nvc;
     }
@@ -2284,10 +2158,6 @@ int sample_rows_args(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t
         return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (n_samples = %d must be >= 1, stride_bytes = %lld >= "
                     "ceil(n_samples / 4))", fn, (int)n_samples, (long long)stride_bytes);
     return VPCA_OK;
-}
-
-cudaError_t sm_grow(void* p, int64_t& cap, int64_t need, size_t elem) {
-    return ld_grow_bytes(reinterpret_cast<void**>(p), cap, need, elem);
 }
 
 // The D2H side of vpca_subset_bed_samples: copies chunk i down once the main thread has launched its kernel, and
@@ -2343,24 +2213,24 @@ int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
     if (lg.rc != VPCA_OK) return lg.rc;
     vpca_ctx::Lane& L = *lg.lane;
     {
-        cudaError_t e = sm_grow(&ctx->d_sm_rows[0], ctx->cap_sm_rows[0], step * stride_bytes, 1);
-        if (e == cudaSuccess) e = sm_grow(&ctx->d_sm_miss, ctx->cap_sm_miss, n_samples, sizeof(int32_t));
+        cudaError_t e = ctx->d_sm_rows[0].ensure(step * stride_bytes);
+        if (e == cudaSuccess) e = ctx->d_sm_miss.ensure(n_samples);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "sample QC buffers for %lld rows of %lld bytes: %s", (long long)step,
                         (long long)stride_bytes, cudaGetErrorString(e));
         }
     }
-    CUDA_OK(ctx, cudaMemsetAsync(ctx->d_sm_miss, 0, (size_t)n_samples * sizeof(int32_t), L.stream));
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->d_sm_miss.get(), 0, (size_t)n_samples * sizeof(int32_t), L.stream));
     for (int64_t v = 0; v < nv; v += step) {
         const int64_t nvc = std::min(step, nv - v);
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[0], rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[0].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
                                      cudaMemcpyHostToDevice, L.stream));
         ctx->c_h2d += nvc * stride_bytes;
-        CUDA_OK(ctx, sample_missing(ctx->d_sm_rows[0], stride_bytes, (int)nvc, n_samples, ctx->d_sm_miss, L.stream));
+        CUDA_OK(ctx, sample_missing(ctx->d_sm_rows[0].get(), stride_bytes, (int)nvc, n_samples, ctx->d_sm_miss.get(), L.stream));
         ctx->c_launches += 1;
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(out_missing, ctx->d_sm_miss, (size_t)n_samples * sizeof(int32_t), cudaMemcpyDeviceToHost,
+    CUDA_OK(ctx, cudaMemcpyAsync(out_missing, ctx->d_sm_miss.get(), (size_t)n_samples * sizeof(int32_t), cudaMemcpyDeviceToHost,
                                  L.stream));
     ctx->c_d2h += 4 * (int64_t)n_samples;
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
@@ -2392,14 +2262,14 @@ int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
     {
         cudaError_t e = cudaSuccess;
         for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-            e = sm_grow(&ctx->d_sm_rows[b], ctx->cap_sm_rows[b], step * stride_bytes, 1);
-            if (e == cudaSuccess) e = sm_grow(&ctx->d_sm_out[b], ctx->cap_sm_out[b], step * mb, 1);
+            e = ctx->d_sm_rows[b].ensure(step * stride_bytes);
+            if (e == cudaSuccess) e = ctx->d_sm_out[b].ensure(step * mb);
             if (e == cudaSuccess && ctx->sm_ev_copy[b] == nullptr)
                 e = cudaEventCreateWithFlags(&ctx->sm_ev_copy[b], cudaEventDisableTiming);
             if (e == cudaSuccess && ctx->sm_ev_kern[b] == nullptr)
                 e = cudaEventCreateWithFlags(&ctx->sm_ev_kern[b], cudaEventDisableTiming);
         }
-        if (e == cudaSuccess) e = sm_grow(&ctx->d_sm_idx, ctx->cap_sm_idx, m, sizeof(int32_t));
+        if (e == cudaSuccess) e = ctx->d_sm_idx.ensure(m);
         if (e == cudaSuccess && ctx->sm_d2h_stream == nullptr)
             e = cudaStreamCreateWithFlags(&ctx->sm_d2h_stream, cudaStreamNonBlocking);
         if (e != cudaSuccess) {
@@ -2408,7 +2278,7 @@ int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
                         (long long)stride_bytes, cudaGetErrorString(e));
         }
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_idx, keep_idx, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, L.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_idx.get(), keep_idx, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, L.stream));
     ctx->c_h2d += 4 * (int64_t)m;
     SubsetDownloader down;
     const int device = ctx->cfg.device;
@@ -2425,9 +2295,9 @@ int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
             e = cudaStreamWaitEvent(ctx->sm_d2h_stream, ctx->sm_ev_kern[b], 0);
             if (e == cudaSuccess)
                 e = out_stride == mb
-                        ? cudaMemcpyAsync(out_rows + (size_t)(v * mb), ctx->d_sm_out[b], (size_t)(nvc * mb),
+                        ? cudaMemcpyAsync(out_rows + (size_t)(v * mb), ctx->d_sm_out[b].get(), (size_t)(nvc * mb),
                                           cudaMemcpyDeviceToHost, ctx->sm_d2h_stream)
-                        : cudaMemcpy2DAsync(out_rows + (size_t)(v * out_stride), (size_t)out_stride, ctx->d_sm_out[b],
+                        : cudaMemcpy2DAsync(out_rows + (size_t)(v * out_stride), (size_t)out_stride, ctx->d_sm_out[b].get(),
                                             (size_t)mb, (size_t)mb, (size_t)nvc, cudaMemcpyDeviceToHost, ctx->sm_d2h_stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->sm_d2h_stream);
             {
@@ -2449,12 +2319,12 @@ int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
         const int b = (int)(i & 1);
         const int64_t v = i * step, nvc = std::min(step, nv - v);
         if (!down.wait_copied(i - 1)) break;   // chunk i - 2, the last user of buffers b, is on the host
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[b], rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[b].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
                                      cudaMemcpyHostToDevice, L.copy_stream));
         CUDA_OK(ctx, cudaEventRecord(ctx->sm_ev_copy[b], L.copy_stream));
         ctx->c_h2d += nvc * stride_bytes;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, ctx->sm_ev_copy[b], 0));
-        CUDA_OK(ctx, subset_samples(ctx->d_sm_rows[b], stride_bytes, (int)nvc, ctx->d_sm_idx, m, ctx->d_sm_out[b], mb,
+        CUDA_OK(ctx, subset_samples(ctx->d_sm_rows[b].get(), stride_bytes, (int)nvc, ctx->d_sm_idx.get(), m, ctx->d_sm_out[b].get(), mb,
                                     L.stream));
         CUDA_OK(ctx, cudaEventRecord(ctx->sm_ev_kern[b], L.stream));
         ctx->c_launches += 1;
@@ -2506,7 +2376,7 @@ int vpca_get_stats(vpca_ctx* ctx, vpca_stats* out) {
 int vpca_gram_export_ipc(vpca_ctx* ctx, void* handle64) {
     if (ctx == nullptr || handle64 == nullptr) return fail(ctx, VPCA_ERR_BAD_ARG, "NULL argument");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (!ctx->own_S) return fail(ctx, VPCA_ERR_STATE, "the peer-reduce mode needs a library-owned Gram (vpca_config.d_gram == NULL)");
+    if (ctx->owned_S.get() == nullptr) return fail(ctx, VPCA_ERR_STATE, "the peer-reduce mode needs a library-owned Gram (vpca_config.d_gram == NULL)");
     if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_STATE, "band-only Grams are shared with vpca_gram_set_peers_local");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t is 64 bytes");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
@@ -2520,7 +2390,7 @@ int vpca_gram_set_peers(vpca_ctx* ctx, const void* handles, int32_t world, int32
     if (ctx == nullptr || handles == nullptr || world < 1 || world > 16 || rank < 0 || rank >= world)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_gram_set_peers: bad argument (world <= 16)");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (!ctx->own_S) return fail(ctx, VPCA_ERR_STATE, "the peer-reduce mode needs a library-owned Gram");
+    if (ctx->owned_S.get() == nullptr) return fail(ctx, VPCA_ERR_STATE, "the peer-reduce mode needs a library-owned Gram");
     if (ctx->plan.num_peers != 0) return fail(ctx, VPCA_ERR_STATE, "peers already set");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     const size_t nn = (size_t)ctx->n * ctx->n;
@@ -2559,7 +2429,7 @@ int vpca_gram_set_peers_local(vpca_ctx* const* ctxs, int32_t world) {
     if (ctxs == nullptr || world < 1 || world > 16) return fail(nullptr, VPCA_ERR_BAD_ARG, "vpca_gram_set_peers_local: world must be in [1, 16]");
     for (int r = 0; r < world; ++r) {
         if (ctxs[r] == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctxs[%d] is NULL", r);
-        if (!ctxs[r]->own_S) return fail(ctxs[r], VPCA_ERR_STATE, "the peer-reduce mode needs a library-owned Gram");
+        if (ctxs[r]->owned_S.get() == nullptr) return fail(ctxs[r], VPCA_ERR_STATE, "the peer-reduce mode needs a library-owned Gram");
         if (ctxs[r]->n != ctxs[0]->n) return fail(ctxs[r], VPCA_ERR_BAD_ARG, "all contexts must have the same n_samples");
         if (ctxs[r]->plan.num_peers != 0) return fail(ctxs[r], VPCA_ERR_STATE, "peers already set");
         for (int q = 0; q < r; ++q)
@@ -2694,13 +2564,15 @@ int vpca_debug_gram_profile(vpca_ctx* ctx, int64_t* out, int32_t max_ctas) {
 int vpca_debug_lanczos_profile(vpca_ctx* ctx, int64_t* out, int32_t max_steps) {
     if (ctx == nullptr || out == nullptr || max_steps <= 0) return fail(ctx, VPCA_ERR_BAD_ARG, "bad argument");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (!ctx->eig_ready || ctx->eig.d_lzprof == nullptr) return 0;
+    if (!ctx->eig_ready || ctx->eig.d_lzprof.get() == nullptr) return 0;
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     const int steps = std::min(max_steps, 32);
-    CUDA_OK(ctx, cudaMemcpy(out, ctx->eig.d_lzprof, (size_t)steps * 8 * sizeof(long long), cudaMemcpyDeviceToHost));
+    CUDA_OK(ctx, cudaMemcpy(out, ctx->eig.d_lzprof.get(), (size_t)steps * 8 * sizeof(long long), cudaMemcpyDeviceToHost));
     return steps;
 }
+
+int64_t vpca_debug_device_bytes(void) { return g_device_bytes.load(); }
 
 int vpca_debug_band_tiles(int32_t n_samples, int32_t cta_group, int32_t row0, int32_t rows, int32_t* out, int32_t max_tiles) {
     if (n_samples < 2 || max_tiles < 0 || row0 < 0 || rows < 1 || row0 + rows > n_samples)

@@ -1,5 +1,7 @@
 // Internal declarations shared by the libvpca translation units (not part of the ABI).
 #pragma once
+#include <algorithm>
+#include <atomic>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include <string>
@@ -9,6 +11,68 @@
 
 namespace vpca {
 
+// ---- device memory -----------------------------------------------------------------------------------------------------
+// Device bytes held by every DeviceBuffer of the process (vpca_debug_device_bytes).
+inline std::atomic<int64_t> g_device_bytes{0};
+
+// Owner of one cudaMalloc allocation of `capacity()` elements, freed on destruction, reset() or when it grows.  There is no
+// conversion to T*: a pointer leaves the buffer through get() only, so no caller can free or replace the allocation.
+// Frees run on whatever device is current; an owner whose buffers live on another device selects it first.
+template <class T>
+class DeviceBuffer {
+public:
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+    DeviceBuffer(DeviceBuffer&& o) noexcept : p_(o.p_), cap_(o.cap_) {
+        o.p_ = nullptr;
+        o.cap_ = 0;
+    }
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+        if (this != &o) {
+            reset();
+            p_ = o.p_;
+            cap_ = o.cap_;
+            o.p_ = nullptr;
+            o.cap_ = 0;
+        }
+        return *this;
+    }
+    ~DeviceBuffer() { reset(); }
+
+    // Grow-only: nothing happens while count <= capacity(); otherwise the old allocation is freed (its contents are not
+    // kept) and max(count, alloc) elements are allocated.  On failure the buffer is empty.
+    cudaError_t ensure(int64_t count, int64_t alloc) {
+        if (count <= cap_) return cudaSuccess;
+        reset();
+        alloc = std::max(alloc, count);
+        void* p = nullptr;
+        const cudaError_t e = cudaMalloc(&p, (size_t)alloc * sizeof(T));
+        if (e != cudaSuccess) return e;
+        p_ = static_cast<T*>(p);
+        cap_ = alloc;
+        g_device_bytes += alloc * (int64_t)sizeof(T);
+        return cudaSuccess;
+    }
+    cudaError_t ensure(int64_t count) { return ensure(count, count); }
+    void reset() {
+        if (p_ == nullptr) return;
+        cudaFree(p_);
+        g_device_bytes -= cap_ * (int64_t)sizeof(T);
+        p_ = nullptr;
+        cap_ = 0;
+    }
+    T* get() const { return p_; }
+    int64_t capacity() const { return cap_; }
+
+private:
+    T* p_ = nullptr;
+    int64_t cap_ = 0;
+};
+
+// Allocation size of the buffers that grow with headroom, so that slowly growing inputs do not reallocate on every call.
+inline int64_t with_slack(int64_t n) { return n + n / 4 + 1024; }
+
 // ---- Gram (gram_sm90.cu) --------------------------------------------------------------------
 struct GramPlan {
     int cta_group = 2;        // CTAs per tile (1: 128 x 256 tiles per CTA; 2: 256 x 256 per CTA pair, one A block each,
@@ -16,7 +80,7 @@ struct GramPlan {
     int kb_window = 0;        // k-blocks per L2 window (0 -> automatic)
     int num_sms = 0;
     int max_pairs[3] = {};    // 2-CTA clusters of the int8 / bf16 / e2m1 kernel the device holds at once (0: not queried)
-    void* d_tiles = nullptr;  // device tile list (TileDesc, gram_sm90.cu)
+    DeviceBuffer<uint8_t> d_tiles;   // device tile list (TileDesc, gram_sm90.cu)
     std::vector<int32_t> h_tiles;   // the same list on the host (8 ints per tile): resident / accumulator-fit decisions
     int num_tiles = 0;
     int num_full = 0;         // leading full-weight tiles (whole-tile waves of the large-N schedule)
@@ -37,12 +101,13 @@ struct GramPlan {
     int* d_err = nullptr;     // device debug words written before a watchdog trap
     static constexpr int kMaxWindows = 1 << 16;
     int sync_lead = 0;        // VPCA_SYNC_LEAD: windows a worker may lead the slowest one by (0 = no pacing)
-    int* d_win_done = nullptr;
+    DeviceBuffer<int> d_win_done;
     bool self_b = true;       // VPCA_SELF_B=0: diagonal tiles load their B rows although they are the pair's own A blocks
     bool red64 = true;        // VPCA_RED64=0: one 32-bit red per cell in the flush instead of two cells per 64-bit red
     double gain = 0.5;        // VPCA_REBALANCE_GAIN: how far a launch moves the shares towards the measured speeds
     bool adaptive = true;     // VPCA_ADAPTIVE=0 keeps the stream-K split equal instead of speed-weighted
-    double* d_cum = nullptr;  // cumulative worker shares (workers + 1 doubles) + update counter
+    DeviceBuffer<uint8_t> d_cum;   // cumulative worker shares (workers + 1 doubles), front/tail split point (a double), update
+                                   // counter (an int)
     int cum_workers = 0, cum_tiles = 0, cum_kbw = 0, cum_for_n = 0, cum_dev = 0, cum_elem = 0;   // what the split in d_cum was made for
     // fused multi-GPU reduction: Gram buffers / barrier flags of all ranks, peer-mapped through CUDA IPC
     int num_peers = 0, peer_rank = 0, peer_epoch = 0;
@@ -55,7 +120,7 @@ struct GramPlan {
     int peer_mode = 0;        // 0: every flush goes to all ranks' Grams; 1: to the owner of the row only (+ gather)
     int own_end[16] = {};     // peer_mode 1: rank q owns Gram rows [own_end[q-1], own_end[q])
     bool profile = false;     // VPCA_GRAM_PROF=1: per-CTA timestamps in d_prof
-    long long* d_prof = nullptr;
+    DeviceBuffer<long long> d_prof;
 };
 // Copies the per-CTA timestamps of the last profiled launch (4 per CTA) to host; returns the CTA count.
 int gram_read_profile(GramPlan& plan, long long* out, int max_ctas);
@@ -129,15 +194,13 @@ struct LdChunk {
     const uint8_t* elig;   // vpca_ld_prune_bed_masked: eligible[v] of every variant v of the call; nullptr = all eligible
 };
 struct LdWork {
-    uint32_t* d_bits = nullptr;     // c x T in-LD bits
-    int32_t* d_seg = nullptr;       // c x T: pairs before word w in row b
-    int32_t* d_row_total = nullptr; // c: in-LD pairs of row b
-    int64_t* d_row_start = nullptr; // c: output position of the first pair of row b
-    int64_t* d_total = nullptr;     // in-LD pairs of the call so far
-    int64_t* d_pairs = nullptr;     // cap pairs: (i, j), then r2
-    double* d_r2 = nullptr;
-    int64_t cap = 0;                // pairs the scratch holds
-    int64_t cap_words = 0, cap_rows = 0;
+    DeviceBuffer<uint32_t> d_bits;      // c x T in-LD bits
+    DeviceBuffer<int32_t> d_seg;        // c x T: pairs before word w in row b
+    DeviceBuffer<int32_t> d_row_total;  // c: in-LD pairs of row b
+    DeviceBuffer<int64_t> d_row_start;  // c: output position of the first pair of row b
+    DeviceBuffer<int64_t> d_total;      // in-LD pairs of the call so far
+    DeviceBuffer<int64_t> d_pairs;      // pair scratch: (i, j) of each pair, then its r2
+    DeviceBuffer<double> d_r2;          // (its capacity is the pairs the scratch holds)
 };
 // Pass 1: bits, per-word prefix, row totals (and their sum into *d_total) of the owned rows.  Never synchronises.
 cudaError_t ld_count(LdWork& w, const LdChunk& ch, cudaStream_t stream);
@@ -170,15 +233,13 @@ constexpr int kKinMaxN = 21845;   // 3n <= 65 535: the plane Gram stays below 2^
 // Device scratch of vpca_kinship_pairs, owned by the context and kept between calls.
 struct KinPairWork {
     int n = 0;
-    int32_t* d_seg = nullptr;        // n x ceil(n / 32): selected pairs per (row b, 32-column tile), then their row-wise scan
-    int32_t* d_row_total = nullptr;  // n: selected pairs per row b
-    int64_t* d_row_start = nullptr;  // n: output position of the first selected pair of row b
-    int32_t* d_ids = nullptr;        // cap pairs: 2 ids, 5 counts, 1 kinship each
-    int32_t* d_counts = nullptr;
-    double* d_kin = nullptr;
-    int64_t cap = 0;
+    DeviceBuffer<int32_t> d_seg;        // n x ceil(n / 32): selected pairs per (row b, 32-column tile), then their row-wise scan
+    DeviceBuffer<int32_t> d_row_total;  // n: selected pairs per row b
+    DeviceBuffer<int64_t> d_row_start;  // n: output position of the first selected pair of row b
+    DeviceBuffer<int32_t> d_ids;        // pair scratch: 2 ids, 5 counts, 1 kinship each (d_kin's capacity: the pairs it holds)
+    DeviceBuffer<int32_t> d_counts;
+    DeviceBuffer<double> d_kin;
 };
-void kin_pair_free(KinPairWork& w);
 cudaError_t kin_pair_alloc(KinPairWork& w, int n);
 // Pass 1: w.d_seg / w.d_row_total for the threshold (select_all: every pair, NaN included).  Never synchronises.
 cudaError_t kin_count(KinPairWork& w, const int32_t* d_G, int n, double min_kinship, bool select_all, cudaStream_t stream);
@@ -189,29 +250,26 @@ cudaError_t kin_emit(KinPairWork& w, const int32_t* d_G, int n, double min_kinsh
 
 // ---- multi-dataset keying: variant keys, join, merge (join.cu)---------------------------------------------
 struct JoinWork {
-    uint64_t* d_hash = nullptr;      // 2 per row: MurmurHash3_x64_128 of the variant key
-    int32_t* d_table = nullptr;      // open-addressing table of row indices (-1 = empty)
+    DeviceBuffer<uint64_t> d_hash;       // 2 per row: MurmurHash3_x64_128 of the variant key
+    DeviceBuffer<int32_t> d_table;       // open-addressing table of row indices (-1 = empty)
     uint64_t table_slots = 0;
-    int64_t* d_rows = nullptr;       // output rows / calls each input row is responsible for, and their exclusive scans
-    int64_t* d_len = nullptr;
-    int64_t* d_row_base = nullptr;
-    int64_t* d_nnz_base = nullptr;
-    int32_t* d_leader = nullptr;
-    int64_t* d_prefix = nullptr;
-    int64_t* d_block = nullptr;      // scan scratch
-    int64_t* d_totals = nullptr;     // {output rows, output calls}
-    int64_t* h_totals = nullptr;     // pinned copy
-    int64_t cap_rows = 0;
-    int64_t* d_out_off = nullptr;    // the joined CSR: out_rows + 1 offsets, out_nnz sample indices
-    int32_t* d_out_idx = nullptr;
-    int64_t cap_out_rows = 0, cap_out_nnz = 0;
+    DeviceBuffer<int64_t> d_rows;        // output rows / calls each input row is responsible for, and their exclusive scans
+    DeviceBuffer<int64_t> d_len;
+    DeviceBuffer<int64_t> d_row_base;
+    DeviceBuffer<int64_t> d_nnz_base;
+    DeviceBuffer<int32_t> d_leader;
+    DeviceBuffer<int64_t> d_prefix;
+    DeviceBuffer<int64_t> d_block;       // scan scratch
+    DeviceBuffer<int64_t> d_totals;      // {output rows, output calls}
+    int64_t* h_totals = nullptr;         // pinned copy
+    DeviceBuffer<int64_t> d_out_off;     // the joined CSR: out_rows + 1 offsets, out_nnz sample indices
+    DeviceBuffer<int32_t> d_out_idx;
     int64_t out_rows = -1, out_nnz = 0;   // result of the last join (-1: none)
     // device copies of the caller's input (grow-only)
-    uint8_t* d_payload = nullptr;
-    int64_t* d_key_off = nullptr;
-    int64_t* d_off = nullptr;
-    int32_t* d_idx = nullptr;
-    int64_t cap_payload = 0, cap_in_rows = 0, cap_in_nnz = 0;
+    DeviceBuffer<uint8_t> d_payload;
+    DeviceBuffer<int64_t> d_key_off;
+    DeviceBuffer<int64_t> d_off;
+    DeviceBuffer<int32_t> d_idx;
 };
 cudaError_t hash_keys(const uint8_t* d_payload, const int64_t* d_off, int64_t nkeys, uint64_t* d_hash, cudaStream_t stream);
 cudaError_t join_rows(JoinWork& w, int mode, int variant_set_count, int64_t n_left, const uint8_t* d_payload,
@@ -228,10 +286,9 @@ struct BandPart {
     cudaStream_t stream = nullptr;
     const int32_t* d_S = nullptr;   // row row0 of the band
     int n = 0, row0 = 0, rows = 0;
-    double* d_v = nullptr;          // n: the Lanczos vector of the step
-    double* d_y = nullptr;          // row0 + rows: the partial product (or partial row sums as int64)
-    double* d_scratch = nullptr;    // tile row partials, then tile column partials
-    size_t scratch_doubles = 0;
+    DeviceBuffer<double> d_v;       // n: the Lanczos vector of the step
+    DeviceBuffer<double> d_y;       // row0 + rows: the partial product (or partial row sums as int64)
+    DeviceBuffer<double> d_scratch; // tile row partials, then tile column partials
     int alloc_n = 0, alloc_row0 = -1, alloc_rows = 0;
     cudaEvent_t ev_done = nullptr;  // the partial has landed on rank 0
 };
@@ -241,18 +298,18 @@ void band_part_free(BandPart& p);
 // doubles for the partials, row sums; no n x n matrix.
 struct BandEigWork {
     int n = 0, kmax = 0;
-    double* d_V = nullptr;
-    double* d_w = nullptr;       // 2 n
-    double* d_small = nullptr;   // alpha | beta | h1 | h2 | e2 | Y | theta2 | res | scal2 | sc | part
-    double* d_slots = nullptr;   // 16 n
-    double* d_rowsum = nullptr;  // n
-    double* d_rbar = nullptr;    // n
-    double* d_scal = nullptr;    // 16: [0] matrixMean, [2] ||T||
-    double* d_evals = nullptr;   // kmax
-    double* d_evecs = nullptr;   // n x kmax, column-major
-    double* d_lu = nullptr;      // 8 kLzCap: inverse-iteration scratch
-    int* d_nz = nullptr;
-    int* d_st = nullptr;         // {step, flag, ticket, step cap}
+    DeviceBuffer<double> d_V;
+    DeviceBuffer<double> d_w;       // 2 n
+    DeviceBuffer<double> d_small;   // alpha | beta | h1 | h2 | e2 | Y | theta2 | res | scal2 | sc | part
+    DeviceBuffer<double> d_slots;   // 16 n
+    DeviceBuffer<double> d_rowsum;  // n
+    DeviceBuffer<double> d_rbar;    // n
+    DeviceBuffer<double> d_scal;    // 16: [0] matrixMean, [2] ||T||
+    DeviceBuffer<double> d_evals;   // kmax
+    DeviceBuffer<double> d_evecs;   // n x kmax, column-major
+    DeviceBuffer<double> d_lu;      // 8 kLzCap: inverse-iteration scratch
+    DeviceBuffer<int> d_nz;
+    DeviceBuffer<int> d_st;         // {step, flag, ticket, step cap}
     cudaEvent_t ev_v = nullptr;  // v_j is ready on rank 0
     int last_iters = 0;
 };
@@ -261,32 +318,32 @@ void band_eig_free(BandEigWork& w);
 // ---- centering + eigensolve (eig.cu) ---------------------------------------------------------------
 struct EigWork {
     int n = 0;
-    double* d_C = nullptr;     // n x n centered matrix, overwritten by the tridiagonalisation
-    double* d_rowsum = nullptr;
-    double* d_v = nullptr;     // Householder vector of the current step (n)
-    double* d_w = nullptr;     // w vector of the current step (n)
-    double* d_p = nullptr;     // p = tau A v (n)
-    double* d_diag = nullptr;  // n
-    double* d_off = nullptr;   // n
-    double* d_tau = nullptr;   // n
-    double* d_scal = nullptr;  // small scalar scratch
-    double* d_evals = nullptr; // k
-    double* d_evecs = nullptr; // n x k (column-major)
-    double* d_lu = nullptr;    // 8 n scratch for inverse iteration
-    int* d_nz = nullptr;
-    int* d_step = nullptr;               // {next step, step of the pending trailing update}
+    DeviceBuffer<double> d_C;     // n x n centered matrix, overwritten by the tridiagonalisation
+    DeviceBuffer<double> d_rowsum;
+    DeviceBuffer<double> d_v;     // Householder vector of the current step (n)
+    DeviceBuffer<double> d_w;     // w vector of the current step (n)
+    DeviceBuffer<double> d_p;     // p = tau A v (n)
+    DeviceBuffer<double> d_diag;  // n
+    DeviceBuffer<double> d_off;   // n
+    DeviceBuffer<double> d_tau;   // n
+    DeviceBuffer<double> d_scal;  // small scalar scratch
+    DeviceBuffer<double> d_evals; // k
+    DeviceBuffer<double> d_evecs; // n x k (column-major)
+    DeviceBuffer<double> d_lu;    // 8 n scratch for inverse iteration
+    DeviceBuffer<int> d_nz;
+    DeviceBuffer<int> d_step;               // {next step, step of the pending trailing update}
     cudaGraphExec_t graph_exec = nullptr; // kGraphSteps tridiagonalisation steps, replayed n / kGraphSteps times
     int graph_n = 0;
     bool graph_fused = false;
     int kmax = 0;
     // persistent Lanczos workspace (allocated on the first solve in that form)
-    double* d_V = nullptr;      // n x kLzCap orthonormal basis, column-major
-    double* d_lzw = nullptr;    // 2 n: w ping-pong
-    double* d_lzs = nullptr;    // alpha | beta | e2 | Y | theta2 | res | scal2 | part | hpart
-    int* d_lzst = nullptr;      // {step, flag, ticket, step cap}
-    unsigned* d_lzbar = nullptr;   // grid barrier counter of the persistent Lanczos kernel
-    double* d_lzG = nullptr;       // kLzCap x kLzCap: V^T V of the Lanczos basis (one-reduction Gram-Schmidt)
-    long long* d_lzprof = nullptr; // VPCA_LZ_PROF=1: phase timestamps of block 0 (first 64 steps)
+    DeviceBuffer<double> d_V;      // n x kLzCap orthonormal basis, column-major
+    DeviceBuffer<double> d_lzw;    // 2 n: w ping-pong
+    DeviceBuffer<double> d_lzs;    // alpha | beta | e2 | Y | theta2 | res | scal2 | part | hpart
+    DeviceBuffer<int> d_lzst;      // {step, flag, ticket, step cap}
+    DeviceBuffer<unsigned> d_lzbar;   // grid barrier counter of the persistent Lanczos kernel
+    DeviceBuffer<double> d_lzG;       // kLzCap x kLzCap: V^T V of the Lanczos basis (one-reduction Gram-Schmidt)
+    DeviceBuffer<long long> d_lzprof; // VPCA_LZ_PROF=1: phase timestamps of block 0 (first 64 steps)
     bool c_valid = false;       // d_C holds the centred matrix of the last center_gram()
     int lz_blocks = -1;         // blocks of the persistent kernel (= SMs; 0: cooperative launch unavailable or
                                 // VPCA_LZ_PERSIST=0; -1: not queried yet, at the first Lanczos solve)

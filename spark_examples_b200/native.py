@@ -54,7 +54,7 @@ EXPORTED_SYMBOLS = (
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
     "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
     "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact", "vpca_sample_missing_bed",
-    "vpca_subset_bed_samples",
+    "vpca_subset_bed_samples", "vpca_debug_device_bytes",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
@@ -228,6 +228,8 @@ def load_library() -> ctypes.CDLL:
     L.vpca_debug_schedule.argtypes = [i32, i32, i32, i32, i32, i32, ctypes.c_double, vp, i32, vp]
     L.vpca_debug_lanczos_profile.restype = ctypes.c_int
     L.vpca_debug_lanczos_profile.argtypes = [vp, vp, i32]
+    L.vpca_debug_device_bytes.restype = i64
+    L.vpca_debug_device_bytes.argtypes = []
     L.vpca_debug_rebalance.restype = ctypes.c_int
     L.vpca_debug_rebalance.argtypes = [vp, i32, i32, i32, i32, vp, vp, i32]
     L.vpca_set_gram.restype = ctypes.c_int

@@ -422,6 +422,40 @@ int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
                         double* out_hwe_p);
 int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out_p);
 
+/* ---- variance-standardized genomic relationship matrix (beyond VariantsPca.scala: PLINK 2 / GCTA / EIGENSOFT's PCA;
+ * DESIGN.md 13) ------------------------------------------------------------------------------------------------------
+ * For each variant of PLINK 1 .bed rows (as vpca_accumulate_bed; bytes past ceil(n_samples / 4) and the padding bits of
+ * the last byte are ignored), with HOM_A1, HET, HOM_A2 the exact counts of vpca_variant_qc_bed over all n_samples
+ * samples, n = HOM_A1 + HET + HOM_A2 and a = 2 HOM_A1 + HET: the variant is USED iff 0 < a < 2n.  For a used variant,
+ * r = min(a, 2n - a) counts the less common allele (A1 at a tie), and, each operation rounded once (no contraction),
+ *   mu = r / n   q = r / (2n)   s = 1 / sqrt(mu (1 - q))   z_d = (d - mu) s
+ * for that allele's count d of a called sample, z = 0 for a missing call.  GRM = (1/M) sum over the M used variants of
+ * z z^T, FP64, each finished cell divided by M once.  Counting A1 or A2 gives the same GRM bit for bit.
+ * The used variants are packed in row order into panels of a fixed number of variants and each panel is multiplied on the
+ * FP64 tensor cores, so the GRM's bits depend only on the ordered sequence of used variants: not on how the rows are
+ * split into calls, on stride_bytes or on skipped variants anywhere.
+ * The sum accumulates in the eigensolver's FP64 N x N matrix (the one vpca_get_centered returns; 34 GB at 65 535
+ * samples), allocated on the first call if no solve has allocated it.  The GRM calls leave the PCA Gram, U, the kinship
+ * counts, the LD state, the QC buffers and the subset state alone.  vpca_compute_pca and vpca_get_centered overwrite
+ * the matrix, and so does a GRM solve by the direct reduction: afterwards vpca_get_grm, vpca_compute_pca_grm and
+ * vpca_grm_bed return VPCA_ERR_STATE until vpca_reset.  Driver-side and synchronous.
+ * vpca_grm_bed: adds the rows; successive calls add up.  Rows are staged in chunks of at most 64 MB on a lane (H2D of
+ *   chunk i + 1 overlapped with the work on chunk i).  VPCA_ERR_STATE after vpca_grm_finalize (until vpca_reset).
+ * vpca_grm_finalize: multiplies the last partial panel, divides by M and mirrors the lower triangle; *n_used = M (may be
+ *   NULL).  Calling it again returns M again.  VPCA_ERR_STATE when M = 0, and from then on every GRM call until vpca_reset.
+ * vpca_get_grm: the finalized GRM, symmetric N x N row-major.
+ * vpca_compute_pca_grm: the k largest eigenpairs of the GRM as it is (no second centring), with the shapes, sign rule and
+ *   k range of vpca_compute_pca: vecs N x k column-major, evals k (may be NULL), 1 <= k <= min(N, max(num_pc, 16)).
+ *   The band solver's Lanczos on the FP64 cells from 512 samples up (the GRM stays valid); below that, with
+ *   VPCA_EIG=direct and as the Lanczos fallback the direct reduction, which consumes the GRM.  It leaves no U:
+ *   vpca_loadings_* return VPCA_ERR_STATE afterwards.
+ * VPCA_ERR_BAD_ARG, before any row is staged: NULL ctx / rows (nv > 0) / out / vecs, nv < 0, stride_bytes <
+ *   ceil(n_samples / 4), k out of range.  VPCA_ERR_UNSUPPORTED above 65 535 samples or on a band-only context. */
+int vpca_grm_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes);
+int vpca_grm_finalize(vpca_ctx* ctx, int64_t* n_used);
+int vpca_get_grm(vpca_ctx* ctx, double* out);
+int vpca_compute_pca_grm(vpca_ctx* ctx, int32_t k, double* vecs, double* evals);
+
 /* ---- sample quality control (beyond VariantsPca.scala: which samples go into S; DESIGN.md 11) -------------------------
  * --keep / --remove / --mind decide the samples of a run before its context exists: the per-sample missing-call counts
  * over every row of a fileset, then the rows repacked to the kept samples, which a plain run reads as its fileset.

@@ -126,4 +126,7 @@ class PcaConf(GenomicsConf):
             ("keep", str, None, False),                   # --bed-path runs: analyse only the samples listed in this ID file
             ("remove", str, None, False),                 # --bed-path runs: leave out the samples listed in this ID file
             ("mind", float, None, False),                 # --bed-path runs: drop samples with missing-call rate > this
+            ("grm", bool, False, False),                  # --bed-path runs: PCs of the variance-standardized relationship
+                                                          # matrix of allele dosages (PLINK 2 / GCTA / EIGENSOFT) instead of S
+            ("makeRel", bool, False, False),              # with --grm and --output-path P: write P.rel.bin and P.rel.id
         ]

@@ -1401,6 +1401,23 @@ __device__ __forceinline__ int4 band_load(const int32_t* __restrict__ S, int n, 
     return s;
 }
 
+// The same for FP64 cells (the GRM), read as two double2.
+template <bool VEC>
+__device__ __forceinline__ double4 band_load(const double* __restrict__ S, int n, int row0, int i, int iend, int c) {
+    double4 s = make_double4(0.0, 0.0, 0.0, 0.0);
+    if (i >= iend || c > i) return s;
+    const double* p = S + (size_t)(i - row0) * n + c;
+    if (VEC && c + 3 <= i) {
+        const double2 lo = __ldg(reinterpret_cast<const double2*>(p)), hi = __ldg(reinterpret_cast<const double2*>(p) + 1);
+        return make_double4(lo.x, lo.y, hi.x, hi.y);
+    }
+    s.x = __ldg(p);
+    if (c + 1 <= i) s.y = __ldg(p + 1);
+    if (c + 2 <= i) s.z = __ldg(p + 2);
+    if (c + 3 <= i) s.w = __ldg(p + 3);
+    return s;
+}
+
 // 32 values per lane in, lane l out with the sum over the warp of value l (fixed order: 31 exchanges, not 32 reductions).
 // Stage OFF: the lane with bit OFF set keeps the upper half of its live values, its partner the lower half.
 template <int OFF, typename T>
@@ -1425,12 +1442,14 @@ __device__ __forceinline__ T warp_transpose_sum(T (&rp)[32], int lane) {
 }
 
 // grid (ceil((row0 + rows) / kBandTC), ceil(rows / kBandTR)).  T = double: the partials of S v.  T = long long: the same
-// traversal with v = 1 in exact integer arithmetic, i.e. the partial row sums of the symmetric S.
-template <typename T, bool VEC>
-__global__ void __launch_bounds__(kBandThreads, 2) band_tile_kernel(const int32_t* __restrict__ S, int n, int row0, int rows,
+// traversal with v = 1 in exact integer arithmetic, i.e. the partial row sums of the symmetric S (int32 cells only).
+// Cell: int32_t (the Gram) or double (the GRM).
+template <typename T, bool VEC, class Cell>
+__global__ void __launch_bounds__(kBandThreads, 2) band_tile_kernel(const Cell* __restrict__ S, int n, int row0, int rows,
                                                                    const double* __restrict__ v, T* __restrict__ rowp,
                                                                    T* __restrict__ colp) {
     constexpr bool kDot = std::is_same<T, double>::value;
+    constexpr int kLoads = std::is_same<Cell, double>::value ? 2 : 8;   // rows loaded at once (FP64: within 128 registers)
     __shared__ double vrow[kBandTR];
     __shared__ T rsum[kBandThreads / 32][kBandTR];
     const int i0 = row0 + (int)blockIdx.y * kBandTR;
@@ -1452,24 +1471,28 @@ __global__ void __launch_bounds__(kBandThreads, 2) band_tile_kernel(const int32_
     for (int h = 0; h < kBandTR / 32; ++h) {
         T rp[32];
 #pragma unroll
-        for (int r0 = 0; r0 < 32; r0 += 8) {
-            int4 sv[8];
+        for (int r0 = 0; r0 < 32; r0 += kLoads) {
+            std::conditional_t<std::is_same<Cell, double>::value, double4, int4> sv[kLoads];
 #pragma unroll
-            for (int u = 0; u < 8; ++u) sv[u] = band_load<VEC>(S, n, row0, i0 + h * 32 + r0 + u, iend, c);   // 8 loads in flight
+            for (int u = 0; u < kLoads; ++u) sv[u] = band_load<VEC>(S, n, row0, i0 + h * 32 + r0 + u, iend, c);   // in flight
 #pragma unroll
-            for (int u = 0; u < 8; ++u) {
+            for (int u = 0; u < kLoads; ++u) {
                 const int i = i0 + h * 32 + r0 + u;
-                const int32_t s[4] = {sv[u].x, sv[u].y, sv[u].z, sv[u].w};
+                const Cell s[4] = {sv[u].x, sv[u].y, sv[u].z, sv[u].w};
                 // cells above the diagonal were loaded as 0; the diagonal cell (column i) feeds the row only
                 if constexpr (kDot) {
                     const double vi = vrow[h * 32 + r0 + u];
                     double d[4];
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) d[e] = lz_i2d(s[e]);
+                    for (int e = 0; e < 4; ++e) {
+                        if constexpr (std::is_same<Cell, double>::value) d[e] = s[e];
+                        else d[e] = lz_i2d(s[e]);
+                    }
                     rp[r0 + u] = (d[0] * vc[0] + d[1] * vc[1]) + (d[2] * vc[2] + d[3] * vc[3]);
 #pragma unroll
                     for (int e = 0; e < 4; ++e) cacc[e] += (c + e < i ? d[e] : 0.0) * vi;
                 } else {
+                    static_assert(std::is_same<Cell, int32_t>::value, "exact row sums are of int32 cells");
                     rp[r0 + u] = ((long long)s[0] + s[1]) + ((long long)s[2] + s[3]);
 #pragma unroll
                     for (int e = 0; e < 4; ++e) cacc[e] += c + e < i ? s[e] : 0;
@@ -1577,7 +1600,8 @@ __global__ void band_scale_kernel(const double* __restrict__ wbuf, int n, const 
 }
 
 // Step j, part 3: S v_j = the ranks' partials added in rank order, then the centring applied to the vector as in
-// lz_persist_kernel: (C v)_i = (S v)_i - rbar_i sum(v) - rbar . v + mean sum(v)  -> w_out
+// lz_persist_kernel: (C v)_i = (S v)_i - rbar_i sum(v) - rbar . v + mean sum(v)  -> w_out.  FP64 cells (the GRM, which
+// is centred already) have rbar = 0 and mean = 0, so w_out = S v exactly.
 __global__ void band_combine_kernel(const double* __restrict__ slots, int n, int world, BandEnds be,
                                     const double* __restrict__ rbar, const double* __restrict__ sc,
                                     const double* __restrict__ scal, double* __restrict__ wbuf, const int* __restrict__ st) {
@@ -1677,11 +1701,12 @@ static cudaError_t lanczos_topk(EigWork& w, int k, cudaStream_t stream, int64_t*
          (size_t)kLzVtCols * kLzVtCols + kLzCap + (((size_t)rows_per + 1) & ~(size_t)1)) * sizeof(double);
     // persistent form (one cooperative launch per chunk) whenever that layout fits; otherwise, and with VPCA_LZ_PERSIST=0,
     // the band solver with the whole Gram as its one band (reads S, no FP64 matrix)
-    if (w.lz_blocks == 0 || base_smem > w.lz_smem_max) {
+    if (w.grm || w.lz_blocks == 0 || base_smem > w.lz_smem_max) {   // (FP64 cells: always the band solver)
         BandPart& p = w.band_part;
         VPCA_TRY(cudaGetDevice(&p.device));
         p.stream = stream;
-        p.d_S = w.d_S;
+        p.d_S = w.grm ? nullptr : w.d_S;
+        p.d_Sd = w.grm ? w.d_C.get() : nullptr;
         p.n = n;
         p.row0 = 0;
         p.rows = n;
@@ -1863,7 +1888,8 @@ cudaError_t eig_topk(EigWork& w, int k, cudaStream_t stream, int64_t* launches) 
         }
         w.last_method = 3;
     }
-    cudaError_t e = center_matrix(w, stream);   // the reduction works on (and overwrites) the FP64 matrix
+    // the reduction works on (and overwrites) the FP64 matrix: the centred Gram, or the GRM d_C holds (symmetric already)
+    cudaError_t e = w.grm ? cudaSuccess : center_matrix(w, stream);
     if (e != cudaSuccess) return e;
     w.c_valid = false;
     e = cudaMemsetAsync(w.d_v.get(), 0, 2 * (size_t)n * sizeof(double), stream);
@@ -1978,9 +2004,18 @@ cudaError_t band_product(const BandPart& p, const double* v, T* y) {
     const dim3 grid((unsigned)((ncols + kBandTC - 1) / kBandTC), (unsigned)((p.rows + kBandTR - 1) / kBandTR));
     T* rowp = reinterpret_cast<T*>(p.d_scratch.get());
     T* colp = rowp + (size_t)grid.x * p.rows;
+    if constexpr (std::is_same<T, double>::value) {
+        if (p.d_Sd != nullptr) {   // FP64 cells
+            const bool vec = (p.n & 3) == 0 && (reinterpret_cast<uintptr_t>(p.d_Sd) & 31) == 0;
+            if (vec) band_tile_kernel<T, true, double><<<grid, kBandThreads, 0, p.stream>>>(p.d_Sd, p.n, p.row0, p.rows, v, rowp, colp);
+            else band_tile_kernel<T, false, double><<<grid, kBandThreads, 0, p.stream>>>(p.d_Sd, p.n, p.row0, p.rows, v, rowp, colp);
+            band_reduce_kernel<T><<<(ncols + 255) / 256, 256, 0, p.stream>>>(rowp, colp, p.row0, p.rows, y);
+            return cudaGetLastError();
+        }
+    }
     const bool vec = (p.n & 3) == 0 && (reinterpret_cast<uintptr_t>(p.d_S) & 15) == 0;
-    if (vec) band_tile_kernel<T, true><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
-    else band_tile_kernel<T, false><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
+    if (vec) band_tile_kernel<T, true, int32_t><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
+    else band_tile_kernel<T, false, int32_t><<<grid, kBandThreads, 0, p.stream>>>(p.d_S, p.n, p.row0, p.rows, v, rowp, colp);
     band_reduce_kernel<T><<<(ncols + 255) / 256, 256, 0, p.stream>>>(rowp, colp, p.row0, p.rows, y);
     return cudaGetLastError();
 }
@@ -2079,13 +2114,20 @@ cudaError_t band_eig_topk(BandEigWork& w, BandPart* const* parts, int world, int
         return cudaGetLastError();
     };
 
-    // ---- row sums (exact, int64), matrixMean and non_zero_rows (VariantsPca.scala:206-211)
-    if (world > 1) VPCA_TRY(cudaEventRecord(w.ev_v, s0));   // the ranks write rank 0's slots after its earlier work
-    VPCA_TRY(gather((long long*)nullptr, nullptr));
-    band_rowsum_kernel<<<(n + 255) / 256, 256, 0, s0>>>(reinterpret_cast<const long long*>(w.d_slots.get()), n, world, be,
-                                                         w.d_rowsum.get(), w.d_rbar.get());
+    // ---- row sums (exact, int64), matrixMean and non_zero_rows (VariantsPca.scala:206-211); FP64 cells are solved as
+    // they are: row sums, rbar and the mean 0
+    if (p0.d_Sd != nullptr) {
+        VPCA_TRY(cudaMemsetAsync(w.d_rowsum.get(), 0, (size_t)n * sizeof(double), s0));
+        VPCA_TRY(cudaMemsetAsync(w.d_rbar.get(), 0, (size_t)n * sizeof(double), s0));
+    } else {
+        if (world > 1) VPCA_TRY(cudaEventRecord(w.ev_v, s0));   // the ranks write rank 0's slots after its earlier work
+        VPCA_TRY(gather((long long*)nullptr, nullptr));
+        band_rowsum_kernel<<<(n + 255) / 256, 256, 0, s0>>>(reinterpret_cast<const long long*>(w.d_slots.get()), n, world, be,
+                                                             w.d_rowsum.get(), w.d_rbar.get());
+        nl += 1;
+    }
     matrix_mean_kernel<<<1, 1024, 0, s0>>>(w.d_rowsum.get(), n, w.d_scal.get(), w.d_nz.get());
-    nl += 2;
+    nl += 1;
 
     // ---- main run: the convergence policy is that of lanczos_topk's persistent form
     LzPolicy policy(n);

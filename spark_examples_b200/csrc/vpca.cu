@@ -104,6 +104,16 @@ struct vpca_ctx {
     cudaEvent_t sm_ev_copy[2] = {nullptr, nullptr}, sm_ev_kern[2] = {nullptr, nullptr};
     GramPlan ld_plan;
     LdWork ld;
+    // GRM (vpca_grm_bed / _finalize, grm.cu): double-buffered raw rows, the chunk's counts, z tables, used flags and used
+    // list, and one FP64 panel; the sum itself accumulates in eig.d_C.  All grow-only.
+    DeviceBuffer<uint8_t> d_grm_rows[2];
+    DeviceBuffer<int32_t> d_grm_counts, d_grm_used, d_grm_inv;
+    DeviceBuffer<double> d_grm_tab, d_grm_Z;
+    DeviceBuffer<int> d_grm_total;
+    int grm_state = 0;      // 0 none, 1 accumulating, 2 finalized (eig.d_C holds the GRM), 3 unusable until vpca_reset
+                            // (finalized with no used variant, or d_C overwritten by another solve)
+    int64_t grm_used = 0;   // used variants so far (M)
+    int grm_fill = 0;       // of which in the current, not yet multiplied panel
 
     struct Slot {
         int64_t pid = -1;
@@ -689,6 +699,9 @@ int vpca_reset(vpca_ctx* ctx) {
     if (ctx->d_kin.get() != nullptr)
         CUDA_OK(ctx, cudaMemsetAsync(ctx->d_kin.get(), 0, (size_t)9 * ctx->n * ctx->n * sizeof(int32_t), ctx->stream));
     ctx->kin_variants = 0;
+    ctx->grm_state = 0;
+    ctx->grm_used = 0;
+    ctx->grm_fill = 0;
     for (auto& s : ctx->slots) s.used = false;
     ctx->finalized = false;
     ctx->pca_done = false;
@@ -1245,6 +1258,7 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
                     "behind VariantsPca.scala:226 refuses more columns); the Gram itself has no such limit");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->pca_k = 0;   // U is overwritten from here on
+    if (ctx->grm_state != 0) ctx->grm_state = 3;   // the solve may use d_C
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_e0, ctx->stream));
     int rc = run_center(ctx, false);   // row sums + mean; the solver materialises C only if it needs it
     if (rc != VPCA_OK) return rc;
@@ -1279,6 +1293,7 @@ int vpca_get_centered(vpca_ctx* ctx, double* out) {
     if (!ctx->finalized) return fail(ctx, VPCA_ERR_STATE, "call vpca_finalize_gram first");
     if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_STATE, "this context stores a row band of the Gram");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (ctx->grm_state != 0) ctx->grm_state = 3;   // d_C is about to hold the centred Gram
     int rc = run_center(ctx, true);   // the eigensolve overwrites C, so recompute it
     if (rc != VPCA_OK) return rc;
     const size_t bytes = (size_t)ctx->n * ctx->n * sizeof(double);
@@ -2137,6 +2152,204 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
         ctx->c_d2h += 8 * nvc;
     }
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+// ---- variance-standardized relationship matrix (grm.cu, DESIGN.md 13) ---------------------------------------------------
+// Driver-side and synchronous.  Rows are staged in chunks of at most kGrmStageBytes on a lane, the upload of chunk i + 1 on
+// the copy stream overlapping the work on chunk i.  Per chunk: counts, tables and the used list, then (after one small
+// read-back of the used count) the used columns expanded into the panel, which is multiplied into eig.d_C whenever it is
+// full.
+namespace {
+constexpr int64_t kGrmStageBytes = 64ll << 20;   // raw .bed bytes per staged chunk
+constexpr int64_t kGrmMaxChunk = 1ll << 20;      // rows per staged chunk
+
+int grm_check(vpca_ctx* ctx) {
+    if (ctx->n > 65535)
+        return fail(ctx, VPCA_ERR_UNSUPPORTED, "the GRM is limited to 65535 samples, like vpca_compute_pca; this context has %d",
+                    ctx->n);
+    if (ctx->band_rows != ctx->n) return fail(ctx, VPCA_ERR_UNSUPPORTED, "the GRM needs a context that stores the whole Gram");
+    return VPCA_OK;
+}
+
+// The eigensolver workspace (whose d_C holds the sum) and the staging buffers; d_C and the panel zeroed on the first call.
+int grm_buffers(vpca_ctx* ctx, vpca_ctx::Lane& L, int64_t step, int64_t stride) {
+    if (!ctx->eig_ready) {
+        cudaError_t e = eig_alloc(ctx->eig, ctx->n, std::max(ctx->num_pc, 16));
+        if (e != cudaSuccess) return fail(ctx, VPCA_ERR_NOMEM, "eigensolver workspace: %s", cudaGetErrorString(e));
+        ctx->eig_ready = true;
+    }
+    const int64_t zc = grm_panel_rows(ctx->n) * kGrmPanelK;
+    cudaError_t e = cudaSuccess;
+    for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride);
+    if (e == cudaSuccess) e = ctx->d_grm_counts.ensure(4 * step);
+    if (e == cudaSuccess) e = ctx->d_grm_tab.ensure(4 * step);
+    if (e == cudaSuccess) e = ctx->d_grm_used.ensure(step);
+    if (e == cudaSuccess) e = ctx->d_grm_inv.ensure(step);
+    if (e == cudaSuccess) e = ctx->d_grm_total.ensure(1);
+    if (e == cudaSuccess) e = ctx->d_grm_Z.ensure(zc);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(ctx, VPCA_ERR_NOMEM, "GRM buffers: %s", cudaGetErrorString(e));
+    }
+    if (ctx->grm_state == 0) {
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->eig.d_C.get(), 0, (size_t)ctx->n * ctx->n * sizeof(double), L.stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->d_grm_Z.get(), 0, (size_t)zc * sizeof(double), L.stream));
+        ctx->eig.c_valid = false;
+        ctx->grm_used = 0;
+        ctx->grm_fill = 0;
+        ctx->grm_state = 1;
+    }
+    return VPCA_OK;
+}
+}   // namespace
+
+int vpca_grm_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    const int n = ctx->n;
+    if (nv < 0 || (nv > 0 && rows == nullptr) || stride_bytes < (n + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_grm_bed: bad argument (rows must be set, nv >= 0, stride_bytes >= "
+                    "ceil(n_samples / 4))");
+    int rc = grm_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->grm_state >= 2)
+            return fail(ctx, VPCA_ERR_STATE, "the GRM was finalized (or its matrix overwritten) since the last vpca_reset");
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int64_t step = std::max<int64_t>(1, std::min({nv, kGrmStageBytes / stride_bytes, kGrmMaxChunk}));
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    rc = grm_buffers(ctx, L, step, stride_bytes);
+    if (rc != VPCA_OK) return rc;
+    const int64_t nchunks = (nv + step - 1) / step;
+    auto upload = [&](int64_t c) -> cudaError_t {
+        const int b = (int)(c & 1);
+        const int64_t v = c * step, nvc = std::min(step, nv - v);
+        cudaError_t e = cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0);
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(ctx->d_grm_rows[b].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+                                cudaMemcpyHostToDevice, L.copy_stream);
+        if (e == cudaSuccess) e = cudaEventRecord(L.ev_copy[b], L.copy_stream);
+        ctx->c_h2d += nvc * stride_bytes;
+        return e;
+    };
+    CUDA_OK(ctx, upload(0));
+    double* Z = ctx->d_grm_Z.get();
+    double* C = ctx->eig.d_C.get();
+    for (int64_t c = 0; c < nchunks; ++c) {
+        const int b = (int)(c & 1);
+        const int nvc = (int)std::min(step, nv - c * step);
+        if (c + 1 < nchunks) CUDA_OK(ctx, upload(c + 1));
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        const uint8_t* d_rows = ctx->d_grm_rows[b].get();
+        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, nvc, n, ctx->d_grm_counts.get(), L.stream));
+        CUDA_OK(ctx, grm_tables(ctx->d_grm_counts.get(), nvc, ctx->d_grm_tab.get(), ctx->d_grm_used.get(),
+                                ctx->d_grm_inv.get(), ctx->d_grm_total.get(), L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, ctx->d_grm_total.get(), sizeof(int), cudaMemcpyDeviceToHost, L.stream));
+        CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+        ctx->c_launches += 3;
+        const int used = *L.h_flags;
+        for (int j = 0; j < used;) {
+            const int cnt = std::min(kGrmPanelK - ctx->grm_fill, used - j);
+            CUDA_OK(ctx, grm_expand(d_rows, stride_bytes, ctx->d_grm_inv.get() + j, ctx->d_grm_tab.get(), cnt, n, Z,
+                                    ctx->grm_fill, L.stream));
+            ctx->c_launches += 1;
+            ctx->grm_fill += cnt;
+            j += cnt;
+            if (ctx->grm_fill == kGrmPanelK) {
+                CUDA_OK(ctx, grm_syrk(Z, n, C, L.stream));
+                ctx->c_launches += 1;
+                ctx->grm_fill = 0;
+            }
+        }
+        ctx->grm_used += used;
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
+    return VPCA_OK;
+}
+
+int vpca_grm_finalize(vpca_ctx* ctx, int64_t* n_used) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int rc = grm_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (ctx->grm_state == 3)
+        return fail(ctx, VPCA_ERR_STATE, "the GRM has no used variant or its matrix was overwritten: call vpca_reset");
+    if (ctx->grm_state == 2) {
+        if (n_used) *n_used = ctx->grm_used;
+        return VPCA_OK;
+    }
+    if (ctx->grm_used == 0) {
+        ctx->grm_state = 3;
+        return fail(ctx, VPCA_ERR_STATE, "no variant of the GRM varies among its called samples (M = 0)");
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    const int n = ctx->n;
+    if (ctx->grm_fill > 0) {   // the partial panel, its unfilled columns zeroed
+        double* Z = ctx->d_grm_Z.get();
+        CUDA_OK(ctx, cudaMemset2DAsync(Z + ctx->grm_fill, kGrmPanelK * sizeof(double), 0,
+                                       (size_t)(kGrmPanelK - ctx->grm_fill) * sizeof(double), (size_t)n, ctx->stream));
+        CUDA_OK(ctx, grm_syrk(Z, n, ctx->eig.d_C.get(), ctx->stream));
+        ctx->c_launches += 1;
+        ctx->grm_fill = 0;
+    }
+    CUDA_OK(ctx, grm_finish(ctx->eig.d_C.get(), n, ctx->grm_used, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_launches += 1;
+    ctx->grm_state = 2;
+    if (n_used) *n_used = ctx->grm_used;
+    return VPCA_OK;
+}
+
+int vpca_get_grm(vpca_ctx* ctx, double* out) {
+    if (ctx == nullptr || out == nullptr) return fail(ctx, VPCA_ERR_BAD_ARG, "NULL argument");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (ctx->grm_state != 2) return fail(ctx, VPCA_ERR_STATE, "no finalized GRM (call vpca_grm_finalize; a solve that "
+                                         "overwrote it needs vpca_reset and the rows again)");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    const size_t bytes = (size_t)ctx->n * ctx->n * sizeof(double);
+    CUDA_OK(ctx, cudaMemcpyAsync(out, ctx->eig.d_C.get(), bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_d2h += (int64_t)bytes;
+    return VPCA_OK;
+}
+
+int vpca_compute_pca_grm(vpca_ctx* ctx, int32_t k, double* vecs, double* evals) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (vecs == nullptr || k < 1 || k > ctx->n || k > std::max(ctx->num_pc, 16))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_compute_pca_grm: k=%d out of range", k);
+    if (ctx->grm_state != 2) return fail(ctx, VPCA_ERR_STATE, "no finalized GRM (call vpca_grm_finalize; a solve that "
+                                         "overwrote it needs vpca_reset and the rows again)");
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    ctx->pca_k = 0;   // a GRM solve leaves no U for the loadings
+    ctx->pca_done = false;
+    {
+        const char* em = getenv("VPCA_EIG");
+        ctx->eig.mode = (em != nullptr && strcmp(em, "direct") == 0) ? 1 : (em != nullptr && strcmp(em, "lanczos") == 0) ? 2 : 0;
+    }
+    CUDA_OK(ctx, cudaEventRecord(ctx->ev_e0, ctx->stream));
+    int64_t launches = 0;
+    ctx->eig.grm = true;
+    const cudaError_t e = eig_topk(ctx->eig, k, ctx->stream, &launches);
+    ctx->eig.grm = false;
+    if (e != cudaSuccess || ctx->eig.last_method != 2) ctx->grm_state = 3;   // the direct reduction consumed d_C
+    CUDA_OK(ctx, e);
+    ctx->c_launches += launches;
+    CUDA_OK(ctx, cudaEventRecord(ctx->ev_e1, ctx->stream));
+    ctx->st.eig_method = ctx->eig.last_method;
+    ctx->st.eig_iterations = ctx->eig.last_iters;
+    ctx->eig_timed = true;
+    const size_t nb = (size_t)ctx->n * k * sizeof(double);
+    CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->eig.d_evecs.get(), nb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, ctx->eig.d_evals.get(), k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0);
     return VPCA_OK;
 }
 

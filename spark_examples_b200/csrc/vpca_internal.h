@@ -218,6 +218,24 @@ cudaError_t qc_count(const uint8_t* d_rows, int64_t pitch, int nv, int n, int32_
 // The exact HWE p-value (vpca.h) of each of nv count rows (layout above, 16-byte aligned).  Never synchronises.
 cudaError_t qc_hwe(const int32_t* d_counts, int nv, double* d_p, cudaStream_t stream);
 
+// ---- variance-standardized relationship matrix (grm.cu, DESIGN.md 13) -----------------------------------------------
+// Used variants per FP64 panel: a constant, so that the panel boundaries, and with them the bits of the sum, depend only
+// on the ordered sequence of used variants.
+constexpr int kGrmPanelK = 1024;
+// Rows of a panel: n rounded up to the SYRK's tile edge (rows >= n stay zero).
+int64_t grm_panel_rows(int n);
+// From nv count rows (qc_count's layout): d_tab[4v ..] = z of each .bed code (0 for missing calls and unused variants),
+// d_used[v] in {0, 1}, d_inv[0 .. *d_total) = the used variants in row order.  Never synchronises.
+cudaError_t grm_tables(const int32_t* d_counts, int nv, double* d_tab, int32_t* d_used, int32_t* d_inv, int* d_total,
+                       cudaStream_t stream);
+// Panel columns [col0, col0 + cnt) = the z columns of rows d_inv[0 .. cnt) (row v at d_rows + v * stride), samples < n.
+cudaError_t grm_expand(const uint8_t* d_rows, int64_t stride, const int32_t* d_inv, const double* d_tab, int cnt, int n,
+                       double* d_Z, int col0, cudaStream_t stream);
+// Lower-triangle tiles of d_C (n x n row-major) += Z Z^T over the kGrmPanelK columns of the panel.  Never synchronises.
+cudaError_t grm_syrk(const double* d_Z, int n, double* d_C, cudaStream_t stream);
+// d_C = its lower triangle / m, mirrored to the upper one.
+cudaError_t grm_finish(double* d_C, int n, int64_t m, cudaStream_t stream);
+
 // ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
 // Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to
 // d_missing[0 .. n) with integer atomics.  Bytes past ceil(n / 4) and the padding bits of the last byte are ignored.
@@ -285,6 +303,7 @@ struct BandPart {
     int device = 0;
     cudaStream_t stream = nullptr;
     const int32_t* d_S = nullptr;   // row row0 of the band
+    const double* d_Sd = nullptr;   // or, when set, the band of an FP64 matrix that is solved as it is (no centring)
     int n = 0, row0 = 0, rows = 0;
     DeviceBuffer<double> d_v;       // n: the Lanczos vector of the step
     DeviceBuffer<double> d_y;       // row0 + rows: the partial product (or partial row sums as int64)
@@ -354,6 +373,8 @@ struct EigWork {
     int last_method = 0;        // 1 direct, 2 Lanczos, 3 Lanczos abandoned -> direct
     int last_iters = 0;         // Lanczos steps of the last solve
     int mode = 0;               // 0 auto, 1 direct, 2 Lanczos whenever n allows
+    bool grm = false;           // eig_topk solves d_C as it is (the GRM, symmetric): the band solver's Lanczos on FP64
+                                // cells, or the direct reduction, which consumes d_C
 };
 cudaError_t eig_alloc(EigWork& w, int n, int kmax);
 void eig_free(EigWork& w);

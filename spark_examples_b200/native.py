@@ -54,11 +54,13 @@ EXPORTED_SYMBOLS = (
     "vpca_project_bed", "vpca_project_panels", "vpca_project_get", "vpca_compute_pca_bands",
     "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
     "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact", "vpca_sample_missing_bed",
-    "vpca_subset_bed_samples", "vpca_debug_device_bytes",
+    "vpca_subset_bed_samples", "vpca_debug_device_bytes", "vpca_grm_bed", "vpca_grm_finalize", "vpca_get_grm",
+    "vpca_compute_pca_grm",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
 LD_MAX_WINDOW = 4096          # vpca_ld_prune_bed: variants a window may reach back (VPCA_LD_MAX_WINDOW)
+GRM_MAX_SAMPLES = 65535       # vpca_grm_* / vpca_compute_pca_grm: the sample limit of vpca_compute_pca
 
 
 class VpcaError(RuntimeError):
@@ -296,6 +298,14 @@ def load_library() -> ctypes.CDLL:
     L.vpca_subset_bed_samples.argtypes = [vp, vp, i64, i64, i32, vp, i32, vp, i64]
     L.vpca_compute_pca_subset.restype = ctypes.c_int
     L.vpca_compute_pca_subset.argtypes = [vp, vp, i32, vp, vp, ctypes.POINTER(i32)]
+    L.vpca_grm_bed.restype = ctypes.c_int
+    L.vpca_grm_bed.argtypes = [vp, vp, i64, i64]
+    L.vpca_grm_finalize.restype = ctypes.c_int
+    L.vpca_grm_finalize.argtypes = [vp, ctypes.POINTER(i64)]
+    L.vpca_get_grm.restype = ctypes.c_int
+    L.vpca_get_grm.argtypes = [vp, vp]
+    L.vpca_compute_pca_grm.restype = ctypes.c_int
+    L.vpca_compute_pca_grm.argtypes = [vp, i32, vp, vp]
     _lib = L
     return L
 
@@ -771,6 +781,37 @@ class NativePca:
         self._check(self._lib.vpca_variant_qc_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv, b.shape[1],
                                                   _host_ptr(counts), _host_ptr(p) if hwe else None))
         return counts[:nv], (p[:nv] if hwe else None)
+
+    # -- variance-standardized relationship matrix (vpca.h, DESIGN.md 13) ---------------------------------------------
+    def grmBed(self, rows: np.ndarray):
+        """Add PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place, not copied) to the GRM; calls add up,
+        and the PCA Gram is not touched.  Synchronises."""
+        b = np.asarray(rows)
+        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
+            b = np.ascontiguousarray(b, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        empty = np.zeros(1, np.uint8)
+        self._check(self._lib.vpca_grm_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), b.shape[0], b.shape[1]))
+
+    def grmFinalize(self) -> int:
+        """Finish the GRM -> M, the number of variants used (VPCA_ERR_STATE when M = 0)."""
+        m = ctypes.c_int64(0)
+        self._check(self._lib.vpca_grm_finalize(self._h, ctypes.byref(m)))
+        return int(m.value)
+
+    def getGrm(self) -> np.ndarray:
+        """The finalized GRM, (n, n) float64, symmetric."""
+        out = np.empty((self.n, self.n), dtype=np.float64)
+        self._check(self._lib.vpca_get_grm(self._h, _host_ptr(out)))
+        return out
+
+    def computePcaGrm(self, k: int = 2):
+        """-> (vecs (n, k) with column c = PC c of the GRM, evals (k,)): computePca's shapes and sign rule."""
+        flat = np.empty(self.n * k, dtype=np.float64)
+        evals = np.empty(k, dtype=np.float64)
+        self._check(self._lib.vpca_compute_pca_grm(self._h, int(k), _host_ptr(flat), _host_ptr(evals)))
+        return flat.reshape(k, self.n).T.copy(), evals
 
     def hweExact(self, counts) -> np.ndarray:
         """Exact HWE p-values of (V, 4) int32 counts (HOM_A1, HET, HOM_A2, MISSING; MISSING ignored) -> (V,) float64."""

@@ -285,6 +285,8 @@ class VariantsPcaDriver:
     def getSimilarityMatrix(self, callsets: CallsRdd) -> SimilarityMatrix:
         """S = sum over variants of x x^T on the GPU: every partition is one `mapPartitions` task (encode + wgmma
         Gram into a private staging Gram, committed on success); `reduceByKey(_ + _)` across ranks is one all-reduce."""
+        if self.conf.grm():
+            return self._getGrm(callsets)
         nat = self._native(callsets.n_samples)
         nat.reset()
         done = self._load_checkpoint(nat, callsets)
@@ -324,6 +326,29 @@ class VariantsPcaDriver:
         nat.finalizeGram()
         return SimilarityMatrix(nat, callsets.n_samples)
 
+    def _getGrm(self, callsets: CallsRdd) -> SimilarityMatrix:
+        """--grm: the variance-standardized relationship matrix of the .bed rows (DESIGN.md 13) instead of S, the KING
+        counts riding on the same rows when asked for; writes P.rel.bin / P.rel.id with --make-rel before the solve."""
+        nat = self._native(callsets.n_samples)
+        nat.reset()
+        V = 0
+        for part in callsets.partitions:
+            rows = part.rows()
+            if self.conf.makeKingTable.isDefined:
+                nat.kinshipBed(rows)
+            nat.grmBed(rows)
+            V += part.n_rows
+        try:
+            M = nat.grmFinalize()
+        except native.VpcaError as e:
+            if e.code != native.VPCA_ERR_STATE:
+                raise
+            raise ValueError(f"--grm: none of the {V} variants varies among its called samples (M = 0)") from None
+        print(f"GRM: {M} of {V} variants used ({V - M} skipped: no variation among called samples).")
+        if self.conf.makeRel() and self._rank == 0:
+            write_rel(self.conf.outputPath(), self._famIds(), nat.getGrm())
+        return SimilarityMatrix(nat, callsets.n_samples)
+
     def getSimilarityMatrixStream(self, calls: CallsRdd) -> SimilarityMatrix:
         """VariantsPca.scala:262-279 yields the same matrix (its sparse-row quirk is not reproduced, SURVEY.md 2 row 3);
         on the GPU there is one implementation."""
@@ -347,7 +372,12 @@ class VariantsPcaDriver:
                 S[i, j] = v                                                      # IndexError like Breeze at :216
             nat = self._native(rowCount)
             nat.setGram(S)
-        if self.conf.kingCutoff.isDefined:
+        if self.conf.grm():
+            vecs, evals = nat.computePcaGrm(numPc)
+            self.pcaSamples = rowCount
+            if self.conf.outputPath.isDefined and self._rank == 0:
+                write_eigen(self.conf.outputPath(), self._famIds(), vecs, evals)
+        elif self.conf.kingCutoff.isDefined:
             vecs, evals, nonZeroRows = self._computePcaUnrelated(nat, rowCount, numPc)
         else:
             vecs, evals, nonZeroRows = nat.computePca(numPc)
@@ -625,6 +655,7 @@ class VariantsPcaDriver:
             print(f"Sample QC: {m} of {n} samples kept ({removed} removed).")
             check_sample_kept(m, n, conf.numPc())
             check_king_flags(conf, m)                   # the kinship limit applies to the kept samples
+            check_grm_flags(conf, m)
             if m == n:
                 return plink.SampleSet(keep, callsets, fam_ids, bed)   # the fileset as it is
             kept = np.flatnonzero(keep)
@@ -780,6 +811,50 @@ def check_king_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
             raise ValueError(f"--project-loadings builds no similarity matrix for {flag} to ride on")
         if n_samples is not None and n_samples > native.KINSHIP_MAX_SAMPLES:
             raise ValueError(f"{flag} is limited to {native.KINSHIP_MAX_SAMPLES} samples; the cohort has {n_samples}")
+
+
+def check_grm_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
+    """Refuse --grm / --make-rel runs the GRM path cannot serve, before any GPU work: without n_samples the flag
+    combinations, with it the cohort size."""
+    if conf.makeRel() and not conf.grm():
+        raise ValueError("--make-rel writes the matrix of --grm: give --grm")
+    if conf.makeRel() and not conf.outputPath.isDefined:
+        raise ValueError("--make-rel writes P.rel.bin and P.rel.id: give --output-path P")
+    if not conf.grm():
+        return
+    if not conf.bedPath.isDefined:
+        raise ValueError("--grm needs allele dosages: give a PLINK fileset with --bed-path")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("--grm runs on one GPU; launch a single process (WORLD_SIZE=1)")
+    for flag, opt in (("--king-cutoff", conf.kingCutoff), ("--save-loadings", conf.saveLoadings),
+                      ("--project-loadings", conf.projectLoadings), ("--checkpoint-path", conf.checkpointPath)):
+        if opt.isDefined:
+            raise ValueError(f"--grm cannot be combined with {flag}" + (
+                " (for the GRM PCs of an unrelated set, run --king-cutoff first and then --keep P.king.cutoff.in.id "
+                "--grm)" if flag == "--king-cutoff" else ""))
+    if n_samples is not None and n_samples > native.GRM_MAX_SAMPLES:
+        raise ValueError(f"--grm is limited to {native.GRM_MAX_SAMPLES} samples; the cohort has {n_samples}")
+
+
+def write_rel(prefix: str, fam: Sequence[Tuple[str, str]], G: np.ndarray) -> None:
+    """--make-rel: prefix.rel.bin (N x N float64, little-endian, row-major: PLINK's `bin square`) and prefix.rel.id
+    (`#FID<TAB>IID`, one line per sample in matrix order)."""
+    np.ascontiguousarray(G, dtype="<f8").tofile(prefix + ".rel.bin")
+    with open(prefix + ".rel.id", "w", encoding="utf-8") as fh:
+        fh.write("#FID\tIID\n")
+        fh.write("".join(f"{f}\t{i}\n" for f, i in fam))
+
+
+def write_eigen(prefix: str, fam: Sequence[Tuple[str, str]], vecs: np.ndarray, evals: np.ndarray) -> None:
+    """--grm with --output-path: prefix.eigenvec (`#FID IID PC1 .. PCk`, tab-separated, the unit-norm eigenvectors) and
+    prefix.eigenval (one eigenvalue per line), every number the shortest text that reads back as the same double."""
+    k = vecs.shape[1]
+    with open(prefix + ".eigenvec", "w", encoding="utf-8") as fh:
+        fh.write("#FID\tIID\t" + "\t".join(f"PC{c + 1}" for c in range(k)) + "\n")
+        fh.write("".join(f"{f}\t{i}\t" + "\t".join(repr(x) for x in row) + "\n"
+                         for (f, i), row in zip(fam, vecs.tolist())))
+    with open(prefix + ".eigenval", "w", encoding="utf-8") as fh:
+        fh.write("".join(f"{x!r}\n" for x in np.asarray(evals, np.float64).tolist()))
 
 
 def check_ld_flags(conf: PcaConf, bim=None) -> Optional[np.ndarray]:
@@ -1129,6 +1204,7 @@ def main(args: Optional[Sequence[str]] = None):
     conf = PcaConf(list(sys.argv[1:] if args is None else args))
     check_sample_flags(conf)
     check_king_flags(conf)
+    check_grm_flags(conf)
     check_ld_flags(conf)
     check_qc_flags(conf)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
@@ -1138,6 +1214,7 @@ def main(args: Optional[Sequence[str]] = None):
         dist.init_process_group("nccl")
     driver = VariantsPcaDriver(conf)
     check_king_flags(conf, len(driver.common.indexes))
+    check_grm_flags(conf, len(driver.common.indexes))
     window_lo = None
     if conf.ldPrune.isDefined:
         from . import plink

@@ -1,7 +1,8 @@
 """Host reference of the variance-standardized relationship matrix (DESIGN.md 13): the z table of each variant restated
 in Python floats with the operations of csrc/grm.cu in the same order (so the bits must match), the same table in exact
-rationals rounded once per step, and the GRM itself in numpy FP64.  Also the .bed helpers and the Balding-Nichols
-cohorts the GRM tests share."""
+rationals rounded once per step, and the GRM itself in numpy FP64.  Its top eigenpairs from the small eigh of Z^T Z
+(Pcs), which never reads the device's GRM, and the checks a GRM solve must pass against them (check_grm_pairs).  Also
+the .bed helpers and the Balding-Nichols cohorts the GRM tests share."""
 from fractions import Fraction
 import math
 
@@ -94,9 +95,116 @@ def tolerance(Z, panel=1024):
     units of the double rounding error, plus one rounding of the division."""
     n, M = Z.shape
     A = np.abs(Z)
-    u = 2.0 ** -53
-    depth = panel + -(-M // panel) + 2 * (256 + -(-M // 256)) + 4
-    return depth * u * (A @ A.T) / max(M, 1)
+    return depth(M, panel) * 2.0 ** -53 * (A @ A.T) / max(M, 1)
+
+
+def depth(M, panel=1024):
+    """The summation depth of tolerance(), in units of the double rounding error."""
+    return panel + -(-M // panel) + 2 * (256 + -(-M // 256)) + 4
+
+
+class Pcs:
+    """FP64 top-k eigenpairs of G = Z Z^T / M that never read the device's GRM: the small eigh of Z^T Z / M (M x M), or
+    of Z Z^T / M when N < M, then u = Z w / sqrt(M lambda).  Z is (N, M) numpy, or a torch float64 tensor (on the GPU
+    for large N).  Residuals G u - lambda u = Z (Z^T u) / M - lambda u cost O(N M) without forming G.
+
+    lam: the top k eigenvalues (zeros past min(N, M)); rank: how many of them are nonzero (above 1e-9 lam[0]); U: (N, rank)
+    numpy, their unit eigenvectors."""
+
+    def __init__(self, Z, k):
+        self.Z = Z
+        self.n, self.M = n, M = Z.shape
+        small = (Z.T @ Z if n >= M else Z @ Z.T) / M
+        if isinstance(Z, np.ndarray):
+            import scipy.linalg
+            self._np = lambda a: a
+            d = small.shape[0]
+            w, W = scipy.linalg.eigh(small, subset_by_index=[max(0, d - k), d - 1])
+        else:
+            import torch
+            self._np = lambda a: a.cpu().numpy()
+            w, W = map(self._np, torch.linalg.eigh(small))
+        del small
+        order = np.argsort(-w, kind="stable")[:k]
+        self.lam = np.zeros(k)
+        self.lam[:len(order)] = w[order]
+        self.rank = int((self.lam > 1e-9 * self.lam[0]).sum())
+        W = W[:, order[:self.rank]]
+        self.U = self._np(Z @ self._like(W)) / np.sqrt(M * self.lam[:self.rank])[None, :] if n >= M else W
+        self.fro2 = float((Z * Z).sum())
+
+    def _like(self, a):
+        """numpy -> Z's kind (and device)"""
+        a = np.ascontiguousarray(a, np.float64)
+        if isinstance(self.Z, np.ndarray):
+            return a
+        import torch
+        return torch.from_numpy(a).to(self.Z.device)
+
+    def gaps_allow(self, k):
+        """the top k + 1 eigenvalues are far enough apart for two solvers' vectors to agree to 1e-8"""
+        return k >= len(self.lam) or np.min(np.abs(np.diff(self.lam[: k + 1]))) / self.lam[0] > 1e-4
+
+    def residuals(self, vecs, evals):
+        """||G u - lambda u|| / lambda_1 per column, G u = Z (Z^T u) / M"""
+        u = self._like(vecs)
+        r = self._np(self.Z @ (self.Z.T @ u) / self.M - u * self._like(evals)[None, :])
+        return np.linalg.norm(r, axis=0) / self.lam[0]
+
+    def residual_bound(self):
+        """1e-11 plus the device GRM's own cellwise error (tolerance()) in Frobenius norm, || |Z| |Z|^T ||_F <= ||Z||_F^2,
+        relative to lambda_1"""
+        return 1e-11 + depth(self.M) * 2.0 ** -53 * self.fro2 / (self.M * self.lam[0])
+
+
+def check_grm_pairs(ref, vecs, evals, k, note=""):
+    """The assertions every GRM solve must meet against the Z^T Z reference.  Pairs past ref.rank belong to a zero
+    eigenvalue: |lambda| <= 1e-12 lambda_1 and the vector orthogonal to every nonzero pair's."""
+    from oracle import oracle
+    r = min(ref.rank, k)
+    assert vecs.shape == (ref.n, k) and evals.shape == (k,), note
+    assert np.all(np.isfinite(vecs)) and np.all(np.isfinite(evals)), note
+    assert np.allclose(evals[:r], ref.lam[:r], rtol=1e-10, atol=0), (note, evals, ref.lam[:k])
+    assert np.all(np.abs(evals[r:]) <= 1e-12 * ref.lam[0]), (note, evals, ref.lam[:k])
+    if r:
+        err = oracle.eigvec_rel_err(vecs[:, :r], ref.U[:, :r])
+        assert np.all(err <= 1e-6), (note, err)
+    if r < k:
+        leak = np.abs(ref.U.T @ vecs[:, r:])
+        assert leak.max() <= 1e-8, (note, leak.max())
+    res = ref.residuals(vecs, evals)
+    assert np.all(res <= ref.residual_bound()), (note, res, ref.residual_bound())
+    assert np.abs(vecs.T @ vecs - np.eye(k)).max() <= 1e-10, note
+    assert np.allclose(np.linalg.norm(vecs, axis=0), 1.0, rtol=0, atol=1e-12), note
+    for c in range(k):
+        assert vecs[np.argmax(np.abs(vecs[:, c])), c] > 0, (note, c)   # sign rule: largest-|.| entry (lowest index) positive
+
+
+class Solve:
+    """computePcaGrm(k) on a context, with the path it took: eig_method (1 direct, 2 Lanczos, 3 Lanczos gave up and the
+    direct reduction ran), eig_iterations and the kernel_launches delta of the call."""
+
+    def __init__(self, nat, k):
+        before = nat.stats()
+        self.vecs, self.evals = nat.computePcaGrm(k)
+        after = nat.stats()
+        self.method = after["eig_method"]
+        self.iters = after["eig_iterations"]
+        self.launches = after["kernel_launches"] - before["kernel_launches"]
+
+    def __repr__(self):
+        return f"Solve(method={self.method}, iters={self.iters}, launches={self.launches})"
+
+
+def assert_path(s, method, n):
+    """The solve took the path claimed.  Band Lanczos (2): norm, scale, tile, reduce, combine and two lz_dots / lz_update
+    pairs, nine launches per step.  Direct (1): ceil(n / 64) replays of the 64-step graph (one launch per step up to
+    n = 3072, two above), then bisection, inverse iteration and the back-transformation; a GRM needs no centring."""
+    assert s.method == method, s
+    if method == 2:
+        assert 16 <= s.iters <= 320 and s.launches >= 9 * s.iters, s
+    elif method == 1:
+        assert s.iters == 0 and s.launches == (1 if n <= 3072 else 2) * 64 * -(-n // 64) + 3, s
 
 
 def pack(code):

@@ -1,7 +1,8 @@
 """The variance-standardized relationship matrix on the GPU (vpca_grm_*, vpca_compute_pca_grm; DESIGN.md 13): the GRM
 against an FP64 reference (numpy up to 2504 samples, torch float64 above) within the bound of DESIGN.md 13, M exact, its
-bits independent of the split of the rows, skipped variants, the counted allele and padding, its PCs against
-numpy.linalg.eigh on every solver path, the state rules and refusals, and the driver end to end."""
+bits independent of the split of the rows, skipped variants, the counted allele and padding, the staging chunks at their
+row caps, its PCs on every solver path and FP64 band-tile layout against the small eigh of Z^T Z, the state rules and
+refusals, and the driver end to end."""
 import numpy as np
 import pytest
 
@@ -80,6 +81,66 @@ def test_grm_many_chunks_through_a_wide_stride():
     G, m = _run(n, wide)
     G0, m0 = _run(n, rows)
     assert m == m0 and np.array_equal(_bits(G), _bits(G0))
+    _check(G, rows, n)
+
+
+def _bed_launches(used, stride, fill=0):
+    """kernel_launches of one grmBed call (vpca_grm_bed), restated: rows are staged in chunks of min(64 MB / stride, 2^20)
+    rows, at least one; each chunk takes 3 (counts, tables, compaction), then one per expand of its used columns into the
+    panel (an expand stops where the panel fills) and one per full panel (the SYRK).  -> (launches, chunks)"""
+    nv = len(used)
+    step = max(1, min(nv, (64 << 20) // stride, 1 << 20))
+    launches = 0
+    for lo in range(0, nv, step):
+        u, j = int(used[lo:lo + step].sum()), 0
+        launches += 3
+        while j < u:
+            cnt = min(KC - fill, u - j)
+            launches += 1
+            fill, j = fill + cnt, j + cnt
+            if fill == KC:
+                launches, fill = launches + 1, 0
+    return launches, -(-nv // step)
+
+
+def _run_counted(n, rows):
+    """_run with the kernel_launches of the grmBed call"""
+    with native.NativePca(n) as nat:
+        before = nat.stats()["kernel_launches"]
+        nat.grmBed(rows)
+        launches = nat.stats()["kernel_launches"] - before
+        m = nat.grmFinalize()
+        return nat.getGrm(), m, launches
+
+
+@pytest.mark.parametrize("n,extra", [(64, 1500), (253, 700)], ids=["row-cap-64", "both-caps-253"])
+def test_grm_chunks_at_the_row_cap(n, extra):
+    """2^20 + extra rows in one call: a staged chunk holds at most kGrmMaxChunk = 2^20 rows, which grm_compact_kernel scans
+    1024 per thread.  At N = 64 (16-byte rows) that cap binds alone; at N = 253 (64-byte rows) 64 MB is 2^20 rows, so the
+    staging cap binds at the same count.  The first chunk is 2^20 rows and about 1000 panels are multiplied in turn."""
+    rows = _cohort(40 + n, n, (1 << 20) + extra)
+    G, m, launches = _run_counted(n, rows)
+    _, used = grm_ref.z_tables(grm_ref.counts(rows, n))
+    want, chunks = _bed_launches(used, rows.shape[1])
+    assert chunks == 2 and launches == want, (launches, want)
+    assert m == int(used.sum()) > 1000 * KC
+    assert m == _check(G, rows, n)
+
+
+def test_grm_one_row_chunks():
+    """Rows 64 MiB + 32 bytes apart: not one whole row fits the 64 MB staging chunk, so every chunk is a single row
+    (step = 1); one of the five rows is monomorphic and uses no column.  The bits are those of the packed rows."""
+    n, nv, stride = 100, 5, (64 << 20) + 32
+    rows = _cohort(43, n, nv)
+    rows[3] = 0xFF                                          # every call HOM_A2: monomorphic
+    wide = np.full((nv, stride), 0x5A, np.uint8)            # junk past the row's 25 bytes
+    wide[:, :rows.shape[1]] = rows
+    G, m, launches = _run_counted(n, wide)
+    _, used = grm_ref.z_tables(grm_ref.counts(rows, n))
+    assert int(used.sum()) == nv - 1 and not used[3]
+    assert (launches, nv) == _bed_launches(used, stride) == (3 * nv + nv - 1, nv)
+    G0, m0 = _run(n, rows)
+    assert m == m0 == nv - 1 and np.array_equal(_bits(G), _bits(G0))
     _check(G, rows, n)
 
 
@@ -172,26 +233,38 @@ def _pcs_check(vecs, evals, G, k):
         assert np.abs(vecs[:, c] - v).max() <= 1e-6, c
 
 
-# pops: populations of the cohort; with k + 1 of them the top k eigenvalues stand apart.  The fallback case asks for PCs 3
-# and 4 of three populations, which lie in the bulk, so Lanczos gives up within 16 steps.
-@pytest.mark.parametrize("n,k,pops,env", [
-    (300, 1, 3, {}), (300, 10, 11, {}), (600, 2, 3, {}), (600, 16, 17, {}), (600, 20, 21, {}),
-    (2504, 10, 11, {"VPCA_EIG": "direct"}), (700, 4, 3, {"VPCA_EIG_MAXIT": "16"}),
+DIRECT, LANCZOS, MAXIT16 = {"VPCA_EIG": "direct"}, {"VPCA_EIG": "lanczos"}, {"VPCA_EIG_MAXIT": "16"}
+# The FP64 band tiles (kBandTR = 64 rows x kBandTC = 1024 columns): N mod 4 picks the vector or the scalar loads, N past
+# 1024 and 2048 a second and third column tile, N mod 64 a partial row tile.
+BAND_N = [512, 513, 1023, 1024, 1025, 1026, 1027, 2047, 2048, 2049, 2503, 2504, 3001]
+FORCED_N = [96, 97, 98, 99, 127, 128, 129, 255]   # VPCA_EIG=lanczos reaches down to kLzForcedMinN = 96
+
+
+# pops: populations of the cohort; with k + 1 of them the top k eigenvalues stand apart.  The fallback cases ask for PCs
+# 3 and 4 of three populations, which lie in the bulk, so Lanczos gives up within 16 steps.
+@pytest.mark.parametrize("n,k,pops,nv,env", [
+    (300, 1, 3, 4000, {}), (300, 10, 11, 4000, {}), (600, 2, 3, 4000, {}), (600, 16, 17, 4000, {}),
+    (600, 20, 21, 4000, {}), (2504, 10, 11, 4000, DIRECT), (700, 4, 3, 4000, MAXIT16),
+    *[(n, 4, 5, 3000, {}) for n in BAND_N], (511, 4, 5, 3000, {}), *[(n, 4, 5, 3000, LANCZOS) for n in FORCED_N],
+    (3073, 4, 5, 3000, DIRECT), (3073, 4, 3, 3000, MAXIT16),
 ], ids=["direct-300-k1", "direct-300-k10", "lanczos-600-k2", "lanczos-600-k16", "lanczos-600-k20", "direct-2504",
-        "fallback-700"])
-def test_grm_pcs(monkeypatch, n, k, pops, env):
+        "fallback-700", *[f"lanczos-{n}" for n in BAND_N], "direct-511", *[f"forced-lanczos-{n}" for n in FORCED_N],
+        "direct-two-kernels-3073", "fallback-3073"])
+def test_grm_pcs(monkeypatch, n, k, pops, nv, env):
+    """Every solver path a GRM reaches, against the small eigh of Z^T Z (never the device's own G).  Lanczos on a GRM is
+    always the band solver on FP64 cells; its tile kernel reads four cells as two double2 when N mod 4 = 0 (d_C is a
+    256-byte-aligned allocation, so every row then starts 32-byte aligned) and one double at a time otherwise."""
     for key, val in env.items():
         monkeypatch.setenv(key, val)
-    rows = _cohort(n + k, n, 4000, pops=pops)
+    rows = _cohort(n + k, n, nv, pops=pops)
     with native.NativePca(n, num_pc=max(k, 2)) as nat:
         nat.grmBed(rows)
         nat.grmFinalize()
-        G = nat.getGrm()
-        vecs, evals = nat.computePcaGrm(k)
-        st = nat.stats()
-    want_method = 1 if (n < 512 or env.get("VPCA_EIG") == "direct") else 3 if "VPCA_EIG_MAXIT" in env else 2
-    assert st["eig_method"] == want_method
-    _pcs_check(vecs, evals, G, k)
+        s = grm_ref.Solve(nat, k)
+    method = 1 if env is DIRECT or (n < 512 and env is not LANCZOS) else 3 if env is MAXIT16 else 2
+    grm_ref.assert_path(s, method, n)
+    Z, _ = grm_ref.z_matrix(rows, n)
+    grm_ref.check_grm_pairs(grm_ref.Pcs(Z, k), s.vecs, s.evals, k, note=repr(s))
 
 
 # ---- 4. state rules and refusals ---------------------------------------------------------------------------------------

@@ -447,14 +447,43 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
  * vpca_compute_pca_grm: the k largest eigenpairs of the GRM as it is (no second centring), with the shapes, sign rule and
  *   k range of vpca_compute_pca: vecs N x k column-major, evals k (may be NULL), 1 <= k <= min(N, max(num_pc, 16)).
  *   The band solver's Lanczos on the FP64 cells from 512 samples up (the GRM stays valid); below that, with
- *   VPCA_EIG=direct and as the Lanczos fallback the direct reduction, which consumes the GRM.  It leaves no U:
- *   vpca_loadings_* return VPCA_ERR_STATE afterwards.
+ *   VPCA_EIG=direct and as the Lanczos fallback the direct reduction, which consumes the GRM.  It leaves no U for the
+ *   carrier loadings: vpca_loadings_* return VPCA_ERR_STATE afterwards.  It keeps the first min(k, 16) columns of U in
+ *   a buffer of its own (N x 16 doubles) for vpca_grm_loadings_bed, valid even after the direct reduction consumed the
+ *   GRM, until the next vpca_reset / vpca_compute_pca* / vpca_set_gram / vpca_load_partial_gram / vpca_finalize_gram.
  * VPCA_ERR_BAD_ARG, before any row is staged: NULL ctx / rows (nv > 0) / out / vecs, nv < 0, stride_bytes <
  *   ceil(n_samples / 4), k out of range.  VPCA_ERR_UNSUPPORTED above 65 535 samples or on a band-only context. */
 int vpca_grm_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes);
 int vpca_grm_finalize(vpca_ctx* ctx, int64_t* n_used);
 int vpca_get_grm(vpca_ctx* ctx, double* out);
 int vpca_compute_pca_grm(vpca_ctx* ctx, int32_t k, double* vecs, double* evals);
+
+/* ---- GRM loadings and projection (DESIGN.md 14) ----------------------------------------------------------------------
+ * With Z the N x M matrix of used z values above (0 for a missing call and for an unused variant), GRM = Z Z^T / M and
+ * GRM u_c = lambda_c u_c:
+ *   loadings of variant v:          w[v][c] = sum_s tab[v][code(s, v)] u_c[s]          (the columns of Z^T U)
+ *   projection of a sample's codes: p_c = sum_v tab_ref[v][y_v] w[v][c] / (M lambda_c)
+ * so a sample of the reference projected with the reference's own tables and loadings gets u_c back.  A missing call
+ * contributes 0 (mean imputation); the new cohort's own frequencies play no part.  Rows are PLINK 1 .bed rows of the
+ * context's n_samples (as vpca_grm_bed; bytes past ceil(n_samples / 4) and padding bits are ignored), staged in chunks
+ * of at most 64 MB and 2^20 rows on a lane.  FP64, no floating-point atomics, every sum in a fixed order.
+ * vpca_grm_loadings_bed: out_w[v * k + c] (nv x k, variant-major) and out_tab[4 v + code] (nv x 4, indexed by the .bed
+ *   code, all zero for an unused variant) for the U of the last vpca_compute_pca_grm.  The tables are recomputed from
+ *   the rows given, with the bits of vpca_grm_bed's, so pass the rows the GRM was built from.  w[v] is the sum over the
+ *   samples in order 0 .. n_samples - 1, one FMA chain per component: it depends on row v's codes, its table, U and
+ *   n_samples only (not on nv, the chunk split or stride_bytes), and the first k' columns have the same bits at any
+ *   k >= k'.  VPCA_ERR_STATE without GRM U; VPCA_ERR_BAD_ARG for k outside [1, min(k solved, 16)] or the argument rules
+ *   of vpca_grm_bed (out_w / out_tab set when nv > 0); VPCA_ERR_UNSUPPORTED where vpca_grm_bed is.
+ * vpca_grm_project_bed: adds sum_v tab[v][code(s, v)] w[v][c] (tab nv x 4 and w nv x k of the reference, aligned with
+ *   the rows; k of vpca_project_begin) into the accumulator of vpca_project_begin; read it with vpca_project_get and
+ *   evals[c] = M lambda_c.  Order: per staged chunk, fixed panels of 1024 variants each summed in variant order, the
+ *   panel sums added into the accumulator in panel order; chunks in row order, calls in call order.  So the bits
+ *   depend on the rows, tables, w and stride_bytes of each call, never on the run.  VPCA_ERR_STATE before
+ *   vpca_project_begin; VPCA_ERR_UNSUPPORTED on a band-only context; VPCA_ERR_BAD_ARG as above. */
+int vpca_grm_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv, int64_t stride_bytes, double* out_w,
+                          double* out_tab);
+int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const double* tab,
+                         const double* w);
 
 /* ---- sample quality control (beyond VariantsPca.scala: which samples go into S; DESIGN.md 11) -------------------------
  * --keep / --remove / --mind decide the samples of a run before its context exists: the per-sample missing-call counts

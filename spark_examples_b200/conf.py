@@ -129,4 +129,5 @@ class PcaConf(GenomicsConf):
             ("grm", bool, False, False),                  # --bed-path runs: PCs of the variance-standardized relationship
                                                           # matrix of allele dosages (PLINK 2 / GCTA / EIGENSOFT) instead of S
             ("makeRel", bool, False, False),              # with --grm and --output-path P: write P.rel.bin and P.rel.id
+            ("saveGrmLoadings", str, None, False),        # with --grm: write per-variant GRM loadings and z tables (.npz)
         ]

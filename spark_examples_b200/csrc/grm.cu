@@ -214,6 +214,12 @@ cudaError_t grm_tables(const int32_t* d_counts, int nv, double* d_tab, int32_t* 
     return cudaGetLastError();
 }
 
+cudaError_t grm_table(const int32_t* d_counts, int nv, double* d_tab, int32_t* d_used, cudaStream_t stream) {
+    if (nv <= 0) return cudaSuccess;
+    grm_table_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, stream>>>(d_counts, nv, d_tab, d_used);
+    return cudaGetLastError();
+}
+
 cudaError_t grm_expand(const uint8_t* d_rows, int64_t stride, const int32_t* d_inv, const double* d_tab, int cnt, int n,
                        double* d_Z, int col0, cudaStream_t stream) {
     if (cnt <= 0) return cudaSuccess;

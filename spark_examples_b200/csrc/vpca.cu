@@ -114,6 +114,11 @@ struct vpca_ctx {
                             // (finalized with no used variant, or d_C overwritten by another solve)
     int64_t grm_used = 0;   // used variants so far (M)
     int grm_fill = 0;       // of which in the current, not yet multiplied panel
+    // GRM loadings and projection (grm_project.cu): U of the last successful vpca_compute_pca_grm (n x 16 column-major,
+    // the first grm_k columns valid; its own buffer, so it outlives the direct solve that consumes d_C), and one chunk of
+    // loadings (out) or of the caller's w and tables (projection, in)
+    DeviceBuffer<double> d_grm_U, d_grm_w, d_grm_ptab;
+    int grm_k = 0;          // 0: no GRM U
 
     struct Slot {
         int64_t pid = -1;
@@ -706,6 +711,7 @@ int vpca_reset(vpca_ctx* ctx) {
     ctx->finalized = false;
     ctx->pca_done = false;
     ctx->pca_k = 0;
+    ctx->grm_k = 0;
     ctx->proj_k = 0;
     ctx->total_variants = 0;
     ctx->inflight_variants = 0;
@@ -1150,6 +1156,7 @@ int vpca_finalize_gram(vpca_ctx* ctx) {
     ctx->finalized = true;
     ctx->pca_done = false;
     ctx->pca_k = 0;
+    ctx->grm_k = 0;
     return VPCA_OK;
 }
 
@@ -1209,6 +1216,7 @@ int vpca_load_partial_gram(vpca_ctx* ctx, const int32_t* gram, int64_t variants_
     ctx->total_variants = variants_in_gram;
     ctx->inflight_variants = 0;
     ctx->pca_k = 0;
+    ctx->grm_k = 0;
     return check_overflow(ctx, 0);
 }
 
@@ -1226,6 +1234,7 @@ int vpca_set_gram(vpca_ctx* ctx, const int32_t* gram) {
     ctx->finalized = true;
     ctx->pca_done = false;
     ctx->pca_k = 0;
+    ctx->grm_k = 0;
     return VPCA_OK;
 }
 
@@ -1258,6 +1267,7 @@ int vpca_compute_pca(vpca_ctx* ctx, int32_t k, double* vecs, double* evals, int3
                     "behind VariantsPca.scala:226 refuses more columns); the Gram itself has no such limit");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->pca_k = 0;   // U is overwritten from here on
+    ctx->grm_k = 0;
     if (ctx->grm_state != 0) ctx->grm_state = 3;   // the solve may use d_C
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_e0, ctx->stream));
     int rc = run_center(ctx, false);   // row sums + mean; the solver materialises C only if it needs it
@@ -1345,6 +1355,7 @@ int vpca_compute_pca_subset(vpca_ctx* ctx, const uint8_t* keep, int32_t k, doubl
         return fail(ctx, VPCA_ERR_UNSUPPORTED, "vpca_compute_pca_subset is limited to 65535 samples, like vpca_compute_pca");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     ctx->pca_k = 0;   // U is overwritten from here on
+    ctx->grm_k = 0;
     ctx->pca_done = false;   // the tridiagonal form of ctx->eig does not belong to this solve
     if (ctx->sub_eig.n != m) {
         eig_free(ctx->sub_eig);   // a new subset size: the whole workspace is allocated afresh
@@ -1428,7 +1439,7 @@ int vpca_compute_pca_bands(vpca_ctx* const* ctxs, int32_t world, int32_t k, doub
     std::vector<std::unique_lock<std::mutex>> locks;   // rank order
     locks.reserve(world);
     for (int r = 0; r < world; ++r) locks.emplace_back(ctxs[r]->mu);
-    for (int r = 0; r < world; ++r) ctxs[r]->pca_k = 0;   // a failed solve leaves no U behind, never a stale one
+    for (int r = 0; r < world; ++r) ctxs[r]->pca_k = ctxs[r]->grm_k = 0;   // a failed solve leaves no U behind, never a stale one
     BandPart* parts[16];
     for (int r = 0; r < world; ++r) {
         vpca_ctx* c = ctxs[r];
@@ -2327,7 +2338,8 @@ int vpca_compute_pca_grm(vpca_ctx* ctx, int32_t k, double* vecs, double* evals) 
     if (ctx->grm_state != 2) return fail(ctx, VPCA_ERR_STATE, "no finalized GRM (call vpca_grm_finalize; a solve that "
                                          "overwrote it needs vpca_reset and the rows again)");
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    ctx->pca_k = 0;   // a GRM solve leaves no U for the loadings
+    ctx->pca_k = 0;   // a GRM solve leaves no U for the carrier loadings
+    ctx->grm_k = 0;   // and a failed one none for the GRM loadings
     ctx->pca_done = false;
     {
         const char* em = getenv("VPCA_EIG");
@@ -2348,8 +2360,155 @@ int vpca_compute_pca_grm(vpca_ctx* ctx, int32_t k, double* vecs, double* evals) 
     const size_t nb = (size_t)ctx->n * k * sizeof(double);
     CUDA_OK(ctx, cudaMemcpyAsync(vecs, ctx->eig.d_evecs.get(), nb, cudaMemcpyDeviceToHost, ctx->stream));
     if (evals) CUDA_OK(ctx, cudaMemcpyAsync(evals, ctx->eig.d_evals.get(), k * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    const int ku = std::min(k, 16);   // U for vpca_grm_loadings_bed
+    CUDA_OK(ctx, ctx->d_grm_U.ensure((int64_t)ctx->n * 16));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_grm_U.get(), ctx->eig.d_evecs.get(), (size_t)ctx->n * ku * sizeof(double),
+                                 cudaMemcpyDeviceToDevice, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->c_d2h += (int64_t)nb + (evals ? k * 8 : 0);
+    ctx->grm_k = ku;
+    return VPCA_OK;
+}
+
+// ---- GRM loadings and projection (grm_project.cu, DESIGN.md 14) ----------------------------------------------------------
+// Driver-side and synchronous.  Rows are staged as in vpca_grm_bed: chunks of at most kGrmStageBytes and kGrmMaxChunk rows
+// on a lane, double-buffered, the upload of chunk i + 1 overlapping the work on chunk i.
+namespace {
+int64_t grm_step(int64_t nv, int64_t stride) { return std::max<int64_t>(1, std::min({nv, kGrmStageBytes / stride, kGrmMaxChunk})); }
+
+// Uploads chunk c of `rows` into d_grm_rows[c & 1] on the lane's copy stream, once the work on that buffer is done.
+cudaError_t grm_upload(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* rows, int64_t nv, int64_t stride, int64_t step,
+                       int64_t c) {
+    const int b = (int)(c & 1);
+    const int64_t v = c * step, nvc = std::min(step, nv - v);
+    cudaError_t e = cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0);
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(ctx->d_grm_rows[b].get(), rows + (size_t)v * stride, (size_t)(nvc * stride),
+                            cudaMemcpyHostToDevice, L.copy_stream);
+    if (e == cudaSuccess) e = cudaEventRecord(L.ev_copy[b], L.copy_stream);
+    ctx->c_h2d += nvc * stride;
+    return e;
+}
+
+int grm_rows_args(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes, bool outs_set) {
+    if (nv < 0 || (nv > 0 && (rows == nullptr || !outs_set)) || stride_bytes < (ctx->n + 3) / 4)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (rows and arrays must be set, nv >= 0, stride_bytes >= "
+                    "ceil(n_samples / 4))", fn);
+    return VPCA_OK;
+}
+}   // namespace
+
+int vpca_grm_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv, int64_t stride_bytes, double* out_w,
+                          double* out_tab) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int rc = grm_rows_args(ctx, "vpca_grm_loadings_bed", rows, nv, stride_bytes, out_w != nullptr && out_tab != nullptr);
+    if (rc != VPCA_OK) return rc;
+    rc = grm_check(ctx);
+    if (rc != VPCA_OK) return rc;
+    const double* U = nullptr;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->grm_k == 0)
+            return fail(ctx, VPCA_ERR_STATE, "GRM loadings need a vpca_compute_pca_grm since the last reset / solve / Gram "
+                        "change");
+        if (k < 1 || k > ctx->grm_k)
+            return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_grm_loadings_bed: k=%d out of range [1, %d]", k, ctx->grm_k);
+        U = ctx->d_grm_U.get();
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int n = ctx->n;
+    const int64_t step = grm_step(nv, stride_bytes);
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = cudaSuccess;
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        if (e == cudaSuccess) e = ctx->d_grm_counts.ensure(4 * step);
+        if (e == cudaSuccess) e = ctx->d_grm_tab.ensure(4 * step);
+        if (e == cudaSuccess) e = ctx->d_grm_used.ensure(step);
+        if (e == cudaSuccess) e = ctx->d_grm_w.ensure(step * k);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GRM loadings buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    const int64_t nchunks = (nv + step - 1) / step;
+    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
+    for (int64_t c = 0; c < nchunks; ++c) {
+        const int b = (int)(c & 1);
+        const int64_t v = c * step;
+        const int nvc = (int)std::min(step, nv - v);
+        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        const uint8_t* d_rows = ctx->d_grm_rows[b].get();
+        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, nvc, n, ctx->d_grm_counts.get(), L.stream));
+        CUDA_OK(ctx, grm_table(ctx->d_grm_counts.get(), nvc, ctx->d_grm_tab.get(), ctx->d_grm_used.get(), L.stream));
+        CUDA_OK(ctx, grm_loadings(d_rows, stride_bytes, nvc, n, ctx->d_grm_tab.get(), U, k, ctx->d_grm_w.get(), L.stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_grm_w.get(), (size_t)nvc * k * sizeof(double),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_tab + 4 * v, ctx->d_grm_tab.get(), (size_t)nvc * 4 * sizeof(double),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        ctx->c_launches += 3;
+        ctx->c_d2h += (int64_t)nvc * (k + 4) * (int64_t)sizeof(double);
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const double* tab,
+                         const double* w) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int k = 0;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        int rc = project_check(ctx);
+        if (rc != VPCA_OK) return rc;
+        k = ctx->proj_k;
+    }
+    int rc = grm_rows_args(ctx, "vpca_grm_project_bed", rows, nv, stride_bytes, tab != nullptr && w != nullptr);
+    if (rc != VPCA_OK) return rc;
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int n = ctx->n;
+    const int64_t step = grm_step(nv, stride_bytes);
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        const int64_t part = grm_project_scratch_doubles(n, step, k);
+        cudaError_t e = cudaSuccess;
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        if (e == cudaSuccess) e = ctx->d_grm_ptab.ensure(4 * step);
+        if (e == cudaSuccess) e = ctx->d_grm_w.ensure(step * k);
+        if (e == cudaSuccess) e = ctx->d_proj_part.ensure(part, with_slack(part));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GRM projection buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    const int64_t nchunks = (nv + step - 1) / step;
+    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
+    for (int64_t c = 0; c < nchunks; ++c) {
+        const int b = (int)(c & 1);
+        const int64_t v = c * step;
+        const int nvc = (int)std::min(step, nv - v);
+        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
+        // the single w / table buffers are reused in stream order: the previous chunk's kernels read them first
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_grm_w.get(), w + v * k, (size_t)nvc * k * sizeof(double),
+                                     cudaMemcpyHostToDevice, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_grm_ptab.get(), tab + 4 * v, (size_t)nvc * 4 * sizeof(double),
+                                     cudaMemcpyHostToDevice, L.stream));
+        ctx->c_h2d += (int64_t)nvc * (k + 4) * (int64_t)sizeof(double);
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        CUDA_OK(ctx, grm_project(ctx->d_grm_rows[b].get(), stride_bytes, nvc, n, ctx->d_grm_ptab.get(), ctx->d_grm_w.get(),
+                                 k, ctx->d_proj_part.get(), ctx->d_proj_acc.get(), kProjLd, L.stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+        ctx->c_launches += 2;
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
     return VPCA_OK;
 }
 

@@ -235,6 +235,20 @@ cudaError_t grm_expand(const uint8_t* d_rows, int64_t stride, const int32_t* d_i
 cudaError_t grm_syrk(const double* d_Z, int n, double* d_C, cudaStream_t stream);
 // d_C = its lower triangle / m, mirrored to the upper one.
 cudaError_t grm_finish(double* d_C, int n, int64_t m, cudaStream_t stream);
+// The z tables and used flags of grm_tables alone (no used list).  Never synchronises.
+cudaError_t grm_table(const int32_t* d_counts, int nv, double* d_tab, int32_t* d_used, cudaStream_t stream);
+
+// ---- GRM loadings and projection (grm_project.cu, DESIGN.md 14) -----------------------------------------------------
+// d_w[v * k + c] = sum over samples s < n, in order, of tab[v][code(s, v)] U[c * n + s] for nv rows (row v at d_rows +
+// v * stride), U n x k column-major, k in [1, 16].  Never synchronises.
+cudaError_t grm_loadings(const uint8_t* d_rows, int64_t stride, int nv, int n, const double* d_tab, const double* d_U,
+                         int k, double* d_w, cudaStream_t stream);
+// Scratch (doubles) grm_project needs for nv rows of n samples at k components.
+int64_t grm_project_scratch_doubles(int n, int64_t nv, int k);
+// d_acc[s * acc_ld + c] += sum over the nv rows of tab[v][code(s, v)] w[v * k + c]: fixed panels of variants summed in
+// variant order, the panel partials (d_part) added in panel order.  Never synchronises.
+cudaError_t grm_project(const uint8_t* d_rows, int64_t stride, int nv, int n, const double* d_tab, const double* d_w,
+                        int k, double* d_part, double* d_acc, int acc_ld, cudaStream_t stream);
 
 // ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
 // Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to

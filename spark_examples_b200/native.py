@@ -55,7 +55,7 @@ EXPORTED_SYMBOLS = (
     "vpca_kinship_bed", "vpca_kinship_pairs", "vpca_compute_pca_subset", "vpca_ld_prune_bed",
     "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact", "vpca_sample_missing_bed",
     "vpca_subset_bed_samples", "vpca_debug_device_bytes", "vpca_grm_bed", "vpca_grm_finalize", "vpca_get_grm",
-    "vpca_compute_pca_grm",
+    "vpca_compute_pca_grm", "vpca_grm_loadings_bed", "vpca_grm_project_bed",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
@@ -306,6 +306,10 @@ def load_library() -> ctypes.CDLL:
     L.vpca_get_grm.argtypes = [vp, vp]
     L.vpca_compute_pca_grm.restype = ctypes.c_int
     L.vpca_compute_pca_grm.argtypes = [vp, i32, vp, vp]
+    L.vpca_grm_loadings_bed.restype = ctypes.c_int
+    L.vpca_grm_loadings_bed.argtypes = [vp, i32, vp, i64, i64, vp, vp]
+    L.vpca_grm_project_bed.restype = ctypes.c_int
+    L.vpca_grm_project_bed.argtypes = [vp, vp, i64, i64, vp, vp]
     _lib = L
     return L
 
@@ -812,6 +816,44 @@ class NativePca:
         evals = np.empty(k, dtype=np.float64)
         self._check(self._lib.vpca_compute_pca_grm(self._h, int(k), _host_ptr(flat), _host_ptr(evals)))
         return flat.reshape(k, self.n).T.copy(), evals
+
+    @staticmethod
+    def _bed_rows(rows):
+        """(V, stride) uint8 rows as they are when already so (a .bed memmap is read in place), else a C-ordered copy."""
+        b = np.asarray(rows)
+        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
+            b = np.ascontiguousarray(b, dtype=np.uint8)
+        if b.ndim != 2:
+            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        return b
+
+    def grmLoadingsBed(self, k: int, rows: np.ndarray):
+        """GRM loadings of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place) for the U of the last
+        computePcaGrm -> (w (V, k) float64 = Z^T U, tab (V, 4) float64 z of each .bed code, zero for an unused variant).
+        Pass the rows the GRM was built from: the tables are recomputed from them.  Synchronises."""
+        b = self._bed_rows(rows)
+        nv = b.shape[0]
+        w = np.zeros((max(nv, 1), int(k)), np.float64)
+        tab = np.zeros((max(nv, 1), 4), np.float64)
+        empty = np.zeros(1, np.uint8)
+        self._check(self._lib.vpca_grm_loadings_bed(self._h, int(k), b.ctypes.data if b.size else _host_ptr(empty), nv,
+                                                    b.shape[1], _host_ptr(w), _host_ptr(tab)))
+        return w[:nv], tab[:nv]
+
+    def projectGrmBed(self, rows: np.ndarray, tab, w):
+        """Add sum_v tab[v][code(s, v)] w[v, :] of PLINK .bed rows ((V, stride) uint8 of this context's samples; a .bed
+        memmap is read in place) to the projection begun by projectBegin; tab (V, 4) and w (V, k) of the reference align
+        with the rows.  Read with projectGet(M * eigenvalues).  Synchronises."""
+        b = self._bed_rows(rows)
+        nv = b.shape[0]
+        tt = np.ascontiguousarray(tab, dtype=np.float64).reshape(nv, 4)
+        ww = np.ascontiguousarray(w, dtype=np.float64).reshape(nv, -1)
+        if nv and ww.shape[1] != getattr(self, "_proj_k", ww.shape[1]):
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"w must have {self._proj_k} columns")
+        empty = np.zeros(4, np.float64)
+        self._check(self._lib.vpca_grm_project_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty.view(np.uint8)),
+                                                   nv, b.shape[1], _host_ptr(tt if nv else empty),
+                                                   _host_ptr(ww if nv else empty)))
 
     def hweExact(self, counts) -> np.ndarray:
         """Exact HWE p-values of (V, 4) int32 counts (HOM_A1, HET, HOM_A2, MISSING; MISSING ignored) -> (V,) float64."""

@@ -17,6 +17,7 @@ Grams are summed with ONE NCCL all-reduce -- the `reduceByKey(_ + _)` of :190.
 """
 from __future__ import annotations
 
+import dataclasses
 import os
 import struct
 import sys
@@ -33,6 +34,7 @@ from .parquet_calls import ParquetSlice
 from .variants_common import BedSlice, CallsBatch, JoinedSlice, SyntheticSlice, VariantsCommon, VariantsDataset
 
 MAX_LOADING_PC = 16   # components vpca_loadings_* / vpca_project_* handle (include/vpca.h)
+SWAP_CODES = [3, 1, 2, 0]   # a z table indexed by the .bed code, re-indexed for the fileset with A1 and A2 swapped
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -184,6 +186,7 @@ class VariantsPcaDriver:
         self._torch_stream = None
         self._bim_cache: Dict[str, list] = {}
         self.pcaSamples: Optional[int] = None   # samples the last computePca solved for (fewer under --king-cutoff)
+        self.grmUsed: Optional[int] = None      # M of the last --grm matrix
 
     # -- VariantsPca.scala:87 ---------------------------------------------------------------------------------------
     @property
@@ -345,6 +348,7 @@ class VariantsPcaDriver:
                 raise
             raise ValueError(f"--grm: none of the {V} variants varies among its called samples (M = 0)") from None
         print(f"GRM: {M} of {V} variants used ({V - M} skipped: no variation among called samples).")
+        self.grmUsed = M
         if self.conf.makeRel() and self._rank == 0:
             write_rel(self.conf.outputPath(), self._famIds(), nat.getGrm())
         return SimilarityMatrix(nat, callsets.n_samples)
@@ -448,14 +452,7 @@ class VariantsPcaDriver:
     def _partition_keys(self, part, row0: int) -> np.ndarray:
         """(nv, 2) uint64 identity of every row of a partition (see keyKind)."""
         if isinstance(part, BedSlice):
-            prefix = part.bed.prefix
-            if prefix not in self._bim_cache:
-                from . import plink
-                self._bim_cache[prefix] = plink.read_bim(prefix)
-            bim = self._bim_cache[prefix][part.v0:part.v0 + part.nv]
-            if part.keep is not None:
-                bim = [b for b, k in zip(bim, part.keep.tolist()) if k]
-            return np.asarray([_hash_words(bimKeyBytes(b)) for b in bim], np.uint64).reshape(-1, 2)
+            return np.asarray([_hash_words(bimKeyBytes(b)) for b in self._partition_bim(part)], np.uint64).reshape(-1, 2)
         if isinstance(part, CallsBatch) and part.keys is not None:
             return np.asarray(part.keys, np.uint64).reshape(-1, 2)
         nv = _partition_len(part)
@@ -515,6 +512,8 @@ class VariantsPcaDriver:
         lacks contribute nothing (mean imputation).  Returns computePca's (callset id, pc1, pc2) rows."""
         path = path if path is not None else self.conf.projectLoadings()
         kind = self.keyKind(callsets)
+        if loadings_matrix(path) == "grm":
+            return self.projectGrmLoadings(callsets, path)
         with np.load(path, allow_pickle=False) as f:
             W, count, keys = f["loadings"], f["count"], f["keys"]
             n_ref, evals = int(f["n_samples"]), np.asarray(f["eigenvalues"], np.float64)
@@ -571,6 +570,91 @@ class VariantsPcaDriver:
         else:
             off, idx = _select_rows(*_partition_csr(part), sel)
             nat.projectCalls(off, idx, w, mean)
+
+    # -- GRM loadings and projection onto the GRM's PCs (beyond the reference; DESIGN.md 14) ----------------------------
+    def _partition_bim(self, part) -> list:
+        """The .bim records of a BedSlice's rows (its kept rows only)."""
+        from . import plink
+        prefix = part.bed.prefix
+        if prefix not in self._bim_cache:
+            self._bim_cache[prefix] = plink.read_bim(prefix)
+        bim = self._bim_cache[prefix][part.v0:part.v0 + part.nv]
+        if part.keep is not None:
+            bim = [b for b, k in zip(bim, part.keep.tolist()) if k]
+        return bim
+
+    def saveGrmLoadings(self, callsets: CallsRdd, path: Optional[str] = None):
+        """After computePca of a --grm run: the GRM loadings w = Z^T U (numPc columns) and z tables of every variant of
+        this run (after sample QC, variant QC and LD pruning), streamed through the GPU a second time, as one .npz."""
+        path = path if path is not None else self.conf.saveGrmLoadings()
+        kind = self.keyKind(callsets)
+        k = self.conf.numPc()
+        starts = _partition_starts(callsets)
+        keys, ws, tabs = [], [], []
+        for pid, part in enumerate(callsets.partitions):
+            w, tab = self._nat.grmLoadingsBed(k, part.rows())
+            keys.append(self._partition_keys(part, starts[pid]))
+            ws.append(np.asarray(w, np.float64).reshape(-1, k))
+            tabs.append(np.asarray(tab, np.float64).reshape(-1, 4))
+
+        def cat(parts, empty):
+            return np.concatenate(parts) if parts else empty
+        with open(path, "wb") as fh:
+            np.savez(fh, matrix=np.str_("grm"), loadings=cat(ws, np.zeros((0, k))), z_table=cat(tabs, np.zeros((0, 4))),
+                     n_used=np.int64(self.grmUsed), eigenvalues=np.asarray(self.eigenvalues[:k], np.float64),
+                     n_samples=np.int64(len(self.common.indexes)), keys=cat(keys, np.zeros((0, 2), np.uint64)),
+                     key_kind=np.str_(kind))
+
+    def projectGrmLoadings(self, callsets: CallsRdd, path: str) -> List[Tuple[str, float, float]]:
+        """Place this cohort on the PCs of a saved GRM loadings file: p_c = sum_v tab[v][code] w[v][c] / (M lambda_c) over
+        the file's variants found in this cohort by .bim key, or failing that with A1 and A2 swapped (then the table's
+        HOM_A1 and HOM_A2 entries are exchanged, so the same allele is counted).  Strand-ambiguous pairs (A/T, C/G) are
+        taken as given.  File variants this cohort lacks contribute nothing.  With --output-path P writes P.eigenvec."""
+        with np.load(path, allow_pickle=False) as f:
+            W, tab, keys = f["loadings"], f["z_table"], f["keys"]
+            M, evals, file_kind = int(f["n_used"]), np.asarray(f["eigenvalues"], np.float64), str(f["key_kind"])
+        kind = self.keyKind(callsets)
+        if file_kind != kind:
+            raise ValueError(f"{path} identifies variants by {file_kind!r} keys, this cohort's rows by {kind!r} keys")
+        k = W.shape[1] if W.ndim == 2 else 0
+        if k < 2:
+            raise ValueError(f"{path} holds {k} component(s); pc1 and pc2 need at least 2")
+        index = {(int(a), int(b)): i for i, (a, b) in enumerate(keys)}
+        plan, found, swapped = [], 0, 0
+        for part in callsets.partitions:
+            bim = self._partition_bim(part)
+            rows = np.asarray([index.get(_hash_words(bimKeyBytes(b)), -1) for b in bim], np.int64).reshape(-1)
+            swap = np.zeros(len(rows), bool)
+            for j in np.flatnonzero(rows < 0).tolist():   # a direct match wins; else the same variant with A1 / A2 swapped
+                b = bim[j]
+                i = index.get(_hash_words(bimKeyBytes(dataclasses.replace(b, a1=b.a2, a2=b.a1))), -1)
+                if i >= 0:
+                    rows[j], swap[j] = i, True
+            sel = rows >= 0
+            found += int(sel.sum())
+            swapped += int(swap.sum())
+            plan.append((part, sel, rows[sel], swap[sel]))
+        print(f"GRM projection: {found} of {len(keys)} loadings variants found in this cohort "
+              f"({swapped} with A1/A2 swapped).")
+        if found == 0:
+            raise ValueError(f"GRM projection: none of the {len(keys)} variants of {path} is in this cohort")
+        rowCount = len(self.common.indexes)
+        nat = self._native(rowCount)
+        nat.reset()
+        nat.projectBegin(k)
+        for part, sel, rows, swap in plan:
+            if not sel.any():
+                continue
+            t = tab[rows]
+            t[swap] = t[swap][:, SWAP_CODES]
+            nat.projectGrmBed(part.rows()[sel], t, W[rows])
+        P = nat.projectGet(M * evals)
+        self.eigenvalues = evals
+        self.components = P
+        if self.conf.outputPath.isDefined and self._rank == 0:
+            write_eigenvec(self.conf.outputPath(), self._famIds(), P)
+        reverse = {i: cid for cid, i in self.common.indexes.items()}
+        return [(reverse[i], float(P[i, 0]), float(P[i, 1])) for i in range(rowCount)]
 
     # -- LD pruning of the variants (beyond the reference; DESIGN.md 9) -------------------------------------------------
     def ldPrune(self, callsets: CallsRdd, window_lo: np.ndarray, eligible: Optional[np.ndarray] = None) -> np.ndarray:
@@ -813,6 +897,32 @@ def check_king_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
             raise ValueError(f"{flag} is limited to {native.KINSHIP_MAX_SAMPLES} samples; the cohort has {n_samples}")
 
 
+GRM_POINTERS = {
+    "--king-cutoff": " (for the GRM PCs of an unrelated set, run --king-cutoff first and then --keep P.king.cutoff.in.id "
+                     "--grm; its relatives go on those axes with --save-grm-loadings and --project-loadings)",
+    "--save-loadings": " (the loadings of the GRM's PCs are written by --save-grm-loadings)",
+    "--project-loadings": " (a GRM loadings file is projected without --grm: a projection builds no matrix)",
+}
+
+
+def loadings_matrix(path: str) -> str:
+    """"grm" for a file of --save-grm-loadings, "carrier" for one of --save-loadings (which has no `matrix` field)."""
+    with np.load(path, allow_pickle=False) as f:
+        return str(f["matrix"]) if "matrix" in f.files else "carrier"
+
+
+def check_projection_flags(conf: PcaConf) -> None:
+    """Refuse a --project-loadings run of a GRM loadings file the GRM projection cannot serve, before any GPU work."""
+    path = conf.projectLoadings.get
+    if path is None or not os.path.exists(path) or loadings_matrix(path) != "grm":
+        return                                          # (a missing file is reported where it is read)
+    if not conf.bedPath.isDefined:
+        raise ValueError(f"{conf.projectLoadings()} holds GRM loadings, which are projected from allele dosages: give a "
+                         "PLINK fileset with --bed-path")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("projecting GRM loadings runs on one GPU; launch a single process (WORLD_SIZE=1)")
+
+
 def check_grm_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
     """Refuse --grm / --make-rel runs the GRM path cannot serve, before any GPU work: without n_samples the flag
     combinations, with it the cohort size."""
@@ -820,6 +930,8 @@ def check_grm_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
         raise ValueError("--make-rel writes the matrix of --grm: give --grm")
     if conf.makeRel() and not conf.outputPath.isDefined:
         raise ValueError("--make-rel writes P.rel.bin and P.rel.id: give --output-path P")
+    if conf.saveGrmLoadings.isDefined and not conf.grm():
+        raise ValueError("--save-grm-loadings writes the loadings of --grm's PCs: give --grm")
     if not conf.grm():
         return
     if not conf.bedPath.isDefined:
@@ -829,9 +941,10 @@ def check_grm_flags(conf: PcaConf, n_samples: Optional[int] = None) -> None:
     for flag, opt in (("--king-cutoff", conf.kingCutoff), ("--save-loadings", conf.saveLoadings),
                       ("--project-loadings", conf.projectLoadings), ("--checkpoint-path", conf.checkpointPath)):
         if opt.isDefined:
-            raise ValueError(f"--grm cannot be combined with {flag}" + (
-                " (for the GRM PCs of an unrelated set, run --king-cutoff first and then --keep P.king.cutoff.in.id "
-                "--grm)" if flag == "--king-cutoff" else ""))
+            raise ValueError(f"--grm cannot be combined with {flag}" + GRM_POINTERS.get(flag, ""))
+    if conf.saveGrmLoadings.isDefined and conf.numPc() > MAX_LOADING_PC:
+        raise ValueError(f"--save-grm-loadings stores at most {MAX_LOADING_PC} components; --num-pc {conf.numPc()} asks "
+                         "for more")
     if n_samples is not None and n_samples > native.GRM_MAX_SAMPLES:
         raise ValueError(f"--grm is limited to {native.GRM_MAX_SAMPLES} samples; the cohort has {n_samples}")
 
@@ -846,15 +959,21 @@ def write_rel(prefix: str, fam: Sequence[Tuple[str, str]], G: np.ndarray) -> Non
 
 
 def write_eigen(prefix: str, fam: Sequence[Tuple[str, str]], vecs: np.ndarray, evals: np.ndarray) -> None:
-    """--grm with --output-path: prefix.eigenvec (`#FID IID PC1 .. PCk`, tab-separated, the unit-norm eigenvectors) and
-    prefix.eigenval (one eigenvalue per line), every number the shortest text that reads back as the same double."""
+    """--grm with --output-path: prefix.eigenvec (write_eigenvec, the unit-norm eigenvectors) and prefix.eigenval (one
+    eigenvalue per line), every number the shortest text that reads back as the same double."""
+    write_eigenvec(prefix, fam, vecs)
+    with open(prefix + ".eigenval", "w", encoding="utf-8") as fh:
+        fh.write("".join(f"{x!r}\n" for x in np.asarray(evals, np.float64).tolist()))
+
+
+def write_eigenvec(prefix: str, fam: Sequence[Tuple[str, str]], vecs: np.ndarray) -> None:
+    """prefix.eigenvec: `#FID IID PC1 .. PCk`, tab-separated, one line per sample, every number the shortest text that
+    reads back as the same double."""
     k = vecs.shape[1]
     with open(prefix + ".eigenvec", "w", encoding="utf-8") as fh:
         fh.write("#FID\tIID\t" + "\t".join(f"PC{c + 1}" for c in range(k)) + "\n")
         fh.write("".join(f"{f}\t{i}\t" + "\t".join(repr(x) for x in row) + "\n"
                          for (f, i), row in zip(fam, vecs.tolist())))
-    with open(prefix + ".eigenval", "w", encoding="utf-8") as fh:
-        fh.write("".join(f"{x!r}\n" for x in np.asarray(evals, np.float64).tolist()))
 
 
 def check_ld_flags(conf: PcaConf, bim=None) -> Optional[np.ndarray]:
@@ -1207,6 +1326,7 @@ def main(args: Optional[Sequence[str]] = None):
     check_grm_flags(conf)
     check_ld_flags(conf)
     check_qc_flags(conf)
+    check_projection_flags(conf)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         import torch
         import torch.distributed as dist
@@ -1241,6 +1361,8 @@ def main(args: Optional[Sequence[str]] = None):
         result = driver.computePca(simMatrix)
         if conf.saveLoadings.isDefined:
             driver.saveLoadings(callsRdd)
+        if conf.saveGrmLoadings.isDefined:
+            driver.saveGrmLoadings(callsRdd)
     driver.emitResult(result)
     if conf.makeKingTable.isDefined:
         driver.writeKingTable()

@@ -485,6 +485,50 @@ int vpca_grm_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t
 int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const double* tab,
                          const double* w);
 
+/* ---- linear association tests (beyond VariantsPca.scala: PLINK 2's linear --glm; DESIGN.md 15) ---------------------
+ * A quantitative trait y, an additive model, per variant on the complete cases.  The REGRESSION SAMPLES are the samples
+ * with a finite phenotype and finite values for every covariate; C (N x q) is an intercept followed by the n_covar
+ * covariate columns over them, q = n_covar + 1 <= 32.  For variant v, g is the count of the counted allele (0 for a
+ * missing call), A_v the regression samples called at v and OBS_CT = |A_v|; least squares over A_v of
+ * y = C gamma + beta g + e gives BETA = beta, SE = sqrt(sigma^2 [(X^T X)^-1]_gg) with sigma^2 = RSS / df and
+ * df = OBS_CT - q - 1, T_STAT = BETA / SE, P = the two-sided Student t p-value I_{df / (df + T^2)}(df / 2, 1 / 2) (0 below
+ * the double range), A1_FREQ = sum over A_v of g / (2 OBS_CT).  ERRCODE, checked in this order:
+ *   VPCA_GLM_TOO_FEW_OBS   df < 1
+ *   VPCA_GLM_CONST_ALLELE  g constant over A_v
+ *   VPCA_GLM_VIF_INFINITE  the Schur term s = sum g^2 - (b^T P^-1 b) is <= 1e-10 x (sum g^2 - (sum g)^2 / OBS_CT), or the
+ *                          covariates are collinear over A_v (a Cholesky pivot of P <= 1e-10; P = Q_A^T Q_A, see below)
+ *   VPCA_GLM_NO_RESIDUAL   RSS <= 1e-12 x the residual phenotype's sum of squares over A_v
+ * A flagged variant has BETA, SE, T_STAT and P NaN; so has A1_FREQ at OBS_CT = 0.
+ * vpca_glm_begin: in FP64 on the host, orthonormalises C over the regression samples into Q (modified Gram-Schmidt applied
+ *   twice), sets y~ = y - Q Q^T y and uploads Q, y~ and the regression mask.  pheno: N doubles, covar: N x n_covar
+ *   row-major (may be NULL when n_covar = 0); NaN is missing.  *n_used (may be NULL) = the regression samples.
+ *   VPCA_ERR_BAD_ARG, leaving no GLM state: pheno NULL, +-Inf in any input, n_covar < 0 or n_covar + 1 > 32, fewer than
+ *   q + 2 regression samples, a constant phenotype, or a covariate collinear with the intercept and the columns before it
+ *   (its residual norm <= 1e-9 x its norm; the message names it).  The state lasts until the next vpca_glm_begin or
+ *   vpca_reset.
+ * vpca_glm_linear_bed: out[6 v ..] = OBS_CT, A1_FREQ, BETA, SE, T_STAT, P and out_err[v] = ERRCODE of each of nv .bed rows
+ *   of n_samples samples (as vpca_grm_bed; bytes past ceil(n_samples / 4) and the padding bits are ignored), counting
+ *   A1 (counted_allele 1) or A2 (2).  Rows are staged as vpca_grm_loadings_bed stages them: chunks of at most 64 MB and
+ *   2^20 rows on a lane.  Per variant one pass over its row sums b = Q^T g, sum g y~, sum g, sum g^2 and OBS_CT in sample
+ *   order (FP64 FMA chains, exact integers), then over the fewer of its missing and its called regression samples the
+ *   terms that turn Q^T Q = I into P = Q_A^T Q_A; a Cholesky solve of the bordered system follows.  Every output of a
+ *   variant depends on its row's codes, Q, y~ and n_samples only: not on the chunk split, stride_bytes or the call.
+ *   VPCA_ERR_STATE without GLM state; VPCA_ERR_BAD_ARG for counted_allele outside {1, 2} or the argument rules of
+ *   vpca_grm_bed (out / out_err set when nv > 0).
+ * Driver-side and synchronous.  The GLM calls leave the PCA Gram, U, the GRM, the kinship counts and the projection
+ * accumulator alone; Q, y~ and the mask take N (q rounded up to 2, 4, 8, 16 or 32, plus 2) doubles and N / 4 bytes. */
+enum {
+    VPCA_GLM_OK = 0,
+    VPCA_GLM_TOO_FEW_OBS = 1,
+    VPCA_GLM_CONST_ALLELE = 2,
+    VPCA_GLM_VIF_INFINITE = 3,
+    VPCA_GLM_NO_RESIDUAL = 4
+};
+#define VPCA_GLM_MAX_Q 32
+int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used);
+int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                        double* out, int32_t* out_err);
+
 /* ---- sample quality control (beyond VariantsPca.scala: which samples go into S; DESIGN.md 11) -------------------------
  * --keep / --remove / --mind decide the samples of a run before its context exists: the per-sample missing-call counts
  * over every row of a fileset, then the rows repacked to the kept samples, which a plain run reads as its fileset.

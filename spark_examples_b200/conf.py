@@ -130,4 +130,9 @@ class PcaConf(GenomicsConf):
                                                           # matrix of allele dosages (PLINK 2 / GCTA / EIGENSOFT) instead of S
             ("makeRel", bool, False, False),              # with --grm and --output-path P: write P.rel.bin and P.rel.id
             ("saveGrmLoadings", str, None, False),        # with --grm: write per-variant GRM loadings and z tables (.npz)
+            ("pheno", str, None, False),                  # with --glm: the phenotype file (PLINK 2's flag names below)
+            ("phenoName", str, None, False),              # with --glm: the --pheno column to test (default: the first)
+            ("covar", str, None, False),                  # with --glm: a file of covariates, all used beside the PCs
+            ("glm", bool, False, False),                  # --bed-path runs: linear association tests with the PCs as
+                                                          # covariates, written to P.<PHENO>.glm.linear
         ]

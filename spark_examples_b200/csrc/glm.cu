@@ -1,0 +1,396 @@
+// Linear association tests (DESIGN.md 15): per .bed variant, the least-squares fit y = C gamma + beta g + e over the
+// regression samples called at that variant, with the covariates C given to vpca_glm_begin as an orthonormal basis Q
+// (n x q over the regression samples, zero elsewhere) and the residual phenotype y~ = y - Q Q^T y.
+//
+//   glm_sums_kernel: a thread owns VT variants and walks ALL samples in order 0 .. n-1 (grm_loadings_kernel's tiling: the
+//     CTA's rows staged through shared memory in 32-byte tiles of 128 samples, Q and y~ in the same sample tiles).  Per
+//     variant, one FMA chain per column: b_c = sum g q_c (c < q) and b_q = sum g y~, plus the exact integer sums OBS_CT,
+//     sum g and sum g^2.  g is the counted allele's dosage, 0 for a missing call and for a sample outside the regression.
+//   glm_solve_kernel: one warp (one CTA) per variant.  Over the fewer of the variant's missing and called regression
+//     samples (in sample order, one FMA chain per entry) the packed lower triangle of [Q | y~]^T [Q | y~]; from it
+//     P = Q_A^T Q_A, t = Q_A^T y~_A and y~_A^T y~_A over the called set A; Cholesky P = L L^T, u = L^-1 b, v = L^-1 t and
+//     the Schur term s = sum g^2 - u^T u, with the ERRCODEs that need no division.
+//   glm_finish_kernel: one thread per variant: A1_FREQ, beta = (b_q - u^T v) / s,
+//     RSS = y~_A^T y~_A - v^T v - (b_q - u^T v) beta, SE = sqrt(RSS / df / s), T_STAT = beta / SE and the two-sided
+//     Student t p-value.
+// A variant's outputs depend on its row's codes, Q, y~, the mask and n only: not on the chunk split, the stride, the
+// padding bits or bytes, or the call.  No floating-point atomics.
+#include <cuda_runtime.h>
+
+#include <cmath>
+#include <cstdint>
+
+#include "vpca_internal.h"
+
+namespace vpca {
+namespace {
+
+// ---- sums ----------------------------------------------------------------------------------------------------------
+constexpr int kSThreads = 128;
+constexpr int kSTileBytes = 32;                 // row bytes per tile (128 samples)
+constexpr int kSPitch = kSTileBytes / 4 + 1;    // words per staged row: odd, so 32 consecutive rows hit 32 banks
+constexpr int kSTileS = 4 * kSTileBytes;        // samples per tile
+
+// grid ceil(nv / (kSThreads VT)).  Qx: n rows of KMAX + 2 doubles, [q_0 .. q_{q-1}, y~, 0 .., mask].  Samples >= n meet a
+// zero tile row (mask 0, so g = 0): fma(0, 0, a) = a for an accumulator that never holds -0, so they change no bit.
+template <int KMAX, int VT>
+__global__ void __launch_bounds__(kSThreads) glm_sums_kernel(const uint8_t* __restrict__ rows, int64_t stride, int nv, int n,
+                                                             const double* __restrict__ Qx, uint32_t lut,
+                                                             double* __restrict__ sums) {
+    constexpr int LD = KMAX + 2;
+    constexpr int RB = kSThreads * VT;
+    __shared__ uint32_t srow[RB * kSPitch];
+    __shared__ __align__(16) double sq[kSTileS * LD];
+    uint8_t* sb = reinterpret_cast<uint8_t*>(srow);
+    const int v0 = blockIdx.x * RB;
+    const int nb = (n + 3) / 4;
+    double acc[VT][KMAX + 1];
+    int obs[VT], sg[VT], gg[VT];
+#pragma unroll
+    for (int i = 0; i < VT; ++i) {
+        obs[i] = sg[i] = gg[i] = 0;
+#pragma unroll
+        for (int c = 0; c <= KMAX; ++c) acc[i][c] = 0.0;
+    }
+#pragma unroll 1
+    for (int b0 = 0; b0 < nb; b0 += kSTileBytes) {
+        __syncthreads();
+        for (int t = threadIdx.x; t < RB * kSTileBytes; t += kSThreads) {
+            const int r = t / kSTileBytes, j = t % kSTileBytes;
+            const int v = v0 + r, b = b0 + j;
+            sb[r * 4 * kSPitch + j] = (v < nv && b < nb) ? rows[(int64_t)v * stride + b] : 0;
+        }
+        const int s0 = 4 * b0;
+        const int lim = min(kSTileS, n - s0) * LD;
+        const double* src = Qx + (int64_t)s0 * LD;
+        for (int t = threadIdx.x; t < kSTileS * LD; t += kSThreads) sq[t] = t < lim ? src[t] : 0.0;
+        __syncthreads();
+#pragma unroll 1
+        for (int wd = 0; wd < kSTileBytes / 4; ++wd) {
+            uint32_t word[VT];
+#pragma unroll
+            for (int i = 0; i < VT; ++i) word[i] = srow[(i * kSThreads + threadIdx.x) * kSPitch + wd];
+#pragma unroll 2
+            for (int j = 0; j < 16; ++j) {   // sample s0 + 16 wd + j is bits 2j, 2j + 1 of the word
+                const double* x = sq + (wd * 16 + j) * LD;
+                const bool in = x[KMAX + 1] != 0.0;
+#pragma unroll
+                for (int i = 0; i < VT; ++i) {
+                    const uint32_t code = (word[i] >> (2 * j)) & 3u;
+                    const int gi = in ? (int)((lut >> (2 * code)) & 3u) : 0;
+                    obs[i] += (in && code != 1u) ? 1 : 0;
+                    sg[i] += gi;
+                    gg[i] += gi * gi;
+                    const double g = (double)gi;
+#pragma unroll
+                    for (int c = 0; c <= KMAX; ++c) acc[i][c] = fma(g, x[c], acc[i][c]);
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < VT; ++i) {
+        const int v = v0 + i * kSThreads + threadIdx.x;
+        if (v >= nv) continue;
+        double* o = sums + (int64_t)v * kGlmRec;
+#pragma unroll
+        for (int c = 0; c <= KMAX; ++c) o[c] = acc[i][c];
+        o[kGlmRec - 3] = obs[i];
+        o[kGlmRec - 2] = sg[i];
+        o[kGlmRec - 1] = gg[i];
+    }
+}
+
+// ---- two-sided Student t p-value -------------------------------------------------------------------------------------
+// ln B(a, 1/2).  From a = 10 up, ln G(a) - ln G(a + 1/2) by Stirling's series written so that nothing large cancels:
+// -ln(a) / 2 + (1/2 - a log1p(1 / (2a))) + the difference of the 1/z series terms; below, lgamma directly (small values).
+__device__ __forceinline__ double lbeta_half(double a) {
+    const double lg_half = 0.57236494292470008707;   // ln G(1/2) = ln(pi) / 2
+    if (a < 10.0) return lgamma(a) + lg_half - lgamma(a + 0.5);
+    const double b = a + 0.5;
+    auto corr = [](double z) {
+        const double r = 1.0 / z, r2 = r * r;
+        return r * (1.0 / 12.0 - r2 * (1.0 / 360.0 - r2 * (1.0 / 1260.0 - r2 * (1.0 / 1680.0))));
+    };
+    return lg_half - 0.5 * log(a) + (0.5 - a * log1p(0.5 / a)) + (corr(a) - corr(b));
+}
+
+// The continued fraction of I_x(a, b) (modified Lentz), converging fast for x < (a + 1) / (a + b + 2).
+__device__ __forceinline__ double betacf(double a, double b, double x) {
+    const double tiny = 1e-300, eps = 1e-16;
+    double c = 1.0, d = 1.0 - (a + b) * x / (a + 1.0);
+    if (fabs(d) < tiny) d = tiny;
+    d = 1.0 / d;
+    double h = d;
+    for (int m = 1; m <= 100000; ++m) {
+        const double m2 = 2.0 * m;
+        double aa = m * (b - m) * x / ((a + m2 - 1.0) * (a + m2));
+        d = 1.0 + aa * d;
+        if (fabs(d) < tiny) d = tiny;
+        c = 1.0 + aa / c;
+        if (fabs(c) < tiny) c = tiny;
+        d = 1.0 / d;
+        h *= d * c;
+        aa = -(a + m) * (a + b + m) * x / ((a + m2) * (a + m2 + 1.0));
+        d = 1.0 + aa * d;
+        if (fabs(d) < tiny) d = tiny;
+        c = 1.0 + aa / c;
+        if (fabs(c) < tiny) c = tiny;
+        d = 1.0 / d;
+        const double del = d * c;
+        h *= del;
+        if (fabs(del - 1.0) <= eps) break;
+    }
+    return h;
+}
+
+// P(|T_df| >= |t|) = I_x(df / 2, 1 / 2), x = df / (df + t^2), 1 - x = t^2 / (df + t^2) (never 1 - x by subtraction).  The
+// continued fraction runs in whichever of x and 1 - x it converges for; a p below the double range comes back as 0.
+__device__ __forceinline__ double t_pvalue(double t, double df) {
+    const double t2 = t * t;
+    const double a = 0.5 * df, b = 0.5;
+    const double x = df / (df + t2), y = t2 / (df + t2);
+    if (y == 0.0) return 1.0;
+    const double lnx = -log1p(t2 / df), lny = log(y);
+    const double front = exp(a * lnx + b * lny - lbeta_half(a));
+    if (x < (a + 1.0) / (a + b + 2.0)) return fmin(1.0, front * betacf(a, b, x) / a);
+    return fmax(0.0, 1.0 - front * betacf(b, a, y) / b);
+}
+
+// ---- solve ---------------------------------------------------------------------------------------------------------
+// 1 / sqrt(d) for d in (1e-10, 1]: the single-precision estimate and two Newton steps in FP64 (24 -> 48 -> ~53 bits), with
+// no call into the slow paths of the FP64 division and square root (their calling convention makes the solve spill).
+__device__ __forceinline__ double rsqrt_newton(double d) {
+    double r = (double)__frsqrt_rn((float)d);
+    r = r * fma(-0.5 * d * r, r, 1.5);
+    r = r * fma(-0.5 * d * r, r, 1.5);
+    return fma(r * fma(-d * r, r, 1.0), 0.5, r);
+}
+
+constexpr int kGWarps = 1;   // one warp per CTA: __syncthreads, which the compiler needs no divergence fallback for
+constexpr double kPivotMin = 1e-10;   // P = Q_A^T Q_A has eigenvalues in [0, 1]: a smaller pivot is collinearity over A
+
+// grid ceil(nv / kGWarps); warp w of CTA c takes variant c kGWarps + w.  mask: bit e of byte j = sample 4 j + e is a
+// regression sample.  out[v * 6 ..] = OBS_CT, sum g, and for ERRCODE `.` the Schur term s, b_q - u^T v,
+// y~_A^T y~_A - v^T v and y~_A^T y~_A, which glm_finish_kernel turns into the statistics; err[v] = VPCA_GLM_*.
+// The lanes exchange values through shared memory and __syncthreads, not shuffles: every branch below is uniform over the
+// warp, but the compiler cannot prove it, and its fallback for a shuffle it cannot prove converged spills.
+template <int KMAX>
+__global__ void __launch_bounds__(kGWarps * 32, KMAX >= 32 ? 8 : 16) glm_solve_kernel(const uint8_t* __restrict__ rows, int64_t stride, int nv,
+                                                                 int n, int q, int n_reg, const double* __restrict__ Qx,
+                                                                 const uint8_t* __restrict__ mask,
+                                                                 const double* __restrict__ z0, double yty,
+                                                                 const double* __restrict__ sums, double* __restrict__ out,
+                                                                 int32_t* __restrict__ err) {
+    constexpr int LD = KMAX + 2;
+    constexpr int PL = KMAX + 1;                             // pitch of L: odd, so lanes reading a column hit distinct banks
+    constexpr int NE = ((KMAX + 1) * (KMAX + 2) / 2 + 31) / 32;   // packed entries of [Q | y~]^T [Q | y~] per lane
+    __shared__ double sL[kGWarps][KMAX * PL];
+    __shared__ double sx[kGWarps][KMAX + 1];   // a sample's [q | y~], then t
+    __shared__ double su[kGWarps][32], sv[kGWarps][32];
+    __shared__ double sd[kGWarps][4];          // pivot, y~_A^T y~_A
+    __shared__ uint32_t ssel[kGWarps][32];
+    __shared__ int sc[kGWarps][4];             // OBS_CT, sum g, sum g^2, ERRCODE
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int v = blockIdx.x * kGWarps + w;
+    if (v >= nv) return;   // the whole warp
+    const double* rec = sums + (int64_t)v * kGlmRec;
+    if (lane == 0) {
+        const int obs = (int)rec[kGlmRec - 3], sg = (int)rec[kGlmRec - 2], gg = (int)rec[kGlmRec - 1];
+        sc[w][0] = obs;
+        sc[w][1] = sg;
+        sc[w][2] = gg;
+        sc[w][3] = obs - q - 1 < 1 ? VPCA_GLM_TOO_FEW_OBS
+                   : (int64_t)obs * gg == (int64_t)sg * sg ? VPCA_GLM_CONST_ALLELE : VPCA_GLM_OK;
+        double* o = out + (int64_t)v * 6;
+        o[0] = obs;
+        o[1] = sg;   // glm_finish_kernel divides
+    }
+    __syncthreads();
+    if (sc[w][3] != VPCA_GLM_OK) {
+        if (lane == 0) err[v] = sc[w][3];
+        return;
+    }
+    // the missing-call terms over the fewer of the missing and the called regression samples
+    const int obs = sc[w][0];
+    const int E = (q + 1) * (q + 2) / 2;
+    uint32_t eab[NE];   // (a << 8) | b of entry lane + 32 j: row a >= column b of the packed triangle
+    double acc[NE];
+#pragma unroll
+    for (int j = 0; j < NE; ++j) {
+        const int e = lane + 32 * j;
+        int a = 0;
+        while ((a + 1) * (a + 2) / 2 <= e) ++a;
+        eab[j] = (uint32_t)a << 8 | (uint32_t)(e - a * (a + 1) / 2);
+        acc[j] = 0.0;
+    }
+    const bool use_missing = n_reg - obs <= obs;
+    if (use_missing ? n_reg > obs : obs > 0) {
+        const uint8_t* row = rows + (int64_t)v * stride;
+        const int nb = (n + 3) / 4;
+        for (int b0 = 0; b0 < nb; b0 += 32) {
+            const int b = b0 + lane;
+            uint32_t sel = 0;
+            if (b < nb) {
+                const uint32_t by = row[b], mk = mask[b];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const bool miss = ((by >> (2 * e)) & 3u) == 1u;
+                    if (((mk >> e) & 1u) && miss == use_missing) sel |= 1u << e;
+                }
+            }
+            __syncthreads();   // the previous block's reads of ssel are done
+            ssel[w][lane] = sel;
+            __syncthreads();
+            for (int src = 0; src < 32; ++src) {
+                uint32_t sm = ssel[w][src];
+                while (sm) {
+                    const int e = __ffs(sm) - 1;
+                    sm &= sm - 1;
+                    const int64_t s = 4 * (int64_t)(b0 + src) + e;
+                    for (int c = lane; c <= q; c += 32) sx[w][c] = Qx[s * LD + c];
+                    __syncthreads();
+#pragma unroll
+                    for (int j = 0; j < NE; ++j)
+                        if (lane + 32 * j < E) acc[j] = fma(sx[w][eab[j] >> 8], sx[w][eab[j] & 255u], acc[j]);
+                    __syncthreads();
+                }
+            }
+        }
+    }
+    // P (lower triangle) into sL, t into sx, y~_A^T y~_A into sd[1]
+#pragma unroll
+    for (int j = 0; j < NE; ++j) {
+        if (lane + 32 * j >= E) continue;
+        const int a = (int)(eab[j] >> 8), b = (int)(eab[j] & 255u);
+        if (a < q) sL[w][a * PL + b] = use_missing ? (a == b ? 1.0 : 0.0) - acc[j] : acc[j];
+        else if (b < q) sx[w][b] = use_missing ? z0[b] - acc[j] : acc[j];
+        else sd[w][1] = use_missing ? yty - acc[j] : acc[j];
+    }
+    __syncthreads();
+    // Cholesky P = L L^T, left-looking by column; lane i owns row i.  sr: 1 / L_jj, so the loops hold no division.
+    double* sr = su[w];
+    for (int j = 0; j < q; ++j) {
+        if (lane == j) {
+            double d = sL[w][j * PL + j];
+            for (int k = 0; k < j; ++k) d = fma(-sL[w][j * PL + k], sL[w][j * PL + k], d);
+            sd[w][0] = d;
+            sr[j] = d > kPivotMin ? rsqrt_newton(d) : 0.0;
+        }
+        __syncthreads();
+        if (!(sd[w][0] > kPivotMin)) {
+            if (lane == 0) err[v] = VPCA_GLM_VIF_INFINITE;
+            return;
+        }
+        if (lane > j && lane < q) {
+            double x = sL[w][lane * PL + j];
+            for (int k = 0; k < j; ++k) x = fma(-sL[w][lane * PL + k], sL[w][j * PL + k], x);
+            sL[w][lane * PL + j] = x * sr[j];
+        }
+        __syncthreads();
+    }
+    // u = L^-1 b, v = L^-1 t by columns: lane i keeps the running right-hand sides of row i
+    double wu = lane < q ? rec[lane] : 0.0, wv = lane < q ? sx[w][lane] : 0.0;
+    for (int j = 0; j < q; ++j) {
+        if (lane == j) {
+            wu *= sr[j];
+            wv *= sr[j];
+            sv[w][j] = wu;
+            sx[w][j] = wv;
+        }
+        __syncthreads();
+        if (lane > j && lane < q) {
+            const double lij = sL[w][lane * PL + j];
+            wu = fma(-lij, sv[w][j], wu);
+            wv = fma(-lij, sx[w][j], wv);
+        }
+    }
+    __syncthreads();
+    if (lane != 0) return;
+    double uu = 0.0, uv = 0.0, vv = 0.0;
+    for (int j = 0; j < q; ++j) {
+        uu = fma(sv[w][j], sv[w][j], uu);
+        uv = fma(sv[w][j], sx[w][j], uv);
+        vv = fma(sx[w][j], sx[w][j], vv);
+    }
+    const int sg = sc[w][1], gg = sc[w][2];
+    const double s = (double)gg - uu;
+    double* o = out + (int64_t)v * 6;
+    // s <= 1e-10 (sum g^2 - (sum g)^2 / OBS_CT), multiplied through by OBS_CT: the divisions wait for glm_finish_kernel
+    if (!(s * obs > 1e-10 * (double)((int64_t)gg * obs - (int64_t)sg * sg))) {
+        err[v] = VPCA_GLM_VIF_INFINITE;
+        return;
+    }
+    const double yyA = sd[w][1];
+    o[2] = s;
+    o[3] = rec[q] - uv;
+    o[4] = yyA - vv;
+    o[5] = yyA;
+    err[v] = VPCA_GLM_OK;
+}
+
+// From what glm_solve_kernel leaves in out[v * 6 ..] (OBS_CT, sum g, and for ERRCODE `.` the Schur term s, b_q - u^T v,
+// y~_A^T y~_A - v^T v and y~_A^T y~_A): A1_FREQ, and for ERRCODE `.` BETA, the RSS check, SE, T_STAT and the two-sided p at
+// df = OBS_CT - q - 1, one thread per variant; NaN where undefined.  The divisions and the p-value run here, apart from the
+// solve's loops, so that none of the solve's registers has to survive their calls.
+__global__ void glm_finish_kernel(int nv, int q, double* __restrict__ out, int32_t* __restrict__ err) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= nv) return;
+    double* o = out + (int64_t)v * 6;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    const double obs = o[0];
+    o[1] = obs > 0.0 ? o[1] / (2.0 * obs) : nan;
+    if (err[v] != VPCA_GLM_OK) {
+        o[2] = o[3] = o[4] = o[5] = nan;
+        return;
+    }
+    const double s = o[2], num = o[3], rpre = o[4], yyA = o[5];
+    const double beta = num / s;
+    const double rss = rpre - num * beta;
+    if (!(rss > 1e-12 * yyA)) {
+        err[v] = VPCA_GLM_NO_RESIDUAL;
+        o[2] = o[3] = o[4] = o[5] = nan;
+        return;
+    }
+    const double df = obs - (double)(q + 1);
+    const double se = sqrt(rss / df / s);
+    const double t = beta / se;
+    o[2] = beta;
+    o[3] = se;
+    o[4] = t;
+    o[5] = t_pvalue(t, df);
+}
+
+template <int KMAX>
+void launch(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, int n_reg, const double* d_Qx,
+            const uint8_t* d_mask, const double* d_z0, double yty, uint32_t lut, double* d_sums, double* d_out,
+            int32_t* d_err, cudaStream_t stream) {
+    constexpr int VT = KMAX >= 32 ? 1 : 2;
+    const unsigned grid = (unsigned)((nv + kSThreads * VT - 1) / (kSThreads * VT));
+    glm_sums_kernel<KMAX, VT><<<grid, kSThreads, 0, stream>>>(d_rows, stride, nv, n, d_Qx, lut, d_sums);
+    glm_solve_kernel<KMAX><<<(unsigned)((nv + kGWarps - 1) / kGWarps), kGWarps * 32, 0, stream>>>(
+        d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, d_sums, d_out, d_err);
+    glm_finish_kernel<<<(unsigned)((nv + 127) / 128), 128, 0, stream>>>(nv, q, d_out, d_err);
+}
+
+}  // namespace
+
+int glm_kmax(int q) { return q <= 2 ? 2 : q <= 4 ? 4 : q <= 8 ? 8 : q <= 16 ? 16 : 32; }
+
+cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, int n_reg, const double* d_Qx,
+                       const uint8_t* d_mask, const double* d_z0, double yty, int counted, double* d_sums, double* d_out,
+                       int32_t* d_err, cudaStream_t stream) {
+    if (nv <= 0) return cudaSuccess;
+    // dosage of the counted allele by .bed code (00 HOM_A1, 01 missing, 10 HET, 11 HOM_A2), two bits each
+    const uint32_t lut = counted == 2 ? (0u | 0u << 2 | 1u << 4 | 2u << 6) : (2u | 0u << 2 | 1u << 4 | 0u << 6);
+    switch (glm_kmax(q)) {
+        case 2: launch<2>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
+        case 4: launch<4>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
+        case 8: launch<8>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
+        case 16: launch<16>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
+        default: launch<32>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
+    }
+    return cudaGetLastError();
+}
+
+}  // namespace vpca

@@ -119,6 +119,15 @@ struct vpca_ctx {
     // loadings (out) or of the caller's w and tables (projection, in)
     DeviceBuffer<double> d_grm_U, d_grm_w, d_grm_ptab;
     int grm_k = 0;          // 0: no GRM U
+    // linear association tests (vpca_glm_*, glm.cu): Q, y~ and the mask of the last vpca_glm_begin (n rows of
+    // glm_kmax(q) + 2 doubles), the regression mask as bits, Q^T y~, and one chunk of sums and outputs; rows are staged in
+    // d_grm_rows.  All grow-only.
+    DeviceBuffer<double> d_glm_Qx, d_glm_z0, d_glm_sums, d_glm_out;
+    DeviceBuffer<uint8_t> d_glm_mask;
+    DeviceBuffer<int32_t> d_glm_err;
+    int glm_q = 0;          // 0: no GLM state
+    int glm_nreg = 0;       // regression samples
+    double glm_yty = 0.0;   // y~^T y~
 
     struct Slot {
         int64_t pid = -1;
@@ -713,6 +722,7 @@ int vpca_reset(vpca_ctx* ctx) {
     ctx->pca_k = 0;
     ctx->grm_k = 0;
     ctx->proj_k = 0;
+    ctx->glm_q = 0;
     ctx->total_variants = 0;
     ctx->inflight_variants = 0;
     ctx->st.variants_accumulated = 0;
@@ -2509,6 +2519,169 @@ int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t
         ctx->c_launches += 2;
     }
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
+    return VPCA_OK;
+}
+
+// ---- linear association tests (glm.cu, DESIGN.md 15) ---------------------------------------------------------------------
+// vpca_glm_begin is host FP64 work and one upload; vpca_glm_linear_bed is driver-side and synchronous, its rows staged as
+// vpca_grm_loadings_bed stages them (grm_upload into d_grm_rows).
+int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        ctx->glm_q = 0;   // a refused call leaves no GLM state
+    }
+    if (pheno == nullptr || n_covar < 0 || (n_covar > 0 && covar == nullptr))
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: bad argument (pheno must be set, n_covar >= 0, covar set when "
+                    "n_covar > 0)");
+    const int q = n_covar + 1;
+    if (q > VPCA_GLM_MAX_Q)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: %d covariates and the intercept exceed %d columns", n_covar,
+                    VPCA_GLM_MAX_Q);
+    const int n = ctx->n;
+    std::vector<int> idx;   // the regression samples
+    for (int s = 0; s < n; ++s) {
+        bool ok = std::isfinite(pheno[s]);
+        if (std::isinf(pheno[s])) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: the phenotype of sample %d is infinite", s);
+        for (int j = 0; j < n_covar; ++j) {
+            const double x = covar[(size_t)s * n_covar + j];
+            if (std::isinf(x))
+                return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: covariate %d of sample %d is infinite", j + 1, s);
+            ok = ok && std::isfinite(x);
+        }
+        if (ok) idx.push_back(s);
+    }
+    const int R = (int)idx.size();
+    if (R < q + 2)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: %d regression samples; %d covariates and the intercept need at "
+                    "least %d", R, n_covar, q + 2);
+    bool constant = true;
+    for (int i = 1; i < R && constant; ++i) constant = pheno[idx[i]] == pheno[idx[0]];
+    if (constant) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: the phenotype is constant over the regression samples");
+    // Q: the columns of C orthonormalised in order, modified Gram-Schmidt applied twice
+    std::vector<double> Q((size_t)q * R), y(R);
+    for (int c = 0; c < q; ++c) {
+        double* col = Q.data() + (size_t)c * R;
+        for (int i = 0; i < R; ++i) col[i] = c == 0 ? 1.0 : covar[(size_t)idx[i] * n_covar + c - 1];
+        double nrm0 = 0.0;
+        for (int i = 0; i < R; ++i) nrm0 += col[i] * col[i];
+        for (int pass = 0; pass < 2; ++pass)
+            for (int k = 0; k < c; ++k) {
+                const double* qk = Q.data() + (size_t)k * R;
+                double r = 0.0;
+                for (int i = 0; i < R; ++i) r += qk[i] * col[i];
+                for (int i = 0; i < R; ++i) col[i] -= r * qk[i];
+            }
+        double nrm = 0.0;
+        for (int i = 0; i < R; ++i) nrm += col[i] * col[i];
+        if (!(nrm > 1e-18 * nrm0))
+            return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: covariate %d is collinear with the intercept and the "
+                        "covariates before it over the %d regression samples", c, R);
+        const double inv = 1.0 / std::sqrt(nrm);
+        for (int i = 0; i < R; ++i) col[i] *= inv;
+    }
+    for (int i = 0; i < R; ++i) y[i] = pheno[idx[i]];
+    for (int pass = 0; pass < 2; ++pass)
+        for (int k = 0; k < q; ++k) {
+            const double* qk = Q.data() + (size_t)k * R;
+            double r = 0.0;
+            for (int i = 0; i < R; ++i) r += qk[i] * y[i];
+            for (int i = 0; i < R; ++i) y[i] -= r * qk[i];
+        }
+    std::vector<double> z0(q, 0.0);
+    double yty = 0.0;
+    for (int i = 0; i < R; ++i) yty += y[i] * y[i];
+    for (int k = 0; k < q; ++k)
+        for (int i = 0; i < R; ++i) z0[k] += Q[(size_t)k * R + i] * y[i];
+    const int ld = glm_kmax(q) + 2;
+    std::vector<double> Qx((size_t)n * ld, 0.0);
+    std::vector<uint8_t> mask((n + 3) / 4, 0);
+    for (int i = 0; i < R; ++i) {
+        double* xr = Qx.data() + (size_t)idx[i] * ld;
+        for (int c = 0; c < q; ++c) xr[c] = Q[(size_t)c * R + i];
+        xr[q] = y[i];
+        xr[ld - 1] = 1.0;
+        mask[idx[i] / 4] |= (uint8_t)(1u << (idx[i] % 4));
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    {
+        cudaError_t e = ctx->d_glm_Qx.ensure((int64_t)n * ld);
+        if (e == cudaSuccess) e = ctx->d_glm_mask.ensure((n + 3) / 4);
+        if (e == cudaSuccess) e = ctx->d_glm_z0.ensure(VPCA_GLM_MAX_Q);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_Qx.get(), Qx.data(), Qx.size() * sizeof(double), cudaMemcpyHostToDevice,
+                                 ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_mask.get(), mask.data(), mask.size(), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_z0.get(), z0.data(), q * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_h2d += (int64_t)(Qx.size() * sizeof(double) + mask.size() + q * sizeof(double));
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    ctx->glm_q = q;
+    ctx->glm_nreg = R;
+    ctx->glm_yty = yty;
+    if (n_used) *n_used = R;
+    return VPCA_OK;
+}
+
+int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                        double* out, int32_t* out_err) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int rc = grm_rows_args(ctx, "vpca_glm_linear_bed", rows, nv, stride_bytes, out != nullptr && out_err != nullptr);
+    if (rc != VPCA_OK) return rc;
+    if (counted_allele != 1 && counted_allele != 2)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_linear_bed: counted_allele must be 1 (A1) or 2 (A2), not %d",
+                    counted_allele);
+    int q = 0, n_reg = 0;
+    double yty = 0.0;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->glm_q == 0) return fail(ctx, VPCA_ERR_STATE, "vpca_glm_linear_bed needs a vpca_glm_begin since the last reset");
+        q = ctx->glm_q;
+        n_reg = ctx->glm_nreg;
+        yty = ctx->glm_yty;
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int n = ctx->n;
+    const int64_t step = grm_step(nv, stride_bytes);
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = cudaSuccess;
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * kGlmRec);
+        if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
+        if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    const int64_t nchunks = (nv + step - 1) / step;
+    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
+    for (int64_t c = 0; c < nchunks; ++c) {
+        const int b = (int)(c & 1);
+        const int64_t v = c * step;
+        const int nvc = (int)std::min(step, nv - v);
+        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        CUDA_OK(ctx, glm_linear(ctx->d_grm_rows[b].get(), stride_bytes, nvc, n, q, n_reg, ctx->d_glm_Qx.get(),
+                                ctx->d_glm_mask.get(), ctx->d_glm_z0.get(), yty, counted_allele, ctx->d_glm_sums.get(),
+                                ctx->d_glm_out.get(), ctx->d_glm_err.get(), L.stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        ctx->c_launches += 3;
+        ctx->c_d2h += (int64_t)nvc * (6 * (int64_t)sizeof(double) + (int64_t)sizeof(int32_t));
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     return VPCA_OK;
 }
 

@@ -250,6 +250,20 @@ int64_t grm_project_scratch_doubles(int n, int64_t nv, int k);
 cudaError_t grm_project(const uint8_t* d_rows, int64_t stride, int nv, int n, const double* d_tab, const double* d_w,
                         int k, double* d_part, double* d_acc, int acc_ld, cudaStream_t stream);
 
+// ---- linear association tests (glm.cu, DESIGN.md 15) ----------------------------------------------------------------
+// Doubles per variant of the sums: b_0 .. b_KMAX (b_c = sum g q_c for c < q, b_q = sum g y~, zero past q), then OBS_CT,
+// sum g and sum g^2 (exact integers).
+constexpr int kGlmRec = VPCA_GLM_MAX_Q + 4;
+// Columns of Q the kernels are instantiated for (2, 4, 8, 16 or 32); Qx has glm_kmax(q) + 2 doubles per sample.
+int glm_kmax(int q);
+// nv .bed rows (row v at d_rows + v * stride) of n samples: the sums into d_sums (nv x kGlmRec), then
+// d_out[v * 6 ..] = OBS_CT, A1_FREQ, BETA, SE, T_STAT, P and d_err[v] (VPCA_GLM_*).  d_Qx: n rows [q_0 .. q_{q-1}, y~, 0 ..,
+// mask]; d_mask: bit e of byte j = sample 4 j + e is a regression sample; d_z0 = Q^T y~ (q); yty = y~^T y~; n_reg the
+// regression samples; counted 1 (A1) or 2 (A2).  Never synchronises.
+cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, int n_reg, const double* d_Qx,
+                       const uint8_t* d_mask, const double* d_z0, double yty, int counted, double* d_sums, double* d_out,
+                       int32_t* d_err, cudaStream_t stream);
+
 // ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
 // Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to
 // d_missing[0 .. n) with integer atomics.  Bytes past ceil(n / 4) and the padding bits of the last byte are ignored.

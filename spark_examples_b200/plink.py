@@ -117,16 +117,15 @@ def read_id_file(path: str) -> List[Tuple[Optional[str], str]]:
     return out
 
 
-def match_sample_ids(fam_ids: Sequence[Tuple[str, str]], ids: Sequence[Tuple[Optional[str], str]], path: str = "ID file"):
-    """(listed (N,) bool over the .fam samples, IDs that match no sample) of read_id_file's entries.  A bare IID matches
-    the sample with that IID; it is refused (ValueError) when several families hold that IID."""
+def sample_rows(fam_ids: Sequence[Tuple[str, str]], ids: Sequence[Tuple[Optional[str], str]], path: str = "ID file"):
+    """(len(ids),) int64: the .fam sample each of read_id_file's entries names, -1 for none.  A bare IID matches the sample
+    with that IID; it is refused (ValueError) when several families hold that IID."""
     pair = {fi: k for k, fi in enumerate(fam_ids)}
     by_iid: dict = {}
     for k, (_, iid) in enumerate(fam_ids):
         by_iid.setdefault(iid, []).append(k)
-    listed = np.zeros(len(fam_ids), bool)
-    unmatched = 0
-    for fid, iid in ids:
+    out = np.full(len(ids), -1, np.int64)
+    for j, (fid, iid) in enumerate(ids):
         if fid is None:
             ks = by_iid.get(iid, [])
             if len(ks) > 1:
@@ -135,11 +134,64 @@ def match_sample_ids(fam_ids: Sequence[Tuple[str, str]], ids: Sequence[Tuple[Opt
             k = ks[0] if ks else None
         else:
             k = pair.get((fid, iid))
-        if k is None:
-            unmatched += 1
-        else:
-            listed[k] = True
-    return listed, unmatched
+        if k is not None:
+            out[j] = k
+    return out
+
+
+def match_sample_ids(fam_ids: Sequence[Tuple[str, str]], ids: Sequence[Tuple[Optional[str], str]], path: str = "ID file"):
+    """(listed (N,) bool over the .fam samples, IDs that match no sample) of read_id_file's entries (sample_rows' rule)."""
+    rows = sample_rows(fam_ids, ids, path)
+    listed = np.zeros(len(fam_ids), bool)
+    listed[rows[rows >= 0]] = True
+    return listed, int(np.count_nonzero(rows < 0))
+
+
+MISSING_TOKENS = ("NA", "nan", "NaN", "-9")   # a missing value in a --pheno / --covar file
+
+
+def read_value_file(path: str, stem: str):
+    """A --pheno / --covar file -> (column names, [(FID or None, IID)], values (rows, columns) float64, NaN = missing).
+    A first line `#FID IID ..`, `FID IID ..` or `#IID ..` is a header; without one every line is `FID IID v1 ..` and the
+    columns are named stem1, stem2, ...  NA, nan and -9 are missing; any other value must be a finite number (ValueError
+    naming the line otherwise), and every line must have the header's number of fields."""
+    names, ids, values = None, [], []
+    bare = False
+    with open(path, "r", encoding="utf-8") as fh:
+        for ln, line in enumerate(fh, 1):
+            tok = line.split()
+            if not tok:
+                continue
+            if names is None and not ids and tok[0] in ("#FID", "FID", "#IID"):
+                bare = tok[0] == "#IID"
+                names = tok[1:] if bare else tok[2:]
+                continue
+            first = 1 if bare else 2
+            if names is None:
+                names = [f"{stem}{c + 1}" for c in range(len(tok) - first)]
+            if len(tok) != first + len(names):
+                raise ValueError(f"{path}: line {ln} has {len(tok)} fields, {first + len(names)} expected")
+            row = []
+            for t in tok[first:]:
+                if t in MISSING_TOKENS:
+                    row.append(np.nan)
+                    continue
+                try:
+                    x = float(t)
+                except ValueError:
+                    x = np.nan
+                    t = None
+                if t is None or not np.isfinite(x):
+                    raise ValueError(f"{path}: line {ln}: {tok[first + len(row)]!r} is not a number (missing values are "
+                                     f"{', '.join(MISSING_TOKENS)})")
+                row.append(x)
+            ids.append((None, tok[0]) if bare else (tok[0], tok[1]))
+            values.append(row)
+    if names is None:
+        names = []
+    if not names:
+        raise ValueError(f"{path}: no value columns")
+    return names, ids, np.asarray(values, np.float64).reshape(len(ids), len(names))
 
 
 class SampleSubset:

@@ -656,6 +656,72 @@ class VariantsPcaDriver:
         reverse = {i: cid for cid, i in self.common.indexes.items()}
         return [(reverse[i], float(P[i, 0]), float(P[i, 1])) for i in range(rowCount)]
 
+    # -- linear association tests with the PCs as covariates (beyond the reference; DESIGN.md 15) -------------------------
+    def glmSamples(self, glm: "GlmInput") -> None:
+        """Place the --pheno / --covar values on this run's samples (after sample QC), print how many IDs match none, and
+        refuse too few regression samples or a phenotype of at most two values among them, before the Gram."""
+        from . import plink
+        # IDs are matched against the whole .fam, as --keep matches them, so only IDs absent from it count as unmatched;
+        # an ID of a sample that sample QC removed matches and is dropped
+        fam = plink.read_fam_ids(self.conf.bedPath())
+        kept = self.samples.keep if self.samples is not None else np.ones(len(fam), bool)
+        run_index = np.where(kept, np.cumsum(kept) - 1, -1)
+        n = int(kept.sum())
+
+        def place(ids, values, flag, path, out):
+            rows = plink.sample_rows(fam, ids, f"{flag} {path}")
+            found = rows >= 0
+            at = np.full(len(rows), -1, np.int64)
+            at[found] = run_index[rows[found]]
+            out[at[at >= 0]] = values[at >= 0]
+            return int(np.count_nonzero(~found))
+        glm.y = np.full(n, np.nan)
+        unmatched = {"--pheno": (glm.pheno_path, place(glm.pheno_ids, glm.pheno_values, "--pheno", glm.pheno_path,
+                                                         glm.y))}
+        glm.c = np.full((n, glm.covar_values.shape[1]), np.nan) if glm.covar_path else np.zeros((n, 0))
+        if glm.covar_path:
+            unmatched["--covar"] = (glm.covar_path, place(glm.covar_ids, glm.covar_values, "--covar", glm.covar_path,
+                                                          glm.c))
+        for flag, (path, k) in unmatched.items():
+            if k:
+                print(f"{flag} {path}: {k} IDs match no sample.")
+        reg = np.isfinite(glm.y) & np.isfinite(glm.c).all(axis=1)
+        if int(reg.sum()) < glm.q + 2:
+            raise ValueError(f"--glm: {int(reg.sum())} of {n} samples have a phenotype and every covariate; {glm.q} "
+                             f"covariates (the intercept included) need at least {glm.q + 2}")
+        check_glm_quantitative(glm.y[reg], glm.name)
+
+    def glmLinear(self, callsets: CallsRdd, glm: "GlmInput", qc_keep: Optional[np.ndarray] = None):
+        """After the PCs (or the projection): the linear test of every variant that passes variant QC, in file order, on
+        this run's rows, with the intercept, the run's PCs and the --covar columns as covariates.  Writes
+        P.<PHENO>.glm.linear and prints the `GLM linear:` line.  Returns (stats (V, 6), err (V,))."""
+        from . import plink
+        pcs = np.asarray(self.components, np.float64)
+        k = pcs.shape[1]
+        nat = self._native(callsets.n_samples)
+        used = nat.glmBegin(glm.y, np.concatenate([pcs, glm.c], axis=1))
+        stats, errs, tested = [], [], []
+        counted = plink.COUNT_A1
+        for part in callsets.partitions:
+            sel = np.ones(part.nv, bool) if qc_keep is None else np.asarray(qc_keep[part.v0:part.v0 + part.nv], bool)
+            rows = part.bed._map[part.v0:part.v0 + part.nv]        # read in place when every variant is tested
+            st, er = nat.glmLinearBed(rows if sel.all() else rows[sel], part.counted)
+            stats.append(np.asarray(st, np.float64).reshape(-1, 6))
+            errs.append(np.asarray(er, np.int32).reshape(-1))
+            tested.extend((part.v0 + np.flatnonzero(sel)).tolist())
+            counted = part.counted
+        stats = np.concatenate(stats) if stats else np.zeros((0, 6))
+        errs = np.concatenate(errs) if errs else np.zeros(0, np.int32)
+        bim = plink.read_bim(self.conf.bedPath())
+        write_glm_linear(f"{self.conf.outputPath()}.{glm.name}.glm.linear", [bim[j] for j in tested], counted, stats, errs)
+        n = callsets.n_samples
+        c = glm.c.shape[1]
+        covs = f"intercept, {k} PCs" + (f", {c} from {glm.covar_path}" if glm.covar_path else "")
+        print(f"GLM linear: {glm.name} on {used} of {n} samples ({n - used} without a phenotype or covariate), "
+              f"{1 + k + c} covariates ({covs}); {len(errs)} variants tested, {int(np.count_nonzero(errs))} with an "
+              f"ERRCODE; lambda_GC = {lambda_gc(stats, errs)!r}.")
+        return stats, errs
+
     # -- LD pruning of the variants (beyond the reference; DESIGN.md 9) -------------------------------------------------
     def ldPrune(self, callsets: CallsRdd, window_lo: np.ndarray, eligible: Optional[np.ndarray] = None) -> np.ndarray:
         """--ld-prune R2: keep-first LD pruning of the whole fileset in one library call; every BedSlice then stands for
@@ -974,6 +1040,98 @@ def write_eigenvec(prefix: str, fam: Sequence[Tuple[str, str]], vecs: np.ndarray
         fh.write("#FID\tIID\t" + "\t".join(f"PC{c + 1}" for c in range(k)) + "\n")
         fh.write("".join(f"{f}\t{i}\t" + "\t".join(repr(x) for x in row) + "\n"
                          for (f, i), row in zip(fam, vecs.tolist())))
+
+
+@dataclasses.dataclass
+class GlmInput:
+    """The --glm inputs read before any GPU work: the --pheno column and the --covar columns by file ID, and q (the
+    intercept, the PCs and the covariates).  glmSamples sets y (N,) and c (N, columns) on the run's samples."""
+    name: str
+    pheno_path: str
+    pheno_ids: list
+    pheno_values: np.ndarray
+    covar_path: Optional[str]
+    covar_ids: list
+    covar_values: np.ndarray
+    q: int
+    y: Optional[np.ndarray] = None
+    c: Optional[np.ndarray] = None
+
+
+LAMBDA_GC_DENOM = 0.45493642311957283   # the median of chi-square with 1 degree of freedom
+
+
+def lambda_gc(stats: np.ndarray, errs: np.ndarray) -> float:
+    """The genomic inflation factor: the median T_STAT^2 over the variants without an ERRCODE / LAMBDA_GC_DENOM."""
+    t = np.asarray(stats, np.float64)[np.asarray(errs) == 0, 4]
+    return float(np.median(t * t) / LAMBDA_GC_DENOM) if len(t) else float("nan")
+
+
+def check_glm_quantitative(values: np.ndarray, name: str) -> None:
+    """Refuse a phenotype with at most two distinct values: a case/control trait, which linear regression does not fit."""
+    distinct = np.unique(values[np.isfinite(values)])
+    if len(distinct) <= 2:
+        raise ValueError(f"--glm: phenotype {name} has {len(distinct)} distinct value(s); case/control traits need "
+                         "logistic regression, which is not implemented")
+
+
+def check_glm_flags(conf: PcaConf) -> Optional[GlmInput]:
+    """Refuse --glm / --pheno / --pheno-name / --covar runs the association path cannot serve, and read the phenotype
+    and covariate files, before any GPU work.  Returns the inputs of a --glm run, else None."""
+    for flag, opt in (("--pheno", conf.pheno), ("--pheno-name", conf.phenoName), ("--covar", conf.covar)):
+        if opt.isDefined and not conf.glm():
+            raise ValueError(f"{flag} is read by --glm: give --glm")
+    if not conf.glm():
+        return None
+    if not conf.pheno.isDefined:
+        raise ValueError("--glm tests a phenotype: give --pheno FILE")
+    if not conf.bedPath.isDefined:
+        raise ValueError("--glm needs allele dosages: give a PLINK fileset with --bed-path")
+    if not conf.outputPath.isDefined:
+        raise ValueError("--glm writes P.<PHENO>.glm.linear: give --output-path P")
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("--glm runs on one GPU; launch a single process (WORLD_SIZE=1)")
+    if conf.checkpointPath.isDefined:
+        raise ValueError("--glm tests the variants in one pass after the PCs; it cannot resume from --checkpoint-path")
+    from . import plink
+    names, ids, values = plink.read_value_file(conf.pheno(), "PHENO")
+    name = conf.phenoName() if conf.phenoName.isDefined else names[0]
+    if name not in names:
+        raise ValueError(f"--pheno-name {name}: {conf.pheno()} has the columns {', '.join(names)}")
+    y = values[:, names.index(name)]
+    covar_ids, covar_values = [], np.zeros((0, 0))
+    if conf.covar.isDefined:
+        _, covar_ids, covar_values = plink.read_value_file(conf.covar(), "COVAR")
+    if conf.projectLoadings.isDefined and os.path.exists(conf.projectLoadings()):
+        with np.load(conf.projectLoadings(), allow_pickle=False) as f:
+            k = int(f["loadings"].shape[1]) if "loadings" in f.files and f["loadings"].ndim == 2 else 0
+        what = f"the {k} PCs of {conf.projectLoadings()}"
+    else:
+        k = conf.numPc()
+        what = f"--num-pc {k}"
+    q = 1 + k + covar_values.shape[1]
+    if q > native.GLM_MAX_Q:
+        raise ValueError(f"--glm fits at most {native.GLM_MAX_Q} covariates, the intercept included; the intercept, {what} "
+                         f"and {covar_values.shape[1]} --covar columns make {q}")
+    check_glm_quantitative(y, name)
+    return GlmInput(name, conf.pheno(), ids, y, conf.covar.get, covar_ids, covar_values, q)
+
+
+def _glm_number(x: float) -> str:
+    return "NA" if not np.isfinite(x) else repr(float(x))
+
+
+def write_glm_linear(path: str, bim, counted: int, stats: np.ndarray, errs: np.ndarray) -> None:
+    """P.<PHENO>.glm.linear, tab-separated, one line per tested variant in file order (PLINK 2's hide-covar columns): REF
+    is A2 and ALT is A1 as in .afreq, A1 the counted allele, TEST ADD; numbers as the shortest text that reads back as the
+    same double, NA where undefined."""
+    with open(path, "w", encoding="utf-8") as fh:
+        fh.write("#CHROM\tPOS\tID\tREF\tALT\tA1\tA1_FREQ\tTEST\tOBS_CT\tBETA\tSE\tT_STAT\tP\tERRCODE\n")
+        fh.write("".join(
+            f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
+            f"ADD\t{int(st[0])}\t{_glm_number(st[2])}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
+            f"{_glm_number(st[5])}\t{native.GLM_ERRCODES[int(e)]}\n"
+            for b, st, e in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist())))
 
 
 def check_ld_flags(conf: PcaConf, bim=None) -> Optional[np.ndarray]:
@@ -1327,6 +1485,7 @@ def main(args: Optional[Sequence[str]] = None):
     check_ld_flags(conf)
     check_qc_flags(conf)
     check_projection_flags(conf)
+    glm = check_glm_flags(conf)
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         import torch
         import torch.distributed as dist
@@ -1335,6 +1494,8 @@ def main(args: Optional[Sequence[str]] = None):
     driver = VariantsPcaDriver(conf)
     check_king_flags(conf, len(driver.common.indexes))
     check_grm_flags(conf, len(driver.common.indexes))
+    if glm is not None:
+        driver.glmSamples(glm)                          # after sample QC, before the Gram
     window_lo = None
     if conf.ldPrune.isDefined:
         from . import plink
@@ -1364,6 +1525,8 @@ def main(args: Optional[Sequence[str]] = None):
         if conf.saveGrmLoadings.isDefined:
             driver.saveGrmLoadings(callsRdd)
     driver.emitResult(result)
+    if glm is not None:
+        driver.glmLinear(callsRdd, glm, qc_keep)       # every QC-passing variant; the pruned set fed the PCs only
     if conf.makeKingTable.isDefined:
         driver.writeKingTable()
     driver.reportIoStats()

@@ -2,17 +2,24 @@
 // regression samples called at that variant, with the covariates C given to vpca_glm_begin as an orthonormal basis Q
 // (n x q over the regression samples, zero elsewhere) and the residual phenotype y~ = y - Q Q^T y.
 //
+//   glm_count_kernel: one warp per variant, popcounts of the row under the regression mask: the exact integer sums
+//     OBS_CT, sum g and sum g^2 of the counted allele's dosage g over the called regression samples A.
 //   glm_sums_kernel: a thread owns VT variants and walks ALL samples in order 0 .. n-1 (grm_loadings_kernel's tiling: the
 //     CTA's rows staged through shared memory in 32-byte tiles of 128 samples, Q and y~ in the same sample tiles).  Per
-//     variant, one FMA chain per column: b_c = sum g q_c (c < q) and b_q = sum g y~, plus the exact integer sums OBS_CT,
-//     sum g and sum g^2.  g is the counted allele's dosage, 0 for a missing call and for a sample outside the regression.
+//     variant, one FMA chain per column: b_c = sum g' q_c (c < q) and b_q = sum g' y~ of the centred dosage g' = g - c
+//     over A and 0 elsewhere, c in {0, 1, 2} the integer nearest the mean of g over A (glm_centre).
 //   glm_solve_kernel: one warp (one CTA) per variant.  Over the fewer of the variant's missing and called regression
 //     samples (in sample order, one FMA chain per entry) the packed lower triangle of [Q | y~]^T [Q | y~]; from it
 //     P = Q_A^T Q_A, t = Q_A^T y~_A and y~_A^T y~_A over the called set A; Cholesky P = L L^T, u = L^-1 b, v = L^-1 t and
-//     the Schur term s = sum g^2 - u^T u, with the ERRCODEs that need no division.
+//     the Schur term s = sum g'^2 - u^T u, with the ERRCODEs that need no division.
 //   glm_finish_kernel: one thread per variant: A1_FREQ, beta = (b_q - u^T v) / s,
 //     RSS = y~_A^T y~_A - v^T v - (b_q - u^T v) beta, SE = sqrt(RSS / df / s), T_STAT = beta / SE and the two-sided
 //     Student t p-value.
+// Why g' and not g: q_0 is constant over the regression samples, so 1_A lies in the span of Q_A and replacing g by g - c
+// over A changes neither s nor b_q - u^T v (nor beta, SE or the RSS) in exact arithmetic.  But with the raw dosage of an
+// almost fixed allele, sum g^2 is about 4 OBS_CT while s is about the number of carriers of the other allele, and the
+// rounding errors of the n-term chains in b, of size n u sum g^2, land on s whole.  With |mean(g')| <= 1/2 (and
+// g'^2 >= |g'|), sum g'^2 <= 2 sum (g' - mean(g'))^2 = 2 VIF s: s cancels by at most a factor of 2 VIF.
 // A variant's outputs depend on its row's codes, Q, y~, the mask and n only: not on the chunk split, the stride, the
 // padding bits or bytes, or the call.  No floating-point atomics.
 #include <cuda_runtime.h>
@@ -25,14 +32,60 @@
 namespace vpca {
 namespace {
 
+// ---- integer sums --------------------------------------------------------------------------------------------------
+// The centre of a variant's dosage: the integer in {0, 1, 2} nearest sum g / OBS_CT, a tie going to 1.  The tie rule
+// makes the centre of 2 - g exactly 2 - c, so counting the other allele centres to -g' and negates BETA and T_STAT
+// exactly.  Any c works for OBS_CT = 0 (TOO_FEW_OBS).
+__device__ __forceinline__ int glm_centre(int obs, int sg) { return 2 * sg < obs ? 0 : 2 * sg > 3 * obs ? 2 : 1; }
+
+// dosage of the counted allele by .bed code (00 HOM_A1, 01 missing, 10 HET, 11 HOM_A2), two bits each
+constexpr uint32_t kLutA1 = 2u | 0u << 2 | 1u << 4 | 0u << 6;
+constexpr uint32_t kLutA2 = 0u | 0u << 2 | 1u << 4 | 2u << 6;
+
+constexpr int kCThreads = 256;
+
+// grid ceil(nv / (kCThreads / 32)): warp w takes variant blockIdx.x kCThreads / 32 + w, lane l its bytes l, l + 32, ...
+// With lo and hi the even and odd bits of a row byte under the byte's 4 mask bits spread to the even bits: MISSING
+// lo & ~hi, HET hi & ~lo, HOM_A2 lo & hi, HOM_A1 ~(lo | hi).  Writes OBS_CT, sum g and sum g^2 (exact) into the last
+// three doubles of the variant's record of sums; glm_sums_kernel leaves them there.
+__global__ void __launch_bounds__(kCThreads) glm_count_kernel(const uint8_t* __restrict__ rows, int64_t stride, int nv,
+                                                              int n, const uint8_t* __restrict__ mask, bool count_a2,
+                                                              double* __restrict__ sums) {
+    const int lane = threadIdx.x & 31;
+    const int v = blockIdx.x * (kCThreads / 32) + (threadIdx.x >> 5);
+    if (v >= nv) return;   // the whole warp
+    const uint8_t* row = rows + (int64_t)v * stride;
+    const int nb = (n + 3) / 4;
+    int obs = 0, hom = 0, het = 0;
+    for (int b = lane; b < nb; b += 32) {
+        uint32_t m = mask[b];
+        m = (m | m << 2) & 0x33u;
+        m = (m | m << 1) & 0x55u;
+        const uint32_t by = row[b], lo = by & m, hi = (by >> 1) & m;
+        obs += __popc(m) - __popc(lo & ~hi);
+        het += __popc(hi & ~lo);
+        hom += __popc(count_a2 ? lo & hi : m & ~(lo | hi));
+    }
+    obs = __reduce_add_sync(0xffffffffu, obs);
+    het = __reduce_add_sync(0xffffffffu, het);
+    hom = __reduce_add_sync(0xffffffffu, hom);
+    if (lane == 0) {
+        double* o = sums + (int64_t)v * kGlmRec;
+        o[kGlmRec - 3] = obs;
+        o[kGlmRec - 2] = 2 * hom + het;
+        o[kGlmRec - 1] = 4 * hom + het;
+    }
+}
+
 // ---- sums ----------------------------------------------------------------------------------------------------------
 constexpr int kSThreads = 128;
 constexpr int kSTileBytes = 32;                 // row bytes per tile (128 samples)
 constexpr int kSPitch = kSTileBytes / 4 + 1;    // words per staged row: odd, so 32 consecutive rows hit 32 banks
 constexpr int kSTileS = 4 * kSTileBytes;        // samples per tile
 
-// grid ceil(nv / (kSThreads VT)).  Qx: n rows of KMAX + 2 doubles, [q_0 .. q_{q-1}, y~, 0 .., mask].  Samples >= n meet a
-// zero tile row (mask 0, so g = 0): fma(0, 0, a) = a for an accumulator that never holds -0, so they change no bit.
+// grid ceil(nv / (kSThreads VT)), after glm_count_kernel.  Qx: n rows of KMAX + 2 doubles, [q_0 .. q_{q-1}, y~, 0 ..,
+// mask].  Samples >= n meet a zero tile row (mask 0, so g' = 0): fma(0, 0, a) = a for an accumulator that never holds -0,
+// so they change no bit.  g' is an integer in [-2, 2], so every product g' x is exact.
 template <int KMAX, int VT>
 __global__ void __launch_bounds__(kSThreads) glm_sums_kernel(const uint8_t* __restrict__ rows, int64_t stride, int nv, int n,
                                                              const double* __restrict__ Qx, uint32_t lut,
@@ -45,10 +98,12 @@ __global__ void __launch_bounds__(kSThreads) glm_sums_kernel(const uint8_t* __re
     const int v0 = blockIdx.x * RB;
     const int nb = (n + 3) / 4;
     double acc[VT][KMAX + 1];
-    int obs[VT], sg[VT], gg[VT];
+    int cv[VT];   // the centre of each variant's dosage, from glm_count_kernel's OBS_CT and sum g
 #pragma unroll
     for (int i = 0; i < VT; ++i) {
-        obs[i] = sg[i] = gg[i] = 0;
+        const int v = v0 + i * kSThreads + threadIdx.x;
+        const double* rec = sums + (int64_t)min(v, nv - 1) * kGlmRec;
+        cv[i] = glm_centre((int)rec[kGlmRec - 3], (int)rec[kGlmRec - 2]);
 #pragma unroll
         for (int c = 0; c <= KMAX; ++c) acc[i][c] = 0.0;
     }
@@ -77,11 +132,7 @@ __global__ void __launch_bounds__(kSThreads) glm_sums_kernel(const uint8_t* __re
 #pragma unroll
                 for (int i = 0; i < VT; ++i) {
                     const uint32_t code = (word[i] >> (2 * j)) & 3u;
-                    const int gi = in ? (int)((lut >> (2 * code)) & 3u) : 0;
-                    obs[i] += (in && code != 1u) ? 1 : 0;
-                    sg[i] += gi;
-                    gg[i] += gi * gi;
-                    const double g = (double)gi;
+                    const double g = (in && code != 1u) ? (double)((int)((lut >> (2 * code)) & 3u) - cv[i]) : 0.0;
 #pragma unroll
                     for (int c = 0; c <= KMAX; ++c) acc[i][c] = fma(g, x[c], acc[i][c]);
                 }
@@ -95,9 +146,6 @@ __global__ void __launch_bounds__(kSThreads) glm_sums_kernel(const uint8_t* __re
         double* o = sums + (int64_t)v * kGlmRec;
 #pragma unroll
         for (int c = 0; c <= KMAX; ++c) o[c] = acc[i][c];
-        o[kGlmRec - 3] = obs[i];
-        o[kGlmRec - 2] = sg[i];
-        o[kGlmRec - 1] = gg[i];
     }
 }
 
@@ -314,9 +362,11 @@ __global__ void __launch_bounds__(kGWarps * 32, KMAX >= 32 ? 8 : 16) glm_solve_k
         vv = fma(sx[w][j], sx[w][j], vv);
     }
     const int sg = sc[w][1], gg = sc[w][2];
-    const double s = (double)gg - uu;
+    const int c = glm_centre(obs, sg);
+    const double s = (double)((int64_t)gg - 2ll * c * sg + (int64_t)c * c * obs) - uu;   // sum g'^2 exactly, - u^T u
     double* o = out + (int64_t)v * 6;
-    // s <= 1e-10 (sum g^2 - (sum g)^2 / OBS_CT), multiplied through by OBS_CT: the divisions wait for glm_finish_kernel
+    // s <= 1e-10 (sum g^2 - (sum g)^2 / OBS_CT), multiplied through by OBS_CT: the divisions wait for glm_finish_kernel.
+    // The centred dosage has the same OBS_CT sum g'^2 - (sum g')^2, so the raw sums serve.
     if (!(s * obs > 1e-10 * (double)((int64_t)gg * obs - (int64_t)sg * sg))) {
         err[v] = VPCA_GLM_VIF_INFINITE;
         return;
@@ -367,6 +417,8 @@ void launch(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, int n_r
             int32_t* d_err, cudaStream_t stream) {
     constexpr int VT = KMAX >= 32 ? 1 : 2;
     const unsigned grid = (unsigned)((nv + kSThreads * VT - 1) / (kSThreads * VT));
+    glm_count_kernel<<<(unsigned)((nv + kCThreads / 32 - 1) / (kCThreads / 32)), kCThreads, 0, stream>>>(
+        d_rows, stride, nv, n, d_mask, lut == kLutA2, d_sums);
     glm_sums_kernel<KMAX, VT><<<grid, kSThreads, 0, stream>>>(d_rows, stride, nv, n, d_Qx, lut, d_sums);
     glm_solve_kernel<KMAX><<<(unsigned)((nv + kGWarps - 1) / kGWarps), kGWarps * 32, 0, stream>>>(
         d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, d_sums, d_out, d_err);
@@ -381,8 +433,7 @@ cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int
                        const uint8_t* d_mask, const double* d_z0, double yty, int counted, double* d_sums, double* d_out,
                        int32_t* d_err, cudaStream_t stream) {
     if (nv <= 0) return cudaSuccess;
-    // dosage of the counted allele by .bed code (00 HOM_A1, 01 missing, 10 HET, 11 HOM_A2), two bits each
-    const uint32_t lut = counted == 2 ? (0u | 0u << 2 | 1u << 4 | 2u << 6) : (2u | 0u << 2 | 1u << 4 | 0u << 6);
+    const uint32_t lut = counted == 2 ? kLutA2 : kLutA1;
     switch (glm_kmax(q)) {
         case 2: launch<2>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
         case 4: launch<4>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;

@@ -251,8 +251,8 @@ cudaError_t grm_project(const uint8_t* d_rows, int64_t stride, int nv, int n, co
                         int k, double* d_part, double* d_acc, int acc_ld, cudaStream_t stream);
 
 // ---- linear association tests (glm.cu, DESIGN.md 15) ----------------------------------------------------------------
-// Doubles per variant of the sums: b_0 .. b_KMAX (b_c = sum g q_c for c < q, b_q = sum g y~, zero past q), then OBS_CT,
-// sum g and sum g^2 (exact integers).
+// Doubles per variant of the sums: b_0 .. b_KMAX (b_c = sum g' q_c for c < q, b_q = sum g' y~, zero past q, g' the
+// centred dosage of glm.cu), then OBS_CT, sum g and sum g^2 of the raw dosage (exact integers).
 constexpr int kGlmRec = VPCA_GLM_MAX_Q + 4;
 // Columns of Q the kernels are instantiated for (2, 4, 8, 16 or 32); Qx has glm_kmax(q) + 2 doubles per sample.
 int glm_kmax(int q);

@@ -25,9 +25,13 @@ def regression_samples(pheno, covar):
     return ok
 
 
-def linear(rows, n, pheno, covar=None, counted=1):
-    """-> (stats (nv, 6): OBS_CT, A1_FREQ, BETA, SE, T_STAT, P with NaN where undefined; err (nv,) int).  lstsq per variant
-    on [1, covar, g] over the called regression samples."""
+def linear(rows, n, pheno, covar=None, counted=1, centre=True):
+    """-> (stats (nv, 6): OBS_CT, A1_FREQ, BETA, SE, T_STAT, P with NaN where undefined; err (nv,) int).  Per variant,
+    over the called regression samples A, the residuals of g - c and of the phenotype after [1, covar - its mean] by
+    lstsq, c the integer nearest the mean of g over A (with centre=False, of g after [1, covar]).  The intercept absorbs
+    both shifts, so BETA, SE and the residuals are those of [1, covar, g]; but the residual of a dosage that is almost constant, such as 2 at all but a few samples, is then
+    computed from values of size at most 2 around a mean within 1/2 of 0, not as a difference of sums of size 4 OBS_CT,
+    and a covariate far from 0 is not nearly collinear with the intercept."""
     pheno = np.asarray(pheno, np.float64)
     covar = np.zeros((n, 0)) if covar is None else np.asarray(covar, np.float64).reshape(n, -1)
     reg = regression_samples(pheno, covar)
@@ -55,25 +59,70 @@ def linear(rows, n, pheno, covar=None, counted=1):
         if np.all(ga == ga[0]):
             err[v] = 2
             continue
+        if centre:
+            ga = ga - nearest_integer_mean(ga.sum(), obs)
+            Ca = Ca - np.concatenate([[0.0], Ca[:, 1:].mean(axis=0)])
         # the dosage's residual sum of squares after the covariates against its centred one
-        gam = np.linalg.lstsq(Ca, ga, rcond=None)[0]
-        s = float(((ga - Ca @ gam) ** 2).sum())
+        gr = ga - Ca @ np.linalg.lstsq(Ca, ga, rcond=None)[0]
+        s = float(gr @ gr)
         css = float(((ga - ga.mean()) ** 2).sum())
         if collinear(Q[A]) or s <= 1e-10 * css:
             err[v] = 3
             continue
-        X = np.concatenate([Ca, ga[:, None]], axis=1)
-        coef = np.linalg.lstsq(X, ya, rcond=None)[0]
-        res = ya - X @ coef
+        # BETA and the residuals from the two residuals after the covariates (Frisch-Waugh-Lovell): no solve with the
+        # dosage beside the intercept, whose condition would be squared into BETA
+        yr = ya - Ca @ np.linalg.lstsq(Ca, ya, rcond=None)[0]
+        beta = float(gr @ yr) / s
+        res = yr - beta * gr
         rss = float(res @ res)
         if rss <= 1e-12 * float((yt[A] ** 2).sum()):
             err[v] = 4
             continue
-        beta = coef[-1]
         se = np.sqrt(rss / df / s)
         t = beta / se
         out[v, 2:] = beta, se, t, 2.0 * scipy.stats.t.sf(abs(t), df)
     return out, err
+
+
+def nearest_integer_mean(sum_g, obs):
+    """The integer in {0, 1, 2} nearest the mean dosage sum_g / obs > 0, a tie going to 1, in integers as glm.cu has it.
+    The tie rule makes the centre of 2 - g exactly 2 minus the centre of g, so the two centred dosages are negatives."""
+    sum_g, obs = int(sum_g), int(obs)
+    return 0 if 2 * sum_g < obs else 2 if 2 * sum_g > 3 * obs else 1
+
+
+def mirror(rows):
+    """.bed rows with codes 00 (HOM_A1) and 11 (HOM_A2) swapped: counting A1 in them counts A2 in `rows`."""
+    rows = np.asarray(rows, np.uint8)
+    lo, hi = rows & 0x55, (rows >> 1) & 0x55
+    hom = ~(lo ^ hi) & 0x55   # 00 or 11
+    return rows ^ (hom * 3).astype(np.uint8)
+
+
+def near_fixed_codes(rng, n, kinds=None):
+    """Codes (k, n) of variants whose counted allele A1 is almost fixed or whose dosage is almost constant: A1 fixed but
+    1, 2, 3 or 10 hets; A1 fixed but one HOM_A2; all het but one or two homs; A1 frequency 0.999 and 0.99.  The carriers
+    of the rarer genotypes sit at random samples, at least one of them.  kinds: a subset of KINDS by name."""
+    out = []
+    for kind in KINDS if kinds is None else kinds:
+        c = np.zeros(n, np.uint8)
+        if kind.startswith("het"):
+            c[rng.choice(n, int(kind[3:]), replace=False)] = 2
+        elif kind == "hom2":
+            c[rng.integers(n)] = 3
+        elif kind.startswith("allhet"):
+            c[:] = 2
+            c[rng.choice(n, int(kind[6:]), replace=False)] = [0, 3][: int(kind[6:])]
+        else:
+            a1 = rng.binomial(2, float(kind[1:]), n)
+            if np.all(a1 == 2):
+                a1[rng.integers(n)] = 1
+            c = np.select([a1 == 2, a1 == 1], [0, 2], 3).astype(np.uint8)
+        out.append(c)
+    return np.stack(out)
+
+
+KINDS = ("het1", "het2", "het3", "het10", "hom2", "allhet1", "allhet2", "f0.999", "f0.99")
 
 
 def collinear(QA, pivot_min=1e-10):

@@ -30,7 +30,7 @@ SUMS_DOUBLES = native.GLM_MAX_Q + 4
 
 
 def kernel_of(name):
-    for key in ("glm_sums_kernel", "glm_solve_kernel", "glm_finish_kernel", "Memcpy HtoD", "Memcpy DtoH"):
+    for key in ("glm_count_kernel", "glm_sums_kernel", "glm_solve_kernel", "glm_finish_kernel", "Memcpy HtoD", "Memcpy DtoH"):
         if key in name:
             return key.replace("Memcpy ", "memcpy_").lower()
     return "other"

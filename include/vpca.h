@@ -522,12 +522,43 @@ enum {
     VPCA_GLM_TOO_FEW_OBS = 1,
     VPCA_GLM_CONST_ALLELE = 2,
     VPCA_GLM_VIF_INFINITE = 3,
-    VPCA_GLM_NO_RESIDUAL = 4
+    VPCA_GLM_NO_RESIDUAL = 4,
+    VPCA_GLM_LOGISTIC_CONVERGE_FAIL = 5
 };
 #define VPCA_GLM_MAX_Q 32
 int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used);
 int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
                         double* out, int32_t* out_err);
+
+/* ---- logistic association tests (beyond VariantsPca.scala: PLINK 2's --glm no-firth for case/control traits;
+ * DESIGN.md 16) ---------------------------------------------------------------------------------------------------------
+ * A case/control trait y in {0 (control), 1 (case)}, an additive model, per variant on the complete cases: with the
+ * regression samples, C, q, g, A_v and OBS_CT as above, maximum likelihood over A_v of logit P(y = 1) = C gamma + beta g
+ * gives BETA = beta, SE = sqrt([H^-1]_gg) with H = X^T W X at the fit, Z = BETA / SE, P = erfc(|Z| / sqrt(2)) (0 below the
+ * double range) and A1_FREQ as in the linear test.  The fit runs in the orthonormal basis Q of C and the centred dosage
+ * of the linear test, by Newton passes from (the null fit, beta = 0): each pass evaluates l, grad l and H over A_v;
+ * a fall of l by more than 1e-10 |l| against the last accepted pass halves the step (at most 8 times in a row);
+ * otherwise H = L L^T and the pass stops at a Newton decrement ||L^-1 grad l|| <= 1e-9, reporting beta + the step's
+ * last entry and SE = 1 / L_gg; at most 25 passes.  ERRCODE, checked in this order:
+ *   VPCA_GLM_TOO_FEW_OBS             OBS_CT - q - 1 < 1
+ *   VPCA_GLM_CONST_ALLELE            g constant over A_v
+ *   VPCA_GLM_LOGISTIC_CONVERGE_FAIL  A_v holds no case or no control (exact counts)
+ *   VPCA_GLM_VIF_INFINITE            on the first pass a Cholesky pivot of H <= 1e-10 x that diagonal entry of H
+ *   VPCA_GLM_LOGISTIC_CONVERGE_FAIL  no convergence in 25 passes or 8 halvings, a pivot <= 0 after the first pass, or a
+ *                                    non-finite l or step (separation lands here)
+ * A flagged variant has BETA, SE, Z and P NaN.
+ * vpca_glm_logistic_begin: pheno is 0, 1 or NaN (missing) per sample, covar as vpca_glm_begin.  Refuses with
+ *   VPCA_ERR_BAD_ARG, leaving no GLM state, everything vpca_glm_begin refuses, a phenotype outside {0, 1, NaN}, no case or
+ *   no control among the regression samples, and a null fit (Q alone, all regression samples, on the host in FP64 by the
+ *   rules above) that does not converge, as when a covariate separates cases from controls; the message names the
+ *   problem.  The GLM state records its model: vpca_glm_linear_bed after this call, and vpca_glm_logistic_bed after
+ *   vpca_glm_begin, return VPCA_ERR_STATE.
+ * vpca_glm_logistic_bed: out[6 v ..] = OBS_CT, A1_FREQ, BETA, SE, Z, P, out_err[v] = ERRCODE and out_passes[v] (may be
+ *   NULL) = the Newton passes run (0 for a variant flagged before the first), with the row, chunk and argument rules of
+ *   vpca_glm_linear_bed.  Every output of a variant depends on its row's codes, Q, y, the null fit and n_samples only. */
+int vpca_glm_logistic_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used);
+int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                          double* out, int32_t* out_err, int32_t* out_passes);
 
 /* ---- sample quality control (beyond VariantsPca.scala: which samples go into S; DESIGN.md 11) -------------------------
  * --keep / --remove / --mind decide the samples of a run before its context exists: the per-sample missing-call counts

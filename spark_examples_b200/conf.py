@@ -135,4 +135,6 @@ class PcaConf(GenomicsConf):
             ("covar", str, None, False),                  # with --glm: a file of covariates, all used beside the PCs
             ("glm", bool, False, False),                  # --bed-path runs: linear association tests with the PCs as
                                                           # covariates, written to P.<PHENO>.glm.linear
+            ("glmLogistic", bool, False, False),          # with --glm: a case/control phenotype (1 control, 2 case) by
+                                                          # logistic regression, written to P.<PHENO>.glm.logistic
         ]

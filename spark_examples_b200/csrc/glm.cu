@@ -46,11 +46,12 @@ constexpr int kCThreads = 256;
 
 // grid ceil(nv / (kCThreads / 32)): warp w takes variant blockIdx.x kCThreads / 32 + w, lane l its bytes l, l + 32, ...
 // With lo and hi the even and odd bits of a row byte under the byte's 4 mask bits spread to the even bits: MISSING
-// lo & ~hi, HET hi & ~lo, HOM_A2 lo & hi, HOM_A1 ~(lo | hi).  Writes OBS_CT, sum g and sum g^2 (exact) into the last
-// three doubles of the variant's record of sums; glm_sums_kernel leaves them there.
+// lo & ~hi, HET hi & ~lo, HOM_A2 lo & hi, HOM_A1 ~(lo | hi).  Writes OBS_CT, sum g and sum g^2 (exact) under the mask
+// to out[v * rec ..]: the linear path points out at the last three doubles of each record of sums (glm_sums_kernel leaves
+// them there), the logistic path runs it twice, under the regression mask and under the case mask.
 __global__ void __launch_bounds__(kCThreads) glm_count_kernel(const uint8_t* __restrict__ rows, int64_t stride, int nv,
                                                               int n, const uint8_t* __restrict__ mask, bool count_a2,
-                                                              double* __restrict__ sums) {
+                                                              double* __restrict__ out, int rec) {
     const int lane = threadIdx.x & 31;
     const int v = blockIdx.x * (kCThreads / 32) + (threadIdx.x >> 5);
     if (v >= nv) return;   // the whole warp
@@ -70,10 +71,10 @@ __global__ void __launch_bounds__(kCThreads) glm_count_kernel(const uint8_t* __r
     het = __reduce_add_sync(0xffffffffu, het);
     hom = __reduce_add_sync(0xffffffffu, hom);
     if (lane == 0) {
-        double* o = sums + (int64_t)v * kGlmRec;
-        o[kGlmRec - 3] = obs;
-        o[kGlmRec - 2] = 2 * hom + het;
-        o[kGlmRec - 1] = 4 * hom + het;
+        double* o = out + (int64_t)v * rec;
+        o[0] = obs;
+        o[1] = 2 * hom + het;
+        o[2] = 4 * hom + het;
     }
 }
 
@@ -206,7 +207,8 @@ __device__ __forceinline__ double t_pvalue(double t, double df) {
 }
 
 // ---- solve ---------------------------------------------------------------------------------------------------------
-// 1 / sqrt(d) for d in (1e-10, 1]: the single-precision estimate and two Newton steps in FP64 (24 -> 48 -> ~53 bits), with
+// 1 / sqrt(d) for d > 0 in the normal float range (the linear solve's pivots lie in (1e-10, 1], the logistic Newton
+// kernel's in (1e-10 H_jj, N]): the single-precision estimate and two Newton steps in FP64 (24 -> 48 -> ~53 bits), with
 // no call into the slow paths of the FP64 division and square root (their calling convention makes the solve spill).
 __device__ __forceinline__ double rsqrt_newton(double d) {
     double r = (double)__frsqrt_rn((float)d);
@@ -418,11 +420,345 @@ void launch(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, int n_r
     constexpr int VT = KMAX >= 32 ? 1 : 2;
     const unsigned grid = (unsigned)((nv + kSThreads * VT - 1) / (kSThreads * VT));
     glm_count_kernel<<<(unsigned)((nv + kCThreads / 32 - 1) / (kCThreads / 32)), kCThreads, 0, stream>>>(
-        d_rows, stride, nv, n, d_mask, lut == kLutA2, d_sums);
+        d_rows, stride, nv, n, d_mask, lut == kLutA2, d_sums + kGlmRec - 3, kGlmRec);
     glm_sums_kernel<KMAX, VT><<<grid, kSThreads, 0, stream>>>(d_rows, stride, nv, n, d_Qx, lut, d_sums);
     glm_solve_kernel<KMAX><<<(unsigned)((nv + kGWarps - 1) / kGWarps), kGWarps * 32, 0, stream>>>(
         d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, d_sums, d_out, d_err);
     glm_finish_kernel<<<(unsigned)((nv + 127) / 128), 128, 0, stream>>>(nv, q, d_out, d_err);
+}
+
+// ---- logistic regression (DESIGN.md 16) ------------------------------------------------------------------------------
+// 1 / d for d in (1, 2]: the single-precision estimate and three Newton steps in FP64, with no call into the slow path of
+// the FP64 division (as rsqrt_newton).
+__device__ __forceinline__ double recip_newton(double d) {
+    double r = (double)__frcp_rn((float)d);
+    r = fma(r, fma(-d, r, 1.0), r);
+    r = fma(r, fma(-d, r, 1.0), r);
+    return fma(r, fma(-d, r, 1.0), r);
+}
+
+constexpr int kLWarps = 8;                 // variants in flight per CTA, all fed by each staged tile of Q and y
+constexpr int kLPerCta = 4 * kLWarps;      // the contiguous range of variants a CTA owns
+constexpr int kLTile = 32;                 // samples per staged tile: one per lane
+constexpr int kLMaxPass = 25;              // passes (evaluations of l, its gradient and H) per variant
+constexpr int kLMaxHalve = 8;              // step halvings in a row
+constexpr double kLDelta2 = 1e-18;         // convergence: the Newton decrement squared, delta <= 1e-9
+constexpr double kLFall = 1e-10;           // l fell: by more than this times |l| of the last accepted pass
+
+// Shared memory of glm_logistic_kernel, in doubles.  LD: pitch of one staged sample, in the tile of Q and y
+// [q_0 .. q_{KMAX-1}, y, mask, 0] and in a warp's tile U [w q_0 .. w q_{q-1}, w g', r, 0 .., g'] (u at 0 .. PMAX - 1,
+// g' at PMAX).  PMAX = KMAX + 2 rows of the augmented lower triangle: H (p = q + 1 <= KMAX + 1 rows) and the gradient
+// (row p).  Once a pass is summed, H and then L take the warp's U tile at pitch KMAX + 1.  Per warp also theta, theta
+// of the last accepted pass, the step, the gradient (then L^-1 grad), 1 / L_jj and the lanes' partial l.
+template <int KMAX>
+struct LogLayout {
+    static constexpr int LD = KMAX + 3;
+    static constexpr int PMAX = KMAX + 2;
+    static constexpr int PH = KMAX + 1;
+    static constexpr int NBK = PMAX / 2;                          // 2 x 2 blocks per side
+    static constexpr int NB = (NBK * (NBK + 1) / 2 + 31) / 32;    // lower-triangle blocks per lane
+    static constexpr int WARP = kLTile * LD + 5 * PMAX + 32;
+    static constexpr int TOTAL = kLTile * LD + kLWarps * WARP;
+    static_assert(PH * PH <= kLTile * LD, "H must fit in the U tile it takes over");
+};
+
+// grid ceil(nv / kLPerCta); CTA c owns variants [c kLPerCta, min(nv, (c + 1) kLPerCta)).  cnt[v * 6 ..]: OBS_CT, sum g,
+// sum g^2 under the regression mask, then OBS_CT under the case mask (glm_count_kernel).  Qx: n rows of KMAX + 2
+// doubles [q_0 .. q_{q-1}, y, 0 .., mask] (y at column q); theta0: the null fit (q).  Per pass every warp holding a
+// variant evaluates l, grad l and H = X^T W X at its theta over A_v, X = [Q | g'], while the CTA walks the sample tiles in
+// order: lane l computes eta, mu, w and r of sample s0 + l and writes its row of U, then every lane adds the 32 samples
+// in order into its 2 x 2 blocks of the augmented triangle (4 shared loads feed 4 FMAs).  Between passes the warp factors
+// H and steps (DESIGN.md 16); a warp whose variant is done takes the CTA's next unstarted variant at the next pass
+// boundary, in warp order.  Out: out[v * 6 ..] = OBS_CT, sum g, BETA, SE (glm_logistic_finish_kernel completes them),
+// err[v], passes[v].  A sample outside A_v adds exactly 0 to every sum (u = 0, g' = 0, l untouched), so a variant's
+// outputs depend on its row's codes, Q, y, theta0, the mask and n only.  No floating-point atomics.
+template <int KMAX>
+__global__ void __launch_bounds__(kLWarps * 32, 2) glm_logistic_kernel(const uint8_t* __restrict__ rows, int64_t stride,
+                                                                      int nv, int n, int q, const double* __restrict__ Qx,
+                                                                      const double* __restrict__ theta0, uint32_t lut,
+                                                                      const double* __restrict__ cnt,
+                                                                      double* __restrict__ out, int32_t* __restrict__ err,
+                                                                      int32_t* __restrict__ passes) {
+    using Lo = LogLayout<KMAX>;
+    constexpr int LD = Lo::LD, PMAX = Lo::PMAX, PH = Lo::PH, NB = Lo::NB;
+    extern __shared__ __align__(16) double lsm[];
+    __shared__ int sst[kLWarps][4];   // variant (-1: none), passes so far, halvings in a row, centre of the dosage
+    __shared__ int sflag[kLWarps];
+    __shared__ double slp[kLWarps][2];   // l of the last accepted pass, l of this pass
+    __shared__ int snext, sany;
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double* const Qt = lsm;
+    const int uoff = kLTile * LD + w * Lo::WARP;
+    double* const U = lsm + uoff;
+    double* const H = U;
+    double* const th = U + kLTile * LD;
+    double* const thp = th + PMAX;
+    double* const del = thp + PMAX;
+    double* const grad = del + PMAX;
+    double* const sr = grad + PMAX;
+    double* const lpart = sr + PMAX;
+    const int p = q + 1;
+    const int nblk = (p + 2) / 2;   // 2 x 2 blocks per side over rows 0 .. p
+    const int nblocks = nblk * (nblk + 1) / 2;
+    // this lane's blocks: rows ba, ba + 1 and columns bb, bb + 1; xo: the offset in lsm of each column's value of sample 0
+    int ba[NB], bb[NB], xo[NB][2];
+#pragma unroll
+    for (int j = 0; j < NB; ++j) {
+        const int t = lane + 32 * j;
+        int I = 0;
+        while ((I + 1) * (I + 2) / 2 <= t) ++I;
+        ba[j] = 2 * I;
+        bb[j] = 2 * (t - I * (I + 1) / 2);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int b = bb[j] + e;
+            xo[j][e] = b < q ? b : b == q ? uoff + PMAX : KMAX + 2;
+        }
+    }
+    const int v_end = min(nv, (int)(blockIdx.x + 1) * kLPerCta);
+    if (threadIdx.x == 0) snext = blockIdx.x * kLPerCta;
+    if (lane == 0) sst[w][0] = -1;
+    const int nt = (n + kLTile - 1) / kLTile;
+    for (;;) {
+        __syncthreads();   // every warp's decision of the last pass is in sst
+        if (threadIdx.x == 0) {
+            int any = 0;
+            for (int ww = 0; ww < kLWarps; ++ww) {
+                while (sst[ww][0] < 0 && snext < v_end) {
+                    const int v = snext++;
+                    const double* c = cnt + (int64_t)v * 6;
+                    const int obs = (int)c[0], sg = (int)c[1], gg = (int)c[2], cases = (int)c[3];
+                    double* o = out + (int64_t)v * 6;
+                    o[0] = obs;
+                    o[1] = sg;   // glm_logistic_finish_kernel divides
+                    const int e = obs - q - 1 < 1                              ? VPCA_GLM_TOO_FEW_OBS
+                                  : (int64_t)obs * gg == (int64_t)sg * sg      ? VPCA_GLM_CONST_ALLELE
+                                  : cases == 0 || cases == obs                 ? VPCA_GLM_LOGISTIC_CONVERGE_FAIL
+                                                                               : VPCA_GLM_OK;
+                    if (e != VPCA_GLM_OK) {
+                        err[v] = e;
+                        passes[v] = 0;
+                        continue;
+                    }
+                    sst[ww][0] = v;
+                    sst[ww][1] = 0;
+                    sst[ww][2] = 0;
+                    sst[ww][3] = glm_centre(obs, sg);
+                }
+                any |= sst[ww][0] >= 0;
+            }
+            sany = any;
+        }
+        __syncthreads();
+        if (!sany) break;
+        const int v = sst[w][0];
+        const bool act = v >= 0;   // uniform over the warp
+        if (act && sst[w][1] == 0)
+            for (int c = lane; c < PMAX; c += 32) th[c] = c < q ? theta0[c] : 0.0;
+        __syncwarp();
+        const uint8_t* row = rows + (int64_t)(act ? v : 0) * stride;
+        const int cen = act ? sst[w][3] : 0;
+        double acc[NB][4];
+#pragma unroll
+        for (int j = 0; j < NB; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.0;
+        double lsum = 0.0;
+#pragma unroll 1
+        for (int t = 0; t < nt; ++t) {
+            const int s0 = t * kLTile;
+            __syncthreads();   // every warp is done with the previous tile
+            for (int i = threadIdx.x; i < kLTile * LD; i += kLWarps * 32) {
+                const int r = i / LD, c = i - r * LD, s = s0 + r;
+                Qt[i] = (c < KMAX + 2 && s < n) ? Qx[(int64_t)s * (KMAX + 2) + c] : 0.0;
+            }
+            __syncthreads();
+            if (!act) continue;
+            {   // sample s0 + lane
+                const int s = s0 + lane;
+                const double* x = Qt + lane * LD;
+                double* u = U + lane * LD;
+                const uint32_t code = s < n ? (row[s >> 2] >> (2 * (s & 3))) & 3u : 1u;
+                const bool in = x[KMAX + 1] != 0.0 && code != 1u;
+                const double g = in ? (double)((int)((lut >> (2 * code)) & 3u) - cen) : 0.0;
+                double eta = 0.0;
+                for (int c = 0; c < q; ++c) eta = fma(x[c], th[c], eta);
+                eta = fma(th[q], g, eta);
+                double wt = 0.0, r = 0.0;
+                if (in) {
+                    const double y = x[q];
+                    const double e = exp(-fabs(eta));
+                    const double rd = recip_newton(1.0 + e);
+                    const double mu = eta >= 0.0 ? rd : e * rd;
+                    wt = e * rd * rd;
+                    r = y - mu;
+                    const double m = y != 0.0 ? -eta : eta;   // l_s = y eta - log(1 + e^eta) = -softplus(m)
+                    lsum -= fmax(m, 0.0) + log1p(e);
+                }
+                for (int c = 0; c < q; ++c) u[c] = wt * x[c];
+                u[q] = wt * g;
+                u[p] = r;
+                for (int c = p + 1; c < 2 * nblk; ++c) u[c] = 0.0;
+                u[PMAX] = g;
+            }
+            __syncwarp();
+#pragma unroll 2
+            for (int s = 0; s < kLTile; ++s) {
+                const double* ur = U + s * LD;
+#pragma unroll
+                for (int j = 0; j < NB; ++j) {
+                    if (lane + 32 * j >= nblocks) continue;
+                    const double u0 = ur[ba[j]], u1 = ur[ba[j] + 1];
+                    const double x0 = lsm[xo[j][0] + s * LD], x1 = lsm[xo[j][1] + s * LD];
+                    acc[j][0] = fma(u0, x0, acc[j][0]);
+                    acc[j][1] = fma(u0, x1, acc[j][1]);
+                    acc[j][2] = fma(u1, x0, acc[j][2]);
+                    acc[j][3] = fma(u1, x1, acc[j][3]);
+                }
+            }
+            __syncwarp();
+        }
+        if (!act) continue;
+        // H (lower triangle, pitch PH, over the U tile) and the gradient from the blocks; each entry has one owner
+#pragma unroll
+        for (int j = 0; j < NB; ++j) {
+            if (lane + 32 * j >= nblocks) continue;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int a = ba[j] + (e >> 1), b = bb[j] + (e & 1);
+                if (b >= p || a < b || a > p) continue;
+                if (a < p) H[a * PH + b] = acc[j][e];
+                else grad[b] = acc[j][e];
+            }
+        }
+        lpart[lane] = lsum;
+        __syncwarp();
+        if (lane == 0) {
+            double l = 0.0;
+            for (int i = 0; i < 32; ++i) l += lpart[i];
+            const int k = ++sst[w][1];
+            int fl = 0;   // 0: factor H; 1: the step was halved; 2: LOGISTIC_CONVERGE_FAIL
+            if (!isfinite(l)) {
+                fl = 2;
+            } else if (k > 1 && l < slp[w][0] - kLFall * fabs(slp[w][0])) {
+                if (sst[w][2] == kLMaxHalve || k == kLMaxPass) {
+                    fl = 2;
+                } else {
+                    ++sst[w][2];
+                    for (int c = 0; c < p; ++c) {
+                        del[c] *= 0.5;
+                        th[c] = thp[c] + del[c];
+                    }
+                    fl = 1;
+                }
+            }
+            slp[w][1] = l;
+            sflag[w] = fl;
+        }
+        __syncwarp();
+        if (sflag[w] == 0) {
+            // Cholesky H = L L^T, left-looking by column; lanes own rows j + 1 + lane, j + 33 + lane; sr[j] = 1 / L_jj.
+            // First pass: a pivot <= kPivotMin H_jj is VIF_INFINITE; later: a pivot <= 0 is LOGISTIC_CONVERGE_FAIL.
+            const bool first = sst[w][1] == 1;
+            for (int j = 0; j < p; ++j) {
+                if (lane == 0) {
+                    const double hjj = H[j * PH + j];
+                    double d = hjj;
+                    for (int k = 0; k < j; ++k) d = fma(-H[j * PH + k], H[j * PH + k], d);
+                    const bool ok = first ? d > kPivotMin * hjj : d > 0.0;
+                    sr[j] = ok ? rsqrt_newton(d) : 0.0;
+                    sflag[w] = ok ? 0 : first ? 3 : 2;
+                }
+                __syncwarp();
+                if (sflag[w] != 0) break;
+                for (int i = j + 1 + lane; i < p; i += 32) {
+                    double x = H[i * PH + j];
+                    for (int k = 0; k < j; ++k) x = fma(-H[i * PH + k], H[j * PH + k], x);
+                    H[i * PH + j] = x * sr[j];
+                }
+                __syncwarp();
+            }
+        }
+        if (lane == 0) {
+            int fl = sflag[w];
+            const int k = sst[w][1];
+            bool done = false;
+            if (fl == 0) {
+                // z = L^-1 grad (over grad), delta^2 = z^T z, the step L^-T z
+                double dd = 0.0;
+                for (int i = 0; i < p; ++i) {
+                    double z = grad[i];
+                    for (int c = 0; c < i; ++c) z = fma(-H[i * PH + c], grad[c], z);
+                    z *= sr[i];
+                    grad[i] = z;
+                    dd = fma(z, z, dd);
+                }
+                for (int i = p - 1; i >= 0; --i) {
+                    double x = grad[i];
+                    for (int c = i + 1; c < p; ++c) x = fma(-H[c * PH + i], del[c], x);
+                    del[i] = x * sr[i];
+                }
+                if (!isfinite(dd)) {
+                    fl = 2;
+                } else if (dd <= kLDelta2) {
+                    double* o = out + (int64_t)v * 6;
+                    o[2] = th[q] + del[q];
+                    o[3] = sr[q];   // sqrt([H^-1]_gg) = 1 / L_gg, g the last column
+                    err[v] = VPCA_GLM_OK;
+                    passes[v] = k;
+                    done = true;
+                } else if (k == kLMaxPass) {
+                    fl = 2;
+                } else {
+                    slp[w][0] = slp[w][1];
+                    sst[w][2] = 0;
+                    for (int c = 0; c < p; ++c) {
+                        thp[c] = th[c];
+                        th[c] += del[c];
+                    }
+                }
+            }
+            if (fl >= 2) {
+                err[v] = fl == 3 ? VPCA_GLM_VIF_INFINITE : VPCA_GLM_LOGISTIC_CONVERGE_FAIL;
+                passes[v] = k;
+                done = true;
+            }
+            if (done) sst[w][0] = -1;
+        }
+        __syncwarp();
+    }
+}
+
+// From what glm_logistic_kernel leaves in out[v * 6 ..] (OBS_CT, sum g, and for ERRCODE `.` BETA and SE): A1_FREQ, and
+// for ERRCODE `.` Z = BETA / SE and P = erfc(|Z| / sqrt(2)); NaN where undefined.  One thread per variant.
+__global__ void glm_logistic_finish_kernel(int nv, double* __restrict__ out, const int32_t* __restrict__ err) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= nv) return;
+    double* o = out + (int64_t)v * 6;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    const double obs = o[0];
+    o[1] = obs > 0.0 ? o[1] / (2.0 * obs) : nan;
+    if (err[v] != VPCA_GLM_OK) {
+        o[2] = o[3] = o[4] = o[5] = nan;
+        return;
+    }
+    const double z = o[2] / o[3];
+    o[4] = z;
+    o[5] = erfc(fabs(z) * 0.70710678118654752440);
+}
+
+template <int KMAX>
+cudaError_t launch_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
+                            const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, uint32_t lut,
+                            double* d_cnt, double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream) {
+    const unsigned cgrid = (unsigned)((nv + kCThreads / 32 - 1) / (kCThreads / 32));
+    glm_count_kernel<<<cgrid, kCThreads, 0, stream>>>(d_rows, stride, nv, n, d_mask, lut == kLutA2, d_cnt, 6);
+    glm_count_kernel<<<cgrid, kCThreads, 0, stream>>>(d_rows, stride, nv, n, d_case, lut == kLutA2, d_cnt + 3, 6);
+    const size_t smem = LogLayout<KMAX>::TOTAL * sizeof(double);
+    cudaError_t e = cudaFuncSetAttribute(glm_logistic_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    glm_logistic_kernel<KMAX><<<(unsigned)((nv + kLPerCta - 1) / kLPerCta), kLWarps * 32, smem, stream>>>(
+        d_rows, stride, nv, n, q, d_Qx, d_theta0, lut, d_cnt, d_out, d_err, d_passes);
+    glm_logistic_finish_kernel<<<(unsigned)((nv + 127) / 128), 128, 0, stream>>>(nv, d_out, d_err);
+    return cudaSuccess;
 }
 
 }  // namespace
@@ -442,6 +778,29 @@ cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int
         default: launch<32>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
     }
     return cudaGetLastError();
+}
+
+cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
+                         const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
+                         double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream) {
+    if (nv <= 0) return cudaSuccess;
+    const uint32_t lut = counted == 2 ? kLutA2 : kLutA1;
+    cudaError_t e;
+    switch (glm_kmax(q)) {
+#define VPCA_GLM_LOGISTIC(K)                                                                                              \
+    case K:                                                                                                               \
+        e = launch_logistic<K>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt, d_out, d_err,       \
+                               d_passes, stream);                                                                         \
+        break;
+        VPCA_GLM_LOGISTIC(2)
+        VPCA_GLM_LOGISTIC(4)
+        VPCA_GLM_LOGISTIC(8)
+        VPCA_GLM_LOGISTIC(16)
+        default: e = launch_logistic<32>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt, d_out,
+                                         d_err, d_passes, stream);
+#undef VPCA_GLM_LOGISTIC
+    }
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 }  // namespace vpca

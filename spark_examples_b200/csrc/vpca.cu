@@ -121,11 +121,13 @@ struct vpca_ctx {
     int grm_k = 0;          // 0: no GRM U
     // linear association tests (vpca_glm_*, glm.cu): Q, y~ and the mask of the last vpca_glm_begin (n rows of
     // glm_kmax(q) + 2 doubles), the regression mask as bits, Q^T y~, and one chunk of sums and outputs; rows are staged in
-    // d_grm_rows.  All grow-only.
+    // d_grm_rows.  All grow-only.  The logistic tests (vpca_glm_logistic_*) keep y in place of y~, the null fit in
+    // d_glm_z0, the cases as bits in d_glm_case, the counts in d_glm_sums and the passes in d_glm_passes.
     DeviceBuffer<double> d_glm_Qx, d_glm_z0, d_glm_sums, d_glm_out;
-    DeviceBuffer<uint8_t> d_glm_mask;
-    DeviceBuffer<int32_t> d_glm_err;
+    DeviceBuffer<uint8_t> d_glm_mask, d_glm_case;
+    DeviceBuffer<int32_t> d_glm_err, d_glm_passes;
     int glm_q = 0;          // 0: no GLM state
+    int glm_logistic = 0;   // the model of the GLM state: 0 linear (vpca_glm_begin), 1 logistic
     int glm_nreg = 0;       // regression samples
     double glm_yty = 0.0;   // y~^T y~
 
@@ -2525,41 +2527,42 @@ int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t
 // ---- linear association tests (glm.cu, DESIGN.md 15) ---------------------------------------------------------------------
 // vpca_glm_begin is host FP64 work and one upload; vpca_glm_linear_bed is driver-side and synchronous, its rows staged as
 // vpca_grm_loadings_bed stages them (grm_upload into d_grm_rows).
-int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used) {
-    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        ctx->glm_q = 0;   // a refused call leaves no GLM state
-    }
+namespace {
+// The checks and the regression samples both begins share; VPCA_OK or the refusal (the message names fn).
+int glm_samples(vpca_ctx* ctx, const char* fn, const double* pheno, const double* covar, int32_t n_covar,
+                std::vector<int>& idx) {
     if (pheno == nullptr || n_covar < 0 || (n_covar > 0 && covar == nullptr))
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: bad argument (pheno must be set, n_covar >= 0, covar set when "
-                    "n_covar > 0)");
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (pheno must be set, n_covar >= 0, covar set when "
+                    "n_covar > 0)", fn);
     const int q = n_covar + 1;
     if (q > VPCA_GLM_MAX_Q)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: %d covariates and the intercept exceed %d columns", n_covar,
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: %d covariates and the intercept exceed %d columns", fn, n_covar,
                     VPCA_GLM_MAX_Q);
     const int n = ctx->n;
-    std::vector<int> idx;   // the regression samples
     for (int s = 0; s < n; ++s) {
         bool ok = std::isfinite(pheno[s]);
-        if (std::isinf(pheno[s])) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: the phenotype of sample %d is infinite", s);
+        if (std::isinf(pheno[s])) return fail(ctx, VPCA_ERR_BAD_ARG, "%s: the phenotype of sample %d is infinite", fn, s);
         for (int j = 0; j < n_covar; ++j) {
             const double x = covar[(size_t)s * n_covar + j];
             if (std::isinf(x))
-                return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: covariate %d of sample %d is infinite", j + 1, s);
+                return fail(ctx, VPCA_ERR_BAD_ARG, "%s: covariate %d of sample %d is infinite", fn, j + 1, s);
             ok = ok && std::isfinite(x);
         }
         if (ok) idx.push_back(s);
     }
     const int R = (int)idx.size();
     if (R < q + 2)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: %d regression samples; %d covariates and the intercept need at "
-                    "least %d", R, n_covar, q + 2);
-    bool constant = true;
-    for (int i = 1; i < R && constant; ++i) constant = pheno[idx[i]] == pheno[idx[0]];
-    if (constant) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: the phenotype is constant over the regression samples");
-    // Q: the columns of C orthonormalised in order, modified Gram-Schmidt applied twice
-    std::vector<double> Q((size_t)q * R), y(R);
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: %d regression samples; %d covariates and the intercept need at "
+                    "least %d", fn, R, n_covar, q + 2);
+    return VPCA_OK;
+}
+
+// Q (q x R, column-major by covariate): the columns of C over the regression samples orthonormalised in order, modified
+// Gram-Schmidt applied twice; VPCA_OK or the refusal of a collinear covariate.
+int glm_basis(vpca_ctx* ctx, const char* fn, const double* covar, int32_t n_covar, const std::vector<int>& idx,
+              std::vector<double>& Q) {
+    const int q = n_covar + 1, R = (int)idx.size();
+    Q.assign((size_t)q * R, 0.0);
     for (int c = 0; c < q; ++c) {
         double* col = Q.data() + (size_t)c * R;
         for (int i = 0; i < R; ++i) col[i] = c == 0 ? 1.0 : covar[(size_t)idx[i] * n_covar + c - 1];
@@ -2575,11 +2578,146 @@ int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int3
         double nrm = 0.0;
         for (int i = 0; i < R; ++i) nrm += col[i] * col[i];
         if (!(nrm > 1e-18 * nrm0))
-            return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: covariate %d is collinear with the intercept and the "
-                        "covariates before it over the %d regression samples", c, R);
+            return fail(ctx, VPCA_ERR_BAD_ARG, "%s: covariate %d is collinear with the intercept and the "
+                        "covariates before it over the %d regression samples", fn, c, R);
         const double inv = 1.0 / std::sqrt(nrm);
         for (int i = 0; i < R; ++i) col[i] *= inv;
     }
+    return VPCA_OK;
+}
+
+// Uploads Qx (n rows [q_0 .. q_{q-1}, y, 0 .., mask], y[i] the value of regression sample idx[i]), the regression mask,
+// z0 (q doubles) and, when cases is set, the regression samples with y = 1 as bits.
+int glm_upload(vpca_ctx* ctx, int q, const std::vector<int>& idx, const std::vector<double>& Q, const std::vector<double>& y,
+               const std::vector<double>& z0, bool cases) {
+    const int n = ctx->n, R = (int)idx.size();
+    const int ld = glm_kmax(q) + 2;
+    std::vector<double> Qx((size_t)n * ld, 0.0);
+    std::vector<uint8_t> mask((n + 3) / 4, 0), cmask(cases ? (n + 3) / 4 : 0, 0);
+    for (int i = 0; i < R; ++i) {
+        double* xr = Qx.data() + (size_t)idx[i] * ld;
+        for (int c = 0; c < q; ++c) xr[c] = Q[(size_t)c * R + i];
+        xr[q] = y[i];
+        xr[ld - 1] = 1.0;
+        mask[idx[i] / 4] |= (uint8_t)(1u << (idx[i] % 4));
+        if (cases && y[i] != 0.0) cmask[idx[i] / 4] |= (uint8_t)(1u << (idx[i] % 4));
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    {
+        cudaError_t e = ctx->d_glm_Qx.ensure((int64_t)n * ld);
+        if (e == cudaSuccess) e = ctx->d_glm_mask.ensure((n + 3) / 4);
+        if (e == cudaSuccess && cases) e = ctx->d_glm_case.ensure((n + 3) / 4);
+        if (e == cudaSuccess) e = ctx->d_glm_z0.ensure(VPCA_GLM_MAX_Q);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_Qx.get(), Qx.data(), Qx.size() * sizeof(double), cudaMemcpyHostToDevice,
+                                 ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_mask.get(), mask.data(), mask.size(), cudaMemcpyHostToDevice, ctx->stream));
+    if (cases)
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_case.get(), cmask.data(), cmask.size(), cudaMemcpyHostToDevice,
+                                     ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_z0.get(), z0.data(), q * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->c_h2d += (int64_t)(Qx.size() * sizeof(double) + mask.size() + cmask.size() + q * sizeof(double));
+    return VPCA_OK;
+}
+
+// The logistic null fit: theta (q) maximising l over all R regression samples with Q alone, by the Newton passes of
+// glm_logistic_kernel (DESIGN.md 16) from theta = 0, in FP64 on the host.  Returns the passes, or 0 without convergence.
+int glm_null_fit(const std::vector<double>& Q, const std::vector<double>& y, int q, std::vector<double>& theta) {
+    const int R = (int)y.size();
+    std::vector<double> Qr((size_t)R * q);   // row-major copy: one sample's q values together
+    for (int c = 0; c < q; ++c)
+        for (int i = 0; i < R; ++i) Qr[(size_t)i * q + c] = Q[(size_t)c * R + i];
+    std::vector<double> th(q, 0.0), thp(q, 0.0), del(q, 0.0), H((size_t)q * q), gr(q), sr(q);
+    double lp = 0.0;
+    int halv = 0;
+    for (int k = 1; k <= 25; ++k) {
+        std::fill(H.begin(), H.end(), 0.0);
+        std::fill(gr.begin(), gr.end(), 0.0);
+        double l = 0.0;
+        for (int i = 0; i < R; ++i) {
+            const double* x = Qr.data() + (size_t)i * q;
+            double eta = 0.0;
+            for (int c = 0; c < q; ++c) eta += x[c] * th[c];
+            const double e = std::exp(-std::fabs(eta)), rd = 1.0 / (1.0 + e);
+            const double mu = eta >= 0.0 ? rd : e * rd, w = e * rd * rd, r = y[i] - mu;
+            const double m = y[i] != 0.0 ? -eta : eta;
+            l -= std::fmax(m, 0.0) + std::log1p(e);
+            for (int a = 0; a < q; ++a) {
+                gr[a] += r * x[a];
+                const double wa = w * x[a];
+                for (int b = 0; b <= a; ++b) H[(size_t)a * q + b] += wa * x[b];
+            }
+        }
+        if (!std::isfinite(l)) return 0;
+        if (k > 1 && l < lp - 1e-10 * std::fabs(lp)) {
+            if (halv == 8) return 0;
+            ++halv;
+            for (int c = 0; c < q; ++c) {
+                del[c] *= 0.5;
+                th[c] = thp[c] + del[c];
+            }
+            continue;
+        }
+        halv = 0;
+        for (int j = 0; j < q; ++j) {   // Cholesky, L below the diagonal of H, sr = 1 / L_jj
+            double d = H[(size_t)j * q + j];
+            for (int c = 0; c < j; ++c) d -= H[(size_t)j * q + c] * H[(size_t)j * q + c];
+            if (!(d > 0.0)) return 0;
+            sr[j] = 1.0 / std::sqrt(d);
+            for (int i = j + 1; i < q; ++i) {
+                double x = H[(size_t)i * q + j];
+                for (int c = 0; c < j; ++c) x -= H[(size_t)i * q + c] * H[(size_t)j * q + c];
+                H[(size_t)i * q + j] = x * sr[j];
+            }
+        }
+        double dd = 0.0;
+        for (int i = 0; i < q; ++i) {
+            double z = gr[i];
+            for (int c = 0; c < i; ++c) z -= H[(size_t)i * q + c] * gr[c];
+            gr[i] = z * sr[i];
+            dd += gr[i] * gr[i];
+        }
+        for (int i = q - 1; i >= 0; --i) {
+            double x = gr[i];
+            for (int c = i + 1; c < q; ++c) x -= H[(size_t)c * q + i] * del[c];
+            del[i] = x * sr[i];
+        }
+        if (!std::isfinite(dd)) return 0;
+        if (dd <= 1e-18) {
+            for (int c = 0; c < q; ++c) theta[c] = th[c] + del[c];
+            return k;
+        }
+        lp = l;
+        for (int c = 0; c < q; ++c) {
+            thp[c] = th[c];
+            th[c] += del[c];
+        }
+    }
+    return 0;
+}
+}  // namespace
+
+int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        ctx->glm_q = 0;   // a refused call leaves no GLM state
+    }
+    std::vector<int> idx;   // the regression samples
+    int rc = glm_samples(ctx, "vpca_glm_begin", pheno, covar, n_covar, idx);
+    if (rc != VPCA_OK) return rc;
+    const int q = n_covar + 1, R = (int)idx.size();
+    bool constant = true;
+    for (int i = 1; i < R && constant; ++i) constant = pheno[idx[i]] == pheno[idx[0]];
+    if (constant) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_begin: the phenotype is constant over the regression samples");
+    std::vector<double> Q, y(R);
+    rc = glm_basis(ctx, "vpca_glm_begin", covar, n_covar, idx, Q);
+    if (rc != VPCA_OK) return rc;
     for (int i = 0; i < R; ++i) y[i] = pheno[idx[i]];
     for (int pass = 0; pass < 2; ++pass)
         for (int k = 0; k < q; ++k) {
@@ -2593,36 +2731,56 @@ int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int3
     for (int i = 0; i < R; ++i) yty += y[i] * y[i];
     for (int k = 0; k < q; ++k)
         for (int i = 0; i < R; ++i) z0[k] += Q[(size_t)k * R + i] * y[i];
-    const int ld = glm_kmax(q) + 2;
-    std::vector<double> Qx((size_t)n * ld, 0.0);
-    std::vector<uint8_t> mask((n + 3) / 4, 0);
-    for (int i = 0; i < R; ++i) {
-        double* xr = Qx.data() + (size_t)idx[i] * ld;
-        for (int c = 0; c < q; ++c) xr[c] = Q[(size_t)c * R + i];
-        xr[q] = y[i];
-        xr[ld - 1] = 1.0;
-        mask[idx[i] / 4] |= (uint8_t)(1u << (idx[i] % 4));
-    }
-    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    {
-        cudaError_t e = ctx->d_glm_Qx.ensure((int64_t)n * ld);
-        if (e == cudaSuccess) e = ctx->d_glm_mask.ensure((n + 3) / 4);
-        if (e == cudaSuccess) e = ctx->d_glm_z0.ensure(VPCA_GLM_MAX_Q);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
-        }
-    }
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_Qx.get(), Qx.data(), Qx.size() * sizeof(double), cudaMemcpyHostToDevice,
-                                 ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_mask.get(), mask.data(), mask.size(), cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_glm_z0.get(), z0.data(), q * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->c_h2d += (int64_t)(Qx.size() * sizeof(double) + mask.size() + q * sizeof(double));
+    rc = glm_upload(ctx, q, idx, Q, y, z0, false);
+    if (rc != VPCA_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ctx->glm_q = q;
+    ctx->glm_logistic = 0;
     ctx->glm_nreg = R;
     ctx->glm_yty = yty;
+    if (n_used) *n_used = R;
+    return VPCA_OK;
+}
+
+int vpca_glm_logistic_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        ctx->glm_q = 0;   // a refused call leaves no GLM state
+    }
+    const char* fn = "vpca_glm_logistic_begin";
+    std::vector<int> idx;
+    int rc = glm_samples(ctx, fn, pheno, covar, n_covar, idx);
+    if (rc != VPCA_OK) return rc;
+    for (int s = 0; s < ctx->n; ++s)
+        if (std::isfinite(pheno[s]) && pheno[s] != 0.0 && pheno[s] != 1.0)
+            return fail(ctx, VPCA_ERR_BAD_ARG, "%s: the phenotype of sample %d is %.17g, not 0 (control), 1 (case) or "
+                        "NaN (missing)", fn, s, pheno[s]);
+    const int q = n_covar + 1, R = (int)idx.size();
+    std::vector<double> y(R);
+    int cases = 0;
+    for (int i = 0; i < R; ++i) {
+        y[i] = pheno[idx[i]];
+        cases += y[i] != 0.0;
+    }
+    if (cases == 0 || cases == R)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: %d cases and %d controls among the %d regression samples; a logistic test "
+                    "needs both", fn, cases, R - cases, R);
+    std::vector<double> Q;
+    rc = glm_basis(ctx, fn, covar, n_covar, idx, Q);
+    if (rc != VPCA_OK) return rc;
+    std::vector<double> theta(q, 0.0);
+    if (glm_null_fit(Q, y, q, theta) == 0)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: the null model (the intercept and the %d covariates, without a variant) "
+                    "does not converge in 25 Newton passes: a covariate separates the cases from the controls", fn,
+                    n_covar);
+    rc = glm_upload(ctx, q, idx, Q, y, theta, true);
+    if (rc != VPCA_OK) return rc;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    ctx->glm_q = q;
+    ctx->glm_logistic = 1;
+    ctx->glm_nreg = R;
+    ctx->glm_yty = 0.0;
     if (n_used) *n_used = R;
     return VPCA_OK;
 }
@@ -2640,6 +2798,9 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         if (ctx->glm_q == 0) return fail(ctx, VPCA_ERR_STATE, "vpca_glm_linear_bed needs a vpca_glm_begin since the last reset");
+        if (ctx->glm_logistic)
+            return fail(ctx, VPCA_ERR_STATE, "vpca_glm_linear_bed: the GLM state is logistic (vpca_glm_logistic_begin); "
+                        "a linear test needs vpca_glm_begin");
         q = ctx->glm_q;
         n_reg = ctx->glm_nreg;
         yty = ctx->glm_yty;
@@ -2680,6 +2841,70 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
                                      cudaMemcpyDeviceToHost, L.stream));
         ctx->c_launches += 3;
         ctx->c_d2h += (int64_t)nvc * (6 * (int64_t)sizeof(double) + (int64_t)sizeof(int32_t));
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                          double* out, int32_t* out_err, int32_t* out_passes) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    int rc = grm_rows_args(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, out != nullptr && out_err != nullptr);
+    if (rc != VPCA_OK) return rc;
+    if (counted_allele != 1 && counted_allele != 2)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_logistic_bed: counted_allele must be 1 (A1) or 2 (A2), not %d",
+                    counted_allele);
+    int q = 0;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (ctx->glm_q == 0)
+            return fail(ctx, VPCA_ERR_STATE, "vpca_glm_logistic_bed needs a vpca_glm_logistic_begin since the last reset");
+        if (!ctx->glm_logistic)
+            return fail(ctx, VPCA_ERR_STATE, "vpca_glm_logistic_bed: the GLM state is linear (vpca_glm_begin); a "
+                        "logistic test needs vpca_glm_logistic_begin");
+        q = ctx->glm_q;
+    }
+    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
+    if (nv == 0) return VPCA_OK;
+    const int n = ctx->n;
+    const int64_t step = grm_step(nv, stride_bytes);
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = cudaSuccess;
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * 6);
+        if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
+        if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
+        if (e == cudaSuccess) e = ctx->d_glm_passes.ensure(step);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
+        }
+    }
+    const int64_t nchunks = (nv + step - 1) / step;
+    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
+    for (int64_t c = 0; c < nchunks; ++c) {
+        const int b = (int)(c & 1);
+        const int64_t v = c * step;
+        const int nvc = (int)std::min(step, nv - v);
+        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        CUDA_OK(ctx, glm_logistic(ctx->d_grm_rows[b].get(), stride_bytes, nvc, n, q, ctx->d_glm_Qx.get(),
+                                  ctx->d_glm_mask.get(), ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele,
+                                  ctx->d_glm_sums.get(), ctx->d_glm_out.get(), ctx->d_glm_err.get(),
+                                  ctx->d_glm_passes.get(), L.stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        if (out_passes)
+            CUDA_OK(ctx, cudaMemcpyAsync(out_passes + v, ctx->d_glm_passes.get(), (size_t)nvc * sizeof(int32_t),
+                                         cudaMemcpyDeviceToHost, L.stream));
+        ctx->c_launches += 5;
+        ctx->c_d2h += (int64_t)nvc * (6 * (int64_t)sizeof(double) + (out_passes ? 2 : 1) * (int64_t)sizeof(int32_t));
     }
     CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
     return VPCA_OK;

@@ -263,6 +263,13 @@ int glm_kmax(int q);
 cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, int n_reg, const double* d_Qx,
                        const uint8_t* d_mask, const double* d_z0, double yty, int counted, double* d_sums, double* d_out,
                        int32_t* d_err, cudaStream_t stream);
+// Logistic tests (DESIGN.md 16) of nv .bed rows: the counts into d_cnt (nv x 6: OBS_CT, sum g, sum g^2 under d_mask, then
+// under d_case), then d_out[v * 6 ..] = OBS_CT, A1_FREQ, BETA, SE, Z, P, d_err[v] (VPCA_GLM_*) and d_passes[v] (Newton
+// passes, 0 for a variant flagged before any).  d_Qx: n rows [q_0 .. q_{q-1}, y, 0 .., mask] with y in {0, 1}; d_case:
+// the regression samples with y = 1 as bits; d_theta0: the null fit in the basis Q (q).  Never synchronises.
+cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
+                         const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
+                         double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream);
 
 // ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
 // Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to

@@ -56,13 +56,15 @@ EXPORTED_SYMBOLS = (
     "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact", "vpca_sample_missing_bed",
     "vpca_subset_bed_samples", "vpca_debug_device_bytes", "vpca_grm_bed", "vpca_grm_finalize", "vpca_get_grm",
     "vpca_compute_pca_grm", "vpca_grm_loadings_bed", "vpca_grm_project_bed", "vpca_glm_begin", "vpca_glm_linear_bed",
+    "vpca_glm_logistic_begin", "vpca_glm_logistic_bed",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
 LD_MAX_WINDOW = 4096          # vpca_ld_prune_bed: variants a window may reach back (VPCA_LD_MAX_WINDOW)
 GRM_MAX_SAMPLES = 65535       # vpca_grm_* / vpca_compute_pca_grm: the sample limit of vpca_compute_pca
 GLM_MAX_Q = 32                # vpca_glm_begin: covariate columns, the intercept included
-GLM_ERRCODES = (".", "TOO_FEW_OBS", "CONST_ALLELE", "VIF_INFINITE", "NO_RESIDUAL")   # by VPCA_GLM_* value
+GLM_ERRCODES = (".", "TOO_FEW_OBS", "CONST_ALLELE", "VIF_INFINITE", "NO_RESIDUAL",
+                "LOGISTIC_CONVERGE_FAIL")   # by VPCA_GLM_* value
 
 
 class VpcaError(RuntimeError):
@@ -316,6 +318,10 @@ def load_library() -> ctypes.CDLL:
     L.vpca_glm_begin.argtypes = [vp, vp, vp, i32, ctypes.POINTER(i64)]
     L.vpca_glm_linear_bed.restype = ctypes.c_int
     L.vpca_glm_linear_bed.argtypes = [vp, vp, i64, i64, i32, vp, vp]
+    L.vpca_glm_logistic_begin.restype = ctypes.c_int
+    L.vpca_glm_logistic_begin.argtypes = [vp, vp, vp, i32, ctypes.POINTER(i64)]
+    L.vpca_glm_logistic_bed.restype = ctypes.c_int
+    L.vpca_glm_logistic_bed.argtypes = [vp, vp, i64, i64, i32, vp, vp, vp]
     _lib = L
     return L
 
@@ -888,6 +894,37 @@ class NativePca:
         self._check(self._lib.vpca_glm_linear_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv, b.shape[1],
                                                   int(counted), _host_ptr(out), _host_ptr(err)))
         return out[:nv], err[:nv]
+
+    # -- logistic association tests (vpca.h, DESIGN.md 16) ---------------------------------------------------------------
+    def glmLogisticBegin(self, pheno, covar=None) -> int:
+        """Set the case/control phenotype ((n,) float64: 1 case, 0 control, NaN missing) and the covariates ((n, c)
+        float64, NaN = missing; None for none) of the logistic tests; the intercept is added.  Returns the regression
+        samples.  VPCA_ERR_BAD_ARG for what glmBegin refuses, a value outside {0, 1, NaN}, no case or no control, or a
+        null model that does not converge."""
+        y = np.ascontiguousarray(pheno, dtype=np.float64).reshape(-1)
+        if y.shape[0] != self.n:
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"pheno must have {self.n} entries")
+        c = np.zeros((self.n, 0)) if covar is None else np.ascontiguousarray(covar, dtype=np.float64).reshape(self.n, -1)
+        m = ctypes.c_int64(0)
+        self._check(self._lib.vpca_glm_logistic_begin(self._h, _host_ptr(y), _host_ptr(c) if c.shape[1] else None,
+                                                      c.shape[1], ctypes.byref(m)))
+        return int(m.value)
+
+    def glmLogisticBed(self, rows: np.ndarray, counted: int = 1):
+        """Logistic tests of PLINK .bed rows ((V, stride) uint8 of this context's samples; a .bed memmap is read in
+        place) against the phenotype of glmLogisticBegin -> (stats (V, 6) float64: OBS_CT, A1_FREQ, BETA, SE, Z, P, NaN
+        where undefined; err (V,) int32: index into GLM_ERRCODES; passes (V,) int32: Newton passes).  counted: 1 counts
+        A1, 2 counts A2.  Synchronises."""
+        b = self._bed_rows(rows)
+        nv = b.shape[0]
+        out = np.zeros((max(nv, 1), 6), np.float64)
+        err = np.zeros(max(nv, 1), np.int32)
+        passes = np.zeros(max(nv, 1), np.int32)
+        empty = np.zeros(1, np.uint8)
+        self._check(self._lib.vpca_glm_logistic_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv,
+                                                    b.shape[1], int(counted), _host_ptr(out), _host_ptr(err),
+                                                    _host_ptr(passes)))
+        return out[:nv], err[:nv], passes[:nv]
 
     def hweExact(self, counts) -> np.ndarray:
         """Exact HWE p-values of (V, 4) int32 counts (HOM_A1, HET, HOM_A2, MISSING; MISSING ignored) -> (V,) float64."""

@@ -689,7 +689,14 @@ class VariantsPcaDriver:
         if int(reg.sum()) < glm.q + 2:
             raise ValueError(f"--glm: {int(reg.sum())} of {n} samples have a phenotype and every covariate; {glm.q} "
                              f"covariates (the intercept included) need at least {glm.q + 2}")
-        check_glm_quantitative(glm.y[reg], glm.name)
+        if glm.logistic:
+            cases = int(np.count_nonzero(glm.y[reg] == 1.0))
+            if cases == 0 or cases == int(reg.sum()):
+                raise ValueError(f"--glm-logistic: phenotype {glm.name} has {cases} cases and {int(reg.sum()) - cases} "
+                                 f"controls among the {int(reg.sum())} samples with a phenotype and every covariate; a "
+                                 "logistic test needs both")
+        else:
+            check_glm_quantitative(glm.y[reg], glm.name)
 
     def glmLinear(self, callsets: CallsRdd, glm: "GlmInput", qc_keep: Optional[np.ndarray] = None):
         """After the PCs (or the projection): the linear test of every variant that passes variant QC, in file order, on
@@ -721,6 +728,41 @@ class VariantsPcaDriver:
               f"{1 + k + c} covariates ({covs}); {len(errs)} variants tested, {int(np.count_nonzero(errs))} with an "
               f"ERRCODE; lambda_GC = {lambda_gc(stats, errs)!r}.")
         return stats, errs
+
+    def glmLogistic(self, callsets: CallsRdd, glm: "GlmInput", qc_keep: Optional[np.ndarray] = None):
+        """glmLinear's logistic counterpart (DESIGN.md 16) for a case/control phenotype: writes P.<PHENO>.glm.logistic
+        and prints the `GLM logistic:` line.  Returns (stats (V, 6), err (V,), passes (V,))."""
+        from . import plink
+        pcs = np.asarray(self.components, np.float64)
+        k = pcs.shape[1]
+        nat = self._native(callsets.n_samples)
+        used = nat.glmLogisticBegin(glm.y, np.concatenate([pcs, glm.c], axis=1))
+        stats, errs, passes, tested = [], [], [], []
+        counted = plink.COUNT_A1
+        for part in callsets.partitions:
+            sel = np.ones(part.nv, bool) if qc_keep is None else np.asarray(qc_keep[part.v0:part.v0 + part.nv], bool)
+            rows = part.bed._map[part.v0:part.v0 + part.nv]        # read in place when every variant is tested
+            st, er, ps = nat.glmLogisticBed(rows if sel.all() else rows[sel], part.counted)
+            stats.append(np.asarray(st, np.float64).reshape(-1, 6))
+            errs.append(np.asarray(er, np.int32).reshape(-1))
+            passes.append(np.asarray(ps, np.int32).reshape(-1))
+            tested.extend((part.v0 + np.flatnonzero(sel)).tolist())
+            counted = part.counted
+        stats = np.concatenate(stats) if stats else np.zeros((0, 6))
+        errs = np.concatenate(errs) if errs else np.zeros(0, np.int32)
+        passes = np.concatenate(passes) if passes else np.zeros(0, np.int32)
+        bim = plink.read_bim(self.conf.bedPath())
+        write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.glm.logistic", [bim[j] for j in tested], counted, stats,
+                           errs)
+        n = callsets.n_samples
+        c = glm.c.shape[1]
+        reg = np.isfinite(glm.y) & np.isfinite(glm.c).all(axis=1)
+        cases = int(np.count_nonzero(glm.y[reg] == 1.0))
+        covs = f"intercept, {k} PCs" + (f", {c} from {glm.covar_path}" if glm.covar_path else "")
+        print(f"GLM logistic: {glm.name} on {used} of {n} samples ({cases} cases, {used - cases} controls, {n - used} "
+              f"without a phenotype or covariate), {1 + k + c} covariates ({covs}); {len(errs)} variants tested, "
+              f"{int(np.count_nonzero(errs))} with an ERRCODE; lambda_GC = {lambda_gc(stats, errs)!r}.")
+        return stats, errs, passes
 
     # -- LD pruning of the variants (beyond the reference; DESIGN.md 9) -------------------------------------------------
     def ldPrune(self, callsets: CallsRdd, window_lo: np.ndarray, eligible: Optional[np.ndarray] = None) -> np.ndarray:
@@ -1054,6 +1096,7 @@ class GlmInput:
     covar_ids: list
     covar_values: np.ndarray
     q: int
+    logistic: bool = False   # --glm-logistic: pheno_values hold 1 (case), 0 (control) and NaN (missing)
     y: Optional[np.ndarray] = None
     c: Optional[np.ndarray] = None
 
@@ -1062,7 +1105,8 @@ LAMBDA_GC_DENOM = 0.45493642311957283   # the median of chi-square with 1 degree
 
 
 def lambda_gc(stats: np.ndarray, errs: np.ndarray) -> float:
-    """The genomic inflation factor: the median T_STAT^2 over the variants without an ERRCODE / LAMBDA_GC_DENOM."""
+    """The genomic inflation factor: the median T_STAT^2 (Z_STAT^2 of a logistic test) over the variants without an
+    ERRCODE / LAMBDA_GC_DENOM."""
     t = np.asarray(stats, np.float64)[np.asarray(errs) == 0, 4]
     return float(np.median(t * t) / LAMBDA_GC_DENOM) if len(t) else float("nan")
 
@@ -1072,7 +1116,23 @@ def check_glm_quantitative(values: np.ndarray, name: str) -> None:
     distinct = np.unique(values[np.isfinite(values)])
     if len(distinct) <= 2:
         raise ValueError(f"--glm: phenotype {name} has {len(distinct)} distinct value(s); case/control traits need "
-                         "logistic regression, which is not implemented")
+                         "logistic regression: add --glm-logistic")
+
+
+def case_control_coding(values: np.ndarray, ids, name: str) -> np.ndarray:
+    """PLINK's case/control coding -> 1 (case), 0 (control), NaN (missing): 2 is a case, 1 a control, and 0, -9, NA
+    and nan are missing.  Any other value is refused with the sample's ID."""
+    values = np.asarray(values, np.float64)
+    out = np.full(len(values), np.nan)
+    out[values == 2.0] = 1.0
+    out[values == 1.0] = 0.0
+    bad = np.flatnonzero(np.isfinite(values) & ~np.isin(values, (0.0, 1.0, 2.0, -9.0)))
+    if len(bad):
+        fid, iid = ids[bad[0]]
+        who = iid if fid is None else f"{fid} {iid}"
+        raise ValueError(f"--glm-logistic: phenotype {name} of sample {who} is {float(values[bad[0]])!r}; case/control "
+                         "phenotypes are 1 (control), 2 (case), or 0, -9, NA or nan (missing)")
+    return out
 
 
 def check_glm_flags(conf: PcaConf) -> Optional[GlmInput]:
@@ -1081,6 +1141,8 @@ def check_glm_flags(conf: PcaConf) -> Optional[GlmInput]:
     for flag, opt in (("--pheno", conf.pheno), ("--pheno-name", conf.phenoName), ("--covar", conf.covar)):
         if opt.isDefined and not conf.glm():
             raise ValueError(f"{flag} is read by --glm: give --glm")
+    if conf.glmLogistic() and not conf.glm():
+        raise ValueError("--glm-logistic is a mode of --glm: give --glm")
     if not conf.glm():
         return None
     if not conf.pheno.isDefined:
@@ -1113,6 +1175,9 @@ def check_glm_flags(conf: PcaConf) -> Optional[GlmInput]:
     if q > native.GLM_MAX_Q:
         raise ValueError(f"--glm fits at most {native.GLM_MAX_Q} covariates, the intercept included; the intercept, {what} "
                          f"and {covar_values.shape[1]} --covar columns make {q}")
+    if conf.glmLogistic():
+        return GlmInput(name, conf.pheno(), ids, case_control_coding(y, ids, name), conf.covar.get, covar_ids,
+                        covar_values, q, logistic=True)
     check_glm_quantitative(y, name)
     return GlmInput(name, conf.pheno(), ids, y, conf.covar.get, covar_ids, covar_values, q)
 
@@ -1130,6 +1195,18 @@ def write_glm_linear(path: str, bim, counted: int, stats: np.ndarray, errs: np.n
         fh.write("".join(
             f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
             f"ADD\t{int(st[0])}\t{_glm_number(st[2])}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
+            f"{_glm_number(st[5])}\t{native.GLM_ERRCODES[int(e)]}\n"
+            for b, st, e in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist())))
+
+
+def write_glm_logistic(path: str, bim, counted: int, stats: np.ndarray, errs: np.ndarray) -> None:
+    """P.<PHENO>.glm.logistic, as write_glm_linear with PLINK 2's logistic columns: OR = exp(BETA), LOG(OR)_SE = SE and
+    Z_STAT in place of BETA, SE and T_STAT."""
+    with open(path, "w", encoding="utf-8") as fh:
+        fh.write("#CHROM\tPOS\tID\tREF\tALT\tA1\tA1_FREQ\tTEST\tOBS_CT\tOR\tLOG(OR)_SE\tZ_STAT\tP\tERRCODE\n")
+        fh.write("".join(
+            f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
+            f"ADD\t{int(st[0])}\t{_glm_number(np.exp(st[2]))}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
             f"{_glm_number(st[5])}\t{native.GLM_ERRCODES[int(e)]}\n"
             for b, st, e in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist())))
 
@@ -1526,7 +1603,10 @@ def main(args: Optional[Sequence[str]] = None):
             driver.saveGrmLoadings(callsRdd)
     driver.emitResult(result)
     if glm is not None:
-        driver.glmLinear(callsRdd, glm, qc_keep)       # every QC-passing variant; the pruned set fed the PCs only
+        if glm.logistic:
+            driver.glmLogistic(callsRdd, glm, qc_keep)
+        else:
+            driver.glmLinear(callsRdd, glm, qc_keep)   # every QC-passing variant; the pruned set fed the PCs only
     if conf.makeKingTable.isDefined:
         driver.writeKingTable()
     driver.reportIoStats()

@@ -412,8 +412,9 @@ int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int
  *   bits of the last byte are ignored); out_counts[4v ..] = HOM_A1, HET, HOM_A2, MISSING (exact, whatever the split of
  *   the rows into calls); out_hwe_p (may be NULL) = the p-value of each row.
  * vpca_hwe_exact: the same p-values from host counts in the layout above (MISSING ignored), for any n.
- * Driver-side and synchronous.  Rows are staged in chunks of at most 64 MB and tested in batches of about 2^18 rows (at
- * least one chunk), so device memory does not grow with nv: the chunk and 24 bytes per batch row are allocated on the
+ * Driver-side and synchronous.  Rows are staged in chunks of at most 64 MB, the upload of chunk i + 1 overlapping the
+ * count of chunk i, and tested in batches of about 2^18 rows (at least one chunk), so device memory does not grow with
+ * nv: two chunk buffers (shared with the other driver-side .bed calls) and 24 bytes per batch row are allocated on the
  * first call and freed by vpca_destroy.  The PCA Gram, U, the kinship counts, the subset state and the LD state are left
  * alone.
  * VPCA_ERR_BAD_ARG, before any row is staged: rows / out_counts / counts / out_p NULL (nv > 0), nv < 0,
@@ -436,7 +437,7 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
  * split into calls, on stride_bytes or on skipped variants anywhere.
  * The sum accumulates in the eigensolver's FP64 N x N matrix (the one vpca_get_centered returns; 34 GB at 65 535
  * samples), allocated on the first call if no solve has allocated it.  The GRM calls leave the PCA Gram, U, the kinship
- * counts, the LD state, the QC buffers and the subset state alone.  vpca_compute_pca and vpca_get_centered overwrite
+ * counts, the LD state, the QC counts and the subset state alone.  vpca_compute_pca and vpca_get_centered overwrite
  * the matrix, and so does a GRM solve by the direct reduction: afterwards vpca_get_grm, vpca_compute_pca_grm and
  * vpca_grm_bed return VPCA_ERR_STATE until vpca_reset.  Driver-side and synchronous.
  * vpca_grm_bed: adds the rows; successive calls add up.  Rows are staged in chunks of at most 64 MB on a lane (H2D of
@@ -571,10 +572,11 @@ int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_
  * vpca_subset_bed_samples: out row v (at out_rows + v * out_stride) = the codes of samples keep_idx[0 .. m) of row v, in
  *   that order, packed as a .bed row of m samples: the padding bits of its last byte are 0, as PLINK writes them, so the
  *   bytes equal those of a fileset of the kept samples.  Bytes of an out row past ceil(m / 4) are not written.
- * Driver-side and synchronous.  Rows are staged in chunks of at most 64 MB, so device memory does not grow with nv or
- *   n_samples; the subset pass double-buffers its chunks and overlaps the upload of chunk i + 1 with the download of
- *   chunk i.  The buffers are allocated on the first call and freed by vpca_destroy.  The PCA Gram, U, the kinship counts,
- *   the subset state, the LD state and the variant QC buffers are left alone.
+ * Driver-side and synchronous.  Rows are staged in chunks of at most 64 MB in two buffers (shared with the other
+ *   driver-side .bed calls), so device memory does not grow with nv or n_samples; the upload of chunk i + 1 overlaps the
+ *   work on chunk i, and the subset pass also overlaps it with the download of chunk i.  The buffers are allocated on the
+ *   first call and freed by vpca_destroy.  The PCA Gram, U, the kinship counts, the subset state, the LD state and the
+ *   variant QC counts are left alone.
  * VPCA_ERR_BAD_ARG, before any row is staged and with the outputs untouched: a NULL rows / out_missing / keep_idx /
  *   out_rows when nv > 0, nv < 0, n_samples < 1, stride_bytes < ceil(n_samples / 4), m < 1, keep_idx not strictly
  *   increasing or outside [0, n_samples), out_stride < ceil(m / 4).  VPCA_ERR_OVERFLOW: nv > 2^31 - 1 for the counts. */

@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <cmath>
 #include <condition_variable>
@@ -90,13 +91,14 @@ struct vpca_ctx {
     DeviceBuffer<int64_t> d_ld_wlo;
     DeviceBuffer<uint8_t> d_ld_keep;
     DeviceBuffer<uint8_t> d_ld_elig;    // vpca_ld_prune_bed_masked: the eligible bytes of the call
-    // variant QC (vpca_variant_qc_bed / vpca_hwe_exact): the raw rows, counts and p-values of one chunk; grow-only
-    DeviceBuffer<uint8_t> d_qc_rows;
+    // .bed rows of the driver-side calls (GRM, its loadings and projection, GLM, variant and sample QC), double-buffered:
+    // those calls never run at the same time, so they share this pair (stage_rows); grow-only
+    DeviceBuffer<uint8_t> d_bed_rows[2];
+    // variant QC (vpca_variant_qc_bed / vpca_hwe_exact): the counts and p-values of one batch; grow-only
     DeviceBuffer<int32_t> d_qc_counts;
     DeviceBuffer<double> d_qc_p;
-    // sample QC (vpca_sample_missing_bed / vpca_subset_bed_samples): double-buffered raw and repacked rows of one chunk, the
+    // sample QC (vpca_sample_missing_bed / vpca_subset_bed_samples): double-buffered repacked rows of one chunk, the
     // per-sample counts, the kept indices, and a stream and events of their own for the D2H copies; grow-only
-    DeviceBuffer<uint8_t> d_sm_rows[2];
     DeviceBuffer<uint8_t> d_sm_out[2];
     DeviceBuffer<int32_t> d_sm_miss;
     DeviceBuffer<int32_t> d_sm_idx;
@@ -104,9 +106,8 @@ struct vpca_ctx {
     cudaEvent_t sm_ev_copy[2] = {nullptr, nullptr}, sm_ev_kern[2] = {nullptr, nullptr};
     GramPlan ld_plan;
     LdWork ld;
-    // GRM (vpca_grm_bed / _finalize, grm.cu): double-buffered raw rows, the chunk's counts, z tables, used flags and used
-    // list, and one FP64 panel; the sum itself accumulates in eig.d_C.  All grow-only.
-    DeviceBuffer<uint8_t> d_grm_rows[2];
+    // GRM (vpca_grm_bed / _finalize, grm.cu): the chunk's counts, z tables, used flags and used list, and one FP64 panel;
+    // the sum itself accumulates in eig.d_C.  All grow-only.
     DeviceBuffer<int32_t> d_grm_counts, d_grm_used, d_grm_inv;
     DeviceBuffer<double> d_grm_tab, d_grm_Z;
     DeviceBuffer<int> d_grm_total;
@@ -120,9 +121,9 @@ struct vpca_ctx {
     DeviceBuffer<double> d_grm_U, d_grm_w, d_grm_ptab;
     int grm_k = 0;          // 0: no GRM U
     // linear association tests (vpca_glm_*, glm.cu): Q, y~ and the mask of the last vpca_glm_begin (n rows of
-    // glm_kmax(q) + 2 doubles), the regression mask as bits, Q^T y~, and one chunk of sums and outputs; rows are staged in
-    // d_grm_rows.  All grow-only.  The logistic tests (vpca_glm_logistic_*) keep y in place of y~, the null fit in
-    // d_glm_z0, the cases as bits in d_glm_case, the counts in d_glm_sums and the passes in d_glm_passes.
+    // glm_kmax(q) + 2 doubles), the regression mask as bits, Q^T y~, and one chunk of sums and outputs.  All grow-only.
+    // The logistic tests (vpca_glm_logistic_*) keep y in place of y~, the null fit in d_glm_z0, the cases as bits in
+    // d_glm_case, the counts in d_glm_sums and the passes in d_glm_passes.
     DeviceBuffer<double> d_glm_Qx, d_glm_z0, d_glm_sums, d_glm_out;
     DeviceBuffer<uint8_t> d_glm_mask, d_glm_case;
     DeviceBuffer<int32_t> d_glm_err, d_glm_passes;
@@ -536,6 +537,52 @@ int process_calls(vpca_ctx* ctx, vpca_ctx::Lane& L, const int64_t* offsets, cons
 }
 
 
+// What the row stager does with one staged chunk: rows [v, v + nvc) of the call sit in d_rows, which is dst[b]; work is
+// enqueued on L.stream.
+using RowsFn = std::function<int(int b, const uint8_t* d_rows, int64_t v, int64_t nvc)>;
+
+// Rows [0, nv) of `rows` (host, `stride` bytes apart) go to the device `step` rows at a time, chunk c into dst[c & 1] on
+// L.copy_stream once the work that last read that buffer (chunk c - 2, L.ev_done) is done; work(b, d_rows, v, nvc)
+// enqueues chunk c's kernels on L.stream and may synchronise it.  The copy of chunk c is enqueued after work(c - 1), not
+// before: from pageable memory cudaMemcpyAsync blocks the host until its stream reaches the copy, so this order is the
+// one that keeps chunk c - 1's kernels running while chunk c is copied.  Counts c_h2d; returns work's first error, else
+// after L.stream has drained (the caller's rows are free on return).
+int stage_rows(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* rows, int64_t nv, int64_t stride, int64_t step,
+               const std::array<uint8_t*, 2>& dst, const RowsFn& work) {
+    for (int64_t v = 0, c = 0; v < nv; v += step, ++c) {
+        const int b = (int)(c & 1);
+        const int64_t nvc = std::min(step, nv - v);
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
+        CUDA_OK(ctx, cudaMemcpyAsync(dst[b], rows + (size_t)v * stride, (size_t)(nvc * stride), cudaMemcpyHostToDevice,
+                                     L.copy_stream));
+        CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
+        ctx->c_h2d += nvc * stride;
+        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
+        if (int rc = work(b, dst[b], v, nvc)) return rc;
+        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
+    return VPCA_OK;
+}
+
+// The argument checks of every packed-row call: nv >= 0, the rows and the outputs (outs_set) given when nv > 0, and rows
+// at least min_stride bytes apart.  The message names fn.
+int rows_args(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int64_t min_stride,
+              bool outs_set = true) {
+    if (nv < 0 || (nv > 0 && (rows == nullptr || !outs_set)) || stride_bytes < min_stride)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (nv = %lld must be >= 0, rows and outputs set when nv > 0, "
+                    "stride_bytes = %lld >= %lld)", fn, (long long)nv, (long long)stride_bytes, (long long)min_stride);
+    return VPCA_OK;
+}
+
+// The context's staging pair for driver-side calls (d_bed_rows); calls on task threads use their lane's L.d_idx instead.
+std::array<uint8_t*, 2> bed_rows(vpca_ctx* ctx) { return {ctx->d_bed_rows[0].get(), ctx->d_bed_rows[1].get()}; }
+
+// Raw rows in the lane's index buffers (the packed accumulate, loadings and projection calls, and kinship).
+std::array<uint8_t*, 2> lane_rows(vpca_ctx::Lane& L) {
+    return {reinterpret_cast<uint8_t*>(L.d_idx[0].get()), reinterpret_cast<uint8_t*>(L.d_idx[1].get())};
+}
+
 // Packed rows (code 0: bitmaps; 1 / 2: PLINK .bed rows counting A1 / A2, see encode.cu) -> encode -> consume(chunk), on
 // lane L; returns after the lane's stream has drained (the caller's buffer is free to reuse).
 int process_packed(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* bits, int64_t nv, int64_t stride_bytes, int code,
@@ -547,25 +594,11 @@ int process_packed(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* bits, int64_
     if (cap_rows < 32) return fail(ctx, VPCA_ERR_BAD_ARG, "stride_bytes too large for the staging buffer");
     const int64_t whole = std::max<int64_t>(P, (cap_rows / P) * P);
     const int64_t step = whole <= cap_rows ? whole : (cap_rows / 32) * 32;
-    int chunk = 0;
-    for (int64_t v = 0; v < nv; v += step, ++chunk) {
-        const int64_t nvc = std::min(step, nv - v);
-        const int b = chunk & 1;
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b].get(), bits + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
-                                     cudaMemcpyHostToDevice, L.copy_stream));
-        CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
-        ctx->c_h2d += nvc * stride_bytes;
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, encode_bits(reinterpret_cast<const uint8_t*>(L.d_idx[b].get()), stride_bytes, nvc, ctx->n, ctx->elem_bits,
-                                 L.d_x[b].get(), P, P, code, L.stream));
+    return stage_rows(ctx, L, bits, nv, stride_bytes, step, lane_rows(L), [&](int b, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
+        CUDA_OK(ctx, encode_bits(d_rows, stride_bytes, nvc, ctx->n, ctx->elem_bits, L.d_x[b].get(), P, P, code, L.stream));
         ctx->c_launches += 1;
-        int r = consume(L, b, v, nvc);
-        if (r != VPCA_OK) return r;
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
-    return VPCA_OK;
+        return consume(L, b, v, nvc);
+    });
 }
 
 }  // namespace
@@ -800,9 +833,9 @@ int vpca_accumulate_calls_u16(vpca_ctx* ctx, int64_t partition_id, const int64_t
 static int accumulate_packed(vpca_ctx* ctx, int64_t partition_id, const uint8_t* bits, int64_t nv, int64_t stride_bytes,
                              int code) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    const int64_t min_stride = code == 0 ? (ctx->n + 7) / 8 : (ctx->n + 3) / 4;
-    if (nv < 0 || (nv > 0 && bits == nullptr) || stride_bytes < min_stride)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "packed rows: stride_bytes must be >= ceil(n_samples / %d)", code == 0 ? 8 : 4);
+    if (int rc = rows_args(ctx, code == 0 ? "vpca_accumulate_bits" : "vpca_accumulate_bed", bits, nv, stride_bytes,
+                           code == 0 ? (ctx->n + 7) / 8 : (ctx->n + 3) / 4))
+        return rc;
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) {
         std::lock_guard<std::mutex> lk(ctx->mu);
@@ -1617,8 +1650,9 @@ int vpca_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv,
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     if (counted_allele != 1 && counted_allele != 2)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: counted_allele must be 1 (A1) or 2 (A2)");
-    if (nv < 0 || (nv > 0 && (rows == nullptr || out_w == nullptr || out_count == nullptr)) || stride_bytes < (ctx->n + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_loadings_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    if (int rc = rows_args(ctx, "vpca_loadings_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4,
+                           out_w != nullptr && out_count != nullptr))
+        return rc;
     const double* U = nullptr;
     const uint8_t* keep = nullptr;
     {
@@ -1698,8 +1732,8 @@ int vpca_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t str
     }
     if (counted_allele != 1 && counted_allele != 2)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_bed: counted_allele must be 1 (A1) or 2 (A2)");
-    if (nv < 0 || (nv > 0 && (rows == nullptr || w == nullptr || mean == nullptr)) || stride_bytes < (ctx->n + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_project_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    if (int rc = rows_args(ctx, "vpca_project_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4, w != nullptr && mean != nullptr))
+        return rc;
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) return VPCA_OK;
     LaneGuard lg(ctx);
@@ -1790,8 +1824,8 @@ int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t str
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     int rc = kinship_check(ctx);
     if (rc != VPCA_OK) return rc;
-    if (nv < 0 || (nv > 0 && rows == nullptr) || stride_bytes < (ctx->n + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_kinship_bed: bad argument (stride_bytes must be >= ceil(n_samples / 4))");
+    rc = rows_args(ctx, "vpca_kinship_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4);
+    if (rc != VPCA_OK) return rc;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         if (ctx->kin_variants + nv > 2147483647ll)
@@ -1810,18 +1844,8 @@ int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t str
     const int64_t cap_rows = (ctx->chunk_nnz * (int64_t)sizeof(int32_t)) / stride_bytes;   // raw rows in L.d_idx[b]
     if (cap_rows < 32) return fail(ctx, VPCA_ERR_BAD_ARG, "stride_bytes too large for the staging buffer");
     const int64_t step = std::min(ctx->kin_chunk, (cap_rows / 32) * 32);
-    int chunk = 0;
-    for (int64_t v = 0; v < nv; v += step, ++chunk) {
-        const int64_t nvc = std::min(step, nv - v);
-        const int b = chunk & 1;
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0));
-        CUDA_OK(ctx, cudaMemcpyAsync(L.d_idx[b].get(), rows + (size_t)v * stride_bytes, (size_t)nvc * stride_bytes,
-                                     cudaMemcpyHostToDevice, L.copy_stream));
-        CUDA_OK(ctx, cudaEventRecord(L.ev_copy[b], L.copy_stream));
-        ctx->c_h2d += nvc * stride_bytes;
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, encode_bed_planes(reinterpret_cast<const uint8_t*>(L.d_idx[b].get()), stride_bytes, nvc, n, ctx->d_kin_x[b].get(), P,
-                                       L.stream));
+    rc = stage_rows(ctx, L, rows, nv, stride_bytes, step, lane_rows(L), [&](int b, const uint8_t* d_rows, int64_t, int64_t nvc) -> int {
+        CUDA_OK(ctx, encode_bed_planes(d_rows, stride_bytes, nvc, n, ctx->d_kin_x[b].get(), P, L.stream));
         std::string msg;
         cudaError_t e = gram_accumulate(ctx->kin_plan, ctx->d_kin_x[b].get(), 8, (int)R, nvc, P, P, ctx->d_kin.get(), L.stream, &msg);
         if (e != cudaSuccess)
@@ -1829,9 +1853,9 @@ int vpca_kinship_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t str
                         "batch, call vpca_reset]", cudaGetErrorString(e), msg.c_str());
         ctx->c_launches += 2;
         ctx->c_gram += 1;
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
+        return VPCA_OK;
+    });
+    if (rc != VPCA_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     ctx->kin_variants += nv;
     return VPCA_OK;
@@ -2077,7 +2101,7 @@ int vpca_ld_prune_bed_masked(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int
 }
 
 // ---- variant QC (qc.cu, DESIGN.md 10) -----------------------------------------------------------------------------------
-// Driver-side and synchronous.  Rows are staged in chunks of at most kQcStageBytes on a lane's stream and counted; the
+// Driver-side and synchronous.  Rows are staged in chunks of at most kQcStageBytes through stage_rows and counted; the
 // counts of whole chunks gather into batches of about kQcHweChunk rows, each tested with one HWE launch and copied back,
 // so that the HWE kernel fills the GPU even when a chunk holds a few thousand wide rows, and device memory stays bounded
 // whatever the number of variants.
@@ -2085,10 +2109,9 @@ namespace {
 constexpr int64_t kQcStageBytes = 64ll << 20;   // raw .bed bytes per staged chunk
 constexpr int64_t kQcHweChunk = 1ll << 18;      // count rows per HWE launch (and per vpca_hwe_exact chunk)
 
-// grows the QC buffers to `row_bytes` staged bytes and `rows` count / p-value rows
-cudaError_t qc_buffers(vpca_ctx* ctx, int64_t row_bytes, int64_t rows) {
-    cudaError_t e = ctx->d_qc_rows.ensure(row_bytes);
-    if (e == cudaSuccess) e = ctx->d_qc_counts.ensure(4 * rows);
+// grows the QC buffers to `rows` count / p-value rows
+cudaError_t qc_buffers(vpca_ctx* ctx, int64_t rows) {
+    cudaError_t e = ctx->d_qc_counts.ensure(4 * rows);
     if (e == cudaSuccess) e = ctx->d_qc_p.ensure(rows);
     return e;
 }
@@ -2098,9 +2121,7 @@ int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
                         double* out_hwe_p) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     const int n = ctx->n;
-    if (nv < 0 || (nv > 0 && (rows == nullptr || out_counts == nullptr)) || stride_bytes < (n + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_variant_qc_bed: bad argument (rows and out_counts must be set, "
-                    "stride_bytes >= ceil(n_samples / 4))");
+    if (int rc = rows_args(ctx, "vpca_variant_qc_bed", rows, nv, stride_bytes, (n + 3) / 4, out_counts != nullptr)) return rc;
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) return VPCA_OK;
     const int64_t step = std::max<int64_t>(1, std::min(nv, kQcStageBytes / stride_bytes));
@@ -2109,23 +2130,20 @@ int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
     if (lg.rc != VPCA_OK) return lg.rc;
     vpca_ctx::Lane& L = *lg.lane;
     {
-        cudaError_t e = qc_buffers(ctx, step * stride_bytes, batch);
+        cudaError_t e = qc_buffers(ctx, batch);
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "variant QC buffers for %lld rows of %lld bytes: %s", (long long)step,
                         (long long)stride_bytes, cudaGetErrorString(e));
         }
     }
-    for (int64_t b0 = 0; b0 < nv; b0 += batch) {
-        const int64_t nb = std::min(batch, nv - b0);
-        for (int64_t v = b0; v < b0 + nb; v += step) {
-            const int64_t nvc = std::min(step, b0 + nb - v);
-            CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_qc_rows.get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
-                                         cudaMemcpyHostToDevice, L.stream));
-            ctx->c_h2d += nvc * stride_bytes;
-            CUDA_OK(ctx, qc_count(ctx->d_qc_rows.get(), stride_bytes, (int)nvc, n, ctx->d_qc_counts.get() + 4 * (v - b0), L.stream));
-            ctx->c_launches += 1;
-        }
+    // chunk boundaries fall on batch boundaries: the last chunk of a batch tests and copies back the whole batch
+    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
+        const int64_t b0 = v / batch * batch, nb = std::min(batch, nv - b0);
+        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, (int)nvc, n, ctx->d_qc_counts.get() + 4 * (v - b0), L.stream));
+        ctx->c_launches += 1;
+        if (v + nvc < b0 + nb) return VPCA_OK;
         CUDA_OK(ctx, cudaMemcpyAsync(out_counts + 4 * b0, ctx->d_qc_counts.get(), (size_t)(4 * nb) * sizeof(int32_t),
                                      cudaMemcpyDeviceToHost, L.stream));
         ctx->c_d2h += 16 * nb;
@@ -2136,9 +2154,8 @@ int vpca_variant_qc_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
             ctx->c_launches += 1;
             ctx->c_d2h += 8 * nb;
         }
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
-    return VPCA_OK;
+        return VPCA_OK;
+    });
 }
 
 int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out_p) {
@@ -2158,7 +2175,7 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
     if (lg.rc != VPCA_OK) return lg.rc;
     vpca_ctx::Lane& L = *lg.lane;
     {
-        cudaError_t e = qc_buffers(ctx, 1, step);
+        cudaError_t e = qc_buffers(ctx, step);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "HWE buffers for %lld rows: %s", (long long)step, cudaGetErrorString(e));
@@ -2179,13 +2196,15 @@ int vpca_hwe_exact(vpca_ctx* ctx, const int32_t* counts, int64_t nv, double* out
 }
 
 // ---- variance-standardized relationship matrix (grm.cu, DESIGN.md 13) ---------------------------------------------------
-// Driver-side and synchronous.  Rows are staged in chunks of at most kGrmStageBytes on a lane, the upload of chunk i + 1 on
-// the copy stream overlapping the work on chunk i.  Per chunk: counts, tables and the used list, then (after one small
-// read-back of the used count) the used columns expanded into the panel, which is multiplied into eig.d_C whenever it is
-// full.
+// Driver-side and synchronous.  Rows are staged in chunks of at most kGrmStageBytes and kGrmMaxChunk rows through
+// stage_rows, the upload of chunk i + 1 overlapping the work on chunk i.  Per chunk: counts, tables and the used list,
+// then (after one small read-back of the used count) the used columns expanded into the panel, which is multiplied into
+// eig.d_C whenever it is full.
 namespace {
 constexpr int64_t kGrmStageBytes = 64ll << 20;   // raw .bed bytes per staged chunk
 constexpr int64_t kGrmMaxChunk = 1ll << 20;      // rows per staged chunk
+
+int64_t grm_step(int64_t nv, int64_t stride) { return std::max<int64_t>(1, std::min({nv, kGrmStageBytes / stride, kGrmMaxChunk})); }
 
 int grm_check(vpca_ctx* ctx) {
     if (ctx->n > 65535)
@@ -2204,7 +2223,7 @@ int grm_buffers(vpca_ctx* ctx, vpca_ctx::Lane& L, int64_t step, int64_t stride) 
     }
     const int64_t zc = grm_panel_rows(ctx->n) * kGrmPanelK;
     cudaError_t e = cudaSuccess;
-    for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride);
+    for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride);
     if (e == cudaSuccess) e = ctx->d_grm_counts.ensure(4 * step);
     if (e == cudaSuccess) e = ctx->d_grm_tab.ensure(4 * step);
     if (e == cudaSuccess) e = ctx->d_grm_used.ensure(step);
@@ -2230,10 +2249,9 @@ int grm_buffers(vpca_ctx* ctx, vpca_ctx::Lane& L, int64_t step, int64_t stride) 
 int vpca_grm_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     const int n = ctx->n;
-    if (nv < 0 || (nv > 0 && rows == nullptr) || stride_bytes < (n + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_grm_bed: bad argument (rows must be set, nv >= 0, stride_bytes >= "
-                    "ceil(n_samples / 4))");
-    int rc = grm_check(ctx);
+    int rc = rows_args(ctx, "vpca_grm_bed", rows, nv, stride_bytes, (n + 3) / 4);
+    if (rc != VPCA_OK) return rc;
+    rc = grm_check(ctx);
     if (rc != VPCA_OK) return rc;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
@@ -2242,35 +2260,17 @@ int vpca_grm_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_
     }
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) return VPCA_OK;
-    const int64_t step = std::max<int64_t>(1, std::min({nv, kGrmStageBytes / stride_bytes, kGrmMaxChunk}));
+    const int64_t step = grm_step(nv, stride_bytes);
     LaneGuard lg(ctx);
     if (lg.rc != VPCA_OK) return lg.rc;
     vpca_ctx::Lane& L = *lg.lane;
     rc = grm_buffers(ctx, L, step, stride_bytes);
     if (rc != VPCA_OK) return rc;
-    const int64_t nchunks = (nv + step - 1) / step;
-    auto upload = [&](int64_t c) -> cudaError_t {
-        const int b = (int)(c & 1);
-        const int64_t v = c * step, nvc = std::min(step, nv - v);
-        cudaError_t e = cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0);
-        if (e == cudaSuccess)
-            e = cudaMemcpyAsync(ctx->d_grm_rows[b].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
-                                cudaMemcpyHostToDevice, L.copy_stream);
-        if (e == cudaSuccess) e = cudaEventRecord(L.ev_copy[b], L.copy_stream);
-        ctx->c_h2d += nvc * stride_bytes;
-        return e;
-    };
-    CUDA_OK(ctx, upload(0));
     double* Z = ctx->d_grm_Z.get();
     double* C = ctx->eig.d_C.get();
-    for (int64_t c = 0; c < nchunks; ++c) {
-        const int b = (int)(c & 1);
-        const int nvc = (int)std::min(step, nv - c * step);
-        if (c + 1 < nchunks) CUDA_OK(ctx, upload(c + 1));
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        const uint8_t* d_rows = ctx->d_grm_rows[b].get();
-        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, nvc, n, ctx->d_grm_counts.get(), L.stream));
-        CUDA_OK(ctx, grm_tables(ctx->d_grm_counts.get(), nvc, ctx->d_grm_tab.get(), ctx->d_grm_used.get(),
+    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t, int64_t nvc) -> int {
+        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, (int)nvc, n, ctx->d_grm_counts.get(), L.stream));
+        CUDA_OK(ctx, grm_tables(ctx->d_grm_counts.get(), (int)nvc, ctx->d_grm_tab.get(), ctx->d_grm_used.get(),
                                 ctx->d_grm_inv.get(), ctx->d_grm_total.get(), L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(L.h_flags, ctx->d_grm_total.get(), sizeof(int), cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
@@ -2290,10 +2290,8 @@ int vpca_grm_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_
             }
         }
         ctx->grm_used += used;
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
-    return VPCA_OK;
+        return VPCA_OK;
+    });
 }
 
 int vpca_grm_finalize(vpca_ctx* ctx, int64_t* n_used) {
@@ -2383,37 +2381,12 @@ int vpca_compute_pca_grm(vpca_ctx* ctx, int32_t k, double* vecs, double* evals) 
 }
 
 // ---- GRM loadings and projection (grm_project.cu, DESIGN.md 14) ----------------------------------------------------------
-// Driver-side and synchronous.  Rows are staged as in vpca_grm_bed: chunks of at most kGrmStageBytes and kGrmMaxChunk rows
-// on a lane, double-buffered, the upload of chunk i + 1 overlapping the work on chunk i.
-namespace {
-int64_t grm_step(int64_t nv, int64_t stride) { return std::max<int64_t>(1, std::min({nv, kGrmStageBytes / stride, kGrmMaxChunk})); }
-
-// Uploads chunk c of `rows` into d_grm_rows[c & 1] on the lane's copy stream, once the work on that buffer is done.
-cudaError_t grm_upload(vpca_ctx* ctx, vpca_ctx::Lane& L, const uint8_t* rows, int64_t nv, int64_t stride, int64_t step,
-                       int64_t c) {
-    const int b = (int)(c & 1);
-    const int64_t v = c * step, nvc = std::min(step, nv - v);
-    cudaError_t e = cudaStreamWaitEvent(L.copy_stream, L.ev_done[b], 0);
-    if (e == cudaSuccess)
-        e = cudaMemcpyAsync(ctx->d_grm_rows[b].get(), rows + (size_t)v * stride, (size_t)(nvc * stride),
-                            cudaMemcpyHostToDevice, L.copy_stream);
-    if (e == cudaSuccess) e = cudaEventRecord(L.ev_copy[b], L.copy_stream);
-    ctx->c_h2d += nvc * stride;
-    return e;
-}
-
-int grm_rows_args(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes, bool outs_set) {
-    if (nv < 0 || (nv > 0 && (rows == nullptr || !outs_set)) || stride_bytes < (ctx->n + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (rows and arrays must be set, nv >= 0, stride_bytes >= "
-                    "ceil(n_samples / 4))", fn);
-    return VPCA_OK;
-}
-}   // namespace
-
+// Driver-side and synchronous.  Rows are staged as in vpca_grm_bed: chunks of grm_step rows through stage_rows.
 int vpca_grm_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t nv, int64_t stride_bytes, double* out_w,
                           double* out_tab) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    int rc = grm_rows_args(ctx, "vpca_grm_loadings_bed", rows, nv, stride_bytes, out_w != nullptr && out_tab != nullptr);
+    int rc = rows_args(ctx, "vpca_grm_loadings_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4,
+                       out_w != nullptr && out_tab != nullptr);
     if (rc != VPCA_OK) return rc;
     rc = grm_check(ctx);
     if (rc != VPCA_OK) return rc;
@@ -2436,7 +2409,7 @@ int vpca_grm_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t
     vpca_ctx::Lane& L = *lg.lane;
     {
         cudaError_t e = cudaSuccess;
-        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
         if (e == cudaSuccess) e = ctx->d_grm_counts.ensure(4 * step);
         if (e == cudaSuccess) e = ctx->d_grm_tab.ensure(4 * step);
         if (e == cudaSuccess) e = ctx->d_grm_used.ensure(step);
@@ -2446,28 +2419,18 @@ int vpca_grm_loadings_bed(vpca_ctx* ctx, int32_t k, const uint8_t* rows, int64_t
             return fail(ctx, VPCA_ERR_NOMEM, "GRM loadings buffers: %s", cudaGetErrorString(e));
         }
     }
-    const int64_t nchunks = (nv + step - 1) / step;
-    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
-    for (int64_t c = 0; c < nchunks; ++c) {
-        const int b = (int)(c & 1);
-        const int64_t v = c * step;
-        const int nvc = (int)std::min(step, nv - v);
-        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        const uint8_t* d_rows = ctx->d_grm_rows[b].get();
-        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, nvc, n, ctx->d_grm_counts.get(), L.stream));
-        CUDA_OK(ctx, grm_table(ctx->d_grm_counts.get(), nvc, ctx->d_grm_tab.get(), ctx->d_grm_used.get(), L.stream));
-        CUDA_OK(ctx, grm_loadings(d_rows, stride_bytes, nvc, n, ctx->d_grm_tab.get(), U, k, ctx->d_grm_w.get(), L.stream));
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
+        CUDA_OK(ctx, qc_count(d_rows, stride_bytes, (int)nvc, n, ctx->d_grm_counts.get(), L.stream));
+        CUDA_OK(ctx, grm_table(ctx->d_grm_counts.get(), (int)nvc, ctx->d_grm_tab.get(), ctx->d_grm_used.get(), L.stream));
+        CUDA_OK(ctx, grm_loadings(d_rows, stride_bytes, (int)nvc, n, ctx->d_grm_tab.get(), U, k, ctx->d_grm_w.get(), L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out_w + v * k, ctx->d_grm_w.get(), (size_t)nvc * k * sizeof(double),
                                      cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out_tab + 4 * v, ctx->d_grm_tab.get(), (size_t)nvc * 4 * sizeof(double),
                                      cudaMemcpyDeviceToHost, L.stream));
         ctx->c_launches += 3;
-        ctx->c_d2h += (int64_t)nvc * (k + 4) * (int64_t)sizeof(double);
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
-    return VPCA_OK;
+        ctx->c_d2h += nvc * (k + 4) * (int64_t)sizeof(double);
+        return VPCA_OK;
+    });
 }
 
 int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, const double* tab,
@@ -2480,7 +2443,7 @@ int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t
         if (rc != VPCA_OK) return rc;
         k = ctx->proj_k;
     }
-    int rc = grm_rows_args(ctx, "vpca_grm_project_bed", rows, nv, stride_bytes, tab != nullptr && w != nullptr);
+    int rc = rows_args(ctx, "vpca_grm_project_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4, tab != nullptr && w != nullptr);
     if (rc != VPCA_OK) return rc;
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
     if (nv == 0) return VPCA_OK;
@@ -2492,7 +2455,7 @@ int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t
     {
         const int64_t part = grm_project_scratch_doubles(n, step, k);
         cudaError_t e = cudaSuccess;
-        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
         if (e == cudaSuccess) e = ctx->d_grm_ptab.ensure(4 * step);
         if (e == cudaSuccess) e = ctx->d_grm_w.ensure(step * k);
         if (e == cudaSuccess) e = ctx->d_proj_part.ensure(part, with_slack(part));
@@ -2501,32 +2464,23 @@ int vpca_grm_project_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t
             return fail(ctx, VPCA_ERR_NOMEM, "GRM projection buffers: %s", cudaGetErrorString(e));
         }
     }
-    const int64_t nchunks = (nv + step - 1) / step;
-    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
-    for (int64_t c = 0; c < nchunks; ++c) {
-        const int b = (int)(c & 1);
-        const int64_t v = c * step;
-        const int nvc = (int)std::min(step, nv - v);
-        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
+    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
         // the single w / table buffers are reused in stream order: the previous chunk's kernels read them first
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_grm_w.get(), w + v * k, (size_t)nvc * k * sizeof(double),
                                      cudaMemcpyHostToDevice, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_grm_ptab.get(), tab + 4 * v, (size_t)nvc * 4 * sizeof(double),
                                      cudaMemcpyHostToDevice, L.stream));
-        ctx->c_h2d += (int64_t)nvc * (k + 4) * (int64_t)sizeof(double);
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, grm_project(ctx->d_grm_rows[b].get(), stride_bytes, nvc, n, ctx->d_grm_ptab.get(), ctx->d_grm_w.get(),
-                                 k, ctx->d_proj_part.get(), ctx->d_proj_acc.get(), kProjLd, L.stream));
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+        ctx->c_h2d += nvc * (k + 4) * (int64_t)sizeof(double);
+        CUDA_OK(ctx, grm_project(d_rows, stride_bytes, (int)nvc, n, ctx->d_grm_ptab.get(), ctx->d_grm_w.get(), k,
+                                 ctx->d_proj_part.get(), ctx->d_proj_acc.get(), kProjLd, L.stream));
         ctx->c_launches += 2;
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));   // the caller's rows are free to reuse on return
-    return VPCA_OK;
+        return VPCA_OK;
+    });
 }
 
 // ---- linear association tests (glm.cu, DESIGN.md 15) ---------------------------------------------------------------------
 // vpca_glm_begin is host FP64 work and one upload; vpca_glm_linear_bed is driver-side and synchronous, its rows staged as
-// vpca_grm_loadings_bed stages them (grm_upload into d_grm_rows).
+// vpca_grm_loadings_bed stages them.
 namespace {
 // The checks and the regression samples both begins share; VPCA_OK or the refusal (the message names fn).
 int glm_samples(vpca_ctx* ctx, const char* fn, const double* pheno, const double* covar, int32_t n_covar,
@@ -2788,7 +2742,7 @@ int vpca_glm_logistic_begin(vpca_ctx* ctx, const double* pheno, const double* co
 int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
                         double* out, int32_t* out_err) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    int rc = grm_rows_args(ctx, "vpca_glm_linear_bed", rows, nv, stride_bytes, out != nullptr && out_err != nullptr);
+    int rc = rows_args(ctx, "vpca_glm_linear_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4, out != nullptr && out_err != nullptr);
     if (rc != VPCA_OK) return rc;
     if (counted_allele != 1 && counted_allele != 2)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_linear_bed: counted_allele must be 1 (A1) or 2 (A2), not %d",
@@ -2814,7 +2768,7 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
     vpca_ctx::Lane& L = *lg.lane;
     {
         cudaError_t e = cudaSuccess;
-        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
         if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * kGlmRec);
         if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
         if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
@@ -2823,33 +2777,25 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
             return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
         }
     }
-    const int64_t nchunks = (nv + step - 1) / step;
-    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
-    for (int64_t c = 0; c < nchunks; ++c) {
-        const int b = (int)(c & 1);
-        const int64_t v = c * step;
-        const int nvc = (int)std::min(step, nv - v);
-        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, glm_linear(ctx->d_grm_rows[b].get(), stride_bytes, nvc, n, q, n_reg, ctx->d_glm_Qx.get(),
-                                ctx->d_glm_mask.get(), ctx->d_glm_z0.get(), yty, counted_allele, ctx->d_glm_sums.get(),
-                                ctx->d_glm_out.get(), ctx->d_glm_err.get(), L.stream));
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
+        CUDA_OK(ctx, glm_linear(d_rows, stride_bytes, (int)nvc, n, q, n_reg, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
+                                ctx->d_glm_z0.get(), yty, counted_allele, ctx->d_glm_sums.get(), ctx->d_glm_out.get(),
+                                ctx->d_glm_err.get(), L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
                                      cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
                                      cudaMemcpyDeviceToHost, L.stream));
         ctx->c_launches += 3;
-        ctx->c_d2h += (int64_t)nvc * (6 * (int64_t)sizeof(double) + (int64_t)sizeof(int32_t));
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
-    return VPCA_OK;
+        ctx->c_d2h += nvc * (6 * (int64_t)sizeof(double) + (int64_t)sizeof(int32_t));
+        return VPCA_OK;
+    });
 }
 
 int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
                           double* out, int32_t* out_err, int32_t* out_passes) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    int rc = grm_rows_args(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, out != nullptr && out_err != nullptr);
+    int rc = rows_args(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4,
+                       out != nullptr && out_err != nullptr);
     if (rc != VPCA_OK) return rc;
     if (counted_allele != 1 && counted_allele != 2)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_logistic_bed: counted_allele must be 1 (A1) or 2 (A2), not %d",
@@ -2873,7 +2819,7 @@ int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_
     vpca_ctx::Lane& L = *lg.lane;
     {
         cudaError_t e = cudaSuccess;
-        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_grm_rows[b].ensure(step * stride_bytes);
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
         if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * 6);
         if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
         if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
@@ -2883,19 +2829,10 @@ int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_
             return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
         }
     }
-    const int64_t nchunks = (nv + step - 1) / step;
-    CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, 0));
-    for (int64_t c = 0; c < nchunks; ++c) {
-        const int b = (int)(c & 1);
-        const int64_t v = c * step;
-        const int nvc = (int)std::min(step, nv - v);
-        if (c + 1 < nchunks) CUDA_OK(ctx, grm_upload(ctx, L, rows, nv, stride_bytes, step, c + 1));
-        CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, L.ev_copy[b], 0));
-        CUDA_OK(ctx, glm_logistic(ctx->d_grm_rows[b].get(), stride_bytes, nvc, n, q, ctx->d_glm_Qx.get(),
-                                  ctx->d_glm_mask.get(), ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele,
-                                  ctx->d_glm_sums.get(), ctx->d_glm_out.get(), ctx->d_glm_err.get(),
-                                  ctx->d_glm_passes.get(), L.stream));
-        CUDA_OK(ctx, cudaEventRecord(L.ev_done[b], L.stream));
+    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
+        CUDA_OK(ctx, glm_logistic(d_rows, stride_bytes, (int)nvc, n, q, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
+                                  ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele, ctx->d_glm_sums.get(),
+                                  ctx->d_glm_out.get(), ctx->d_glm_err.get(), ctx->d_glm_passes.get(), L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
                                      cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
@@ -2904,31 +2841,19 @@ int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_
             CUDA_OK(ctx, cudaMemcpyAsync(out_passes + v, ctx->d_glm_passes.get(), (size_t)nvc * sizeof(int32_t),
                                          cudaMemcpyDeviceToHost, L.stream));
         ctx->c_launches += 5;
-        ctx->c_d2h += (int64_t)nvc * (6 * (int64_t)sizeof(double) + (out_passes ? 2 : 1) * (int64_t)sizeof(int32_t));
-    }
-    CUDA_OK(ctx, cudaStreamSynchronize(L.stream));
-    return VPCA_OK;
+        ctx->c_d2h += nvc * (6 * (int64_t)sizeof(double) + (out_passes ? 2 : 1) * (int64_t)sizeof(int32_t));
+        return VPCA_OK;
+    });
 }
 
 // ---- sample QC (samples.cu, DESIGN.md 11) -------------------------------------------------------------------------------
 // Driver-side and synchronous, on rows of their own sample count: the context lends its device, a lane and scratch.  Rows
-// are staged in chunks of at most kSmStageBytes.  The subset pass copies both ways: chunk i + 1 goes up on the lane's copy
-// stream while a helper thread brings chunk i down on a stream of its own, so that the two copies (pageable, hence each
-// blocking the thread that issues it) run at once on the two copy engines.
+// are staged in chunks of at most kSmStageBytes in the context's driver-side pair (d_bed_rows).  The subset pass copies
+// both ways: chunk i + 1 goes up on the lane's copy stream while a helper thread brings chunk i down on a stream of its
+// own, so that the two copies (pageable, hence each blocking the thread that issues it) run at once on the two copy
+// engines.
 namespace {
 constexpr int64_t kSmStageBytes = 64ll << 20;   // raw .bed bytes per staged chunk
-
-// the checks both calls share; 0 when the arguments are good
-int sample_rows_args(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
-                     int32_t n_samples) {
-    if (nv < 0 || (nv > 0 && rows == nullptr))
-        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (nv = %lld must be >= 0, rows set when nv > 0)", fn,
-                    (long long)nv);
-    if (n_samples < 1 || stride_bytes < ((int64_t)n_samples + 3) / 4)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: bad argument (n_samples = %d must be >= 1, stride_bytes = %lld >= "
-                    "ceil(n_samples / 4))", fn, (int)n_samples, (long long)stride_bytes);
-    return VPCA_OK;
-}
 
 // The D2H side of vpca_subset_bed_samples: copies chunk i down once the main thread has launched its kernel, and
 // reports each finished copy, which frees the chunk's two buffers for chunk i + 2.
@@ -2967,9 +2892,10 @@ struct SubsetDownloader {
 int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t n_samples,
                             int32_t* out_missing) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    if (int rc = sample_rows_args(ctx, "vpca_sample_missing_bed", rows, nv, stride_bytes, n_samples)) return rc;
-    if (nv > 0 && out_missing == nullptr)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_sample_missing_bed: out_missing is NULL");
+    if (n_samples < 1) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_sample_missing_bed: n_samples = %d must be >= 1", (int)n_samples);
+    if (int rc = rows_args(ctx, "vpca_sample_missing_bed", rows, nv, stride_bytes, ((int64_t)n_samples + 3) / 4,
+                           out_missing != nullptr))
+        return rc;
     if (nv > 2147483647ll)
         return fail(ctx, VPCA_ERR_OVERFLOW, "vpca_sample_missing_bed: %lld rows could overflow an int32 count",
                     (long long)nv);
@@ -2983,8 +2909,8 @@ int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
     if (lg.rc != VPCA_OK) return lg.rc;
     vpca_ctx::Lane& L = *lg.lane;
     {
-        cudaError_t e = ctx->d_sm_rows[0].ensure(step * stride_bytes);
-        if (e == cudaSuccess) e = ctx->d_sm_miss.ensure(n_samples);
+        cudaError_t e = ctx->d_sm_miss.ensure(n_samples);
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "sample QC buffers for %lld rows of %lld bytes: %s", (long long)step,
@@ -2992,14 +2918,12 @@ int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
         }
     }
     CUDA_OK(ctx, cudaMemsetAsync(ctx->d_sm_miss.get(), 0, (size_t)n_samples * sizeof(int32_t), L.stream));
-    for (int64_t v = 0; v < nv; v += step) {
-        const int64_t nvc = std::min(step, nv - v);
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[0].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
-                                     cudaMemcpyHostToDevice, L.stream));
-        ctx->c_h2d += nvc * stride_bytes;
-        CUDA_OK(ctx, sample_missing(ctx->d_sm_rows[0].get(), stride_bytes, (int)nvc, n_samples, ctx->d_sm_miss.get(), L.stream));
+    int rc = stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t, int64_t nvc) -> int {
+        CUDA_OK(ctx, sample_missing(d_rows, stride_bytes, (int)nvc, n_samples, ctx->d_sm_miss.get(), L.stream));
         ctx->c_launches += 1;
-    }
+        return VPCA_OK;
+    });
+    if (rc != VPCA_OK) return rc;
     CUDA_OK(ctx, cudaMemcpyAsync(out_missing, ctx->d_sm_miss.get(), (size_t)n_samples * sizeof(int32_t), cudaMemcpyDeviceToHost,
                                  L.stream));
     ctx->c_d2h += 4 * (int64_t)n_samples;
@@ -3010,9 +2934,10 @@ int vpca_sample_missing_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
 int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t n_samples,
                             const int32_t* keep_idx, int32_t m, uint8_t* out_rows, int64_t out_stride) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    if (int rc = sample_rows_args(ctx, "vpca_subset_bed_samples", rows, nv, stride_bytes, n_samples)) return rc;
-    if (nv > 0 && (keep_idx == nullptr || out_rows == nullptr))
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_subset_bed_samples: keep_idx and out_rows must be set");
+    if (n_samples < 1) return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_subset_bed_samples: n_samples = %d must be >= 1", (int)n_samples);
+    if (int rc = rows_args(ctx, "vpca_subset_bed_samples", rows, nv, stride_bytes, ((int64_t)n_samples + 3) / 4,
+                           keep_idx != nullptr && out_rows != nullptr))
+        return rc;
     if (m < 1 || out_stride < ((int64_t)m + 3) / 4)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_subset_bed_samples: bad argument (m = %d must be >= 1, out_stride = %lld "
                     ">= ceil(m / 4))", (int)m, (long long)out_stride);
@@ -3032,7 +2957,7 @@ int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
     {
         cudaError_t e = cudaSuccess;
         for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-            e = ctx->d_sm_rows[b].ensure(step * stride_bytes);
+            e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
             if (e == cudaSuccess) e = ctx->d_sm_out[b].ensure(step * mb);
             if (e == cudaSuccess && ctx->sm_ev_copy[b] == nullptr)
                 e = cudaEventCreateWithFlags(&ctx->sm_ev_copy[b], cudaEventDisableTiming);
@@ -3089,12 +3014,12 @@ int vpca_subset_bed_samples(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int6
         const int b = (int)(i & 1);
         const int64_t v = i * step, nvc = std::min(step, nv - v);
         if (!down.wait_copied(i - 1)) break;   // chunk i - 2, the last user of buffers b, is on the host
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_sm_rows[b].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->d_bed_rows[b].get(), rows + (size_t)v * stride_bytes, (size_t)(nvc * stride_bytes),
                                      cudaMemcpyHostToDevice, L.copy_stream));
         CUDA_OK(ctx, cudaEventRecord(ctx->sm_ev_copy[b], L.copy_stream));
         ctx->c_h2d += nvc * stride_bytes;
         CUDA_OK(ctx, cudaStreamWaitEvent(L.stream, ctx->sm_ev_copy[b], 0));
-        CUDA_OK(ctx, subset_samples(ctx->d_sm_rows[b].get(), stride_bytes, (int)nvc, ctx->d_sm_idx.get(), m, ctx->d_sm_out[b].get(), mb,
+        CUDA_OK(ctx, subset_samples(ctx->d_bed_rows[b].get(), stride_bytes, (int)nvc, ctx->d_sm_idx.get(), m, ctx->d_sm_out[b].get(), mb,
                                     L.stream));
         CUDA_OK(ctx, cudaEventRecord(ctx->sm_ev_kern[b], L.stream));
         ctx->c_launches += 1;

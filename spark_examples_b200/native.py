@@ -330,6 +330,20 @@ def _host_ptr(a: np.ndarray) -> int:
     return a.ctypes.data
 
 
+_NO_ROWS = np.zeros(1, np.uint8)   # the address passed for zero rows: vpca_ld_prune_bed refuses NULL rows even then
+
+
+def _bed_rows(rows) -> Tuple[np.ndarray, int]:
+    """(V, stride) uint8 rows as they are when already so (a .bed memmap is read in place), else a C-ordered copy, and
+    their address, valid even for V = 0."""
+    b = np.asarray(rows)
+    if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
+        b = np.ascontiguousarray(b, dtype=np.uint8)
+    if b.ndim != 2:
+        raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+    return b, b.ctypes.data if b.size else _NO_ROWS.ctypes.data
+
+
 class NativePca:
     """One GPU's VariantsPca state.  Method names follow the JNI class of INTEGRATION.md 1:1."""
 
@@ -487,10 +501,8 @@ class NativePca:
     def accumulateBed(self, partition_id: int, rows: np.ndarray, counted_allele: int = 1):
         """rows: (nv, stride) uint8 PLINK .bed rows (2 bits per sample: 00 hom A1, 01 missing, 10 het, 11 hom A2);
         counted_allele 1: carriers of A1, 2: carriers of A2 (plink.py)."""
-        b = np.ascontiguousarray(rows, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
-        self._check(self._lib.vpca_accumulate_bed(self._h, int(partition_id), _host_ptr(b), b.shape[0], b.shape[1],
+        b, ptr = _bed_rows(rows)
+        self._check(self._lib.vpca_accumulate_bed(self._h, int(partition_id), ptr, b.shape[0], b.shape[1],
                                                   int(counted_allele)))
 
     def accumulateBitsRaw(self, partition_id: int, ptr: int, nv: int, stride_bytes: int):
@@ -666,12 +678,10 @@ class NativePca:
 
     def loadingsBed(self, k: int, rows: np.ndarray, counted_allele: int = 1):
         """Same for PLINK .bed rows (see accumulateBed), with the same U and the same bits."""
-        b = np.ascontiguousarray(rows, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        b, ptr = _bed_rows(rows)
         w = np.zeros((max(b.shape[0], 1), int(k)), dtype=np.float64)
         cnt = np.zeros(max(b.shape[0], 1), dtype=np.int32)
-        self._check(self._lib.vpca_loadings_bed(self._h, int(k), _host_ptr(b), b.shape[0], b.shape[1], int(counted_allele),
+        self._check(self._lib.vpca_loadings_bed(self._h, int(k), ptr, b.shape[0], b.shape[1], int(counted_allele),
                                                 _host_ptr(w), _host_ptr(cnt)))
         return w[:b.shape[0]], cnt[:b.shape[0]]
 
@@ -695,12 +705,10 @@ class NativePca:
                                                  _host_ptr(ww), _host_ptr(mm)))
 
     def projectBed(self, rows: np.ndarray, w, mean, counted_allele: int = 1):
-        b = np.ascontiguousarray(rows, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        b, ptr = _bed_rows(rows)
         ww = np.ascontiguousarray(w, dtype=np.float64).reshape(b.shape[0], -1)
         mm = np.ascontiguousarray(mean, dtype=np.float64).reshape(b.shape[0])
-        self._check(self._lib.vpca_project_bed(self._h, _host_ptr(b), b.shape[0], b.shape[1], int(counted_allele),
+        self._check(self._lib.vpca_project_bed(self._h, ptr, b.shape[0], b.shape[1], int(counted_allele),
                                                _host_ptr(ww), _host_ptr(mm)))
 
     def projectPanels(self, d_ptr: int, nv: int, panel_variants: int, d_w: int, d_mean: int):
@@ -720,10 +728,8 @@ class NativePca:
     def kinshipBed(self, rows: np.ndarray):
         """Add PLINK .bed rows ((nv, stride) uint8, see accumulateBed) to the kinship counts of every sample pair; calls
         add up, and the PCA Gram is not touched.  Synchronises."""
-        b = np.ascontiguousarray(rows, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
-        self._check(self._lib.vpca_kinship_bed(self._h, _host_ptr(b) if b.size else None, b.shape[0], b.shape[1]))
+        b, ptr = _bed_rows(rows)
+        self._check(self._lib.vpca_kinship_bed(self._h, ptr, b.shape[0], b.shape[1]))
 
     def kinshipPairs(self, min_kinship: float = float("-inf"), max_pairs: Optional[int] = None):
         """-> (ids (P, 2) int32 with a < b, counts (P, 5) int32 NSNP, HETHET, IBS0, HET1_HOM2, HET2_HOM1, kinship (P,)
@@ -747,11 +753,7 @@ class NativePca:
         the first min(total, max_pairs) in-LD pairs in order of j, then i.  eligible ((V,) bool, e.g. the variant QC
         mask): only eligible variants are paired or kept -- the result of pruning the eligible rows alone, indexed over
         all V.  Synchronises."""
-        b = np.asarray(rows)
-        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
-            b = np.ascontiguousarray(b, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        b, rows_ptr = _bed_rows(rows)
         nv = b.shape[0]
         lo = np.ascontiguousarray(window_lo, dtype=np.int64).reshape(-1)
         if len(lo) != nv:
@@ -762,7 +764,6 @@ class NativePca:
         r2 = np.zeros(max(p, 1), np.float64)
         total = ctypes.c_int64(0)
         empty = np.zeros(1, np.int64)          # a valid address for zero variants
-        rows_ptr = b.ctypes.data if b.size else _host_ptr(empty)
         lo_ptr = lo.ctypes.data if lo.size else _host_ptr(empty)
         if eligible is None:
             self._check(self._lib.vpca_ld_prune_bed(self._h, rows_ptr, nv, b.shape[1], lo_ptr, float(r2_max),
@@ -785,16 +786,11 @@ class NativePca:
         """Genotype counts of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place, not copied) ->
         (counts (V, 4) int32 of HOM_A1, HET, HOM_A2, MISSING; p (V,) float64 exact HWE p-values, or None without
         `hwe`).  Synchronises."""
-        b = np.asarray(rows)
-        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
-            b = np.ascontiguousarray(b, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
+        b, ptr = _bed_rows(rows)
         nv = b.shape[0]
         counts = np.zeros((max(nv, 1), 4), np.int32)
         p = np.zeros(max(nv, 1), np.float64)
-        empty = np.zeros(1, np.uint8)
-        self._check(self._lib.vpca_variant_qc_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv, b.shape[1],
+        self._check(self._lib.vpca_variant_qc_bed(self._h, ptr, nv, b.shape[1],
                                                   _host_ptr(counts), _host_ptr(p) if hwe else None))
         return counts[:nv], (p[:nv] if hwe else None)
 
@@ -802,13 +798,8 @@ class NativePca:
     def grmBed(self, rows: np.ndarray):
         """Add PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place, not copied) to the GRM; calls add up,
         and the PCA Gram is not touched.  Synchronises."""
-        b = np.asarray(rows)
-        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
-            b = np.ascontiguousarray(b, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
-        empty = np.zeros(1, np.uint8)
-        self._check(self._lib.vpca_grm_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), b.shape[0], b.shape[1]))
+        b, ptr = _bed_rows(rows)
+        self._check(self._lib.vpca_grm_bed(self._h, ptr, b.shape[0], b.shape[1]))
 
     def grmFinalize(self) -> int:
         """Finish the GRM -> M, the number of variants used (VPCA_ERR_STATE when M = 0)."""
@@ -829,26 +820,15 @@ class NativePca:
         self._check(self._lib.vpca_compute_pca_grm(self._h, int(k), _host_ptr(flat), _host_ptr(evals)))
         return flat.reshape(k, self.n).T.copy(), evals
 
-    @staticmethod
-    def _bed_rows(rows):
-        """(V, stride) uint8 rows as they are when already so (a .bed memmap is read in place), else a C-ordered copy."""
-        b = np.asarray(rows)
-        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
-            b = np.ascontiguousarray(b, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
-        return b
-
     def grmLoadingsBed(self, k: int, rows: np.ndarray):
         """GRM loadings of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in place) for the U of the last
         computePcaGrm -> (w (V, k) float64 = Z^T U, tab (V, 4) float64 z of each .bed code, zero for an unused variant).
         Pass the rows the GRM was built from: the tables are recomputed from them.  Synchronises."""
-        b = self._bed_rows(rows)
+        b, ptr = _bed_rows(rows)
         nv = b.shape[0]
         w = np.zeros((max(nv, 1), int(k)), np.float64)
         tab = np.zeros((max(nv, 1), 4), np.float64)
-        empty = np.zeros(1, np.uint8)
-        self._check(self._lib.vpca_grm_loadings_bed(self._h, int(k), b.ctypes.data if b.size else _host_ptr(empty), nv,
+        self._check(self._lib.vpca_grm_loadings_bed(self._h, int(k), ptr, nv,
                                                     b.shape[1], _host_ptr(w), _host_ptr(tab)))
         return w[:nv], tab[:nv]
 
@@ -856,15 +836,14 @@ class NativePca:
         """Add sum_v tab[v][code(s, v)] w[v, :] of PLINK .bed rows ((V, stride) uint8 of this context's samples; a .bed
         memmap is read in place) to the projection begun by projectBegin; tab (V, 4) and w (V, k) of the reference align
         with the rows.  Read with projectGet(M * eigenvalues).  Synchronises."""
-        b = self._bed_rows(rows)
+        b, ptr = _bed_rows(rows)
         nv = b.shape[0]
         tt = np.ascontiguousarray(tab, dtype=np.float64).reshape(nv, 4)
         ww = np.ascontiguousarray(w, dtype=np.float64).reshape(nv, -1)
         if nv and ww.shape[1] != getattr(self, "_proj_k", ww.shape[1]):
             raise VpcaError(VPCA_ERR_BAD_ARG, f"w must have {self._proj_k} columns")
         empty = np.zeros(4, np.float64)
-        self._check(self._lib.vpca_grm_project_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty.view(np.uint8)),
-                                                   nv, b.shape[1], _host_ptr(tt if nv else empty),
+        self._check(self._lib.vpca_grm_project_bed(self._h, ptr, nv, b.shape[1], _host_ptr(tt if nv else empty),
                                                    _host_ptr(ww if nv else empty)))
 
     # -- linear association tests (vpca.h, DESIGN.md 15) -----------------------------------------------------------------
@@ -886,12 +865,11 @@ class NativePca:
         """Linear tests of PLINK .bed rows ((V, stride) uint8 of this context's samples; a .bed memmap is read in place)
         against the phenotype of glmBegin -> (stats (V, 6) float64: OBS_CT, A1_FREQ, BETA, SE, T_STAT, P, NaN where
         undefined; err (V,) int32: index into GLM_ERRCODES).  counted: 1 counts A1, 2 counts A2.  Synchronises."""
-        b = self._bed_rows(rows)
+        b, ptr = _bed_rows(rows)
         nv = b.shape[0]
         out = np.zeros((max(nv, 1), 6), np.float64)
         err = np.zeros(max(nv, 1), np.int32)
-        empty = np.zeros(1, np.uint8)
-        self._check(self._lib.vpca_glm_linear_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv, b.shape[1],
+        self._check(self._lib.vpca_glm_linear_bed(self._h, ptr, nv, b.shape[1],
                                                   int(counted), _host_ptr(out), _host_ptr(err)))
         return out[:nv], err[:nv]
 
@@ -915,13 +893,12 @@ class NativePca:
         place) against the phenotype of glmLogisticBegin -> (stats (V, 6) float64: OBS_CT, A1_FREQ, BETA, SE, Z, P, NaN
         where undefined; err (V,) int32: index into GLM_ERRCODES; passes (V,) int32: Newton passes).  counted: 1 counts
         A1, 2 counts A2.  Synchronises."""
-        b = self._bed_rows(rows)
+        b, ptr = _bed_rows(rows)
         nv = b.shape[0]
         out = np.zeros((max(nv, 1), 6), np.float64)
         err = np.zeros(max(nv, 1), np.int32)
         passes = np.zeros(max(nv, 1), np.int32)
-        empty = np.zeros(1, np.uint8)
-        self._check(self._lib.vpca_glm_logistic_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), nv,
+        self._check(self._lib.vpca_glm_logistic_bed(self._h, ptr, nv,
                                                     b.shape[1], int(counted), _host_ptr(out), _host_ptr(err),
                                                     _host_ptr(passes)))
         return out[:nv], err[:nv], passes[:nv]
@@ -936,22 +913,13 @@ class NativePca:
         return p[:nv]
 
     # -- sample QC (vpca.h, DESIGN.md 11) ----------------------------------------------------------------------------
-    @staticmethod
-    def _bed_rows(rows) -> np.ndarray:
-        b = np.asarray(rows)
-        if b.ndim != 2 or b.dtype != np.uint8 or not b.flags.c_contiguous:
-            b = np.ascontiguousarray(b, dtype=np.uint8)
-        if b.ndim != 2:
-            raise VpcaError(VPCA_ERR_BAD_ARG, "rows must be (nv, stride_bytes)")
-        return b
 
     def sampleMissingBed(self, rows: np.ndarray, n_samples: int) -> np.ndarray:
         """Missing calls of each of the n_samples samples of PLINK .bed rows ((V, stride) uint8; a .bed memmap is read in
         place, not copied) -> (n_samples,) int32.  The rows need not have this context's sample count.  Synchronises."""
-        b = self._bed_rows(rows)
+        b, ptr = _bed_rows(rows)
         out = np.zeros(max(int(n_samples), 1), np.int32)
-        empty = np.zeros(1, np.uint8)
-        self._check(self._lib.vpca_sample_missing_bed(self._h, b.ctypes.data if b.size else _host_ptr(empty), b.shape[0],
+        self._check(self._lib.vpca_sample_missing_bed(self._h, ptr, b.shape[0],
                                                       b.shape[1], int(n_samples), _host_ptr(out)))
         return out[:int(n_samples)]
 
@@ -959,15 +927,15 @@ class NativePca:
         """PLINK .bed rows of n_samples samples ((V, stride) uint8; a .bed memmap is read in place, not copied) repacked to
         the samples keep (strictly increasing indices) -> (V, ceil(M / 4)) uint8, the rows of a fileset of those samples.
         The rows need not have this context's sample count.  Synchronises."""
-        b = self._bed_rows(rows)
+        b, ptr = _bed_rows(rows)
         idx = np.ascontiguousarray(keep, dtype=np.int32).reshape(-1)
         m = len(idx)
         mb = (m + 3) // 4
         out = np.empty((b.shape[0], mb), np.uint8)
         empty = np.zeros(1, np.uint8)
         self._check(self._lib.vpca_subset_bed_samples(
-            self._h, b.ctypes.data if b.size else _host_ptr(empty), b.shape[0], b.shape[1], int(n_samples),
-            _host_ptr(idx) if m else None, m, out.ctypes.data if out.size else _host_ptr(empty), mb))
+            self._h, ptr, b.shape[0], b.shape[1], int(n_samples), _host_ptr(idx) if m else None, m,
+            out.ctypes.data if out.size else _host_ptr(empty), mb))
         return out
 
     def computePcaSubset(self, keep, k: int = 2):
@@ -1182,8 +1150,8 @@ class NativePcaPool:
         self._check(self._lib.vpca_pool_accumulate_bits(self._h, int(partition_id), _host_ptr(b), b.shape[0], b.shape[1]))
 
     def accumulateBed(self, partition_id: int, rows: np.ndarray, counted_allele: int = 1):
-        b = np.ascontiguousarray(rows, dtype=np.uint8)
-        self._check(self._lib.vpca_pool_accumulate_bed(self._h, int(partition_id), _host_ptr(b), b.shape[0], b.shape[1],
+        b, ptr = _bed_rows(rows)
+        self._check(self._lib.vpca_pool_accumulate_bed(self._h, int(partition_id), ptr, b.shape[0], b.shape[1],
                                                        int(counted_allele)))
 
     def commit(self, partition_id: int):

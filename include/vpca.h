@@ -524,7 +524,8 @@ enum {
     VPCA_GLM_CONST_ALLELE = 2,
     VPCA_GLM_VIF_INFINITE = 3,
     VPCA_GLM_NO_RESIDUAL = 4,
-    VPCA_GLM_LOGISTIC_CONVERGE_FAIL = 5
+    VPCA_GLM_LOGISTIC_CONVERGE_FAIL = 5,
+    VPCA_GLM_FIRTH_CONVERGE_FAIL = 6
 };
 #define VPCA_GLM_MAX_Q 32
 int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used);
@@ -560,6 +561,33 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
 int vpca_glm_logistic_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used);
 int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
                           double* out, int32_t* out_err, int32_t* out_passes);
+
+/* ---- Firth-penalized logistic tests (beyond VariantsPca.scala: PLINK 2's --glm firth-fallback / firth; DESIGN.md 17) --
+ * The model, samples, basis and start of the logistic tests above, maximising the penalized log-likelihood
+ * l*(theta) = l(theta) + log det(H(theta)) / 2 (H = X^T W X) instead of l.  It has a finite maximum where l has none, as
+ * when every carrier of a rare allele is a case.  Each pass evaluates l and H at a trial point, H = L L^T, and
+ * l* = l + sum log L_jj, then the Firth score U* = sum_i x_i (y_i - mu_i + h_i (1/2 - mu_i)), h_i = w_i ||L^-1 x_i||^2.
+ * A trial point theta_prev + t Delta is backtracked (t halved) when l is not finite, a pivot of H is <= 0 or l* fell by
+ * more than 1e-10 |l*_prev|, and by the secant t <- t s0 / (s0 - s1) when s1 = U*^T Delta < -0.45 s0, s0 = delta^2 at
+ * theta_prev; at most 30 backtracks in a row.  An accepted point takes z = L^-1 U*, delta^2 = z^T z, Delta = L^-T z, and
+ * stops at delta <= 1e-9, reporting BETA = beta + Delta_g and SE = 1 / L_gg (sqrt([H^-1]_gg) of the unpenalized
+ * information), Z = BETA / SE and P = erfc(|Z| / sqrt(2)); else the next trial point is at t = min(1, 5 / delta).  At most
+ * 100 passes, backtracked ones included.
+ * vpca_glm_firth_bed: as vpca_glm_logistic_bed (the same state, rows, chunks, outputs and argument rules), in one of two
+ *   modes:
+ *   VPCA_GLM_FIRTH_FALLBACK  the maximum-likelihood fit of vpca_glm_logistic_bed (the same bits), and the Firth fit, from
+ *                            the same start, of the variants it ends with VPCA_GLM_LOGISTIC_CONVERGE_FAIL after at least
+ *                            one pass.  A variant without a case or a control among its called samples keeps that code.
+ *   VPCA_GLM_FIRTH_ALWAYS    the Firth fit of every variant past the checks that come before the first pass.
+ *   The Firth fit's ERRCODE is VPCA_GLM_VIF_INFINITE by the first-pass rule of the logistic test, or
+ *   VPCA_GLM_FIRTH_CONVERGE_FAIL (100 passes, 30 backtracks in a row, or a non-finite l or step on the first pass or at
+ *   an accepted point).  out_passes[v] (may be NULL) = the passes of the fit reported; out_firth[v] (may be NULL) = 1
+ *   where the Firth fit ran.  A variant's Firth outputs depend on its row's codes, Q, y, the null fit and n_samples only,
+ *   and are the same bits in both modes.  VPCA_ERR_STATE without vpca_glm_logistic_begin state (after vpca_glm_begin
+ *   too); VPCA_ERR_BAD_ARG for a mode outside {1, 2}, besides the rules of vpca_glm_logistic_bed. */
+enum { VPCA_GLM_FIRTH_FALLBACK = 1, VPCA_GLM_FIRTH_ALWAYS = 2 };
+int vpca_glm_firth_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                       int32_t mode, double* out, int32_t* out_err, int32_t* out_passes, uint8_t* out_firth);
 
 /* ---- sample quality control (beyond VariantsPca.scala: which samples go into S; DESIGN.md 11) -------------------------
  * --keep / --remove / --mind decide the samples of a run before its context exists: the per-sample missing-call counts

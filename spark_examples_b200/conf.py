@@ -137,4 +137,7 @@ class PcaConf(GenomicsConf):
                                                           # covariates, written to P.<PHENO>.glm.linear
             ("glmLogistic", bool, False, False),          # with --glm: a case/control phenotype (1 control, 2 case) by
                                                           # logistic regression, written to P.<PHENO>.glm.logistic
+            ("glmFirth", str, None, False),               # with --glm --glm-logistic: fallback (Firth regression where
+                                                          # the plain fit fails; P.<PHENO>.glm.logistic.hybrid) or
+                                                          # always (P.<PHENO>.glm.firth)
         ]

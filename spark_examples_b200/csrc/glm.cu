@@ -745,18 +745,427 @@ __global__ void glm_logistic_finish_kernel(int nv, double* __restrict__ out, con
     o[5] = erfc(fabs(z) * 0.70710678118654752440);
 }
 
+// ---- Firth-penalized logistic regression (DESIGN.md 17) --------------------------------------------------------------
+constexpr int kFMaxPass = 100;         // passes (walk A, and walk B unless A backtracks) per variant
+constexpr int kFMaxBack = 30;          // backtracks in a row
+constexpr double kFMaxDelta = 5.0;     // the first trial point of a step lies at most this Newton decrement away
+constexpr double kFSecant = 0.45;      // the secant backtrack: U*^T Delta at the trial point < -kFSecant delta^2_prev
+
+// Shared memory of glm_firth_kernel, in doubles: the tile of Q and y as in LogLayout, and per warp a U tile (walk A:
+// rows [w q_0 .. w q_{q-1}, w g', 0 .., g'] as in glm_logistic_kernel; between the walks H, then L, then L^-1 over it at
+// pitch PH), theta, theta of the last accepted point, the step, the Firth score, 1 / L_jj (then z = L^-1 U*), the lanes'
+// partial l, and a tile's u and g' (walk B).
+template <int KMAX>
+struct FirthLayout {
+    static constexpr int LD = KMAX + 3;
+    static constexpr int PV = KMAX + 2;
+    static constexpr int PH = KMAX + 1;
+    static constexpr int NBK = (KMAX + 2) / 2;                    // 2 x 2 blocks per side of H (p <= KMAX + 1 rows)
+    static constexpr int NB = (NBK * (NBK + 1) / 2 + 31) / 32;    // lower-triangle blocks per lane
+    static constexpr int WARP = kLTile * LD + 5 * PV + 3 * 32;
+    static constexpr int TOTAL = kLTile * LD + kLWarps * WARP;
+    static_assert(PH * PH <= kLTile * LD, "H must fit in the U tile it takes over");
+};
+
+// grid ceil(nv / kLPerCta).  The variants to fit: list positions [0, nf) with nf = *d_nf (idx[i] the chunk's variant), or
+// with idx == nullptr every variant of the chunk (nf = nv); CTA c owns positions [c kLPerCta, (c + 1) kLPerCta).  cnt,
+// Qx, theta0 and out as glm_logistic_kernel.  Per variant, from (theta0, beta = 0), the passes of DESIGN.md 17: a warp is
+// in walk A (l and H at theta: glm_logistic_kernel's walk without the gradient row) or in walk B (the Firth score U* with
+// L^-1 in shared memory: lane l takes sample s0 + l, z = L^-1 x by independent FMA chains over the rows of L^-1, h =
+// w z^T z and u = y - mu + h (1/2 - mu), then lanes own the score's entries and add the 32 samples in order).  All warps
+// read the same staged tile whichever walk they are in; between walks a warp factors H, takes l* = l + sum log L_jj,
+// inverts L in place, or backtracks / steps (lane 0).  Writes out[v * 6 + 2 ..] = BETA, SE for ERRCODE `.`, err[v],
+// passes[v] and firth[v] = 1 where a pass ran, 0 where the ERRCODE came before any.  A sample outside A_v adds exactly 0
+// to every sum, so a variant's outputs depend on its row's codes, Q, y, theta0, the mask and n only.
+template <int KMAX>
+__global__ void __launch_bounds__(kLWarps * 32, 2) glm_firth_kernel(const uint8_t* __restrict__ rows, int64_t stride,
+                                                                   int nv, int n, int q, const double* __restrict__ Qx,
+                                                                   const double* __restrict__ theta0, uint32_t lut,
+                                                                   const double* __restrict__ cnt,
+                                                                   const int32_t* __restrict__ idx,
+                                                                   const int32_t* __restrict__ d_nf,
+                                                                   double* __restrict__ out, int32_t* __restrict__ err,
+                                                                   int32_t* __restrict__ passes,
+                                                                   uint8_t* __restrict__ firth) {
+    using Lo = FirthLayout<KMAX>;
+    constexpr int LD = Lo::LD, PV = Lo::PV, PH = Lo::PH, NB = Lo::NB;
+    extern __shared__ __align__(16) double fsm[];
+    __shared__ int sst[kLWarps][5];      // variant (-1: none), passes so far, backtracks in a row, centre, walk (0 A, 1 B)
+    __shared__ int sflag[kLWarps];
+    __shared__ double sdp[kLWarps][4];   // l* of the last accepted point, l* of this point, s0 = its delta^2, t
+    __shared__ int snext, sany;
+    const int nf = idx ? *d_nf : nv;
+    const int p0 = blockIdx.x * kLPerCta;
+    if (p0 >= nf) return;   // the whole CTA
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double* const Qt = fsm;
+    const int uoff = kLTile * LD + w * Lo::WARP;
+    double* const U = fsm + uoff;
+    double* const H = U;
+    double* const th = U + kLTile * LD;
+    double* const thp = th + PV;
+    double* const del = thp + PV;
+    double* const grad = del + PV;
+    double* const sr = grad + PV;
+    double* const lpart = sr + PV;
+    double* const su = lpart + 32;
+    double* const sg = su + 32;
+    const int p = q + 1;
+    const int nblk = (p + 1) / 2;   // 2 x 2 blocks per side over rows 0 .. p - 1
+    const int nblocks = nblk * (nblk + 1) / 2;
+    int ba[NB], bb[NB], xo[NB][2];
+#pragma unroll
+    for (int j = 0; j < NB; ++j) {
+        const int t = lane + 32 * j;
+        int I = 0;
+        while ((I + 1) * (I + 2) / 2 <= t) ++I;
+        ba[j] = 2 * I;
+        bb[j] = 2 * (t - I * (I + 1) / 2);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int b = bb[j] + e;
+            xo[j][e] = b < q ? b : b == q ? uoff + KMAX + 2 : KMAX + 2;
+        }
+    }
+    const int p_end = min(nf, p0 + kLPerCta);
+    if (threadIdx.x == 0) snext = p0;
+    if (lane == 0) sst[w][0] = -1;
+    const int nt = (n + kLTile - 1) / kLTile;
+    for (;;) {
+        __syncthreads();   // every warp's decision of the last walk is in sst
+        if (threadIdx.x == 0) {
+            int any = 0;
+            for (int ww = 0; ww < kLWarps; ++ww) {
+                while (sst[ww][0] < 0 && snext < p_end) {
+                    const int v = idx ? idx[snext] : snext;
+                    ++snext;
+                    const double* c = cnt + (int64_t)v * 6;
+                    const int obs = (int)c[0], sg_ = (int)c[1], gg = (int)c[2], cases = (int)c[3];
+                    double* o = out + (int64_t)v * 6;
+                    o[0] = obs;
+                    o[1] = sg_;   // glm_logistic_finish_kernel divides
+                    const int e = obs - q - 1 < 1                              ? VPCA_GLM_TOO_FEW_OBS
+                                  : (int64_t)obs * gg == (int64_t)sg_ * sg_    ? VPCA_GLM_CONST_ALLELE
+                                  : cases == 0 || cases == obs                 ? VPCA_GLM_LOGISTIC_CONVERGE_FAIL
+                                                                               : VPCA_GLM_OK;
+                    firth[v] = e == VPCA_GLM_OK;
+                    if (e != VPCA_GLM_OK) {
+                        err[v] = e;
+                        passes[v] = 0;
+                        continue;
+                    }
+                    sst[ww][0] = v;
+                    sst[ww][1] = 0;
+                    sst[ww][2] = 0;
+                    sst[ww][3] = glm_centre(obs, sg_);
+                    sst[ww][4] = 0;
+                }
+                any |= sst[ww][0] >= 0;
+            }
+            sany = any;
+        }
+        __syncthreads();
+        if (!sany) break;
+        const int v = sst[w][0];
+        const bool act = v >= 0;   // uniform over the warp
+        const bool walk_b = act && sst[w][4] == 1;
+        if (act && sst[w][1] == 0)
+            for (int c = lane; c < PV; c += 32) th[c] = c < q ? theta0[c] : 0.0;
+        __syncwarp();
+        const uint8_t* row = rows + (int64_t)(act ? v : 0) * stride;
+        const int cen = act ? sst[w][3] : 0;
+        double acc[NB][4];
+#pragma unroll
+        for (int j = 0; j < NB; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.0;
+        double gacc0 = 0.0, gacc1 = 0.0;   // walk B: score entries lane and lane + 32
+        double lsum = 0.0;
+#pragma unroll 1
+        for (int t = 0; t < nt; ++t) {
+            const int s0 = t * kLTile;
+            __syncthreads();   // every warp is done with the previous tile
+            for (int i = threadIdx.x; i < kLTile * LD; i += kLWarps * 32) {
+                const int r = i / LD, c = i - r * LD, s = s0 + r;
+                Qt[i] = (c < KMAX + 2 && s < n) ? Qx[(int64_t)s * (KMAX + 2) + c] : 0.0;
+            }
+            __syncthreads();
+            if (!act) continue;
+            const int s = s0 + lane;
+            const double* x = Qt + lane * LD;
+            const uint32_t code = s < n ? (row[s >> 2] >> (2 * (s & 3))) & 3u : 1u;
+            const bool in = x[KMAX + 1] != 0.0 && code != 1u;
+            const double g = in ? (double)((int)((lut >> (2 * code)) & 3u) - cen) : 0.0;
+            double eta = 0.0;
+            for (int c = 0; c < q; ++c) eta = fma(x[c], th[c], eta);
+            eta = fma(th[q], g, eta);
+            double wt = 0.0, mu = 0.0, e = 0.0;
+            if (in) {
+                e = exp(-fabs(eta));
+                const double rd = recip_newton(1.0 + e);
+                mu = eta >= 0.0 ? rd : e * rd;
+                wt = e * rd * rd;
+            }
+            if (!walk_b) {
+                if (in) {
+                    const double m = x[q] != 0.0 ? -eta : eta;   // l_s = y eta - log(1 + e^eta) = -softplus(m)
+                    lsum -= fmax(m, 0.0) + log1p(e);
+                }
+                double* u = U + lane * LD;
+                for (int c = 0; c < q; ++c) u[c] = wt * x[c];
+                u[q] = wt * g;
+                for (int c = p; c < 2 * nblk; ++c) u[c] = 0.0;
+                u[KMAX + 2] = g;
+                __syncwarp();
+#pragma unroll 2
+                for (int r = 0; r < kLTile; ++r) {
+                    const double* ur = U + r * LD;
+#pragma unroll
+                    for (int j = 0; j < NB; ++j) {
+                        if (lane + 32 * j >= nblocks) continue;
+                        const double u0 = ur[ba[j]], u1 = ur[ba[j] + 1];
+                        const double x0 = fsm[xo[j][0] + r * LD], x1 = fsm[xo[j][1] + r * LD];
+                        acc[j][0] = fma(u0, x0, acc[j][0]);
+                        acc[j][1] = fma(u0, x1, acc[j][1]);
+                        acc[j][2] = fma(u1, x0, acc[j][2]);
+                        acc[j][3] = fma(u1, x1, acc[j][3]);
+                    }
+                }
+            } else {
+                double uu = 0.0;
+                if (in) {
+                    // h = w ||L^-1 x||^2, one FMA chain per row of L^-1 (H holds L^-1)
+                    double hh = 0.0;
+                    for (int j = 0; j < q; ++j) {
+                        const double* li = H + j * PH;
+                        double z = 0.0;
+                        for (int k = 0; k <= j; ++k) z = fma(li[k], x[k], z);
+                        hh = fma(z, z, hh);
+                    }
+                    {
+                        const double* li = H + q * PH;
+                        double z = 0.0;
+                        for (int k = 0; k < q; ++k) z = fma(li[k], x[k], z);
+                        z = fma(li[q], g, z);
+                        hh = fma(z, z, hh);
+                    }
+                    uu = fma(wt * hh, 0.5 - mu, x[q] - mu);
+                }
+                su[lane] = uu;
+                sg[lane] = g;
+                __syncwarp();
+                const int c1 = lane + 32;
+#pragma unroll 2
+                for (int r = 0; r < kLTile; ++r) {
+                    const double ur = su[r];
+                    if (lane < p) gacc0 = fma(ur, lane < q ? Qt[r * LD + lane] : sg[r], gacc0);
+                    if (c1 < p) gacc1 = fma(ur, c1 < q ? Qt[r * LD + c1] : sg[r], gacc1);
+                }
+            }
+            __syncwarp();
+        }
+        if (!act) continue;
+        if (!walk_b) {
+            // H (lower triangle, pitch PH, over the U tile) from the blocks; each entry has one owner
+#pragma unroll
+            for (int j = 0; j < NB; ++j) {
+                if (lane + 32 * j >= nblocks) continue;
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int a = ba[j] + (e >> 1), b = bb[j] + (e & 1);
+                    if (a >= p || a < b) continue;
+                    H[a * PH + b] = acc[j][e];
+                }
+            }
+            lpart[lane] = lsum;
+            __syncwarp();
+            if (lane == 0) {
+                double l = 0.0;
+                for (int i = 0; i < 32; ++i) l += lpart[i];
+                sdp[w][1] = l;
+                ++sst[w][1];
+                sflag[w] = isfinite(l) ? 0 : 2;   // 0: factor H; 2: not finite
+            }
+            __syncwarp();
+            const int k = sst[w][1];
+            const bool first = k == 1;
+            double ldet = 0.0;   // lane 0: sum log L_jj = sum log(pivot) / 2, in column order
+            if (sflag[w] == 0) {
+                // Cholesky H = L L^T as glm_logistic_kernel.  First pass: a pivot <= kPivotMin H_jj is VIF_INFINITE (3);
+                // later a pivot <= 0 backtracks (2).
+                for (int j = 0; j < p; ++j) {
+                    if (lane == 0) {
+                        const double hjj = H[j * PH + j];
+                        double d = hjj;
+                        for (int c = 0; c < j; ++c) d = fma(-H[j * PH + c], H[j * PH + c], d);
+                        const bool ok = first ? d > kPivotMin * hjj : d > 0.0;
+                        sr[j] = ok ? rsqrt_newton(d) : 0.0;
+                        if (ok) ldet += 0.5 * log(d);
+                        sflag[w] = ok ? 0 : first ? 3 : 2;
+                    }
+                    __syncwarp();
+                    if (sflag[w] != 0) break;
+                    for (int i = j + 1 + lane; i < p; i += 32) {
+                        double x = H[i * PH + j];
+                        for (int c = 0; c < j; ++c) x = fma(-H[i * PH + c], H[j * PH + c], x);
+                        H[i * PH + j] = x * sr[j];
+                    }
+                    __syncwarp();
+                }
+            }
+            if (lane == 0) {
+                int fl = sflag[w];
+                const double ls = sdp[w][1] + ldet;
+                sdp[w][1] = ls;
+                if (first) {
+                    if (fl != 0) fl = fl == 3 ? 3 : 4;   // 4: FIRTH_CONVERGE_FAIL
+                } else if (fl != 0 || ls < sdp[w][0] - kLFall * fabs(sdp[w][0])) {
+                    // halve the step
+                    if (sst[w][2] == kFMaxBack || k == kFMaxPass) {
+                        fl = 4;
+                    } else {
+                        ++sst[w][2];
+                        const double t = 0.5 * sdp[w][3];
+                        sdp[w][3] = t;
+                        for (int c = 0; c < p; ++c) th[c] = __dadd_rn(thp[c], __dmul_rn(t, del[c]));
+                        fl = 1;
+                    }
+                }
+                if (fl >= 3) {
+                    err[v] = fl == 3 ? VPCA_GLM_VIF_INFINITE : VPCA_GLM_FIRTH_CONVERGE_FAIL;
+                    passes[v] = k;
+                    sst[w][0] = -1;
+                } else if (fl == 0) {
+                    sst[w][4] = 1;
+                }
+                sflag[w] = fl;
+            }
+            __syncwarp();
+            if (sflag[w] == 0) {
+                // L^-1 in place by rows: row i of L^-1 from row i of L and the rows of L^-1 above it
+                for (int i = 0; i < p; ++i) {
+                    double x = 0.0;
+                    if (lane < i) {
+                        for (int c = lane; c < i; ++c) x = fma(H[i * PH + c], H[c * PH + lane], x);
+                        x = -x * sr[i];
+                    }
+                    __syncwarp();
+                    if (lane < i) H[i * PH + lane] = x;
+                    if (lane == (i & 31)) H[i * PH + i] = sr[i];
+                    __syncwarp();
+                }
+            }
+        } else {
+            if (lane < p) grad[lane] = gacc0;
+            if (lane + 32 < p) grad[lane + 32] = gacc1;
+            __syncwarp();
+            if (lane == 0) {
+                const int k = sst[w][1];
+                bool done = false;
+                sst[w][4] = 0;
+                double s1 = 0.0;
+                if (k > 1)
+                    for (int c = 0; c < p; ++c) s1 = fma(grad[c], del[c], s1);
+                const double s0 = sdp[w][2];
+                if (k > 1 && s1 < -kFSecant * s0) {
+                    // the secant on the directional derivative of l* along the step
+                    if (sst[w][2] == kFMaxBack || k == kFMaxPass) {
+                        err[v] = VPCA_GLM_FIRTH_CONVERGE_FAIL;
+                        passes[v] = k;
+                        done = true;
+                    } else {
+                        ++sst[w][2];
+                        const double t = sdp[w][3] * s0 / (s0 - s1);
+                        sdp[w][3] = t;
+                        for (int c = 0; c < p; ++c) th[c] = __dadd_rn(thp[c], __dmul_rn(t, del[c]));
+                    }
+                } else {
+                    // z = L^-1 U* (over sr), delta^2 = z^T z, the step L^-T z
+                    double dd = 0.0;
+                    for (int i = 0; i < p; ++i) {
+                        double z = 0.0;
+                        for (int c = 0; c <= i; ++c) z = fma(H[i * PH + c], grad[c], z);
+                        sr[i] = z;
+                        dd = fma(z, z, dd);
+                    }
+                    for (int j = 0; j < p; ++j) {
+                        double x = 0.0;
+                        for (int i = j; i < p; ++i) x = fma(H[i * PH + j], sr[i], x);
+                        del[j] = x;
+                    }
+                    if (!isfinite(dd) || (dd > kLDelta2 && k == kFMaxPass)) {
+                        err[v] = VPCA_GLM_FIRTH_CONVERGE_FAIL;
+                        passes[v] = k;
+                        done = true;
+                    } else if (dd <= kLDelta2) {
+                        double* o = out + (int64_t)v * 6;
+                        o[2] = th[q] + del[q];
+                        o[3] = H[q * PH + q];   // 1 / L_gg
+                        err[v] = VPCA_GLM_OK;
+                        passes[v] = k;
+                        done = true;
+                    } else {
+                        const double t = dd > kFMaxDelta * kFMaxDelta ? kFMaxDelta / sqrt(dd) : 1.0;
+                        sdp[w][0] = sdp[w][1];
+                        sdp[w][2] = dd;
+                        sdp[w][3] = t;
+                        sst[w][2] = 0;
+                        for (int c = 0; c < p; ++c) {
+                            thp[c] = th[c];
+                            th[c] = __dadd_rn(thp[c], __dmul_rn(t, del[c]));
+                        }
+                    }
+                }
+                if (done) sst[w][0] = -1;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// The variants a fallback refits: those the maximum-likelihood kernel ended with LOGISTIC_CONVERGE_FAIL after at least
+// one pass, into idx[0 .. *nf) (in any order: a variant's outputs do not depend on its place); firth[v] = 0 elsewhere.
+__global__ void glm_firth_select_kernel(int nv, const int32_t* __restrict__ err, const int32_t* __restrict__ passes,
+                                        uint8_t* __restrict__ firth, int32_t* __restrict__ idx, int32_t* __restrict__ nf) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= nv) return;
+    const bool f = err[v] == VPCA_GLM_LOGISTIC_CONVERGE_FAIL && passes[v] > 0;
+    firth[v] = f;
+    if (f) idx[atomicAdd(nf, 1)] = v;
+}
+
+// firth_mode 0: the maximum-likelihood fit alone; VPCA_GLM_FIRTH_FALLBACK: then the Firth fit of the variants it could
+// not fit; VPCA_GLM_FIRTH_ALWAYS: the Firth fit alone.  d_firth, d_idx, d_nf: unused in mode 0.
 template <int KMAX>
 cudaError_t launch_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
                             const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, uint32_t lut,
-                            double* d_cnt, double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream) {
+                            double* d_cnt, double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode,
+                            uint8_t* d_firth, int32_t* d_idx, int32_t* d_nf, cudaStream_t stream) {
     const unsigned cgrid = (unsigned)((nv + kCThreads / 32 - 1) / (kCThreads / 32));
+    const unsigned lgrid = (unsigned)((nv + kLPerCta - 1) / kLPerCta);
     glm_count_kernel<<<cgrid, kCThreads, 0, stream>>>(d_rows, stride, nv, n, d_mask, lut == kLutA2, d_cnt, 6);
     glm_count_kernel<<<cgrid, kCThreads, 0, stream>>>(d_rows, stride, nv, n, d_case, lut == kLutA2, d_cnt + 3, 6);
-    const size_t smem = LogLayout<KMAX>::TOTAL * sizeof(double);
-    cudaError_t e = cudaFuncSetAttribute(glm_logistic_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    glm_logistic_kernel<KMAX><<<(unsigned)((nv + kLPerCta - 1) / kLPerCta), kLWarps * 32, smem, stream>>>(
-        d_rows, stride, nv, n, q, d_Qx, d_theta0, lut, d_cnt, d_out, d_err, d_passes);
+    cudaError_t e = cudaSuccess;
+    if (firth_mode != VPCA_GLM_FIRTH_ALWAYS) {
+        const size_t smem = LogLayout<KMAX>::TOTAL * sizeof(double);
+        e = cudaFuncSetAttribute(glm_logistic_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        glm_logistic_kernel<KMAX><<<lgrid, kLWarps * 32, smem, stream>>>(d_rows, stride, nv, n, q, d_Qx, d_theta0, lut,
+                                                                          d_cnt, d_out, d_err, d_passes);
+    }
+    if (firth_mode != 0) {
+        const bool fallback = firth_mode == VPCA_GLM_FIRTH_FALLBACK;
+        if (fallback) {
+            e = cudaMemsetAsync(d_nf, 0, sizeof(int32_t), stream);
+            if (e != cudaSuccess) return e;
+            glm_firth_select_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, stream>>>(nv, d_err, d_passes, d_firth,
+                                                                                      d_idx, d_nf);
+        }
+        const size_t smem = FirthLayout<KMAX>::TOTAL * sizeof(double);
+        e = cudaFuncSetAttribute(glm_firth_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        glm_firth_kernel<KMAX><<<lgrid, kLWarps * 32, smem, stream>>>(d_rows, stride, nv, n, q, d_Qx, d_theta0, lut,
+                                                                       d_cnt, fallback ? d_idx : nullptr, d_nf, d_out,
+                                                                       d_err, d_passes, d_firth);
+    }
     glm_logistic_finish_kernel<<<(unsigned)((nv + 127) / 128), 128, 0, stream>>>(nv, d_out, d_err);
     return cudaSuccess;
 }
@@ -780,9 +1189,10 @@ cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int
     return cudaGetLastError();
 }
 
-cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
-                         const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
-                         double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream) {
+cudaError_t glm_firth(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
+                      const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
+                      double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode, uint8_t* d_firth, int32_t* d_idx,
+                      int32_t* d_nf, cudaStream_t stream) {
     if (nv <= 0) return cudaSuccess;
     const uint32_t lut = counted == 2 ? kLutA2 : kLutA1;
     cudaError_t e;
@@ -790,17 +1200,24 @@ cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, i
 #define VPCA_GLM_LOGISTIC(K)                                                                                              \
     case K:                                                                                                               \
         e = launch_logistic<K>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt, d_out, d_err,       \
-                               d_passes, stream);                                                                         \
+                               d_passes, firth_mode, d_firth, d_idx, d_nf, stream);                                       \
         break;
         VPCA_GLM_LOGISTIC(2)
         VPCA_GLM_LOGISTIC(4)
         VPCA_GLM_LOGISTIC(8)
         VPCA_GLM_LOGISTIC(16)
         default: e = launch_logistic<32>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt, d_out,
-                                         d_err, d_passes, stream);
+                                         d_err, d_passes, firth_mode, d_firth, d_idx, d_nf, stream);
 #undef VPCA_GLM_LOGISTIC
     }
     return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
+                         const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
+                         double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream) {
+    return glm_firth(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, counted, d_cnt, d_out, d_err, d_passes, 0,
+                     nullptr, nullptr, nullptr, stream);
 }
 
 }  // namespace vpca

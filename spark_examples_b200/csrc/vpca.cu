@@ -125,8 +125,10 @@ struct vpca_ctx {
     // The logistic tests (vpca_glm_logistic_*) keep y in place of y~, the null fit in d_glm_z0, the cases as bits in
     // d_glm_case, the counts in d_glm_sums and the passes in d_glm_passes.
     DeviceBuffer<double> d_glm_Qx, d_glm_z0, d_glm_sums, d_glm_out;
-    DeviceBuffer<uint8_t> d_glm_mask, d_glm_case;
-    DeviceBuffer<int32_t> d_glm_err, d_glm_passes;
+    // The Firth tests (vpca_glm_firth_bed) add the chunk's Firth flags, and for a fallback the list of the variants to
+    // refit and its length, built on the device.
+    DeviceBuffer<uint8_t> d_glm_mask, d_glm_case, d_glm_firth;
+    DeviceBuffer<int32_t> d_glm_err, d_glm_passes, d_glm_idx, d_glm_nf;
     int glm_q = 0;          // 0: no GLM state
     int glm_logistic = 0;   // the model of the GLM state: 0 linear (vpca_glm_begin), 1 logistic
     int glm_nreg = 0;       // regression samples
@@ -2791,23 +2793,24 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
     });
 }
 
-int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
-                          double* out, int32_t* out_err, int32_t* out_passes) {
-    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    int rc = rows_args(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4,
-                       out != nullptr && out_err != nullptr);
+namespace {
+// vpca_glm_logistic_bed (firth_mode 0) and vpca_glm_firth_bed: the argument and state rules, then the rows through
+// stage_rows with glm_firth's kernels per chunk.
+int glm_logistic_rows(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
+                      int32_t counted_allele, int firth_mode, double* out, int32_t* out_err, int32_t* out_passes,
+                      uint8_t* out_firth) {
+    int rc = rows_args(ctx, fn, rows, nv, stride_bytes, (ctx->n + 3) / 4, out != nullptr && out_err != nullptr);
     if (rc != VPCA_OK) return rc;
     if (counted_allele != 1 && counted_allele != 2)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_logistic_bed: counted_allele must be 1 (A1) or 2 (A2), not %d",
-                    counted_allele);
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: counted_allele must be 1 (A1) or 2 (A2), not %d", fn, counted_allele);
     int q = 0;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         if (ctx->glm_q == 0)
-            return fail(ctx, VPCA_ERR_STATE, "vpca_glm_logistic_bed needs a vpca_glm_logistic_begin since the last reset");
+            return fail(ctx, VPCA_ERR_STATE, "%s needs a vpca_glm_logistic_begin since the last reset", fn);
         if (!ctx->glm_logistic)
-            return fail(ctx, VPCA_ERR_STATE, "vpca_glm_logistic_bed: the GLM state is linear (vpca_glm_begin); a "
-                        "logistic test needs vpca_glm_logistic_begin");
+            return fail(ctx, VPCA_ERR_STATE, "%s: the GLM state is linear (vpca_glm_begin); a logistic test needs "
+                        "vpca_glm_logistic_begin", fn);
         q = ctx->glm_q;
     }
     CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
@@ -2824,15 +2827,21 @@ int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_
         if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
         if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
         if (e == cudaSuccess) e = ctx->d_glm_passes.ensure(step);
+        if (e == cudaSuccess && firth_mode) e = ctx->d_glm_firth.ensure(step);
+        if (e == cudaSuccess && firth_mode == VPCA_GLM_FIRTH_FALLBACK) e = ctx->d_glm_idx.ensure(step);
+        if (e == cudaSuccess && firth_mode == VPCA_GLM_FIRTH_FALLBACK) e = ctx->d_glm_nf.ensure(1);
         if (e != cudaSuccess) {
             cudaGetLastError();
             return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
         }
     }
+    const bool fallback = firth_mode == VPCA_GLM_FIRTH_FALLBACK;
     return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
-        CUDA_OK(ctx, glm_logistic(d_rows, stride_bytes, (int)nvc, n, q, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
-                                  ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele, ctx->d_glm_sums.get(),
-                                  ctx->d_glm_out.get(), ctx->d_glm_err.get(), ctx->d_glm_passes.get(), L.stream));
+        CUDA_OK(ctx, glm_firth(d_rows, stride_bytes, (int)nvc, n, q, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
+                               ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele, ctx->d_glm_sums.get(),
+                               ctx->d_glm_out.get(), ctx->d_glm_err.get(), ctx->d_glm_passes.get(), firth_mode,
+                               firth_mode ? ctx->d_glm_firth.get() : nullptr, fallback ? ctx->d_glm_idx.get() : nullptr,
+                               fallback ? ctx->d_glm_nf.get() : nullptr, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
                                      cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
@@ -2840,10 +2849,33 @@ int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_
         if (out_passes)
             CUDA_OK(ctx, cudaMemcpyAsync(out_passes + v, ctx->d_glm_passes.get(), (size_t)nvc * sizeof(int32_t),
                                          cudaMemcpyDeviceToHost, L.stream));
-        ctx->c_launches += 5;
-        ctx->c_d2h += nvc * (6 * (int64_t)sizeof(double) + (out_passes ? 2 : 1) * (int64_t)sizeof(int32_t));
+        if (out_firth)
+            CUDA_OK(ctx, cudaMemcpyAsync(out_firth + v, ctx->d_glm_firth.get(), (size_t)nvc, cudaMemcpyDeviceToHost,
+                                         L.stream));
+        // count kernels, then the maximum-likelihood and finish kernels (5 as counted before the Firth tests), the
+        // selection and the Firth kernel (fallback), or the Firth and finish kernels (always)
+        ctx->c_launches += firth_mode == 0 ? 5 : fallback ? 6 : 4;
+        ctx->c_d2h += nvc * (6 * (int64_t)sizeof(double) + (out_passes ? 2 : 1) * (int64_t)sizeof(int32_t) +
+                             (out_firth ? 1 : 0));
         return VPCA_OK;
     });
+}
+}  // namespace
+
+int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                          double* out, int32_t* out_err, int32_t* out_passes) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    return glm_logistic_rows(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, counted_allele, 0, out, out_err,
+                             out_passes, nullptr);
+}
+
+int vpca_glm_firth_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                       int32_t mode, double* out, int32_t* out_err, int32_t* out_passes, uint8_t* out_firth) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    if (mode != VPCA_GLM_FIRTH_FALLBACK && mode != VPCA_GLM_FIRTH_ALWAYS)
+        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_firth_bed: mode must be 1 (fallback) or 2 (always), not %d", mode);
+    return glm_logistic_rows(ctx, "vpca_glm_firth_bed", rows, nv, stride_bytes, counted_allele, mode, out, out_err,
+                             out_passes, out_firth);
 }
 
 // ---- sample QC (samples.cu, DESIGN.md 11) -------------------------------------------------------------------------------

@@ -270,6 +270,13 @@ cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int
 cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
                          const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
                          double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream);
+// Firth tests (DESIGN.md 17): glm_logistic with firth_mode VPCA_GLM_FIRTH_FALLBACK (then the Firth fit of the variants the
+// maximum-likelihood fit ends with LOGISTIC_CONVERGE_FAIL after a pass, listed on the device in d_idx (nv) and d_nf (1))
+// or VPCA_GLM_FIRTH_ALWAYS (the Firth fit alone); d_firth[v] (nv) = 1 where the Firth fit ran.  Never synchronises.
+cudaError_t glm_firth(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
+                      const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
+                      double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode, uint8_t* d_firth, int32_t* d_idx,
+                      int32_t* d_nf, cudaStream_t stream);
 
 // ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
 // Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to

@@ -56,7 +56,7 @@ EXPORTED_SYMBOLS = (
     "vpca_ld_prune_bed_masked", "vpca_variant_qc_bed", "vpca_hwe_exact", "vpca_sample_missing_bed",
     "vpca_subset_bed_samples", "vpca_debug_device_bytes", "vpca_grm_bed", "vpca_grm_finalize", "vpca_get_grm",
     "vpca_compute_pca_grm", "vpca_grm_loadings_bed", "vpca_grm_project_bed", "vpca_glm_begin", "vpca_glm_linear_bed",
-    "vpca_glm_logistic_begin", "vpca_glm_logistic_bed",
+    "vpca_glm_logistic_begin", "vpca_glm_logistic_bed", "vpca_glm_firth_bed",
 )
 
 KINSHIP_MAX_SAMPLES = 21845   # vpca_kinship_*: the 3N x 3N plane Gram stays below 2^32 cells
@@ -64,7 +64,8 @@ LD_MAX_WINDOW = 4096          # vpca_ld_prune_bed: variants a window may reach b
 GRM_MAX_SAMPLES = 65535       # vpca_grm_* / vpca_compute_pca_grm: the sample limit of vpca_compute_pca
 GLM_MAX_Q = 32                # vpca_glm_begin: covariate columns, the intercept included
 GLM_ERRCODES = (".", "TOO_FEW_OBS", "CONST_ALLELE", "VIF_INFINITE", "NO_RESIDUAL",
-                "LOGISTIC_CONVERGE_FAIL")   # by VPCA_GLM_* value
+                "LOGISTIC_CONVERGE_FAIL", "FIRTH_CONVERGE_FAIL")   # by VPCA_GLM_* value
+GLM_FIRTH_MODES = {"fallback": 1, "always": 2}   # vpca_glm_firth_bed: VPCA_GLM_FIRTH_FALLBACK, VPCA_GLM_FIRTH_ALWAYS
 
 
 class VpcaError(RuntimeError):
@@ -322,6 +323,8 @@ def load_library() -> ctypes.CDLL:
     L.vpca_glm_logistic_begin.argtypes = [vp, vp, vp, i32, ctypes.POINTER(i64)]
     L.vpca_glm_logistic_bed.restype = ctypes.c_int
     L.vpca_glm_logistic_bed.argtypes = [vp, vp, i64, i64, i32, vp, vp, vp]
+    L.vpca_glm_firth_bed.restype = ctypes.c_int
+    L.vpca_glm_firth_bed.argtypes = [vp, vp, i64, i64, i32, i32, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -902,6 +905,24 @@ class NativePca:
                                                     b.shape[1], int(counted), _host_ptr(out), _host_ptr(err),
                                                     _host_ptr(passes)))
         return out[:nv], err[:nv], passes[:nv]
+
+    # -- Firth-penalized logistic tests (vpca.h, DESIGN.md 17) -----------------------------------------------------------
+    def glmFirthBed(self, rows: np.ndarray, counted: int = 1, mode: str = "fallback"):
+        """Logistic tests with Firth's penalized likelihood of PLINK .bed rows (as glmLogisticBed, on the state of
+        glmLogisticBegin).  mode "fallback": the maximum-likelihood fit, and the Firth fit where it does not converge;
+        "always": the Firth fit of every variant -> (stats (V, 6), err (V,), passes (V,) of the fit reported, firth (V,)
+        uint8: 1 where the Firth fit ran).  Synchronises."""
+        if mode not in GLM_FIRTH_MODES:
+            raise VpcaError(VPCA_ERR_BAD_ARG, f"mode must be one of {', '.join(GLM_FIRTH_MODES)}, not {mode!r}")
+        b, ptr = _bed_rows(rows)
+        nv = b.shape[0]
+        out = np.zeros((max(nv, 1), 6), np.float64)
+        err = np.zeros(max(nv, 1), np.int32)
+        passes = np.zeros(max(nv, 1), np.int32)
+        firth = np.zeros(max(nv, 1), np.uint8)
+        self._check(self._lib.vpca_glm_firth_bed(self._h, ptr, nv, b.shape[1], int(counted), GLM_FIRTH_MODES[mode],
+                                                 _host_ptr(out), _host_ptr(err), _host_ptr(passes), _host_ptr(firth)))
+        return out[:nv], err[:nv], passes[:nv], firth[:nv]
 
     def hweExact(self, counts) -> np.ndarray:
         """Exact HWE p-values of (V, 4) int32 counts (HOM_A1, HET, HOM_A2, MISSING; MISSING ignored) -> (V,) float64."""

@@ -731,18 +731,24 @@ class VariantsPcaDriver:
 
     def glmLogistic(self, callsets: CallsRdd, glm: "GlmInput", qc_keep: Optional[np.ndarray] = None):
         """glmLinear's logistic counterpart (DESIGN.md 16) for a case/control phenotype: writes P.<PHENO>.glm.logistic
-        and prints the `GLM logistic:` line.  Returns (stats (V, 6), err (V,), passes (V,))."""
+        and prints the `GLM logistic:` line.  Returns (stats (V, 6), err (V,), passes (V,)).  With --glm-firth
+        (DESIGN.md 17): fallback writes P.<PHENO>.glm.logistic.hybrid with the FIRTH? column and counts the Firth fits in
+        the line; always writes P.<PHENO>.glm.firth and prints `GLM Firth:`."""
         from . import plink
         pcs = np.asarray(self.components, np.float64)
         k = pcs.shape[1]
         nat = self._native(callsets.n_samples)
         used = nat.glmLogisticBegin(glm.y, np.concatenate([pcs, glm.c], axis=1))
-        stats, errs, passes, tested = [], [], [], []
+        stats, errs, passes, firths, tested = [], [], [], [], []
         counted = plink.COUNT_A1
         for part in callsets.partitions:
             sel = np.ones(part.nv, bool) if qc_keep is None else np.asarray(qc_keep[part.v0:part.v0 + part.nv], bool)
             rows = part.bed._map[part.v0:part.v0 + part.nv]        # read in place when every variant is tested
-            st, er, ps = nat.glmLogisticBed(rows if sel.all() else rows[sel], part.counted)
+            if glm.firth:
+                st, er, ps, fi = nat.glmFirthBed(rows if sel.all() else rows[sel], part.counted, glm.firth)
+                firths.append(np.asarray(fi, np.uint8).reshape(-1))
+            else:
+                st, er, ps = nat.glmLogisticBed(rows if sel.all() else rows[sel], part.counted)
             stats.append(np.asarray(st, np.float64).reshape(-1, 6))
             errs.append(np.asarray(er, np.int32).reshape(-1))
             passes.append(np.asarray(ps, np.int32).reshape(-1))
@@ -752,16 +758,25 @@ class VariantsPcaDriver:
         errs = np.concatenate(errs) if errs else np.zeros(0, np.int32)
         passes = np.concatenate(passes) if passes else np.zeros(0, np.int32)
         bim = plink.read_bim(self.conf.bedPath())
-        write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.glm.logistic", [bim[j] for j in tested], counted, stats,
-                           errs)
+        firths = np.concatenate(firths) if firths else np.zeros(0, np.uint8)
+        fitted = ""
+        if glm.firth == "fallback":
+            write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.glm.logistic.hybrid", [bim[j] for j in tested],
+                               counted, stats, errs, firths)
+            fitted = f", {int(np.count_nonzero(firths))} fitted by Firth regression"
+        else:
+            ext = "glm.firth" if glm.firth == "always" else "glm.logistic"
+            write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.{ext}", [bim[j] for j in tested], counted, stats,
+                               errs)
         n = callsets.n_samples
         c = glm.c.shape[1]
         reg = np.isfinite(glm.y) & np.isfinite(glm.c).all(axis=1)
         cases = int(np.count_nonzero(glm.y[reg] == 1.0))
         covs = f"intercept, {k} PCs" + (f", {c} from {glm.covar_path}" if glm.covar_path else "")
-        print(f"GLM logistic: {glm.name} on {used} of {n} samples ({cases} cases, {used - cases} controls, {n - used} "
+        model = "Firth" if glm.firth == "always" else "logistic"
+        print(f"GLM {model}: {glm.name} on {used} of {n} samples ({cases} cases, {used - cases} controls, {n - used} "
               f"without a phenotype or covariate), {1 + k + c} covariates ({covs}); {len(errs)} variants tested, "
-              f"{int(np.count_nonzero(errs))} with an ERRCODE; lambda_GC = {lambda_gc(stats, errs)!r}.")
+              f"{int(np.count_nonzero(errs))} with an ERRCODE{fitted}; lambda_GC = {lambda_gc(stats, errs)!r}.")
         return stats, errs, passes
 
     # -- LD pruning of the variants (beyond the reference; DESIGN.md 9) -------------------------------------------------
@@ -1097,6 +1112,7 @@ class GlmInput:
     covar_values: np.ndarray
     q: int
     logistic: bool = False   # --glm-logistic: pheno_values hold 1 (case), 0 (control) and NaN (missing)
+    firth: Optional[str] = None   # --glm-firth: "fallback" or "always"
     y: Optional[np.ndarray] = None
     c: Optional[np.ndarray] = None
 
@@ -1143,6 +1159,11 @@ def check_glm_flags(conf: PcaConf) -> Optional[GlmInput]:
             raise ValueError(f"{flag} is read by --glm: give --glm")
     if conf.glmLogistic() and not conf.glm():
         raise ValueError("--glm-logistic is a mode of --glm: give --glm")
+    if conf.glmFirth.isDefined:
+        if not (conf.glm() and conf.glmLogistic()):
+            raise ValueError("--glm-firth is a mode of the logistic test: give --glm --glm-logistic")
+        if conf.glmFirth() not in native.GLM_FIRTH_MODES:
+            raise ValueError(f"--glm-firth takes fallback or always, not {conf.glmFirth()!r}")
     if not conf.glm():
         return None
     if not conf.pheno.isDefined:
@@ -1177,7 +1198,7 @@ def check_glm_flags(conf: PcaConf) -> Optional[GlmInput]:
                          f"and {covar_values.shape[1]} --covar columns make {q}")
     if conf.glmLogistic():
         return GlmInput(name, conf.pheno(), ids, case_control_coding(y, ids, name), conf.covar.get, covar_ids,
-                        covar_values, q, logistic=True)
+                        covar_values, q, logistic=True, firth=conf.glmFirth.get)
     check_glm_quantitative(y, name)
     return GlmInput(name, conf.pheno(), ids, y, conf.covar.get, covar_ids, covar_values, q)
 
@@ -1199,16 +1220,20 @@ def write_glm_linear(path: str, bim, counted: int, stats: np.ndarray, errs: np.n
             for b, st, e in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist())))
 
 
-def write_glm_logistic(path: str, bim, counted: int, stats: np.ndarray, errs: np.ndarray) -> None:
+def write_glm_logistic(path: str, bim, counted: int, stats: np.ndarray, errs: np.ndarray,
+                       firth: Optional[np.ndarray] = None) -> None:
     """P.<PHENO>.glm.logistic, as write_glm_linear with PLINK 2's logistic columns: OR = exp(BETA), LOG(OR)_SE = SE and
-    Z_STAT in place of BETA, SE and T_STAT."""
+    Z_STAT in place of BETA, SE and T_STAT.  firth (the .hybrid file of --glm-firth fallback): a FIRTH? column after
+    A1_FREQ, Y where the Firth fit produced the row."""
+    fcol = "" if firth is None else "FIRTH?\t"
+    flags = [""] * len(errs) if firth is None else ["Y\t" if f else "N\t" for f in np.asarray(firth).tolist()]
     with open(path, "w", encoding="utf-8") as fh:
-        fh.write("#CHROM\tPOS\tID\tREF\tALT\tA1\tA1_FREQ\tTEST\tOBS_CT\tOR\tLOG(OR)_SE\tZ_STAT\tP\tERRCODE\n")
+        fh.write(f"#CHROM\tPOS\tID\tREF\tALT\tA1\tA1_FREQ\t{fcol}TEST\tOBS_CT\tOR\tLOG(OR)_SE\tZ_STAT\tP\tERRCODE\n")
         fh.write("".join(
             f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
-            f"ADD\t{int(st[0])}\t{_glm_number(np.exp(st[2]))}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
+            f"{fl}ADD\t{int(st[0])}\t{_glm_number(np.exp(st[2]))}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
             f"{_glm_number(st[5])}\t{native.GLM_ERRCODES[int(e)]}\n"
-            for b, st, e in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist())))
+            for b, st, e, fl in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist(), flags)))
 
 
 def check_ld_flags(conf: PcaConf, bim=None) -> Optional[np.ndarray]:

@@ -26,6 +26,7 @@
 
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 
 #include "vpca_internal.h"
 
@@ -445,22 +446,224 @@ constexpr int kLMaxHalve = 8;              // step halvings in a row
 constexpr double kLDelta2 = 1e-18;         // convergence: the Newton decrement squared, delta <= 1e-9
 constexpr double kLFall = 1e-10;           // l fell: by more than this times |l| of the last accepted pass
 
-// Shared memory of glm_logistic_kernel, in doubles.  LD: pitch of one staged sample, in the tile of Q and y
-// [q_0 .. q_{KMAX-1}, y, mask, 0] and in a warp's tile U [w q_0 .. w q_{q-1}, w g', r, 0 .., g'] (u at 0 .. PMAX - 1,
-// g' at PMAX).  PMAX = KMAX + 2 rows of the augmented lower triangle: H (p = q + 1 <= KMAX + 1 rows) and the gradient
-// (row p).  Once a pass is summed, H and then L take the warp's U tile at pitch KMAX + 1.  Per warp also theta, theta
-// of the last accepted pass, the step, the gradient (then L^-1 grad), 1 / L_jj and the lanes' partial l.
-template <int KMAX>
-struct LogLayout {
+// Shared memory of glm_logistic_kernel and glm_firth_kernel, in doubles.  LD: pitch of one staged sample, in the tile of
+// Q and y [q_0 .. q_{KMAX-1}, y, mask, 0] and in a warp's tile U [w q_0 .. w q_{q-1}, w g', r, 0 .., g'] (u at
+// 0 .. PMAX - 1, g' at PMAX).  PMAX = KMAX + 2 rows of the augmented lower triangle: H (p = q + 1 <= KMAX + 1 rows) and,
+// in the logistic kernel, the gradient (row p; the Firth kernel's r is 0).  Once a pass is summed, H and then L (and the
+// Firth kernel's L^-1) take the warp's U tile at pitch PH.  Per warp also theta, theta of the last accepted point, the
+// step, the gradient or the Firth score (then L^-1 of it), 1 / L_jj, and NLANE arrays of one double per lane: the lanes'
+// partial l, and the Firth kernel's u and g' of a tile (walk B).
+template <int KMAX, int NLANE>
+struct NewtonLayout {
     static constexpr int LD = KMAX + 3;
     static constexpr int PMAX = KMAX + 2;
     static constexpr int PH = KMAX + 1;
     static constexpr int NBK = PMAX / 2;                          // 2 x 2 blocks per side
     static constexpr int NB = (NBK * (NBK + 1) / 2 + 31) / 32;    // lower-triangle blocks per lane
-    static constexpr int WARP = kLTile * LD + 5 * PMAX + 32;
+    static constexpr int WARP = kLTile * LD + 5 * PMAX + NLANE * 32;
     static constexpr int TOTAL = kLTile * LD + kLWarps * WARP;
     static_assert(PH * PH <= kLTile * LD, "H must fit in the U tile it takes over");
 };
+
+// The pass boundary of both Newton kernels, once every warp's decision of the last pass is in sst[w] (variant, -1 for
+// none; passes so far; backtracks in a row; centre of the dosage; the Firth kernel's walk).  Thread 0 gives each warp
+// without a variant the CTA's next list position in [snext, end), in warp order: the variant idx[i], or i itself with
+// idx == nullptr.  It writes OBS_CT and sum g from cnt[v * 6 ..] (OBS_CT, sum g, sum g^2 under the regression mask,
+// then OBS_CT under the case mask) to out[v * 6 ..], and err[v] and passes[v] = 0 for the ERRCODEs that need no pass;
+// firth[v], if firth is set, says whether a pass runs.  A warp that starts a variant starts from theta = (theta0, 0).
+// Returns whether any warp holds a variant.
+template <class Lo, int NST>
+__device__ __forceinline__ bool newton_next_pass(int (*sst)[NST], int& snext, int& sany, int end, const int32_t* idx,
+                                                 int q, const double* cnt, const double* theta0, double* th,
+                                                 double* out, int32_t* err, int32_t* passes, uint8_t* firth) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int any = 0;
+        for (int ww = 0; ww < kLWarps; ++ww) {
+            while (sst[ww][0] < 0 && snext < end) {
+                const int v = idx ? idx[snext] : snext;
+                ++snext;
+                const double* c = cnt + (int64_t)v * 6;
+                const int obs = (int)c[0], sg = (int)c[1], gg = (int)c[2], cases = (int)c[3];
+                double* o = out + (int64_t)v * 6;
+                o[0] = obs;
+                o[1] = sg;   // glm_logistic_finish_kernel divides
+                const int e = obs - q - 1 < 1                              ? VPCA_GLM_TOO_FEW_OBS
+                              : (int64_t)obs * gg == (int64_t)sg * sg      ? VPCA_GLM_CONST_ALLELE
+                              : cases == 0 || cases == obs                 ? VPCA_GLM_LOGISTIC_CONVERGE_FAIL
+                                                                           : VPCA_GLM_OK;
+                if (firth) firth[v] = e == VPCA_GLM_OK;
+                if (e != VPCA_GLM_OK) {
+                    err[v] = e;
+                    passes[v] = 0;
+                    continue;
+                }
+                sst[ww][0] = v;
+                sst[ww][1] = 0;
+                sst[ww][2] = 0;
+                sst[ww][3] = glm_centre(obs, sg);
+                if (NST > 4) sst[ww][4] = 0;
+            }
+            any |= sst[ww][0] >= 0;
+        }
+        sany = any;
+    }
+    __syncthreads();
+    if (!sany) return false;
+    const int w = threadIdx.x >> 5;
+    if (sst[w][0] >= 0 && sst[w][1] == 0)
+        for (int c = threadIdx.x & 31; c < Lo::PMAX; c += 32) th[c] = c < q ? theta0[c] : 0.0;
+    __syncwarp();
+    return true;
+}
+
+// Once every warp is done with the previous tile, the CTA stages samples [s0, s0 + kLTile) of Qx (n rows of KMAX + 2
+// doubles; zero past n) into Qt at pitch LD.
+template <class Lo>
+__device__ __forceinline__ void newton_stage_tile(double* Qt, const double* __restrict__ Qx, int s0, int n) {
+    constexpr int LD = Lo::LD, QLD = Lo::PMAX;
+    __syncthreads();
+    for (int i = threadIdx.x; i < kLTile * LD; i += kLWarps * 32) {
+        const int r = i / LD, c = i - r * LD, s = s0 + r;
+        Qt[i] = (c < QLD && s < n) ? Qx[(int64_t)s * QLD + c] : 0.0;
+    }
+    __syncthreads();
+}
+
+// This lane's 2 x 2 blocks of the lower triangle: rows ba, ba + 1 and columns bb, bb + 1; xo: the offset in the shared
+// memory of each column's value of sample 0 (q_b in the tile of Q and y, g' in the warp's U tile at uoff, and past g'
+// the tile's zero column).
+template <class Lo>
+__device__ __forceinline__ void newton_blocks(int lane, int q, int uoff, int (&ba)[Lo::NB], int (&bb)[Lo::NB],
+                                              int (&xo)[Lo::NB][2]) {
+#pragma unroll
+    for (int j = 0; j < Lo::NB; ++j) {
+        const int t = lane + 32 * j;
+        int I = 0;
+        while ((I + 1) * (I + 2) / 2 <= t) ++I;
+        ba[j] = 2 * I;
+        bb[j] = 2 * (t - I * (I + 1) / 2);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int b = bb[j] + e;
+            xo[j][e] = b < q ? b : b == q ? uoff + Lo::PMAX : Lo::PMAX;
+        }
+    }
+}
+
+// The link at sample s of the warp's variant (x: its row of the staged tile): in says s is in A_v, g' the centred
+// dosage (0 outside A_v), eta = x^T theta; inside A_v also e = exp(-|eta|), mu and the weight w = mu (1 - mu) (0
+// outside).
+struct NewtonLink {
+    bool in;
+    double g, eta, e, mu, wt;
+};
+template <class Lo>
+__device__ __forceinline__ NewtonLink newton_link(const double* x, const uint8_t* row, int s, int n, int q, uint32_t lut,
+                                                  int cen, const double* th) {
+    NewtonLink k;
+    const uint32_t code = s < n ? (row[s >> 2] >> (2 * (s & 3))) & 3u : 1u;
+    k.in = x[Lo::PMAX - 1] != 0.0 && code != 1u;
+    k.g = k.in ? (double)((int)((lut >> (2 * code)) & 3u) - cen) : 0.0;
+    k.eta = 0.0;
+    for (int c = 0; c < q; ++c) k.eta = fma(x[c], th[c], k.eta);
+    k.eta = fma(th[q], k.g, k.eta);
+    k.wt = k.mu = k.e = 0.0;
+    if (k.in) {
+        k.e = exp(-fabs(k.eta));
+        const double rd = recip_newton(1.0 + k.e);
+        k.mu = k.eta >= 0.0 ? rd : k.e * rd;
+        k.wt = k.e * rd * rd;
+    }
+    return k;
+}
+
+// -l_s of a sample in A_v, from y, eta and e = exp(-|eta|): l_s = y eta - log(1 + e^eta) = -softplus(m).
+__device__ __forceinline__ double newton_nll(double y, double eta, double e) {
+    const double m = y != 0.0 ? -eta : eta;
+    return fmax(m, 0.0) + log1p(e);
+}
+
+// One tile of the sums of H (and the gradient): lane l writes the row of U of sample s0 + l (x its row of the tile, r
+// its gradient term), then every lane adds the 32 samples in order into its 2 x 2 blocks of the augmented triangle
+// (4 shared loads feed 4 FMAs).  nblk: 2 x 2 blocks per side.
+template <class Lo>
+__device__ __forceinline__ void newton_tile_sums(const double* sm, double* U, int lane, const double* x, int q,
+                                                 const NewtonLink& k, double r, int nblk, const int (&ba)[Lo::NB],
+                                                 const int (&xo)[Lo::NB][2], double (&acc)[Lo::NB][4]) {
+    constexpr int LD = Lo::LD;
+    double* u = U + lane * LD;
+    for (int c = 0; c < q; ++c) u[c] = k.wt * x[c];
+    u[q] = k.wt * k.g;
+    u[q + 1] = r;
+    for (int c = q + 2; c < 2 * nblk; ++c) u[c] = 0.0;
+    u[Lo::PMAX] = k.g;
+    __syncwarp();
+    const int nblocks = nblk * (nblk + 1) / 2;
+#pragma unroll 2
+    for (int s = 0; s < kLTile; ++s) {
+        const double* ur = U + s * LD;
+#pragma unroll
+        for (int j = 0; j < Lo::NB; ++j) {
+            if (lane + 32 * j >= nblocks) continue;
+            const double u0 = ur[ba[j]], u1 = ur[ba[j] + 1];
+            const double x0 = sm[xo[j][0] + s * LD], x1 = sm[xo[j][1] + s * LD];
+            acc[j][0] = fma(u0, x0, acc[j][0]);
+            acc[j][1] = fma(u0, x1, acc[j][1]);
+            acc[j][2] = fma(u1, x0, acc[j][2]);
+            acc[j][3] = fma(u1, x1, acc[j][3]);
+        }
+    }
+}
+
+// H (lower triangle, pitch PH, over the U tile) from the blocks, and with nrow = p + 1 the gradient (row p); each entry
+// has one owner.
+template <class Lo>
+__device__ __forceinline__ void newton_unpack(double* H, double* grad, int p, int nrow, int lane, int nblk,
+                                              const int (&ba)[Lo::NB], const int (&bb)[Lo::NB],
+                                              const double (&acc)[Lo::NB][4]) {
+    const int nblocks = nblk * (nblk + 1) / 2;
+#pragma unroll
+    for (int j = 0; j < Lo::NB; ++j) {
+        if (lane + 32 * j >= nblocks) continue;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int a = ba[j] + (e >> 1), b = bb[j] + (e & 1);
+            if (b >= p || a < b || a >= nrow) continue;
+            if (a < p) H[a * Lo::PH + b] = acc[j][e];
+            else grad[b] = acc[j][e];
+        }
+    }
+}
+
+// Cholesky H = L L^T over H (p x p, pitch PH), left-looking by column; lanes own rows j + 1 + lane, j + 33 + lane;
+// sr[j] = 1 / L_jj.  First pass: a pivot <= kPivotMin H_jj sets flag (the warp's, in shared memory) to 3
+// (VIF_INFINITE); later a pivot <= 0 sets it to 2; else it stays 0.  ldet, if set (lane 0): += sum log L_jj =
+// sum log(pivot) / 2, in column order.
+template <class Lo>
+__device__ __forceinline__ void newton_cholesky(double* H, double* sr, int p, int lane, bool first, int& flag,
+                                                double* ldet) {
+    constexpr int PH = Lo::PH;
+    for (int j = 0; j < p; ++j) {
+        if (lane == 0) {
+            const double hjj = H[j * PH + j];
+            double d = hjj;
+            for (int c = 0; c < j; ++c) d = fma(-H[j * PH + c], H[j * PH + c], d);
+            const bool ok = first ? d > kPivotMin * hjj : d > 0.0;
+            sr[j] = ok ? rsqrt_newton(d) : 0.0;
+            if (ldet && ok) *ldet += 0.5 * log(d);
+            flag = ok ? 0 : first ? 3 : 2;
+        }
+        __syncwarp();
+        if (flag != 0) break;
+        for (int i = j + 1 + lane; i < p; i += 32) {
+            double x = H[i * PH + j];
+            for (int c = 0; c < j; ++c) x = fma(-H[i * PH + c], H[j * PH + c], x);
+            H[i * PH + j] = x * sr[j];
+        }
+        __syncwarp();
+    }
+}
 
 // grid ceil(nv / kLPerCta); CTA c owns variants [c kLPerCta, min(nv, (c + 1) kLPerCta)).  cnt[v * 6 ..]: OBS_CT, sum g,
 // sum g^2 under the regression mask, then OBS_CT under the case mask (glm_count_kernel).  Qx: n rows of KMAX + 2
@@ -479,7 +682,7 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_logistic_kernel(const uin
                                                                       const double* __restrict__ cnt,
                                                                       double* __restrict__ out, int32_t* __restrict__ err,
                                                                       int32_t* __restrict__ passes) {
-    using Lo = LogLayout<KMAX>;
+    using Lo = NewtonLayout<KMAX, 1>;
     constexpr int LD = Lo::LD, PMAX = Lo::PMAX, PH = Lo::PH, NB = Lo::NB;
     extern __shared__ __align__(16) double lsm[];
     __shared__ int sst[kLWarps][4];   // variant (-1: none), passes so far, halvings in a row, centre of the dosage
@@ -499,63 +702,15 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_logistic_kernel(const uin
     double* const lpart = sr + PMAX;
     const int p = q + 1;
     const int nblk = (p + 2) / 2;   // 2 x 2 blocks per side over rows 0 .. p
-    const int nblocks = nblk * (nblk + 1) / 2;
-    // this lane's blocks: rows ba, ba + 1 and columns bb, bb + 1; xo: the offset in lsm of each column's value of sample 0
     int ba[NB], bb[NB], xo[NB][2];
-#pragma unroll
-    for (int j = 0; j < NB; ++j) {
-        const int t = lane + 32 * j;
-        int I = 0;
-        while ((I + 1) * (I + 2) / 2 <= t) ++I;
-        ba[j] = 2 * I;
-        bb[j] = 2 * (t - I * (I + 1) / 2);
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const int b = bb[j] + e;
-            xo[j][e] = b < q ? b : b == q ? uoff + PMAX : KMAX + 2;
-        }
-    }
+    newton_blocks<Lo>(lane, q, uoff, ba, bb, xo);
     const int v_end = min(nv, (int)(blockIdx.x + 1) * kLPerCta);
     if (threadIdx.x == 0) snext = blockIdx.x * kLPerCta;
     if (lane == 0) sst[w][0] = -1;
     const int nt = (n + kLTile - 1) / kLTile;
-    for (;;) {
-        __syncthreads();   // every warp's decision of the last pass is in sst
-        if (threadIdx.x == 0) {
-            int any = 0;
-            for (int ww = 0; ww < kLWarps; ++ww) {
-                while (sst[ww][0] < 0 && snext < v_end) {
-                    const int v = snext++;
-                    const double* c = cnt + (int64_t)v * 6;
-                    const int obs = (int)c[0], sg = (int)c[1], gg = (int)c[2], cases = (int)c[3];
-                    double* o = out + (int64_t)v * 6;
-                    o[0] = obs;
-                    o[1] = sg;   // glm_logistic_finish_kernel divides
-                    const int e = obs - q - 1 < 1                              ? VPCA_GLM_TOO_FEW_OBS
-                                  : (int64_t)obs * gg == (int64_t)sg * sg      ? VPCA_GLM_CONST_ALLELE
-                                  : cases == 0 || cases == obs                 ? VPCA_GLM_LOGISTIC_CONVERGE_FAIL
-                                                                               : VPCA_GLM_OK;
-                    if (e != VPCA_GLM_OK) {
-                        err[v] = e;
-                        passes[v] = 0;
-                        continue;
-                    }
-                    sst[ww][0] = v;
-                    sst[ww][1] = 0;
-                    sst[ww][2] = 0;
-                    sst[ww][3] = glm_centre(obs, sg);
-                }
-                any |= sst[ww][0] >= 0;
-            }
-            sany = any;
-        }
-        __syncthreads();
-        if (!sany) break;
+    while (newton_next_pass<Lo>(sst, snext, sany, v_end, nullptr, q, cnt, theta0, th, out, err, passes, nullptr)) {
         const int v = sst[w][0];
         const bool act = v >= 0;   // uniform over the warp
-        if (act && sst[w][1] == 0)
-            for (int c = lane; c < PMAX; c += 32) th[c] = c < q ? theta0[c] : 0.0;
-        __syncwarp();
         const uint8_t* row = rows + (int64_t)(act ? v : 0) * stride;
         const int cen = act ? sst[w][3] : 0;
         double acc[NB][4];
@@ -565,70 +720,20 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_logistic_kernel(const uin
 #pragma unroll 1
         for (int t = 0; t < nt; ++t) {
             const int s0 = t * kLTile;
-            __syncthreads();   // every warp is done with the previous tile
-            for (int i = threadIdx.x; i < kLTile * LD; i += kLWarps * 32) {
-                const int r = i / LD, c = i - r * LD, s = s0 + r;
-                Qt[i] = (c < KMAX + 2 && s < n) ? Qx[(int64_t)s * (KMAX + 2) + c] : 0.0;
-            }
-            __syncthreads();
+            newton_stage_tile<Lo>(Qt, Qx, s0, n);
             if (!act) continue;
-            {   // sample s0 + lane
-                const int s = s0 + lane;
-                const double* x = Qt + lane * LD;
-                double* u = U + lane * LD;
-                const uint32_t code = s < n ? (row[s >> 2] >> (2 * (s & 3))) & 3u : 1u;
-                const bool in = x[KMAX + 1] != 0.0 && code != 1u;
-                const double g = in ? (double)((int)((lut >> (2 * code)) & 3u) - cen) : 0.0;
-                double eta = 0.0;
-                for (int c = 0; c < q; ++c) eta = fma(x[c], th[c], eta);
-                eta = fma(th[q], g, eta);
-                double wt = 0.0, r = 0.0;
-                if (in) {
-                    const double y = x[q];
-                    const double e = exp(-fabs(eta));
-                    const double rd = recip_newton(1.0 + e);
-                    const double mu = eta >= 0.0 ? rd : e * rd;
-                    wt = e * rd * rd;
-                    r = y - mu;
-                    const double m = y != 0.0 ? -eta : eta;   // l_s = y eta - log(1 + e^eta) = -softplus(m)
-                    lsum -= fmax(m, 0.0) + log1p(e);
-                }
-                for (int c = 0; c < q; ++c) u[c] = wt * x[c];
-                u[q] = wt * g;
-                u[p] = r;
-                for (int c = p + 1; c < 2 * nblk; ++c) u[c] = 0.0;
-                u[PMAX] = g;
+            const double* x = Qt + lane * LD;
+            const NewtonLink k = newton_link<Lo>(x, row, s0 + lane, n, q, lut, cen, th);
+            double r = 0.0;
+            if (k.in) {
+                r = x[q] - k.mu;
+                lsum -= newton_nll(x[q], k.eta, k.e);
             }
-            __syncwarp();
-#pragma unroll 2
-            for (int s = 0; s < kLTile; ++s) {
-                const double* ur = U + s * LD;
-#pragma unroll
-                for (int j = 0; j < NB; ++j) {
-                    if (lane + 32 * j >= nblocks) continue;
-                    const double u0 = ur[ba[j]], u1 = ur[ba[j] + 1];
-                    const double x0 = lsm[xo[j][0] + s * LD], x1 = lsm[xo[j][1] + s * LD];
-                    acc[j][0] = fma(u0, x0, acc[j][0]);
-                    acc[j][1] = fma(u0, x1, acc[j][1]);
-                    acc[j][2] = fma(u1, x0, acc[j][2]);
-                    acc[j][3] = fma(u1, x1, acc[j][3]);
-                }
-            }
+            newton_tile_sums<Lo>(lsm, U, lane, x, q, k, r, nblk, ba, xo, acc);
             __syncwarp();
         }
         if (!act) continue;
-        // H (lower triangle, pitch PH, over the U tile) and the gradient from the blocks; each entry has one owner
-#pragma unroll
-        for (int j = 0; j < NB; ++j) {
-            if (lane + 32 * j >= nblocks) continue;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int a = ba[j] + (e >> 1), b = bb[j] + (e & 1);
-                if (b >= p || a < b || a > p) continue;
-                if (a < p) H[a * PH + b] = acc[j][e];
-                else grad[b] = acc[j][e];
-            }
-        }
+        newton_unpack<Lo>(H, grad, p, p + 1, lane, nblk, ba, bb, acc);
         lpart[lane] = lsum;
         __syncwarp();
         if (lane == 0) {
@@ -654,29 +759,7 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_logistic_kernel(const uin
             sflag[w] = fl;
         }
         __syncwarp();
-        if (sflag[w] == 0) {
-            // Cholesky H = L L^T, left-looking by column; lanes own rows j + 1 + lane, j + 33 + lane; sr[j] = 1 / L_jj.
-            // First pass: a pivot <= kPivotMin H_jj is VIF_INFINITE; later: a pivot <= 0 is LOGISTIC_CONVERGE_FAIL.
-            const bool first = sst[w][1] == 1;
-            for (int j = 0; j < p; ++j) {
-                if (lane == 0) {
-                    const double hjj = H[j * PH + j];
-                    double d = hjj;
-                    for (int k = 0; k < j; ++k) d = fma(-H[j * PH + k], H[j * PH + k], d);
-                    const bool ok = first ? d > kPivotMin * hjj : d > 0.0;
-                    sr[j] = ok ? rsqrt_newton(d) : 0.0;
-                    sflag[w] = ok ? 0 : first ? 3 : 2;
-                }
-                __syncwarp();
-                if (sflag[w] != 0) break;
-                for (int i = j + 1 + lane; i < p; i += 32) {
-                    double x = H[i * PH + j];
-                    for (int k = 0; k < j; ++k) x = fma(-H[i * PH + k], H[j * PH + k], x);
-                    H[i * PH + j] = x * sr[j];
-                }
-                __syncwarp();
-            }
-        }
+        if (sflag[w] == 0) newton_cholesky<Lo>(H, sr, p, lane, sst[w][1] == 1, sflag[w], nullptr);
         if (lane == 0) {
             int fl = sflag[w];
             const int k = sst[w][1];
@@ -751,22 +834,6 @@ constexpr int kFMaxBack = 30;          // backtracks in a row
 constexpr double kFMaxDelta = 5.0;     // the first trial point of a step lies at most this Newton decrement away
 constexpr double kFSecant = 0.45;      // the secant backtrack: U*^T Delta at the trial point < -kFSecant delta^2_prev
 
-// Shared memory of glm_firth_kernel, in doubles: the tile of Q and y as in LogLayout, and per warp a U tile (walk A:
-// rows [w q_0 .. w q_{q-1}, w g', 0 .., g'] as in glm_logistic_kernel; between the walks H, then L, then L^-1 over it at
-// pitch PH), theta, theta of the last accepted point, the step, the Firth score, 1 / L_jj (then z = L^-1 U*), the lanes'
-// partial l, and a tile's u and g' (walk B).
-template <int KMAX>
-struct FirthLayout {
-    static constexpr int LD = KMAX + 3;
-    static constexpr int PV = KMAX + 2;
-    static constexpr int PH = KMAX + 1;
-    static constexpr int NBK = (KMAX + 2) / 2;                    // 2 x 2 blocks per side of H (p <= KMAX + 1 rows)
-    static constexpr int NB = (NBK * (NBK + 1) / 2 + 31) / 32;    // lower-triangle blocks per lane
-    static constexpr int WARP = kLTile * LD + 5 * PV + 3 * 32;
-    static constexpr int TOTAL = kLTile * LD + kLWarps * WARP;
-    static_assert(PH * PH <= kLTile * LD, "H must fit in the U tile it takes over");
-};
-
 // grid ceil(nv / kLPerCta).  The variants to fit: list positions [0, nf) with nf = *d_nf (idx[i] the chunk's variant), or
 // with idx == nullptr every variant of the chunk (nf = nv); CTA c owns positions [c kLPerCta, (c + 1) kLPerCta).  cnt,
 // Qx, theta0 and out as glm_logistic_kernel.  Per variant, from (theta0, beta = 0), the passes of DESIGN.md 17: a warp is
@@ -787,8 +854,8 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_firth_kernel(const uint8_
                                                                    double* __restrict__ out, int32_t* __restrict__ err,
                                                                    int32_t* __restrict__ passes,
                                                                    uint8_t* __restrict__ firth) {
-    using Lo = FirthLayout<KMAX>;
-    constexpr int LD = Lo::LD, PV = Lo::PV, PH = Lo::PH, NB = Lo::NB;
+    using Lo = NewtonLayout<KMAX, 3>;
+    constexpr int LD = Lo::LD, PV = Lo::PMAX, PH = Lo::PH, NB = Lo::NB;
     extern __shared__ __align__(16) double fsm[];
     __shared__ int sst[kLWarps][5];      // variant (-1: none), passes so far, backtracks in a row, centre, walk (0 A, 1 B)
     __shared__ int sflag[kLWarps];
@@ -812,66 +879,16 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_firth_kernel(const uint8_
     double* const sg = su + 32;
     const int p = q + 1;
     const int nblk = (p + 1) / 2;   // 2 x 2 blocks per side over rows 0 .. p - 1
-    const int nblocks = nblk * (nblk + 1) / 2;
     int ba[NB], bb[NB], xo[NB][2];
-#pragma unroll
-    for (int j = 0; j < NB; ++j) {
-        const int t = lane + 32 * j;
-        int I = 0;
-        while ((I + 1) * (I + 2) / 2 <= t) ++I;
-        ba[j] = 2 * I;
-        bb[j] = 2 * (t - I * (I + 1) / 2);
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const int b = bb[j] + e;
-            xo[j][e] = b < q ? b : b == q ? uoff + KMAX + 2 : KMAX + 2;
-        }
-    }
+    newton_blocks<Lo>(lane, q, uoff, ba, bb, xo);
     const int p_end = min(nf, p0 + kLPerCta);
     if (threadIdx.x == 0) snext = p0;
     if (lane == 0) sst[w][0] = -1;
     const int nt = (n + kLTile - 1) / kLTile;
-    for (;;) {
-        __syncthreads();   // every warp's decision of the last walk is in sst
-        if (threadIdx.x == 0) {
-            int any = 0;
-            for (int ww = 0; ww < kLWarps; ++ww) {
-                while (sst[ww][0] < 0 && snext < p_end) {
-                    const int v = idx ? idx[snext] : snext;
-                    ++snext;
-                    const double* c = cnt + (int64_t)v * 6;
-                    const int obs = (int)c[0], sg_ = (int)c[1], gg = (int)c[2], cases = (int)c[3];
-                    double* o = out + (int64_t)v * 6;
-                    o[0] = obs;
-                    o[1] = sg_;   // glm_logistic_finish_kernel divides
-                    const int e = obs - q - 1 < 1                              ? VPCA_GLM_TOO_FEW_OBS
-                                  : (int64_t)obs * gg == (int64_t)sg_ * sg_    ? VPCA_GLM_CONST_ALLELE
-                                  : cases == 0 || cases == obs                 ? VPCA_GLM_LOGISTIC_CONVERGE_FAIL
-                                                                               : VPCA_GLM_OK;
-                    firth[v] = e == VPCA_GLM_OK;
-                    if (e != VPCA_GLM_OK) {
-                        err[v] = e;
-                        passes[v] = 0;
-                        continue;
-                    }
-                    sst[ww][0] = v;
-                    sst[ww][1] = 0;
-                    sst[ww][2] = 0;
-                    sst[ww][3] = glm_centre(obs, sg_);
-                    sst[ww][4] = 0;
-                }
-                any |= sst[ww][0] >= 0;
-            }
-            sany = any;
-        }
-        __syncthreads();
-        if (!sany) break;
+    while (newton_next_pass<Lo>(sst, snext, sany, p_end, idx, q, cnt, theta0, th, out, err, passes, firth)) {
         const int v = sst[w][0];
         const bool act = v >= 0;   // uniform over the warp
         const bool walk_b = act && sst[w][4] == 1;
-        if (act && sst[w][1] == 0)
-            for (int c = lane; c < PV; c += 32) th[c] = c < q ? theta0[c] : 0.0;
-        __syncwarp();
         const uint8_t* row = rows + (int64_t)(act ? v : 0) * stride;
         const int cen = act ? sst[w][3] : 0;
         double acc[NB][4];
@@ -882,75 +899,35 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_firth_kernel(const uint8_
 #pragma unroll 1
         for (int t = 0; t < nt; ++t) {
             const int s0 = t * kLTile;
-            __syncthreads();   // every warp is done with the previous tile
-            for (int i = threadIdx.x; i < kLTile * LD; i += kLWarps * 32) {
-                const int r = i / LD, c = i - r * LD, s = s0 + r;
-                Qt[i] = (c < KMAX + 2 && s < n) ? Qx[(int64_t)s * (KMAX + 2) + c] : 0.0;
-            }
-            __syncthreads();
+            newton_stage_tile<Lo>(Qt, Qx, s0, n);
             if (!act) continue;
-            const int s = s0 + lane;
             const double* x = Qt + lane * LD;
-            const uint32_t code = s < n ? (row[s >> 2] >> (2 * (s & 3))) & 3u : 1u;
-            const bool in = x[KMAX + 1] != 0.0 && code != 1u;
-            const double g = in ? (double)((int)((lut >> (2 * code)) & 3u) - cen) : 0.0;
-            double eta = 0.0;
-            for (int c = 0; c < q; ++c) eta = fma(x[c], th[c], eta);
-            eta = fma(th[q], g, eta);
-            double wt = 0.0, mu = 0.0, e = 0.0;
-            if (in) {
-                e = exp(-fabs(eta));
-                const double rd = recip_newton(1.0 + e);
-                mu = eta >= 0.0 ? rd : e * rd;
-                wt = e * rd * rd;
-            }
+            const NewtonLink k = newton_link<Lo>(x, row, s0 + lane, n, q, lut, cen, th);
             if (!walk_b) {
-                if (in) {
-                    const double m = x[q] != 0.0 ? -eta : eta;   // l_s = y eta - log(1 + e^eta) = -softplus(m)
-                    lsum -= fmax(m, 0.0) + log1p(e);
-                }
-                double* u = U + lane * LD;
-                for (int c = 0; c < q; ++c) u[c] = wt * x[c];
-                u[q] = wt * g;
-                for (int c = p; c < 2 * nblk; ++c) u[c] = 0.0;
-                u[KMAX + 2] = g;
-                __syncwarp();
-#pragma unroll 2
-                for (int r = 0; r < kLTile; ++r) {
-                    const double* ur = U + r * LD;
-#pragma unroll
-                    for (int j = 0; j < NB; ++j) {
-                        if (lane + 32 * j >= nblocks) continue;
-                        const double u0 = ur[ba[j]], u1 = ur[ba[j] + 1];
-                        const double x0 = fsm[xo[j][0] + r * LD], x1 = fsm[xo[j][1] + r * LD];
-                        acc[j][0] = fma(u0, x0, acc[j][0]);
-                        acc[j][1] = fma(u0, x1, acc[j][1]);
-                        acc[j][2] = fma(u1, x0, acc[j][2]);
-                        acc[j][3] = fma(u1, x1, acc[j][3]);
-                    }
-                }
+                if (k.in) lsum -= newton_nll(x[q], k.eta, k.e);
+                newton_tile_sums<Lo>(fsm, U, lane, x, q, k, 0.0, nblk, ba, xo, acc);
             } else {
                 double uu = 0.0;
-                if (in) {
+                if (k.in) {
                     // h = w ||L^-1 x||^2, one FMA chain per row of L^-1 (H holds L^-1)
                     double hh = 0.0;
                     for (int j = 0; j < q; ++j) {
                         const double* li = H + j * PH;
                         double z = 0.0;
-                        for (int k = 0; k <= j; ++k) z = fma(li[k], x[k], z);
+                        for (int c = 0; c <= j; ++c) z = fma(li[c], x[c], z);
                         hh = fma(z, z, hh);
                     }
                     {
                         const double* li = H + q * PH;
                         double z = 0.0;
-                        for (int k = 0; k < q; ++k) z = fma(li[k], x[k], z);
-                        z = fma(li[q], g, z);
+                        for (int c = 0; c < q; ++c) z = fma(li[c], x[c], z);
+                        z = fma(li[q], k.g, z);
                         hh = fma(z, z, hh);
                     }
-                    uu = fma(wt * hh, 0.5 - mu, x[q] - mu);
+                    uu = fma(k.wt * hh, 0.5 - k.mu, x[q] - k.mu);
                 }
                 su[lane] = uu;
-                sg[lane] = g;
+                sg[lane] = k.g;
                 __syncwarp();
                 const int c1 = lane + 32;
 #pragma unroll 2
@@ -964,17 +941,7 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_firth_kernel(const uint8_
         }
         if (!act) continue;
         if (!walk_b) {
-            // H (lower triangle, pitch PH, over the U tile) from the blocks; each entry has one owner
-#pragma unroll
-            for (int j = 0; j < NB; ++j) {
-                if (lane + 32 * j >= nblocks) continue;
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int a = ba[j] + (e >> 1), b = bb[j] + (e & 1);
-                    if (a >= p || a < b) continue;
-                    H[a * PH + b] = acc[j][e];
-                }
-            }
+            newton_unpack<Lo>(H, grad, p, p, lane, nblk, ba, bb, acc);
             lpart[lane] = lsum;
             __syncwarp();
             if (lane == 0) {
@@ -987,30 +954,9 @@ __global__ void __launch_bounds__(kLWarps * 32, 2) glm_firth_kernel(const uint8_
             __syncwarp();
             const int k = sst[w][1];
             const bool first = k == 1;
-            double ldet = 0.0;   // lane 0: sum log L_jj = sum log(pivot) / 2, in column order
-            if (sflag[w] == 0) {
-                // Cholesky H = L L^T as glm_logistic_kernel.  First pass: a pivot <= kPivotMin H_jj is VIF_INFINITE (3);
-                // later a pivot <= 0 backtracks (2).
-                for (int j = 0; j < p; ++j) {
-                    if (lane == 0) {
-                        const double hjj = H[j * PH + j];
-                        double d = hjj;
-                        for (int c = 0; c < j; ++c) d = fma(-H[j * PH + c], H[j * PH + c], d);
-                        const bool ok = first ? d > kPivotMin * hjj : d > 0.0;
-                        sr[j] = ok ? rsqrt_newton(d) : 0.0;
-                        if (ok) ldet += 0.5 * log(d);
-                        sflag[w] = ok ? 0 : first ? 3 : 2;
-                    }
-                    __syncwarp();
-                    if (sflag[w] != 0) break;
-                    for (int i = j + 1 + lane; i < p; i += 32) {
-                        double x = H[i * PH + j];
-                        for (int c = 0; c < j; ++c) x = fma(-H[i * PH + c], H[j * PH + c], x);
-                        H[i * PH + j] = x * sr[j];
-                    }
-                    __syncwarp();
-                }
-            }
+            double ldet = 0.0;   // lane 0: sum log L_jj
+            // first pass: VIF_INFINITE (3); later a pivot <= 0 backtracks (2)
+            if (sflag[w] == 0) newton_cholesky<Lo>(H, sr, p, lane, first, sflag[w], &ldet);
             if (lane == 0) {
                 int fl = sflag[w];
                 const double ls = sdp[w][1] + ldet;
@@ -1145,7 +1091,7 @@ cudaError_t launch_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n
     glm_count_kernel<<<cgrid, kCThreads, 0, stream>>>(d_rows, stride, nv, n, d_case, lut == kLutA2, d_cnt + 3, 6);
     cudaError_t e = cudaSuccess;
     if (firth_mode != VPCA_GLM_FIRTH_ALWAYS) {
-        const size_t smem = LogLayout<KMAX>::TOTAL * sizeof(double);
+        const size_t smem = NewtonLayout<KMAX, 1>::TOTAL * sizeof(double);
         e = cudaFuncSetAttribute(glm_logistic_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         glm_logistic_kernel<KMAX><<<lgrid, kLWarps * 32, smem, stream>>>(d_rows, stride, nv, n, q, d_Qx, d_theta0, lut,
@@ -1159,7 +1105,7 @@ cudaError_t launch_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n
             glm_firth_select_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, stream>>>(nv, d_err, d_passes, d_firth,
                                                                                       d_idx, d_nf);
         }
-        const size_t smem = FirthLayout<KMAX>::TOTAL * sizeof(double);
+        const size_t smem = NewtonLayout<KMAX, 3>::TOTAL * sizeof(double);
         e = cudaFuncSetAttribute(glm_firth_kernel<KMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         glm_firth_kernel<KMAX><<<lgrid, kLWarps * 32, smem, stream>>>(d_rows, stride, nv, n, q, d_Qx, d_theta0, lut,
@@ -1168,6 +1114,18 @@ cudaError_t launch_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n
     }
     glm_logistic_finish_kernel<<<(unsigned)((nv + 127) / 128), 128, 0, stream>>>(nv, d_out, d_err);
     return cudaSuccess;
+}
+
+// Calls f(std::integral_constant<int, glm_kmax(q)>()): the one place a q picks the kernels' instantiation.
+template <class F>
+auto with_kmax(int q, F&& f) {
+    switch (glm_kmax(q)) {
+        case 2: return f(std::integral_constant<int, 2>());
+        case 4: return f(std::integral_constant<int, 4>());
+        case 8: return f(std::integral_constant<int, 8>());
+        case 16: return f(std::integral_constant<int, 16>());
+        default: return f(std::integral_constant<int, 32>());
+    }
 }
 
 }  // namespace
@@ -1179,45 +1137,24 @@ cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int
                        int32_t* d_err, cudaStream_t stream) {
     if (nv <= 0) return cudaSuccess;
     const uint32_t lut = counted == 2 ? kLutA2 : kLutA1;
-    switch (glm_kmax(q)) {
-        case 2: launch<2>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
-        case 4: launch<4>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
-        case 8: launch<8>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
-        case 16: launch<16>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
-        default: launch<32>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err, stream); break;
-    }
+    with_kmax(q, [&](auto K) {
+        launch<decltype(K)::value>(d_rows, stride, nv, n, q, n_reg, d_Qx, d_mask, d_z0, yty, lut, d_sums, d_out, d_err,
+                                   stream);
+    });
     return cudaGetLastError();
-}
-
-cudaError_t glm_firth(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
-                      const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
-                      double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode, uint8_t* d_firth, int32_t* d_idx,
-                      int32_t* d_nf, cudaStream_t stream) {
-    if (nv <= 0) return cudaSuccess;
-    const uint32_t lut = counted == 2 ? kLutA2 : kLutA1;
-    cudaError_t e;
-    switch (glm_kmax(q)) {
-#define VPCA_GLM_LOGISTIC(K)                                                                                              \
-    case K:                                                                                                               \
-        e = launch_logistic<K>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt, d_out, d_err,       \
-                               d_passes, firth_mode, d_firth, d_idx, d_nf, stream);                                       \
-        break;
-        VPCA_GLM_LOGISTIC(2)
-        VPCA_GLM_LOGISTIC(4)
-        VPCA_GLM_LOGISTIC(8)
-        VPCA_GLM_LOGISTIC(16)
-        default: e = launch_logistic<32>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt, d_out,
-                                         d_err, d_passes, firth_mode, d_firth, d_idx, d_nf, stream);
-#undef VPCA_GLM_LOGISTIC
-    }
-    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
                          const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
-                         double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream) {
-    return glm_firth(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, counted, d_cnt, d_out, d_err, d_passes, 0,
-                     nullptr, nullptr, nullptr, stream);
+                         double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode, uint8_t* d_firth,
+                         int32_t* d_idx, int32_t* d_nf, cudaStream_t stream) {
+    if (nv <= 0) return cudaSuccess;
+    const uint32_t lut = counted == 2 ? kLutA2 : kLutA1;
+    const cudaError_t e = with_kmax(q, [&](auto K) {
+        return launch_logistic<decltype(K)::value>(d_rows, stride, nv, n, q, d_Qx, d_mask, d_case, d_theta0, lut, d_cnt,
+                                                   d_out, d_err, d_passes, firth_mode, d_firth, d_idx, d_nf, stream);
+    });
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 }  // namespace vpca

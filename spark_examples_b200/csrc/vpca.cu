@@ -2581,6 +2581,16 @@ int glm_upload(vpca_ctx* ctx, int q, const std::vector<int>& idx, const std::vec
     return VPCA_OK;
 }
 
+// Sets the GLM state under ctx->mu: q columns (0: none), the model, R regression samples and y~^T y~ (linear).
+void glm_commit(vpca_ctx* ctx, int q, bool logistic, int R, double yty, int64_t* n_used) {
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    ctx->glm_q = q;
+    ctx->glm_logistic = logistic;
+    ctx->glm_nreg = R;
+    ctx->glm_yty = yty;
+    if (n_used) *n_used = R;
+}
+
 // The logistic null fit: theta (q) maximising l over all R regression samples with Q alone, by the Newton passes of
 // glm_logistic_kernel (DESIGN.md 16) from theta = 0, in FP64 on the host.  Returns the passes, or 0 without convergence.
 int glm_null_fit(const std::vector<double>& Q, const std::vector<double>& y, int q, std::vector<double>& theta) {
@@ -2660,10 +2670,7 @@ int glm_null_fit(const std::vector<double>& Q, const std::vector<double>& y, int
 
 int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        ctx->glm_q = 0;   // a refused call leaves no GLM state
-    }
+    glm_commit(ctx, 0, false, 0, 0.0, nullptr);   // a refused call leaves no GLM state
     std::vector<int> idx;   // the regression samples
     int rc = glm_samples(ctx, "vpca_glm_begin", pheno, covar, n_covar, idx);
     if (rc != VPCA_OK) return rc;
@@ -2689,21 +2696,13 @@ int vpca_glm_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int3
         for (int i = 0; i < R; ++i) z0[k] += Q[(size_t)k * R + i] * y[i];
     rc = glm_upload(ctx, q, idx, Q, y, z0, false);
     if (rc != VPCA_OK) return rc;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    ctx->glm_q = q;
-    ctx->glm_logistic = 0;
-    ctx->glm_nreg = R;
-    ctx->glm_yty = yty;
-    if (n_used) *n_used = R;
+    glm_commit(ctx, q, false, R, yty, n_used);
     return VPCA_OK;
 }
 
 int vpca_glm_logistic_begin(vpca_ctx* ctx, const double* pheno, const double* covar, int32_t n_covar, int64_t* n_used) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        ctx->glm_q = 0;   // a refused call leaves no GLM state
-    }
+    glm_commit(ctx, 0, false, 0, 0.0, nullptr);   // a refused call leaves no GLM state
     const char* fn = "vpca_glm_logistic_begin";
     std::vector<int> idx;
     int rc = glm_samples(ctx, fn, pheno, covar, n_covar, idx);
@@ -2732,31 +2731,31 @@ int vpca_glm_logistic_begin(vpca_ctx* ctx, const double* pheno, const double* co
                     n_covar);
     rc = glm_upload(ctx, q, idx, Q, y, theta, true);
     if (rc != VPCA_OK) return rc;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    ctx->glm_q = q;
-    ctx->glm_logistic = 1;
-    ctx->glm_nreg = R;
-    ctx->glm_yty = 0.0;
-    if (n_used) *n_used = R;
+    glm_commit(ctx, q, true, R, 0.0, n_used);
     return VPCA_OK;
 }
 
-int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
-                        double* out, int32_t* out_err) {
-    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    int rc = rows_args(ctx, "vpca_glm_linear_bed", rows, nv, stride_bytes, (ctx->n + 3) / 4, out != nullptr && out_err != nullptr);
+namespace {
+// The three GLM *_bed calls: the argument and state rules (the state's model must be logistic, or linear), then the
+// rows through stage_rows with the model's kernels per chunk: glm_linear, or glm_logistic in firth_mode.  out_passes and
+// out_firth (logistic only) may be null.
+int glm_bed_rows(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
+                 int32_t counted_allele, bool logistic, int firth_mode, double* out, int32_t* out_err, int32_t* out_passes,
+                 uint8_t* out_firth) {
+    int rc = rows_args(ctx, fn, rows, nv, stride_bytes, (ctx->n + 3) / 4, out != nullptr && out_err != nullptr);
     if (rc != VPCA_OK) return rc;
     if (counted_allele != 1 && counted_allele != 2)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_linear_bed: counted_allele must be 1 (A1) or 2 (A2), not %d",
-                    counted_allele);
+        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: counted_allele must be 1 (A1) or 2 (A2), not %d", fn, counted_allele);
+    const char* begin = logistic ? "vpca_glm_logistic_begin" : "vpca_glm_begin";
     int q = 0, n_reg = 0;
     double yty = 0.0;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
-        if (ctx->glm_q == 0) return fail(ctx, VPCA_ERR_STATE, "vpca_glm_linear_bed needs a vpca_glm_begin since the last reset");
-        if (ctx->glm_logistic)
-            return fail(ctx, VPCA_ERR_STATE, "vpca_glm_linear_bed: the GLM state is logistic (vpca_glm_logistic_begin); "
-                        "a linear test needs vpca_glm_begin");
+        if (ctx->glm_q == 0) return fail(ctx, VPCA_ERR_STATE, "%s needs a %s since the last reset", fn, begin);
+        if (ctx->glm_logistic != (int)logistic)
+            return fail(ctx, VPCA_ERR_STATE, "%s: the GLM state is %s (%s); a %s test needs %s", fn,
+                        logistic ? "linear" : "logistic", logistic ? "vpca_glm_begin" : "vpca_glm_logistic_begin",
+                        logistic ? "logistic" : "linear", begin);
         q = ctx->glm_q;
         n_reg = ctx->glm_nreg;
         yty = ctx->glm_yty;
@@ -2765,83 +2764,37 @@ int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t 
     if (nv == 0) return VPCA_OK;
     const int n = ctx->n;
     const int64_t step = grm_step(nv, stride_bytes);
-    LaneGuard lg(ctx);
-    if (lg.rc != VPCA_OK) return lg.rc;
-    vpca_ctx::Lane& L = *lg.lane;
-    {
-        cudaError_t e = cudaSuccess;
-        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
-        if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * kGlmRec);
-        if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
-        if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
-        }
-    }
-    return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
-        CUDA_OK(ctx, glm_linear(d_rows, stride_bytes, (int)nvc, n, q, n_reg, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
-                                ctx->d_glm_z0.get(), yty, counted_allele, ctx->d_glm_sums.get(), ctx->d_glm_out.get(),
-                                ctx->d_glm_err.get(), L.stream));
-        CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
-                                     cudaMemcpyDeviceToHost, L.stream));
-        CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
-                                     cudaMemcpyDeviceToHost, L.stream));
-        ctx->c_launches += 3;
-        ctx->c_d2h += nvc * (6 * (int64_t)sizeof(double) + (int64_t)sizeof(int32_t));
-        return VPCA_OK;
-    });
-}
-
-namespace {
-// vpca_glm_logistic_bed (firth_mode 0) and vpca_glm_firth_bed: the argument and state rules, then the rows through
-// stage_rows with glm_firth's kernels per chunk.
-int glm_logistic_rows(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_t nv, int64_t stride_bytes,
-                      int32_t counted_allele, int firth_mode, double* out, int32_t* out_err, int32_t* out_passes,
-                      uint8_t* out_firth) {
-    int rc = rows_args(ctx, fn, rows, nv, stride_bytes, (ctx->n + 3) / 4, out != nullptr && out_err != nullptr);
-    if (rc != VPCA_OK) return rc;
-    if (counted_allele != 1 && counted_allele != 2)
-        return fail(ctx, VPCA_ERR_BAD_ARG, "%s: counted_allele must be 1 (A1) or 2 (A2), not %d", fn, counted_allele);
-    int q = 0;
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        if (ctx->glm_q == 0)
-            return fail(ctx, VPCA_ERR_STATE, "%s needs a vpca_glm_logistic_begin since the last reset", fn);
-        if (!ctx->glm_logistic)
-            return fail(ctx, VPCA_ERR_STATE, "%s: the GLM state is linear (vpca_glm_begin); a logistic test needs "
-                        "vpca_glm_logistic_begin", fn);
-        q = ctx->glm_q;
-    }
-    CUDA_OK(ctx, cudaSetDevice(ctx->cfg.device));
-    if (nv == 0) return VPCA_OK;
-    const int n = ctx->n;
-    const int64_t step = grm_step(nv, stride_bytes);
-    LaneGuard lg(ctx);
-    if (lg.rc != VPCA_OK) return lg.rc;
-    vpca_ctx::Lane& L = *lg.lane;
-    {
-        cudaError_t e = cudaSuccess;
-        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
-        if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * 6);
-        if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
-        if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
-        if (e == cudaSuccess) e = ctx->d_glm_passes.ensure(step);
-        if (e == cudaSuccess && firth_mode) e = ctx->d_glm_firth.ensure(step);
-        if (e == cudaSuccess && firth_mode == VPCA_GLM_FIRTH_FALLBACK) e = ctx->d_glm_idx.ensure(step);
-        if (e == cudaSuccess && firth_mode == VPCA_GLM_FIRTH_FALLBACK) e = ctx->d_glm_nf.ensure(1);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
-        }
-    }
     const bool fallback = firth_mode == VPCA_GLM_FIRTH_FALLBACK;
+    LaneGuard lg(ctx);
+    if (lg.rc != VPCA_OK) return lg.rc;
+    vpca_ctx::Lane& L = *lg.lane;
+    {
+        cudaError_t e = cudaSuccess;
+        for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = ctx->d_bed_rows[b].ensure(step * stride_bytes);
+        if (e == cudaSuccess) e = ctx->d_glm_sums.ensure(step * (logistic ? 6 : kGlmRec));
+        if (e == cudaSuccess) e = ctx->d_glm_out.ensure(step * 6);
+        if (e == cudaSuccess) e = ctx->d_glm_err.ensure(step);
+        if (e == cudaSuccess && logistic) e = ctx->d_glm_passes.ensure(step);
+        if (e == cudaSuccess && firth_mode) e = ctx->d_glm_firth.ensure(step);
+        if (e == cudaSuccess && fallback) e = ctx->d_glm_idx.ensure(step);
+        if (e == cudaSuccess && fallback) e = ctx->d_glm_nf.ensure(1);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(ctx, VPCA_ERR_NOMEM, "GLM buffers: %s", cudaGetErrorString(e));
+        }
+    }
     return stage_rows(ctx, L, rows, nv, stride_bytes, step, bed_rows(ctx), [&](int, const uint8_t* d_rows, int64_t v, int64_t nvc) -> int {
-        CUDA_OK(ctx, glm_firth(d_rows, stride_bytes, (int)nvc, n, q, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
-                               ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele, ctx->d_glm_sums.get(),
-                               ctx->d_glm_out.get(), ctx->d_glm_err.get(), ctx->d_glm_passes.get(), firth_mode,
-                               firth_mode ? ctx->d_glm_firth.get() : nullptr, fallback ? ctx->d_glm_idx.get() : nullptr,
-                               fallback ? ctx->d_glm_nf.get() : nullptr, L.stream));
+        if (logistic)
+            CUDA_OK(ctx, glm_logistic(d_rows, stride_bytes, (int)nvc, n, q, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
+                                      ctx->d_glm_case.get(), ctx->d_glm_z0.get(), counted_allele, ctx->d_glm_sums.get(),
+                                      ctx->d_glm_out.get(), ctx->d_glm_err.get(), ctx->d_glm_passes.get(), firth_mode,
+                                      firth_mode ? ctx->d_glm_firth.get() : nullptr,
+                                      fallback ? ctx->d_glm_idx.get() : nullptr, fallback ? ctx->d_glm_nf.get() : nullptr,
+                                      L.stream));
+        else
+            CUDA_OK(ctx, glm_linear(d_rows, stride_bytes, (int)nvc, n, q, n_reg, ctx->d_glm_Qx.get(), ctx->d_glm_mask.get(),
+                                    ctx->d_glm_z0.get(), yty, counted_allele, ctx->d_glm_sums.get(), ctx->d_glm_out.get(),
+                                    ctx->d_glm_err.get(), L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out + v * 6, ctx->d_glm_out.get(), (size_t)nvc * 6 * sizeof(double),
                                      cudaMemcpyDeviceToHost, L.stream));
         CUDA_OK(ctx, cudaMemcpyAsync(out_err + v, ctx->d_glm_err.get(), (size_t)nvc * sizeof(int32_t),
@@ -2852,9 +2805,10 @@ int glm_logistic_rows(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_
         if (out_firth)
             CUDA_OK(ctx, cudaMemcpyAsync(out_firth + v, ctx->d_glm_firth.get(), (size_t)nvc, cudaMemcpyDeviceToHost,
                                          L.stream));
-        // count kernels, then the maximum-likelihood and finish kernels (5 as counted before the Firth tests), the
-        // selection and the Firth kernel (fallback), or the Firth and finish kernels (always)
-        ctx->c_launches += firth_mode == 0 ? 5 : fallback ? 6 : 4;
+        // linear: 3 as counted since the linear tests began; logistic: the count kernels, then the maximum-likelihood
+        // and finish kernels (5 as counted before the Firth tests), the selection and the Firth kernel (fallback), or
+        // the Firth and finish kernels (always)
+        ctx->c_launches += !logistic ? 3 : firth_mode == 0 ? 5 : fallback ? 6 : 4;
         ctx->c_d2h += nvc * (6 * (int64_t)sizeof(double) + (out_passes ? 2 : 1) * (int64_t)sizeof(int32_t) +
                              (out_firth ? 1 : 0));
         return VPCA_OK;
@@ -2862,11 +2816,18 @@ int glm_logistic_rows(vpca_ctx* ctx, const char* fn, const uint8_t* rows, int64_
 }
 }  // namespace
 
+int vpca_glm_linear_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
+                        double* out, int32_t* out_err) {
+    if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
+    return glm_bed_rows(ctx, "vpca_glm_linear_bed", rows, nv, stride_bytes, counted_allele, false, 0, out, out_err,
+                        nullptr, nullptr);
+}
+
 int vpca_glm_logistic_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
                           double* out, int32_t* out_err, int32_t* out_passes) {
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
-    return glm_logistic_rows(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, counted_allele, 0, out, out_err,
-                             out_passes, nullptr);
+    return glm_bed_rows(ctx, "vpca_glm_logistic_bed", rows, nv, stride_bytes, counted_allele, true, 0, out, out_err,
+                        out_passes, nullptr);
 }
 
 int vpca_glm_firth_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t stride_bytes, int32_t counted_allele,
@@ -2874,8 +2835,8 @@ int vpca_glm_firth_bed(vpca_ctx* ctx, const uint8_t* rows, int64_t nv, int64_t s
     if (ctx == nullptr) return fail(nullptr, VPCA_ERR_BAD_ARG, "ctx is NULL");
     if (mode != VPCA_GLM_FIRTH_FALLBACK && mode != VPCA_GLM_FIRTH_ALWAYS)
         return fail(ctx, VPCA_ERR_BAD_ARG, "vpca_glm_firth_bed: mode must be 1 (fallback) or 2 (always), not %d", mode);
-    return glm_logistic_rows(ctx, "vpca_glm_firth_bed", rows, nv, stride_bytes, counted_allele, mode, out, out_err,
-                             out_passes, out_firth);
+    return glm_bed_rows(ctx, "vpca_glm_firth_bed", rows, nv, stride_bytes, counted_allele, true, mode, out, out_err,
+                        out_passes, out_firth);
 }
 
 // ---- sample QC (samples.cu, DESIGN.md 11) -------------------------------------------------------------------------------

@@ -266,17 +266,15 @@ cudaError_t glm_linear(const uint8_t* d_rows, int64_t stride, int nv, int n, int
 // Logistic tests (DESIGN.md 16) of nv .bed rows: the counts into d_cnt (nv x 6: OBS_CT, sum g, sum g^2 under d_mask, then
 // under d_case), then d_out[v * 6 ..] = OBS_CT, A1_FREQ, BETA, SE, Z, P, d_err[v] (VPCA_GLM_*) and d_passes[v] (Newton
 // passes, 0 for a variant flagged before any).  d_Qx: n rows [q_0 .. q_{q-1}, y, 0 .., mask] with y in {0, 1}; d_case:
-// the regression samples with y = 1 as bits; d_theta0: the null fit in the basis Q (q).  Never synchronises.
+// the regression samples with y = 1 as bits; d_theta0: the null fit in the basis Q (q).  firth_mode 0: the
+// maximum-likelihood fit alone.  With Firth's penalized likelihood (DESIGN.md 17): VPCA_GLM_FIRTH_FALLBACK, then the
+// Firth fit of the variants the maximum-likelihood fit ends with LOGISTIC_CONVERGE_FAIL after a pass, listed on the
+// device in d_idx (nv) and d_nf (1); VPCA_GLM_FIRTH_ALWAYS, the Firth fit alone; d_firth[v] (nv) = 1 where the Firth fit
+// ran.  d_firth, d_idx and d_nf are unused in mode 0.  Never synchronises.
 cudaError_t glm_logistic(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
                          const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
-                         double* d_out, int32_t* d_err, int32_t* d_passes, cudaStream_t stream);
-// Firth tests (DESIGN.md 17): glm_logistic with firth_mode VPCA_GLM_FIRTH_FALLBACK (then the Firth fit of the variants the
-// maximum-likelihood fit ends with LOGISTIC_CONVERGE_FAIL after a pass, listed on the device in d_idx (nv) and d_nf (1))
-// or VPCA_GLM_FIRTH_ALWAYS (the Firth fit alone); d_firth[v] (nv) = 1 where the Firth fit ran.  Never synchronises.
-cudaError_t glm_firth(const uint8_t* d_rows, int64_t stride, int nv, int n, int q, const double* d_Qx,
-                      const uint8_t* d_mask, const uint8_t* d_case, const double* d_theta0, int counted, double* d_cnt,
-                      double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode, uint8_t* d_firth, int32_t* d_idx,
-                      int32_t* d_nf, cudaStream_t stream);
+                         double* d_out, int32_t* d_err, int32_t* d_passes, int firth_mode, uint8_t* d_firth,
+                         int32_t* d_idx, int32_t* d_nf, cudaStream_t stream);
 
 // ---- sample QC (samples.cu, DESIGN.md 11) ---------------------------------------------------------------------------
 // Adds the MISSING calls (code 01) of each of the n samples over nv .bed rows (row v at d_rows + v * pitch) to

@@ -855,26 +855,31 @@ class NativePca:
         none) of the linear tests; the intercept is added.  Returns the regression samples (finite phenotype and
         covariates).  VPCA_ERR_BAD_ARG for +-Inf, more than 31 covariates, too few samples, a constant phenotype or a
         collinear covariate."""
+        return self._glm_begin(self._lib.vpca_glm_begin, pheno, covar)
+
+    def _glm_begin(self, fn, pheno, covar) -> int:
         y = np.ascontiguousarray(pheno, dtype=np.float64).reshape(-1)
         if y.shape[0] != self.n:
             raise VpcaError(VPCA_ERR_BAD_ARG, f"pheno must have {self.n} entries")
         c = np.zeros((self.n, 0)) if covar is None else np.ascontiguousarray(covar, dtype=np.float64).reshape(self.n, -1)
         m = ctypes.c_int64(0)
-        self._check(self._lib.vpca_glm_begin(self._h, _host_ptr(y), _host_ptr(c) if c.shape[1] else None, c.shape[1],
-                                             ctypes.byref(m)))
+        self._check(fn(self._h, _host_ptr(y), _host_ptr(c) if c.shape[1] else None, c.shape[1], ctypes.byref(m)))
         return int(m.value)
+
+    def _glm_bed(self, fn, rows, counted, *extra, dtypes=()):
+        """Calls fn(ctx, rows, V, stride, counted, *extra, stats, err, *outputs) with outputs of dtypes -> (stats (V, 6),
+        err (V,), *outputs (V,))."""
+        b, ptr = _bed_rows(rows)
+        nv = b.shape[0]
+        outs = [np.zeros((max(nv, 1), 6), np.float64)] + [np.zeros(max(nv, 1), t) for t in (np.int32, *dtypes)]
+        self._check(fn(self._h, ptr, nv, b.shape[1], int(counted), *extra, *(_host_ptr(o) for o in outs)))
+        return tuple(o[:nv] for o in outs)
 
     def glmLinearBed(self, rows: np.ndarray, counted: int = 1):
         """Linear tests of PLINK .bed rows ((V, stride) uint8 of this context's samples; a .bed memmap is read in place)
         against the phenotype of glmBegin -> (stats (V, 6) float64: OBS_CT, A1_FREQ, BETA, SE, T_STAT, P, NaN where
         undefined; err (V,) int32: index into GLM_ERRCODES).  counted: 1 counts A1, 2 counts A2.  Synchronises."""
-        b, ptr = _bed_rows(rows)
-        nv = b.shape[0]
-        out = np.zeros((max(nv, 1), 6), np.float64)
-        err = np.zeros(max(nv, 1), np.int32)
-        self._check(self._lib.vpca_glm_linear_bed(self._h, ptr, nv, b.shape[1],
-                                                  int(counted), _host_ptr(out), _host_ptr(err)))
-        return out[:nv], err[:nv]
+        return self._glm_bed(self._lib.vpca_glm_linear_bed, rows, counted)
 
     # -- logistic association tests (vpca.h, DESIGN.md 16) ---------------------------------------------------------------
     def glmLogisticBegin(self, pheno, covar=None) -> int:
@@ -882,29 +887,14 @@ class NativePca:
         float64, NaN = missing; None for none) of the logistic tests; the intercept is added.  Returns the regression
         samples.  VPCA_ERR_BAD_ARG for what glmBegin refuses, a value outside {0, 1, NaN}, no case or no control, or a
         null model that does not converge."""
-        y = np.ascontiguousarray(pheno, dtype=np.float64).reshape(-1)
-        if y.shape[0] != self.n:
-            raise VpcaError(VPCA_ERR_BAD_ARG, f"pheno must have {self.n} entries")
-        c = np.zeros((self.n, 0)) if covar is None else np.ascontiguousarray(covar, dtype=np.float64).reshape(self.n, -1)
-        m = ctypes.c_int64(0)
-        self._check(self._lib.vpca_glm_logistic_begin(self._h, _host_ptr(y), _host_ptr(c) if c.shape[1] else None,
-                                                      c.shape[1], ctypes.byref(m)))
-        return int(m.value)
+        return self._glm_begin(self._lib.vpca_glm_logistic_begin, pheno, covar)
 
     def glmLogisticBed(self, rows: np.ndarray, counted: int = 1):
         """Logistic tests of PLINK .bed rows ((V, stride) uint8 of this context's samples; a .bed memmap is read in
         place) against the phenotype of glmLogisticBegin -> (stats (V, 6) float64: OBS_CT, A1_FREQ, BETA, SE, Z, P, NaN
         where undefined; err (V,) int32: index into GLM_ERRCODES; passes (V,) int32: Newton passes).  counted: 1 counts
         A1, 2 counts A2.  Synchronises."""
-        b, ptr = _bed_rows(rows)
-        nv = b.shape[0]
-        out = np.zeros((max(nv, 1), 6), np.float64)
-        err = np.zeros(max(nv, 1), np.int32)
-        passes = np.zeros(max(nv, 1), np.int32)
-        self._check(self._lib.vpca_glm_logistic_bed(self._h, ptr, nv,
-                                                    b.shape[1], int(counted), _host_ptr(out), _host_ptr(err),
-                                                    _host_ptr(passes)))
-        return out[:nv], err[:nv], passes[:nv]
+        return self._glm_bed(self._lib.vpca_glm_logistic_bed, rows, counted, dtypes=(np.int32,))
 
     # -- Firth-penalized logistic tests (vpca.h, DESIGN.md 17) -----------------------------------------------------------
     def glmFirthBed(self, rows: np.ndarray, counted: int = 1, mode: str = "fallback"):
@@ -914,15 +904,8 @@ class NativePca:
         uint8: 1 where the Firth fit ran).  Synchronises."""
         if mode not in GLM_FIRTH_MODES:
             raise VpcaError(VPCA_ERR_BAD_ARG, f"mode must be one of {', '.join(GLM_FIRTH_MODES)}, not {mode!r}")
-        b, ptr = _bed_rows(rows)
-        nv = b.shape[0]
-        out = np.zeros((max(nv, 1), 6), np.float64)
-        err = np.zeros(max(nv, 1), np.int32)
-        passes = np.zeros(max(nv, 1), np.int32)
-        firth = np.zeros(max(nv, 1), np.uint8)
-        self._check(self._lib.vpca_glm_firth_bed(self._h, ptr, nv, b.shape[1], int(counted), GLM_FIRTH_MODES[mode],
-                                                 _host_ptr(out), _host_ptr(err), _host_ptr(passes), _host_ptr(firth)))
-        return out[:nv], err[:nv], passes[:nv], firth[:nv]
+        return self._glm_bed(self._lib.vpca_glm_firth_bed, rows, counted, GLM_FIRTH_MODES[mode],
+                             dtypes=(np.int32, np.uint8))
 
     def hweExact(self, counts) -> np.ndarray:
         """Exact HWE p-values of (V, 4) int32 counts (HOM_A1, HET, HOM_A2, MISSING; MISSING ignored) -> (V,) float64."""

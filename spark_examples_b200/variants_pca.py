@@ -698,34 +698,43 @@ class VariantsPcaDriver:
         else:
             check_glm_quantitative(glm.y[reg], glm.name)
 
-    def glmLinear(self, callsets: CallsRdd, glm: "GlmInput", qc_keep: Optional[np.ndarray] = None):
-        """After the PCs (or the projection): the linear test of every variant that passes variant QC, in file order, on
-        this run's rows, with the intercept, the run's PCs and the --covar columns as covariates.  Writes
-        P.<PHENO>.glm.linear and prints the `GLM linear:` line.  Returns (stats (V, 6), err (V,))."""
+    def _glmRun(self, callsets: CallsRdd, glm: "GlmInput", qc_keep, begin, bed, spec):
+        """The driver loop of every association test: begin(nat, y, covariates) with the intercept, the run's PCs and the
+        --covar columns as covariates, then bed(nat, rows, counted) on every variant that passes variant QC, in file
+        order, on this run's rows.  spec: (dtype, shape of one variant's entry) of each output of bed.  Returns (the
+        regression samples, the outputs concatenated over the partitions, the tested variants' .bim records, the
+        counted allele, the covariates' description for the summary line)."""
         from . import plink
         pcs = np.asarray(self.components, np.float64)
         k = pcs.shape[1]
         nat = self._native(callsets.n_samples)
-        used = nat.glmBegin(glm.y, np.concatenate([pcs, glm.c], axis=1))
-        stats, errs, tested = [], [], []
+        used = begin(nat, glm.y, np.concatenate([pcs, glm.c], axis=1))
+        chunks, tested = [], []
         counted = plink.COUNT_A1
         for part in callsets.partitions:
             sel = np.ones(part.nv, bool) if qc_keep is None else np.asarray(qc_keep[part.v0:part.v0 + part.nv], bool)
             rows = part.bed._map[part.v0:part.v0 + part.nv]        # read in place when every variant is tested
-            st, er = nat.glmLinearBed(rows if sel.all() else rows[sel], part.counted)
-            stats.append(np.asarray(st, np.float64).reshape(-1, 6))
-            errs.append(np.asarray(er, np.int32).reshape(-1))
+            chunks.append(bed(nat, rows if sel.all() else rows[sel], part.counted))
             tested.extend((part.v0 + np.flatnonzero(sel)).tolist())
             counted = part.counted
-        stats = np.concatenate(stats) if stats else np.zeros((0, 6))
-        errs = np.concatenate(errs) if errs else np.zeros(0, np.int32)
+        outs = [np.concatenate([np.asarray(ch[i], t).reshape((-1,) + tail) for ch in chunks]) if chunks
+                else np.zeros((0,) + tail, t) for i, (t, tail) in enumerate(spec)]
         bim = plink.read_bim(self.conf.bedPath())
-        write_glm_linear(f"{self.conf.outputPath()}.{glm.name}.glm.linear", [bim[j] for j in tested], counted, stats, errs)
-        n = callsets.n_samples
         c = glm.c.shape[1]
-        covs = f"intercept, {k} PCs" + (f", {c} from {glm.covar_path}" if glm.covar_path else "")
+        covs = f"{1 + k + c} covariates (intercept, {k} PCs" + (f", {c} from {glm.covar_path}" if glm.covar_path else "")
+        return used, outs, [bim[j] for j in tested], counted, covs + ")"
+
+    def glmLinear(self, callsets: CallsRdd, glm: "GlmInput", qc_keep: Optional[np.ndarray] = None):
+        """After the PCs (or the projection): the linear test of every variant that passes variant QC, in file order, on
+        this run's rows, with the intercept, the run's PCs and the --covar columns as covariates.  Writes
+        P.<PHENO>.glm.linear and prints the `GLM linear:` line.  Returns (stats (V, 6), err (V,))."""
+        used, (stats, errs), bim, counted, covs = self._glmRun(
+            callsets, glm, qc_keep, lambda nat, y, c: nat.glmBegin(y, c), lambda nat, rows, a: nat.glmLinearBed(rows, a),
+            ((np.float64, (6,)), (np.int32, ())))
+        write_glm_linear(f"{self.conf.outputPath()}.{glm.name}.glm.linear", bim, counted, stats, errs)
+        n = callsets.n_samples
         print(f"GLM linear: {glm.name} on {used} of {n} samples ({n - used} without a phenotype or covariate), "
-              f"{1 + k + c} covariates ({covs}); {len(errs)} variants tested, {int(np.count_nonzero(errs))} with an "
+              f"{covs}; {len(errs)} variants tested, {int(np.count_nonzero(errs))} with an "
               f"ERRCODE; lambda_GC = {lambda_gc(stats, errs)!r}.")
         return stats, errs
 
@@ -734,48 +743,29 @@ class VariantsPcaDriver:
         and prints the `GLM logistic:` line.  Returns (stats (V, 6), err (V,), passes (V,)).  With --glm-firth
         (DESIGN.md 17): fallback writes P.<PHENO>.glm.logistic.hybrid with the FIRTH? column and counts the Firth fits in
         the line; always writes P.<PHENO>.glm.firth and prints `GLM Firth:`."""
-        from . import plink
-        pcs = np.asarray(self.components, np.float64)
-        k = pcs.shape[1]
-        nat = self._native(callsets.n_samples)
-        used = nat.glmLogisticBegin(glm.y, np.concatenate([pcs, glm.c], axis=1))
-        stats, errs, passes, firths, tested = [], [], [], [], []
-        counted = plink.COUNT_A1
-        for part in callsets.partitions:
-            sel = np.ones(part.nv, bool) if qc_keep is None else np.asarray(qc_keep[part.v0:part.v0 + part.nv], bool)
-            rows = part.bed._map[part.v0:part.v0 + part.nv]        # read in place when every variant is tested
-            if glm.firth:
-                st, er, ps, fi = nat.glmFirthBed(rows if sel.all() else rows[sel], part.counted, glm.firth)
-                firths.append(np.asarray(fi, np.uint8).reshape(-1))
-            else:
-                st, er, ps = nat.glmLogisticBed(rows if sel.all() else rows[sel], part.counted)
-            stats.append(np.asarray(st, np.float64).reshape(-1, 6))
-            errs.append(np.asarray(er, np.int32).reshape(-1))
-            passes.append(np.asarray(ps, np.int32).reshape(-1))
-            tested.extend((part.v0 + np.flatnonzero(sel)).tolist())
-            counted = part.counted
-        stats = np.concatenate(stats) if stats else np.zeros((0, 6))
-        errs = np.concatenate(errs) if errs else np.zeros(0, np.int32)
-        passes = np.concatenate(passes) if passes else np.zeros(0, np.int32)
-        bim = plink.read_bim(self.conf.bedPath())
-        firths = np.concatenate(firths) if firths else np.zeros(0, np.uint8)
+        spec = ((np.float64, (6,)), (np.int32, ()), (np.int32, ()))
+        if glm.firth:
+            bed = lambda nat, rows, a: nat.glmFirthBed(rows, a, glm.firth)   # noqa: E731
+            spec += ((np.uint8, ()),)
+        else:
+            bed = lambda nat, rows, a: nat.glmLogisticBed(rows, a)   # noqa: E731
+        used, outs, bim, counted, covs = self._glmRun(callsets, glm, qc_keep,
+                                                      lambda nat, y, c: nat.glmLogisticBegin(y, c), bed, spec)
+        stats, errs, passes = outs[:3]
         fitted = ""
         if glm.firth == "fallback":
-            write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.glm.logistic.hybrid", [bim[j] for j in tested],
-                               counted, stats, errs, firths)
-            fitted = f", {int(np.count_nonzero(firths))} fitted by Firth regression"
+            write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.glm.logistic.hybrid", bim, counted, stats, errs,
+                               outs[3])
+            fitted = f", {int(np.count_nonzero(outs[3]))} fitted by Firth regression"
         else:
             ext = "glm.firth" if glm.firth == "always" else "glm.logistic"
-            write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.{ext}", [bim[j] for j in tested], counted, stats,
-                               errs)
+            write_glm_logistic(f"{self.conf.outputPath()}.{glm.name}.{ext}", bim, counted, stats, errs)
         n = callsets.n_samples
-        c = glm.c.shape[1]
         reg = np.isfinite(glm.y) & np.isfinite(glm.c).all(axis=1)
         cases = int(np.count_nonzero(glm.y[reg] == 1.0))
-        covs = f"intercept, {k} PCs" + (f", {c} from {glm.covar_path}" if glm.covar_path else "")
         model = "Firth" if glm.firth == "always" else "logistic"
         print(f"GLM {model}: {glm.name} on {used} of {n} samples ({cases} cases, {used - cases} controls, {n - used} "
-              f"without a phenotype or covariate), {1 + k + c} covariates ({covs}); {len(errs)} variants tested, "
+              f"without a phenotype or covariate), {covs}; {len(errs)} variants tested, "
               f"{int(np.count_nonzero(errs))} with an ERRCODE{fitted}; lambda_GC = {lambda_gc(stats, errs)!r}.")
         return stats, errs, passes
 
@@ -1207,6 +1197,11 @@ def _glm_number(x: float) -> str:
     return "NA" if not np.isfinite(x) else repr(float(x))
 
 
+def _glm_row_prefix(b, counted: int, st) -> str:
+    """The first seven columns of a .glm.* row, through A1_FREQ and its tab."""
+    return f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
+
+
 def write_glm_linear(path: str, bim, counted: int, stats: np.ndarray, errs: np.ndarray) -> None:
     """P.<PHENO>.glm.linear, tab-separated, one line per tested variant in file order (PLINK 2's hide-covar columns): REF
     is A2 and ALT is A1 as in .afreq, A1 the counted allele, TEST ADD; numbers as the shortest text that reads back as the
@@ -1214,8 +1209,7 @@ def write_glm_linear(path: str, bim, counted: int, stats: np.ndarray, errs: np.n
     with open(path, "w", encoding="utf-8") as fh:
         fh.write("#CHROM\tPOS\tID\tREF\tALT\tA1\tA1_FREQ\tTEST\tOBS_CT\tBETA\tSE\tT_STAT\tP\tERRCODE\n")
         fh.write("".join(
-            f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
-            f"ADD\t{int(st[0])}\t{_glm_number(st[2])}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
+            f"{_glm_row_prefix(b, counted, st)}ADD\t{int(st[0])}\t{_glm_number(st[2])}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
             f"{_glm_number(st[5])}\t{native.GLM_ERRCODES[int(e)]}\n"
             for b, st, e in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist())))
 
@@ -1230,8 +1224,7 @@ def write_glm_logistic(path: str, bim, counted: int, stats: np.ndarray, errs: np
     with open(path, "w", encoding="utf-8") as fh:
         fh.write(f"#CHROM\tPOS\tID\tREF\tALT\tA1\tA1_FREQ\t{fcol}TEST\tOBS_CT\tOR\tLOG(OR)_SE\tZ_STAT\tP\tERRCODE\n")
         fh.write("".join(
-            f"{b.contig}\t{b.position}\t{b.id}\t{b.a2}\t{b.a1}\t{b.a1 if counted == 1 else b.a2}\t{_glm_number(st[1])}\t"
-            f"{fl}ADD\t{int(st[0])}\t{_glm_number(np.exp(st[2]))}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
+            f"{_glm_row_prefix(b, counted, st)}{fl}ADD\t{int(st[0])}\t{_glm_number(np.exp(st[2]))}\t{_glm_number(st[3])}\t{_glm_number(st[4])}\t"
             f"{_glm_number(st[5])}\t{native.GLM_ERRCODES[int(e)]}\n"
             for b, st, e, fl in zip(bim, np.asarray(stats, np.float64).tolist(), np.asarray(errs).tolist(), flags)))
 
